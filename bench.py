@@ -1,18 +1,20 @@
 #!/usr/bin/env python
-"""bench.py -- LM iterations/s of the B200-native DynOSAM batch solver (BASELINE.json metric).
+"""bench.py -- LM iterations/s of the H100-native DynOSAM batch solver (BASELINE.json metric).
 
 One "step" = one outer Levenberg-Marquardt iteration (1 materialising linearize + >= 1 damped Schur solve +
 >= 1 chi^2 sweep) on the synthetic 10k-key-frame / 100-object / 2M-landmark dynamic graph (BASELINE.json
-configs[4]; it fits one B200, so it is also the N=1 workload).  N > 1: landmarks are sharded in time over the ranks and
+configs[4]; its run peaks at 27 GB of device memory, so it fits one 80 GB H100 and is also the N=1 workload).  N > 1: landmarks are sharded in time over the ranks and
 the reduced solve is distributed (one cell of the banded system per rank: a reduce per cell, an all-reduce of the small
 boundary-separator system and of the pose update); strong scaling: total work fixed.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config C5|C3|C2|C1] [--scale s]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config C5|C3|C2|C1] [--scale s] [--dump-outputs DIR]
     python bench.py --impl reference ...    # CPU arm: the oracle port on the host cores, same config at full size
 
 The JSON line carries `roofline` (Jacobian-build kernel vs measured HBM bandwidth), `reduced_solve` (vs the fp64 rate
 measured on the box), `e2e` (through the C ABI from host arrays), `cpu_baseline` + `parity_check` (one full-size LM
 iteration of the oracle port, compared with the GPU's first iteration) and `configs` (C2, C3, front-end C4).
+--dump-outputs DIR writes what the timed optimize() returned after its last step as DIR/<name>.npy (see dump_outputs), so
+that two builds can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -248,17 +250,31 @@ def cpu_oracle_leg(cfg_name, formulation, seed, scale, iters):
     return r
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant Jacobian-build kernel, from an `ncu --set full`
-# capture of this very launch (a counter value cannot be measured inside a timed run); the capture is named next to it.
-# Only valid for the exact launch that was profiled: C5 at full scale on one GPU; anything else reports null.
-NCU_TRAFFIC = {("C5", "hybrid", 5, 11376204): (576.973e6 + 4550.677e6, "profiles/r02_final.md section 3 (ncu --set full of the same launch)")}
+DUMP_BUDGET = 64 << 20      # bytes of --dump-outputs in all
 
 
-def ncu_traffic(args, world, blk):
-    if world != 1 or args.scale != 1.0:
-        return None, None
-    v = NCU_TRAFFIC.get((args.config, args.formulation, int(blk.type), int(blk.n)))
-    return (float(v[0]), v[1]) if v else (None, None)
+def dump_outputs(out_dir, s, st):
+    """Writes what the timed optimize() hands its caller after the last step, float64: pose [n_pose, 12] (row-major
+    3x4 [R | t]), point [n_point, 3], flow [n_flow, 2] (when the problem has optical-flow variables) and chi2 = [error at
+    the initial values, error after the last step].  With N > 1 ranks it runs on rank 0 only, so `point` holds rank 0's
+    shard (its kept landmarks, in that rank's order) and chi2 is the global error.  When the arrays exceed DUMP_BUDGET,
+    every variable array is cut to the same share of its rows, chosen by numpy.random.default_rng(0) and kept in ascending
+    order (the same rows on every run with the same arguments)."""
+    pose, point, flow = s.values()
+    arrays = {"pose": pose, "point": point, "chi2": np.array([st["error_initial"], st["error_final"]])}
+    if flow.shape[0]:
+        arrays["flow"] = flow
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_BUDGET:
+        frac = 0.95*DUMP_BUDGET/total
+        rng = np.random.default_rng(0)
+        for k in ("pose", "point", "flow"):
+            if k in arrays:
+                a = arrays[k]
+                arrays[k] = a[np.sort(rng.choice(a.shape[0], int(a.shape[0]*frac), replace=False))]
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def quick_config_rate(cfg_name, formulation, seed, device, steps=3):
@@ -293,6 +309,7 @@ def main():
     ap.add_argument("--cells", type=int, default=0, help="cells of the reduced solve (0 automatic, -1 plain band)")
     ap.add_argument("--replicated-solve", action="store_true", help="N > 1: all-reduce the reduced system and solve it on every rank")
     ap.add_argument("--tune", default="", help="name=value,... performance parameters (dynoba_set_tuning)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the variables and chi^2 of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     K, W = args.steps, max(args.warmup, 0)
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -303,7 +320,7 @@ def main():
               "parallelism": (f"landmarks sharded in time x{world}; reduced solve " + ("replicated" if args.replicated_solve else "distributed: one cell of the band per rank, "
                               "reduce per cell + all-reduce of the boundary system")) if world > 1 else "1 GPU",
               "seed": args.seed,
-              "l2_policy": "working set (Jacobian tiles, GBs) >> 126 MB L2; no explicit flush",
+              "l2_policy": "working set (Jacobian tiles, GBs) >> 50 MB L2; no explicit flush",
               "noise": "sigma_point 0.2, Huber k 1e-4, LM defaults with rel/abs tol 0 so that exactly K iterations run",
               "timed_region": "LM iterations 1..K from the initial values (after W warm-up iterations and a value reset)"}
 
@@ -397,6 +414,10 @@ def main():
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms_total = float(ms[0]); steps_done = st["iterations"]
     value = steps_done/(ms_total*1e-3) if ms_total > 0 else 0.0
+    if steps_done != K:
+        print(f"bench.py: LM stopped after {steps_done} of {K} iterations (converged or lambda bound)", file=sys.stderr)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, s, st)
 
     # ---- end-to-end through the C-ABI with host buffers: ingest (H2D) + K iterations + read-back (D2H)
     e2e = None
@@ -433,12 +454,11 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = peaks.get("hbm_gbs", 6650.0); peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback"
+    peak = peaks.get("hbm_gbs", 3350.0); peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "H100 SXM data sheet (HBM3)"
     lin = float(np.median(lin_ms))
     pass_ach = info["jacobian_bytes"]/(lin*1e-3)/1e9 if lin > 0 else 0.0
     dms = float(np.median(dom_ms))
     ach = dom_bytes/(dms*1e-3)/1e9 if dms > 0 else 0.0
-    traffic, traffic_src = ncu_traffic(args, world, prob.blocks[dom])
     from dynosam_b200.problem import TYPE_NAMES
     solves = max(st["inner_iterations"], 1)
     chol_flops = float(info["reduced_dim"])*float(info["bandwidth"])**2
@@ -452,7 +472,7 @@ def main():
            "roofline": {"kernel": f"linearize_kernel<{TYPE_NAMES[prob.blocks[dom].type]}> (materialising Jacobian build of the largest factor block, "
                                   f"{prob.blocks[dom].n} factors)",
                         "bound": "hbm", "achieved": ach, "peak": peak, "peak_source": peak_src, "unit": "GB/s",
-                        "frac": ach/peak if peak else None, "traffic": traffic, "traffic_source": traffic_src,
+                        "frac": ach/peak if peak else None,
                         "algorithmic_bytes": int(dom_bytes), "ms_per_launch": dms,
                         "whole_pass": {"algorithmic_bytes": info["jacobian_bytes"], "ms": lin, "achieved": pass_ach,
                                        "frac": pass_ach/peak if peak else None,
@@ -460,7 +480,7 @@ def main():
            "reduced_solve": {"kernel": "band_cholesky_dataflow_kernel_v3 + band_backward_cluster_kernel (this rank's share)", "bound": "fp64 latency chain / DMMA",
                              "flops_per_solve": chol_flops, "note": "n*bw^2 of the plain band Cholesky, whole system; spiked chains do up to 4x that per column",
                              "ms_per_solve": solve_ms, "achieved_tflops": chol_flops/(solve_ms*1e-3)/1e12 if solve_ms > 0 else None,
-                             "fp64_peak_tflops": fp64_peak, "fp64_peak_source": "dynoba_fp64_rate: register-only DFMA kernel on this GPU (MEASURED_PEAKS.json has no fp64 entry)",
+                             "fp64_peak_tflops": fp64_peak, "fp64_peak_source": "dynoba_fp64_rate: best of register-only DFMA, DMMA m8n8k4 and DMMA m16n8k16 kernels on this GPU",
                              "frac": chol_flops/(solve_ms*1e-3)/1e12/fp64_peak if solve_ms > 0 and fp64_peak > 0 else None}}
     if e2e:
         out["e2e"] = e2e

@@ -138,7 +138,7 @@ def run_dynoba(n, warmup, streaming=True):
            "klt_device_ms_per_frame": float(np.mean(klt_ms)), "h2d_bytes_per_frame": int(h2d),
            "note": "end to end through the C ABI from host images (H2D/D2H inside the timed region); a frame moves a few MB and "
                    "launches ~40 small kernels, so it is PCIe / launch bound, not HBM bound: the dense passes' 21 B/px "
-                   f"({dense_bytes/1e6:.1f} MB) would take {dense_bytes/6.57e12*1e6:.1f} us at the measured HBM rate"}
+                   f"({dense_bytes/1e6:.1f} MB) would take {dense_bytes/3.35e12*1e6:.1f} us at the H100 data-sheet HBM rate (3.35 TB/s)"}
     return out
 
 

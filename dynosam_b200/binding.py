@@ -1,5 +1,5 @@
 """ctypes binding of libdynoba.so (include/dynoba.h).  No CPU fallback: a missing library or a
-missing sm_100 device raises."""
+missing sm_90 device raises."""
 from __future__ import annotations
 
 import ctypes as C
@@ -154,7 +154,7 @@ class Solver:
         self.h = C.c_void_p()
         st = self.lib.dynoba_create(device, C.byref(self.h))
         if st != OK:
-            raise DynobaError(st, self.lib.dynoba_status_string(st).decode() + " (no sm_100 CUDA device: libdynoba has no CPU path)")
+            raise DynobaError(st, self.lib.dynoba_status_string(st).decode() + " (no sm_90 CUDA device: libdynoba has no CPU path)")
         self.problem = None
         self._cb = None
         if problem is not None:

@@ -102,7 +102,7 @@ PinnedArena g_arena;
 // Process-wide cache of device allocations: a closed solver's blocks are kept and handed to the next one that asks for
 // (about) the same size, because cudaMalloc / cudaFree of multi-GB blocks cost hundreds of milliseconds per optimize()
 // call when the caller builds one solver per batch.  DYNOBA_NO_DEVCACHE=1 turns it off; the cache is trimmed when an
-// allocation fails or when it holds more than DYNOBA_DEVCACHE_GB (default 96) gigabytes.
+// allocation fails or when it holds more than DYNOBA_DEVCACHE_GB (default 48, 60 % of an 80 GB H100) gigabytes.
 namespace {
 struct DevCache {
   std::mutex mu; std::multimap<std::pair<int, size_t>, void*> blocks; size_t bytes = 0;   // keyed by (device, bytes)
@@ -114,7 +114,7 @@ struct DevCache {
   }
   void give(int dev, void* p, size_t n) {
     static const bool off = getenv("DYNOBA_NO_DEVCACHE") != nullptr;
-    static const size_t cap = (size_t)(getenv("DYNOBA_DEVCACHE_GB") ? atof(getenv("DYNOBA_DEVCACHE_GB")) : 96.0)*(1ull << 30);
+    static const size_t cap = (size_t)(getenv("DYNOBA_DEVCACHE_GB") ? atof(getenv("DYNOBA_DEVCACHE_GB")) : 48.0)*(1ull << 30);
     std::lock_guard<std::mutex> l(mu);
     if (off || bytes + n > cap) { cudaFree(p); return; }
     blocks.emplace(std::make_pair(dev, n), p); bytes += n;
@@ -199,7 +199,7 @@ int dynoba_create(int device, dynoba_handle* out) {
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return DYNOBA_ERR_CUDA;  // no CPU fallback
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major < 10) return DYNOBA_ERR_CUDA;
+  if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0) return DYNOBA_ERR_CUDA;   // sm_90a code only
   dynoba_solver* h = new dynoba_solver();
   h->device = device;
   if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { delete h; return DYNOBA_ERR_CUDA; }
@@ -858,7 +858,8 @@ static int finalize_impl(dynoba_solver* h) {
 }
 
 // ------------------------------------------------------------------------------------------------ device steps
-// fp64 FMA rate of the device (the roofline denominator of the reduced solve; DMMA m8n8k4 runs at the same rate)
+// fp64 peak of the device, the roofline denominator of the reduced solve: the best of plain FMAs (DFMA) and the fp64
+// tensor-core shapes m8n8k4 (what the band kernel's tile updates use) and m16n8k16 (sm_90)
 __global__ void fp64_rate_kernel(double* out, int iters) {
   double a[8];
 #pragma unroll
@@ -869,6 +870,33 @@ __global__ void fp64_rate_kernel(double* out, int iters) {
     for (int k = 0; k < 8; k++) a[k] = fma(a[k], m, c);
   }
   double s = 0; for (int k = 0; k < 8; k++) s += a[k];
+  out[(size_t)blockIdx.x*blockDim.x + threadIdx.x] = s;
+}
+__global__ void fp64_dmma_k4_rate_kernel(double* out, int iters) {      // 8 independent m8n8k4 per step: 8*512 flops per warp
+  const double a = 1.0 + 1e-3*(threadIdx.x & 31), b = 1.0 - 1e-9;
+  double c[8][2];
+#pragma unroll
+  for (int k = 0; k < 8; k++) { c[k][0] = k; c[k][1] = -k; }
+  for (int i = 0; i < iters; i++) {
+#pragma unroll
+    for (int k = 0; k < 8; k++)
+      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};" : "+d"(c[k][0]), "+d"(c[k][1]) : "d"(a), "d"(b));
+  }
+  double s = 0; for (int k = 0; k < 8; k++) s += c[k][0] + c[k][1];
+  out[(size_t)blockIdx.x*blockDim.x + threadIdx.x] = s;
+}
+__global__ void fp64_dmma_k16_rate_kernel(double* out, int iters) {     // 4 independent m16n8k16 per step: 4*4096 flops per warp
+  const double a = 1e-3*(threadIdx.x & 31), b = 1e-3;
+  double c[4][4];
+#pragma unroll
+  for (int k = 0; k < 4; k++) for (int j = 0; j < 4; j++) c[k][j] = k - j;
+  for (int i = 0; i < iters; i++) {
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+      asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0, %1, %2, %3}, {%4, %4, %4, %4, %4, %4, %4, %4}, {%5, %5, %5, %5}, "
+                   "{%0, %1, %2, %3};" : "+d"(c[k][0]), "+d"(c[k][1]), "+d"(c[k][2]), "+d"(c[k][3]) : "d"(a), "d"(b));
+  }
+  double s = 0; for (int k = 0; k < 4; k++) for (int j = 0; j < 4; j++) s += c[k][j];
   out[(size_t)blockIdx.x*blockDim.x + threadIdx.x] = s;
 }
 
@@ -973,14 +1001,21 @@ int dynoba_fp64_rate(dynoba_handle h, double* tflops) {
   int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
   const int grid = sms*8, block = 256, iters = 1 << 15;
   double* d; int rc = dalloc(h, &d, (size_t)grid*block, false); if (rc) return rc;
-  float best = 1e30f;
-  for (int rep = 0; rep < 4; rep++) {
-    CK(cudaEventRecord(h->ev[0], h->stream));
-    fp64_rate_kernel<<<grid, block, 0, h->stream>>>(d, iters);
-    CK(cudaEventRecord(h->ev[1], h->stream)); CK(cudaStreamSynchronize(h->stream));
-    float ms; CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1])); if (rep && ms < best) best = ms;
+  void (*kern[3])(double*, int) = { fp64_rate_kernel, fp64_dmma_k4_rate_kernel, fp64_dmma_k16_rate_kernel };
+  const double flops_per_thread_step[3] = { 2.0*8, 8*512.0/32, 4*4096.0/32 };
+  const int kiters[3] = { iters, iters/2, iters/8 };
+  double peak = 0;
+  for (int k = 0; k < 3; k++) {
+    float best = 1e30f;
+    for (int rep = 0; rep < 4; rep++) {
+      CK(cudaEventRecord(h->ev[0], h->stream));
+      kern[k]<<<grid, block, 0, h->stream>>>(d, kiters[k]);
+      CK(cudaEventRecord(h->ev[1], h->stream)); CK(cudaStreamSynchronize(h->stream));
+      float ms; CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1])); if (rep && ms < best) best = ms;
+    }
+    peak = std::max(peak, flops_per_thread_step[k]*kiters[k]*(double)grid*block/(best*1e-3)/1e12);
   }
-  *tflops = 2.0*8.0*iters*(double)grid*block/(best*1e-3)/1e12;
+  *tflops = peak;
   return DYNOBA_OK;
 }
 

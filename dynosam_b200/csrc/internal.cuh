@@ -9,6 +9,12 @@ namespace dynoba {
 
 constexpr int TILE = 32;           // band-Cholesky tile edge
 constexpr int TILE2 = TILE*TILE;
+// SM count of the current device: grid of the grid-stride clear / accumulate kernels (any value is correct)
+inline int device_sm_count() {
+  int dev = 0, n = 0;
+  cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  return n > 0 ? n : 1;
+}
 
 // Variables, SoA, fp64.  Pose-like variables are stored in *solver order* (ordered by the frame hint),
 // landmarks in group order (sorted by the first pose they touch).  strides are padded to 32.
@@ -145,7 +151,7 @@ struct BandBlockRef { double* base; int tpc, oi, oj, rev, fast; };
 #if defined(__CUDACC__)
 // fire-and-forget fp64 addition into the reduced system: RED on the GLOBAL window.  A plain atomicAdd through a pointer the
 // compiler cannot prove global (loaded from a descriptor) becomes a generic, value-returning ATOM with an address-space
-// query per call -- measured +6 ms per damped solve on C5
+// query per call
 __device__ __forceinline__ void red_add(double* p, double v) {
   asm volatile("red.global.add.f64 [%0], %1;" :: "l"(__cvta_generic_to_global(p)), "d"(v) : "memory");
 }

@@ -3,7 +3,7 @@
 // Replaces GTSAM's multifrontal Cholesky on the COLAMD ordering (SURVEY.md 8a row a11, [GTSAM-ext]) for the
 // reduced system that is left after the landmarks are eliminated.  With pose-like variables ordered by frame
 // the system is banded (half-width = the co-visibility window, <= max track age), stored as 32x32 tiles.
-// tcgen05/UMMA has no fp64 path: tile updates run on mma.sync.m8n8k4.f64 (DMMA), triangular work on fp64 FMAs.
+// Hopper's wgmma has no fp64 shape: tile updates run on mma.sync.m8n8k4.f64 (DMMA), triangular work on fp64 FMAs.
 //
 // A band Cholesky is one long dependency chain (potrf(K,K) -> trsm -> update -> potrf(K+1,K+1)), so the time axis is
 // cut into CELLS (nested dissection in time; internal.cuh, tools/cell_proto.py): every cell is two chains that are
@@ -1181,7 +1181,8 @@ static int chol_launch(const BandProb* dprobs, const BandProb* hprobs, int np, i
   if (grid > want) grid = (int)want;
   if (grid < np + 1 + (job.any_spiked ? 1 : 0)) grid = np + 1 + (job.any_spiked ? 1 : 0);
   // worker CTAs: without spikes all of them work on band tiles; else the two pools share them in proportion to their work
-  // (measured per column: band tiles ~330 us of one CTA, spike + FF updates ~730 us), pool A never below what keeps a chain
+  // (relative work per column 330 : 730, band tiles : spike + FF updates, timed on B200 and not re-timed on H100), pool A
+  // never below what keeps a chain
   // at the spine's pace (~22 CTAs per chain)
   const int workers = grid - np;
   if (!job.any_spiked) job.band_ctas = workers;
@@ -1250,9 +1251,9 @@ int band_plan_layout(BandPlan& P, int n, int bw, int ncell_request, int rank, in
   } else {
     const long long free_tiles = (long long)NT - (long long)(2*C - 1)*WB;
     // relative chain lengths.  One GPU: plain end chains 4.5x the spiked ones.  Several GPUs (one cell per rank): a rank in
-    // the middle runs two spiked chains (weight 0.5 each); an end rank runs its plain chain at the spine's pace
-    // (10.4 us per column against the ~12.9 us a middle rank needs per spiked column: weight 1.24) and, with the worker
-    // CTAs that leaves for the spike pool, a shorter spiked chain (0.6) -- measured rates of C5, see DESIGN.md section 6.
+    // the middle runs two spiked chains (weight 0.5 each); an end rank runs its plain chain at the spine's pace (weight
+    // 1.24) and, with the worker CTAs that leaves for the spike pool, a shorter spiked chain (0.6).  All of these weights
+    // come from per-column timings of C5 on B200 and have not been re-timed on H100 (tuning: outer_weight, band_profile).
     std::vector<double> wgt(2*C, 1.0);
     if (P.outer_weight > 0 || world == 1 || C != world) { wgt[0] = wgt[2*C - 1] = P.outer_weight > 0 ? P.outer_weight : (C >= 2 ? 4.5 : 1.0); }
     else { for (auto& x : wgt) x = 0.5; wgt[0] = wgt[2*C - 1] = 1.24; wgt[1] = wgt[2*C - 2] = 0.6; }
@@ -1438,7 +1439,7 @@ int launch_band_factor(const BandPlan& P, int* fail, cudaStream_t s) {
   }
   if (C >= 2) {
     cudaMemsetAsync(P.gq_base, 0, P.gq_count*sizeof(double), s);
-    for (int c : P.local_cells) { gq_add_cell_kernel<<<148, 256, 0, s>>>(cell_refs(P), c, P.TPCgq); launches++; }
+    for (int c : P.local_cells) { gq_add_cell_kernel<<<device_sm_count(), 256, 0, s>>>(cell_refs(P), c, P.TPCgq); launches++; }
     tm.lap("boundary system: assemble");
   }
   return launches;

@@ -65,7 +65,7 @@ int launch_prior_eval(const DevPrior& P, const DevVars& v, double* partial, int 
 }
 int launch_prior_accum(const DevPrior& P, const DevBand& B, cudaStream_t s) {
   const int dim = 6*P.n;
-  prior_accum_kernel<<<std::min(148, (dim*dim + 255)/256), 256, 0, s>>>(P, B);
+  prior_accum_kernel<<<std::min(device_sm_count(), (dim*dim + 255)/256), 256, 0, s>>>(P, B);
   return 1;
 }
 int launch_prior_model(const DevPrior& P, const DevBand& B, double* partial, cudaStream_t s) {

@@ -73,7 +73,7 @@ __global__ void band_diag_kernel(DevBand B, double lambda, int rank, int world) 
   *band_at(B, i, i) = i < B.n ? lambda : 1.0;
 }
 int launch_band_clear(const DevBand& B, double lambda, int rank, int world, cudaStream_t s) {
-  band_clear_kernel<<<148*8, 256, 0, s>>>(B);
+  band_clear_kernel<<<device_sm_count()*8, 256, 0, s>>>(B);
   band_diag_kernel<<<(B.n_pad + 255)/256, 256, 0, s>>>(B, lambda, rank, world);
   return 2;
 }

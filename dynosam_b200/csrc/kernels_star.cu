@@ -567,7 +567,7 @@ static int star_device_ready(int device) {
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return DYNOBA_ERR_CUDA;     // no CPU fallback
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major < 10) return DYNOBA_ERR_CUDA;
+  if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0) return DYNOBA_ERR_CUDA;
   if (device >= 64 || cudaSetDevice(device) != cudaSuccess) return DYNOBA_ERR_CUDA;
   StarContext& c = g_star[device];
   if (!c.stream && cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking) != cudaSuccess) { c.stream = nullptr; return DYNOBA_ERR_CUDA; }

@@ -89,7 +89,7 @@ class FeatureTrackerGPU:
         self.h = C.c_void_p()
         st = self.lib.dynofront_create(device, self.W, self.H, C.byref(self.h))
         if st != 0:
-            raise FrontendError(f"dynofront_create failed ({st}): no sm_100 CUDA device; libdynofront has no CPU path")
+            raise FrontendError(f"dynofront_create failed ({st}): no sm_90 CUDA device; libdynofront has no CPU path")
 
     def _ck(self, st):
         if st != 0:

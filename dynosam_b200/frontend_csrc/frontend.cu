@@ -1,4 +1,4 @@
-// frontend.cu -- libdynofront: front-end rows a13 / a14 of SURVEY.md section 8 as sm_100a kernels (include/dynofront.h).
+// frontend.cu -- libdynofront: front-end rows a13 / a14 of SURVEY.md section 8 as sm_90a kernels (include/dynofront.h).
 // Compiled with -fmad=false: the KLT arithmetic follows OpenCV's scalar float code, which is not FMA-contracted.
 //
 // Ordering semantics that make the reference sequential are kept exactly:
@@ -515,7 +515,7 @@ int dynofront_create(int device, int width, int height, dynofront_handle* out) {
   *out = nullptr;
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return -3;
-  cudaDeviceProp prop; if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major < 10) return -3;
+  cudaDeviceProp prop; if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0) return -3;   // sm_90a code only
   dynofront_ctx* h = new dynofront_ctx(); h->dev = device; h->W = width; h->H = height;
   cudaSetDevice(device);
   if (cudaStreamCreateWithFlags(&h->s, cudaStreamNonBlocking) != cudaSuccess) { delete h; return -3; }

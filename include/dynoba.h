@@ -1,5 +1,5 @@
 /*
- * dynoba.h -- C ABI of libdynoba: B200-native (sm_100a) batch nonlinear-least-squares hot path for DynOSAM.
+ * dynoba.h -- C ABI of libdynoba: H100-native (sm_90a) batch nonlinear-least-squares hot path for DynOSAM.
  *
  * This is the drop-in boundary for the reference's solver call
  *     gtsam::LevenbergMarquardtOptimizer problem(graph, theta, params);
@@ -13,7 +13,7 @@
  * dynoba_status (0 = ok, < 0 = error); no exception crosses the ABI.  A handle is NOT thread-safe;
  * use one handle per optimiser instance (the reference calls from exactly one backend thread,
  * src/pipeline/PipelineManager.cc:175-250).  Host arrays are copied during the call; nothing is retained.
- * There is no CPU fallback: every compute entry point fails with DYNOBA_ERR_CUDA when no sm_100 device works.
+ * There is no CPU fallback: every compute entry point fails with DYNOBA_ERR_CUDA when no sm_90 (compute capability 9.0) device works.
  */
 #ifndef DYNOBA_H
 #define DYNOBA_H
@@ -159,8 +159,9 @@ int dynoba_optimize(dynoba_handle h, const dynoba_lm_params* p, dynoba_lm_stats*
 int dynoba_get_variables(dynoba_handle h, int kind, int64_t n, double* out);
 int dynoba_get_keys(dynoba_handle h, int kind, int64_t n, uint64_t* out);
 int dynoba_num_variables(dynoba_handle h, int kind, int64_t* out);
-/* Measured fp64 FMA throughput of the device in TFLOP/s (a few milliseconds of a register-only FMA kernel): the
- * roofline denominator bench.py prints next to the reduced solve (tcgen05 has no fp64; DMMA runs at the FMA rate). */
+/* Measured fp64 peak of the device in TFLOP/s: the best of three register-only kernels of a few milliseconds each -- plain
+ * FMAs, and the fp64 tensor-core shapes mma.sync m8n8k4 and m16n8k16.  The roofline denominator bench.py prints next to
+ * the reduced solve. */
 int dynoba_fp64_rate(dynoba_handle h, double* tflops);
 int dynoba_problem_info(dynoba_handle h, int32_t* reduced_dim, int32_t* bandwidth, int64_t* jacobian_bytes);
 

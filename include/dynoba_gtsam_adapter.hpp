@@ -56,7 +56,7 @@ class LevenbergMarquardtOptimizer {
     // h_ is an RAII member: if anything below throws, the members are destroyed and the handle (with its CUDA streams
     // and device blocks) is released
     int st = dynoba_create(device, &h_.h);
-    if (st != DYNOBA_OK) throw std::runtime_error(std::string("libdynoba: ") + dynoba_status_string(st) + " (no usable sm_100 device)");
+    if (st != DYNOBA_OK) throw std::runtime_error(std::string("libdynoba: ") + dynoba_status_string(st) + " (no usable sm_90 device)");
     ingestValues(initial);
     ingestFactors(graph);
     dynoba_lm_default_params(&p_);

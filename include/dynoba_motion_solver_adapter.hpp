@@ -10,7 +10,7 @@
  * caller keeps its Frame / Feature containers: gather per object what optimize() reads from them (-inl.hpp:117-160, :343-366).
  *
  * Compiled by tests/test_host.py against tests/stubs/ (GTSAM is absent from the build container); nothing here needs CUDA
- * headers.  Throws std::runtime_error on a non-OK status (no usable sm_100 device included: there is no CPU path behind it).
+ * headers.  Throws std::runtime_error on a non-OK status (no usable sm_90 device included: there is no CPU path behind it).
  */
 #ifndef DYNOBA_MOTION_SOLVER_ADAPTER_HPP
 #define DYNOBA_MOTION_SOLVER_ADAPTER_HPP

@@ -1,5 +1,5 @@
 /*
- * dynofront.h -- C ABI of libdynofront: the front-end half of the DynOSAM hot path on sm_100a
+ * dynofront.h -- C ABI of libdynofront: the front-end half of the DynOSAM hot path on sm_90a
  * (SURVEY.md section 8 rows a13 "dense-flow warp / label correlate" and a14 "pyramidal KLT").
  *
  * Replaces, with the same inputs / outputs and the same ordering semantics:

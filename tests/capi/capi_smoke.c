@@ -12,7 +12,7 @@
 int main(void) {
   dynoba_handle h = NULL;
   int st = dynoba_create(0, &h);
-  if (st == DYNOBA_ERR_CUDA) { printf("no usable sm_100 device: %s\n", dynoba_status_string(st)); return 3; }
+  if (st == DYNOBA_ERR_CUDA) { printf("no usable sm_90 device: %s\n", dynoba_status_string(st)); return 3; }
   if (st != DYNOBA_OK) return 1;
   /* poses: R row-major | t.  pose 1 starts 0.3 m off its true place (1, 0, 0) */
   double poses[2][12] = { {1,0,0, 0,1,0, 0,0,1, 0,0,0}, {1,0,0, 0,1,0, 0,0,1, 1.3,0.1,-0.1} };

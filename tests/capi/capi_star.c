@@ -18,7 +18,7 @@ int main(void) {
   dynoba_flow_pose_params fp; dynoba_flow_pose_default_params(&fp);
   double pose_out[12], flow_out[6][2], eb = 0.0, ea = 0.0; uint8_t inl[6]; int32_t its = 0, inner = 0, rounds = 0;
   const int st = dynoba_flow_pose_batch(0, 1, off, guess, I12, K5, &kp[0][0], depth, &flow[0][0], &fp, pose_out, &flow_out[0][0], inl, &eb, &ea, &its, &inner, &rounds);
-  if (st == DYNOBA_ERR_CUDA) { printf("no usable sm_100 device: %s\n", dynoba_status_string(st)); return 3; }
+  if (st == DYNOBA_ERR_CUDA) { printf("no usable sm_90 device: %s\n", dynoba_status_string(st)); return 3; }
   if (st != DYNOBA_OK) { fprintf(stderr, "dynoba_flow_pose_batch -> %s\n", dynoba_status_string(st)); return 1; }
   printf("flow+pose: error %.6g -> %.6g in %d iterations, t_z %.4f\n", eb, ea, (int)its, pose_out[11]);
   dynoba_batch_release(0);

@@ -1,5 +1,5 @@
-"""torchrun worker (N GPUs): the time-sharded solver against the unsharded oracle.  Run through
-`gpurun --gpus 2 -- python -m torch.distributed.run --nproc-per-node 2 ... tests/multi/check_sharded.py`.
+"""torchrun worker (N GPUs): the time-sharded solver against the unsharded oracle.  Run on a machine with 2 GPUs
+through `python -m torch.distributed.run --nproc-per-node 2 ... tests/multi/check_sharded.py`.
 
 Covers both multi-GPU modes of libdynoba: the replicated reduced solve (one all-reduce of the whole reduced system) and
 the distributed one (dynoba_set_reduce: cells of the band owned by ranks, a reduce per cell, all-reduce of the boundary

@@ -221,6 +221,34 @@ def test_bench_own_arm_fails_loudly_without_gpu():
     assert not any(l.strip().startswith("{") for l in out.stdout.splitlines())
 
 
+def test_bench_dump_outputs_names_dtypes_and_budget(tmp_path, monkeypatch):
+    """bench.dump_outputs writes pose / point / chi2 (+ flow when present) as float64 .npy; above the byte budget it writes
+    the same seeded row sample on every call and stays under the budget."""
+    import bench
+    rng = np.random.default_rng(3)
+    pose, point, flow = rng.normal(size=(500, 12)), rng.normal(size=(20000, 3)), rng.normal(size=(300, 2))
+
+    class Stub:
+        def values(self):
+            return pose, point, flow
+    st = {"error_initial": 2.0, "error_final": 1.0}
+    bench.dump_outputs(str(tmp_path / "full"), Stub(), st)
+    full = {f: np.load(tmp_path / "full" / f) for f in os.listdir(tmp_path / "full")}
+    assert sorted(full) == ["chi2.npy", "flow.npy", "point.npy", "pose.npy"]
+    assert all(a.dtype == np.float64 for a in full.values())
+    assert np.array_equal(full["point.npy"], point) and np.array_equal(full["chi2.npy"], [2.0, 1.0])
+    monkeypatch.setattr(bench, "DUMP_BUDGET", 100_000)
+    for d in ("a", "b"):
+        bench.dump_outputs(str(tmp_path / d), Stub(), st)
+    sizes = sum(os.path.getsize(tmp_path / "a" / f) for f in os.listdir(tmp_path / "a"))
+    assert sizes <= 100_000 + 4*128                                # (+ one .npy header per file)
+    for f in os.listdir(tmp_path / "a"):
+        a, b = np.load(tmp_path / "a" / f), np.load(tmp_path / "b" / f)
+        assert a.dtype == np.float64 and np.array_equal(a, b)
+    p = np.load(tmp_path / "a" / "point.npy")
+    assert 0 < p.shape[0] < point.shape[0] and (p[:, None, :] == point[None, :200, :]).all(2).any(1).sum() > 0
+
+
 def test_gtsam_adapter_compiles_against_api_stubs():
     """include/dynoba_gtsam_adapter.hpp (the drop-in for RegularBackendModule.cc:405-428) is real code: it must compile,
     with every factor branch incl. stereo and flow projection, against declarations of the GTSAM 4.2 / DynOSAM API it

@@ -1,5 +1,5 @@
 """N > 1: the time-sharded solver (replicated and distributed reduced solve over NCCL) against the unsharded oracle.
-Needs >= 2 GPUs on the box (gpurun --gpus 2); skipped otherwise."""
+Needs >= 2 GPUs on the machine; skipped otherwise."""
 import os
 import subprocess
 import sys

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Summarise ncu outputs into profiles/: a launch list (gpu__time_duration CSV) and raw-page metrics of a report."""
+"""Summarise ncu outputs as markdown tables: a launch list (gpu__time_duration CSV) and raw-page metrics of a report."""
 import collections, csv, re, subprocess, sys
 
 def launch_summary(path):

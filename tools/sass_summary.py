@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Opcode census of the shipped sm_100a kernels (cuobjdump -sass): writes profiles/r02_sass_<kernel>.txt (full SASS of
-the kernels DESIGN.md discusses) and prints a table of the opcodes that matter for the Blackwell evidence: DMMA (fp64
+"""Opcode census of the shipped sm_90a kernels (cuobjdump -sass): writes profiles/sass_<kernel>.txt (full SASS of
+the kernels DESIGN.md discusses) and prints a table of the opcodes that matter for the Hopper evidence: DMMA (fp64
 tensor core), DFMA, UBLKCP / LDGSTS (bulk and per-thread async copies), SYNCS (mbarrier), RED / ATOM, LDG / STG widths.
     python tools/sass_summary.py            # after __graft_entry__.build()
 """
@@ -11,7 +11,7 @@ LIBS = {"libdynoba.so": ["linearize_kernel<5", "schur_accum_kernel<2", "schur_st
         "libdynofront.so": ["klt_kernel", "sc_count_kernel", "pm_warp_kernel"]}
 CENSUS_ONLY = ("flow_pose_kernel", "motion_refine_kernel")
 KEYS = ["DMMA", "DFMA", "DADD", "DMUL", "MUFU", "UBLKCP", "LDGSTS", "SYNCS", "RED", "ATOM", "LDG.E.64", "LDG.E.128", "LDG.E.U8", "LDG.E ", "STG.E.64", "STG.E.128",
-        "STG.E ", "LDS", "STS", "LDL", "STL", "BAR", "SHFL", "UTMALDG", "UTCMMA"]
+        "STG.E ", "LDS", "STS", "LDL", "STL", "BAR", "SHFL", "UTMALDG", "HGMMA"]
 
 def demangle(n):
     try:
@@ -41,8 +41,9 @@ def main():
                     if op.startswith(k.strip()) and (not k.endswith(" ") or op == k.strip()):
                         ops[k.strip() if not k.endswith(" ") else k.strip() + " (32-bit)"] += 1
             short = re.sub(r"\(.*", "", name).replace("dynoba::", "")
-            fn = os.path.join(ROOT, "profiles", "r02_sass_" + re.sub(r"[^A-Za-z0-9]+", "_", short).strip("_") + ".txt")
+            fn = os.path.join(ROOT, "profiles", "sass_" + re.sub(r"[^A-Za-z0-9]+", "_", short).strip("_") + ".txt")
             if not any(w in name for w in CENSUS_ONLY):           # large scalar kernels: census row only, no multi-MB dump in the repo
+                os.makedirs(os.path.dirname(fn), exist_ok=True)
                 open(fn, "w").write(f"// cuobjdump -sass {lib}, function {name}\n" + b)
             rows.append((lib, short, n_inst, ops))
     print("| kernel | instructions | " + " | ".join(k.strip() for k in KEYS) + " |")

@@ -1,4 +1,4 @@
-// micro-benchmark: fp64 DFMA issue rate / latency, SHFL and LDS cost for one warp and for a full SM (B200)
+// micro-benchmark: fp64 DFMA and DMMA (m8n8k4, m16n8k16) issue rate / latency, SHFL and LDS cost for one warp and for a full GPU (H100)
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void dfma_kernel(double* out, int iters, long long* cyc) {
@@ -89,6 +89,25 @@ __global__ void dmma_kernel(double* out, int iters, long long* cyc, int nacc) {
   out[blockIdx.x*blockDim.x + threadIdx.x] = s;
   if (threadIdx.x == 0 && blockIdx.x == 0) *cyc = t1 - t0;
 }
+__global__ void dmma16_kernel(double* out, int iters, long long* cyc) {   // mma.sync m16n8k16 f64 (sm_90), 4 independent
+  double a0 = 1e-3*(threadIdx.x & 31), b0 = 1e-3;
+  double c[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) c[i][j] = i - j;
+  long long t0 = clock64();
+  for (int it = 0; it < iters; it++) {
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+      asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%4,%4,%4,%4,%4,%4,%4}, {%5,%5,%5,%5}, {%0,%1,%2,%3};"
+                   : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3]) : "d"(a0), "d"(b0));
+  }
+  long long t1 = clock64();
+  double s = 0;
+#pragma unroll
+  for (int i = 0; i < 4; i++) s += c[i][0] + c[i][1] + c[i][2] + c[i][3];
+  out[blockIdx.x*blockDim.x + threadIdx.x] = s;
+  if (threadIdx.x == 0 && blockIdx.x == 0) *cyc = t1 - t0;
+}
 __global__ void dmma_dep_kernel(double* out, int iters, long long* cyc) {
   double a0 = out[threadIdx.x & 31] + 1.0, b0 = 1.0000001, c0 = 0, c1 = 0;
   long long t0 = clock64();
@@ -104,8 +123,9 @@ __global__ void dmma_dep_kernel(double* out, int iters, long long* cyc) {
 int main() {
   double* d; long long* c; cudaMalloc(&d, 1 << 24); cudaMemset(d, 0, 1 << 24); cudaMalloc(&c, 8);
   long long h; const int it = 2000;
+  int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   for (int cfg = 0; cfg < 3; cfg++) {
-    int blocks = cfg == 0 ? 1 : 148*(cfg == 1 ? 1 : 4), threads = cfg == 0 ? 32 : (cfg == 1 ? 128 : 256);
+    int blocks = cfg == 0 ? 1 : sms*(cfg == 1 ? 1 : 4), threads = cfg == 0 ? 32 : (cfg == 1 ? 128 : 256);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); float ms;
     dfma_kernel<<<blocks, threads>>>(d, it, c); cudaDeviceSynchronize();
     cudaEventRecord(e0); dfma_kernel<<<blocks, threads>>>(d, it, c); cudaEventRecord(e1); cudaDeviceSynchronize();
@@ -117,12 +137,20 @@ int main() {
   lds_kernel<<<1, 32>>>(d, it, c); cudaDeviceSynchronize(); cudaMemcpy(&h, c, 8, cudaMemcpyDeviceToHost); printf("lds.128 bcast + 2 dadd, 1 warp: %.2f cyc each\n", (double)h/(it*8));
   rsqrt_kernel<<<1, 32>>>(d, it, c); cudaDeviceSynchronize(); cudaMemcpy(&h, c, 8, cudaMemcpyDeviceToHost); printf("rsqrt(double)+dadd dependent: %.2f cyc\n", (double)h/it);
   for (int cfg = 0; cfg < 3; cfg++) {
-    int blocks = cfg == 0 ? 1 : 148*(cfg == 1 ? 1 : 4), threads = cfg == 0 ? 32 : (cfg == 1 ? 128 : 256);
+    int blocks = cfg == 0 ? 1 : sms*(cfg == 1 ? 1 : 4), threads = cfg == 0 ? 32 : (cfg == 1 ? 128 : 256);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); float ms;
     dmma_kernel<<<blocks, threads>>>(d, it, c, 16); cudaDeviceSynchronize();
     cudaEventRecord(e0); dmma_kernel<<<blocks, threads>>>(d, it, c, 16); cudaEventRecord(e1); cudaDeviceSynchronize();
     cudaMemcpy(&h, c, 8, cudaMemcpyDeviceToHost); cudaEventElapsedTime(&ms, e0, e1);
     printf("dmma m8n8k4 indep blocks %4d x %3d thr: %.2f cyc per warp-DMMA (warp 0), chip %.2f TFLOP/s\n", blocks, threads, (double)h/(it*16), 2.0*256*(double)blocks*(threads/32)*it*16/(ms*1e-3)/1e12);
+  }
+  for (int cfg = 1; cfg < 3; cfg++) {
+    int blocks = sms*(cfg == 1 ? 1 : 4), threads = cfg == 1 ? 128 : 256;
+    cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); float ms;
+    dmma16_kernel<<<blocks, threads>>>(d, it, c); cudaDeviceSynchronize();
+    cudaEventRecord(e0); dmma16_kernel<<<blocks, threads>>>(d, it, c); cudaEventRecord(e1); cudaDeviceSynchronize();
+    cudaMemcpy(&h, c, 8, cudaMemcpyDeviceToHost); cudaEventElapsedTime(&ms, e0, e1);
+    printf("dmma m16n8k16 indep blocks %4d x %3d thr: %.2f cyc per warp-DMMA (warp 0), chip %.2f TFLOP/s\n", blocks, threads, (double)h/(it*4), 4096.0*(double)blocks*(threads/32)*it*4/(ms*1e-3)/1e12);
   }
   dmma_dep_kernel<<<1, 32>>>(d, it, c); cudaDeviceSynchronize(); cudaMemcpy(&h, c, 8, cudaMemcpyDeviceToHost); printf("dmma dependent chain: %.2f cyc latency\n", (double)h/(it*16));
   return 0;

@@ -1,5 +1,5 @@
 // Micro-benchmark of the spine's 32x32 potrf variants in isolation (one warp), optionally with spinning sibling warps.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -Xcompiler -fopenmp -I../../dynosam_b200/csrc potrf_bench.cu -o potrf_bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -Xcompiler -fopenmp -I../../dynosam_b200/csrc potrf_bench.cu -o potrf_bench
 #include <cstdio>
 #include "../../dynosam_b200/csrc/kernels_band.cu"
 using namespace dynoba;
