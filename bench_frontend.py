@@ -139,7 +139,51 @@ def run_dynoba(n, warmup, streaming=True):
            "note": "end to end through the C ABI from host images (H2D/D2H inside the timed region); a frame moves a few MB and "
                    "launches ~40 small kernels, so it is PCIe / launch bound, not HBM bound: the dense passes' 21 B/px "
                    f"({dense_bytes/1e6:.1f} MB) would take {dense_bytes/3.35e12*1e6:.1f} us at the H100 data-sheet HBM rate (3.35 TB/s)"}
+    if streaming:
+        out.update(full_frame(t, frames, static_pts, feats, n, warmup))
+    out.update(card())
     return out
+
+
+def full_frame(t, frames, static_pts, feats, n, warmup):
+    """The streaming frame loop again, with sampleDynamic completed on the device (scan + range-tree ANMS + new features,
+    dynofront_sample_dynamic) in place of the candidate scan: per object K = 200 - the features track_dynamic kept."""
+    from dynosam_b200.frontend import TrackParams
+    prm = TrackParams(); static_age = np.zeros(N_STATIC, np.int32); objs = list(range(1, 11))
+    t.next_frame(frames[0][0], frames[0][2], frames[0][1])
+
+    def one(k):
+        g1, m1, f1 = frames[k]
+        kp, lab, age, tid = feats[k-1]
+        t.next_frame(g1, f1, m1)
+        t.propagate_mask_resident(kp, lab, prm)
+        acc, *_ = t.track_dynamic(kp, lab, age, tid, prm, 10**6, want_masks=False)
+        num_track = np.bincount(lab[acc.astype(bool)], minlength=11)[1:11].astype(np.int32)
+        r = t.sample_dynamic(objs, num_track, prm, 10**6, max_features=PER_OBJECT); sd_ms = t.last_ms
+        t.klt_track_fb(None, None, static_pts, prm, static_age, 25)
+        return sd_ms, int(r["num_sampled"].sum())
+    for k in range(1, warmup + 1):
+        one(k)
+    sd = []; sampled = []; t0 = time.perf_counter()
+    for k in range(1, n + 1):
+        ms, s = one(k); sd.append(ms); sampled.append(s)
+    dt = time.perf_counter() - t0
+    return {"full_frame_fps": n/dt, "sample_dynamic_ms": float(np.mean(sd)), "sampled_per_frame": float(np.mean(sampled)),
+            "full_frame_note": "streaming loop with dynofront_sample_dynamic in place of dynofront_sample_candidates; "
+                               "static feature detection is not on the device yet and is not part of the loop"}
+
+
+def card():
+    """name and power limit of the GPU the numbers were measured on, read in the same run"""
+    import subprocess
+    import torch
+    info = {"gpu": torch.cuda.get_device_name(0), "power_limit": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True, timeout=30)
+        info["power_limit"] = r.stdout.strip() or None
+    except (OSError, subprocess.SubprocessError):
+        pass
+    return info
 
 
 if __name__ == "__main__":

@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libdynofront.so")
 EXPORTS = ["dynofront_create", "dynofront_destroy", "dynofront_last_error", "dynofront_set_frame", "dynofront_track_dynamic",
            "dynofront_sample_candidates", "dynofront_propagate_mask", "dynofront_klt_track", "dynofront_klt_track_fb",
            "dynofront_klt_last_min_eig", "dynofront_stereo_track", "dynofront_track_static_flow", "dynofront_next_frame", "dynofront_pin_host", "dynofront_unpin_host",
-           "dynofront_get_motion_mask", "dynofront_get_pyramid_level"]
+           "dynofront_get_motion_mask", "dynofront_get_pyramid_level", "dynofront_anms_range_tree", "dynofront_sample_dynamic"]
 
 
 class TrackParamsC(C.Structure):
@@ -68,6 +68,9 @@ def load():
         L.dynofront_pin_host.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         L.dynofront_unpin_host.argtypes = [C.c_void_p, C.c_void_p]
         L.dynofront_get_motion_mask.argtypes = [C.c_void_p, C.c_void_p]
+        L.dynofront_anms_range_tree.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p]*4 + [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)]
+        L.dynofront_sample_dynamic.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(TrackParamsC), C.POINTER(C.c_int64),
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p]*5 + [C.POINTER(C.c_int32), C.POINTER(C.c_float)]
         L.dynofront_get_pyramid_level.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]
         _LIB = L
     return _LIB
@@ -154,6 +157,40 @@ class FeatureTrackerGPU:
         pc = prm.c()
         self._ck(self.lib.dynofront_sample_candidates(self.h, n, _p(objs), C.byref(pc), _p(counts), _p(offs), _p(zero), _p(idx), cap))
         return {int(o): idx[offs[i]:offs[i] + counts[i]].copy() for i, o in enumerate(objs)}, {int(o): int(zero[i]) for i, o in enumerate(objs)}
+
+    def anms_range_tree(self, lists, k_needed, tolerance, cols=None, rows=None):
+        """Range-tree ANMS (suppressNonMax, response-0 key-points) on several integer key-point lists in one launch.
+        lists: sequence of [n_l, 2] (col, row) arrays; k_needed / tolerance: one value per list (or a scalar).
+        Returns one int32 array per list: indices of the selected key-points, in selection order."""
+        lists = [np.ascontiguousarray(a, dtype=np.int32).reshape(-1, 2) for a in lists]; m = len(lists)
+        offs = np.zeros(m + 1, np.int32); offs[1:] = np.cumsum([len(a) for a in lists])
+        xy = np.ascontiguousarray(np.concatenate(lists) if m else np.zeros((0, 2), np.int32), dtype=np.int32)
+        k = np.ascontiguousarray(np.broadcast_to(np.asarray(k_needed, np.int32), (m,)))
+        tol = np.ascontiguousarray(np.broadcast_to(np.asarray(tolerance, np.float32), (m,)))
+        sel = np.zeros(max(int(offs[-1]), 1), np.int32); nsel = np.zeros(max(m, 1), np.int32); ms = C.c_float()
+        self._ck(self.lib.dynofront_anms_range_tree(self.h, m, _p(offs), _p(xy), _p(k), _p(tol), int(cols or self.W), int(rows or self.H),
+                                                    _p(sel), _p(nsel), C.byref(ms)))
+        self.last_ms = ms.value
+        return [sel[offs[l]:offs[l] + nsel[l]].copy() for l in range(m)]
+
+    def sample_dynamic(self, objects, num_track, prm: TrackParams, next_tracklet_id: int, max_features=200, capacity=None):
+        """FeatureTracker::sampleDynamic on the device: candidate scan, range-tree ANMS per object, new features.  Uses the
+        detection mask left by track_dynamic (or the uploaded one).  Returns a dict: per object counts / num_sampled /
+        zero_flow, per feature keypoint / flow / predicted / tracklet / label (packed object after object), next_tracklet_id."""
+        objs = np.ascontiguousarray(objects, dtype=np.int32); n = objs.shape[0]
+        ntr = np.ascontiguousarray(np.broadcast_to(np.asarray(num_track, np.int32), (n,)))
+        cap = int(capacity if capacity is not None else n*max(int(max_features), 1)*2 + 64)
+        counts = np.zeros(n, np.int32); ns = np.zeros(n, np.int32); zero = np.zeros(n, np.int32)
+        kp = np.zeros((cap, 2)); fl = np.zeros((cap, 2)); pk = np.zeros((cap, 2)); tid = np.zeros(cap, np.int64); lab = np.zeros(cap, np.int32)
+        nid = C.c_int64(int(next_tracklet_id)); nf = C.c_int32(); ms = C.c_float(); pc = prm.c()
+        self._ck(self.lib.dynofront_sample_dynamic(self.h, n, _p(objs), _p(ntr), int(max_features), C.byref(pc), C.byref(nid), _p(counts), _p(ns),
+                                                   _p(zero), cap, _p(kp), _p(fl), _p(pk), _p(tid), _p(lab), C.byref(nf), C.byref(ms)))
+        self.last_ms = ms.value
+        if nf.value > cap:                                        # more than the guess: run again with room for all
+            return self.sample_dynamic(objects, num_track, prm, next_tracklet_id, max_features, nf.value)
+        s = nf.value
+        return dict(counts=counts, num_sampled=ns, zero_flow=zero, keypoint=kp[:s], flow=fl[:s], predicted=pk[:s], tracklet=tid[:s], label=lab[:s],
+                    next_tracklet_id=nid.value)
 
     def propagate_mask(self, prev_pred_kp, prev_label, prev_mask, prev_flow, current_mask, prm: TrackParams, min_votes=150):
         kp = np.ascontiguousarray(prev_pred_kp, dtype=np.float64).reshape(-1, 2)

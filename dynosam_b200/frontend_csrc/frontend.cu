@@ -42,6 +42,11 @@ struct dynofront_ctx {
   int sf_cap = 0, sf_cells = 0; double* sf_kp = nullptr; int32_t* sf_age = nullptr; uint8_t* sf_use = nullptr; int32_t* sf_det = nullptr;
   int *sf_cell = nullptr, *sf_win = nullptr, *sf_win2 = nullptr, *sf_cnt = nullptr; uint8_t* sf_pass = nullptr; uint8_t* sf_acc = nullptr; double* sf_out = nullptr;
   int32_t* sf_oage = nullptr; long long* sf_otid = nullptr;
+  // ANMS work arrays (grow-only: points, lists) and sampleDynamic selection scratch
+  int sel_cap = 0, sel_lists = 0; int *sel_xy = nullptr, *sel_px = nullptr, *sel_py = nullptr, *sel_orig = nullptr, *sel_next = nullptr, *sel_out = nullptr;
+  int *sel_off = nullptr, *sel_cnt = nullptr, *sel_k = nullptr, *sel_n = nullptr; float* sel_tol = nullptr;
+  int* sd_idx = nullptr; int *sd_off = nullptr, *sd_k = nullptr, *sd_ntrack = nullptr; int sd_cap = 0; double* sd_out = nullptr;
+  long long* sd_tid = nullptr; int32_t* sd_lab = nullptr;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   std::vector<void*> allocs;
 };
@@ -229,6 +234,179 @@ __global__ void __launch_bounds__(ST_TILE) sc_scatter_kernel(size_t npx, int W, 
     for (int w = 0; w < warp; w++) base += wc[w][s];
     const long long dst = (long long)obj_off[s] + tile_off[(size_t)blockIdx.x*ST_MAXOBJ + s] + base + myrank;
     if (dst < capacity) indices[dst] = (int)p;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------- ANMS (range tree)
+// AdaptiveNonMaximumSuppression::suppressNonMax with AnmsAlgorithmType::RangeTree (NonMaximumSupression.cc:33-116,
+// anms.cc:278-362), one CTA per key-point list, every list of a frame in one launch.
+//  * Order.  Both call sites hand over responses that truncate to int 0, so cv::sortIdx(SORT_DESCENDING) sorts all-equal
+//    keys: libstdc++'s introsort then yields a fixed permutation P_n of the input (equal_keys_sort_position).
+//  * Width.  The reference's binary search over the square half-width w, with its quadratic-formula bounds, float
+//    Kmin / Kmax and the fall-back to the last computed result (which can hold more than Kmax points).
+//  * Greedy.  For one w, a point is kept when no earlier KEPT point lies in the inclusive square |dx| <= w, |dy| <= w.
+//    Chunks of SEL_THREADS points are first tested in parallel against the points kept by earlier chunks (a bucket grid
+//    in shared memory, cells >= w so a square touches <= 3x3 cells); the survivors of a chunk are then resolved in order
+//    by one warp, 32 at a time: pairwise conflicts as a bit mask, a serial 32-step scan, insertion into the grid.
+// Undefined inputs of the reference, defined here: K = 0 selects nothing (the reference converts +inf to int), K = 1
+// selects the first point in processing order (the reference computes 0/0).
+constexpr int SEL_THREADS = 256, SEL_GRID = 4096;
+__device__ __forceinline__ int equal_keys_sort_position(int e, int n) {
+  int pos = e, lo = 0, hi = n;
+  while (hi - lo > 16) {                                   // std::__introsort_loop; depth never reaches 2*floor(log2 n)
+    const int mid = lo + (hi - lo)/2;
+    if (pos == lo) pos = mid; else if (pos == mid) pos = lo;   // __move_median_to_first, every comparison false: swap(first, mid)
+    if (pos != lo) pos = lo + hi - pos;                        // __unguarded_partition: reverses [lo + 1, hi)
+    const int cut = lo + 1 + (hi - lo - 1)/2;
+    if (pos >= cut) lo = cut; else hi = cut;                   // recurse right, loop left (insertion sort moves nothing)
+  }
+  return n - 1 - pos;                                          // SORT_DESCENDING reverses the ascending result
+}
+// upper bound of the width search, anms.cc:282-297 in the reference's types (int / long long / double), K >= 2.  Every width
+// tried is <= this, so key-points with coordinate + anms_high <= 65535 never reach the u16 wrap of rangetree<u16,u16>::search.
+__host__ __device__ inline int anms_high(int K, int cols, int rows) {
+  const int exp1 = rows + cols + 2*K;
+  const long long exp2 = 4LL*cols + 4LL*K + 4LL*rows*K + (long long)rows*rows + (long long)cols*cols - 2LL*rows*cols + 4LL*rows*cols*K;
+  const double exp3 = sqrt((double)exp2), exp4 = K - 1;
+  const double sol1 = -round((exp1 + exp3)/exp4), sol2 = -round((exp1 - exp3)/exp4);
+  return (int)(sol1 > sol2 ? sol1 : sol2);
+}
+struct SelGrid { int x0, y0, s, nx, ny, w; };
+__device__ __forceinline__ bool sel_conflict(const SelGrid& g, const int* head, const int* px, const int* py, const int* nxt, int x, int y) {
+  const int cx0 = max(x - g.w - g.x0, 0)/g.s, cx1 = min((x + g.w - g.x0)/g.s, g.nx - 1);
+  const int cy0 = max(y - g.w - g.y0, 0)/g.s, cy1 = min((y + g.w - g.y0)/g.s, g.ny - 1);
+  for (int cy = cy0; cy <= cy1; cy++)
+    for (int cx = cx0; cx <= cx1; cx++)
+      for (int q = head[cy*g.nx + cx]; q >= 0; q = nxt[q]) {
+        const int dx = px[q] - x, dy = py[q] - y;
+        if (dx <= g.w && dx >= -g.w && dy <= g.w && dy >= -g.w) return true;
+      }
+  return false;
+}
+// Points of list l: pixel (lin % W, lin / W) of lin[off + e] when lin is given, else xy[off + e].  Work arrays px / py /
+// porig / nxt and the result sel are indexed like the input (off + position).  sel[off + r] = index within the list of
+// the r-th selected point, nsel[l] = how many (never more than the list holds).
+__global__ void __launch_bounds__(SEL_THREADS, 1) anms_range_tree_kernel(const int* __restrict__ off, const int* __restrict__ cnt, const int* __restrict__ kneed,
+                                                                      const float* __restrict__ tol, float tol_all, const int* __restrict__ lin,
+                                                                      const int* __restrict__ xy, int W, int cols, int rows,
+                                                                      int* px, int* py, int* porig, int* nxt, int* sel, int* __restrict__ nsel) {
+  __shared__ int head[SEL_GRID];
+  __shared__ uint8_t pend[SEL_THREADS];
+  __shared__ int s_bb[4], s_kept, s_width, s_stop, s_done;   // (two flags: no thread rewrites one that a slow warp may still read)
+  __shared__ SelGrid s_g;
+  const int l = blockIdx.x, o = off[l], n = cnt[l], K = kneed[l], tid = threadIdx.x, lane = tid & 31;
+  if (n <= 0 || K <= 0) { if (tid == 0) nsel[l] = 0; return; }
+  px += o; py += o; porig += o; nxt += o; sel += o;
+  if (tid == 0) { s_bb[0] = s_bb[1] = 0x7fffffff; s_bb[2] = s_bb[3] = -1; }
+  __syncthreads();
+  int bx0 = 0x7fffffff, by0 = 0x7fffffff, bx1 = -1, by1 = -1;
+  for (int e = tid; e < n; e += SEL_THREADS) {
+    int x, y;
+    if (lin) { const int p = lin[o + e]; x = p % W; y = p / W; } else { x = xy[2*(o + e)]; y = xy[2*(o + e) + 1]; }
+    const int k = equal_keys_sort_position(e, n);
+    px[k] = x; py[k] = y; porig[k] = e;
+    bx0 = min(bx0, x); by0 = min(by0, y); bx1 = max(bx1, x); by1 = max(by1, y);
+  }
+  atomicMin(&s_bb[0], bx0); atomicMin(&s_bb[1], by0); atomicMax(&s_bb[2], bx1); atomicMax(&s_bb[3], by1);
+  __syncthreads();
+  if (K == 1) { if (tid == 0) { sel[0] = porig[0]; nsel[l] = 1; } return; }
+  // anms.cc:282-310, same types: int / long long / double, float Kmin / Kmax
+  int low = 0, high = 0, prevwidth = -1; unsigned Kmin = 0, Kmax = 0;
+  if (tid == 0) {
+    high = anms_high(K, cols, rows);
+    low = (int)floor(sqrt((double)n/K));
+    const float t = tol ? tol[l] : tol_all, Kf = (float)(unsigned)K;
+    Kmin = (unsigned)roundf(Kf - Kf*t); Kmax = (unsigned)roundf(Kf + Kf*t);
+    s_kept = 0;
+  }
+  for (;;) {
+    if (tid == 0) {
+      const int width = low + (high - low)/2;
+      s_stop = (width == prevwidth || low > high) ? 1 : 0;         // keep the last computed result
+      if (!s_stop) {
+        SelGrid g; g.w = width; g.x0 = s_bb[0]; g.y0 = s_bb[1];
+        const int bw = s_bb[2] - s_bb[0] + 1, bh = s_bb[3] - s_bb[1] + 1;
+        g.s = max(max(width, 1), (int)sqrt((double)bw*bh/SEL_GRID));
+        while ((long long)((bw + g.s - 1)/g.s)*((bh + g.s - 1)/g.s) > SEL_GRID) g.s++;
+        g.nx = (bw + g.s - 1)/g.s; g.ny = (bh + g.s - 1)/g.s;
+        s_g = g; s_width = width;
+      }
+    }
+    __syncthreads();
+    if (s_stop) break;
+    const SelGrid g = s_g;
+    for (int c = tid; c < g.nx*g.ny; c += SEL_THREADS) head[c] = -1;
+    __syncthreads();
+    int kept = 0;                                                  // (warp 0's running count)
+    for (int c0 = 0; c0 < n; c0 += SEL_THREADS) {
+      const int i = c0 + tid;
+      pend[tid] = (i < n && !sel_conflict(g, head, px, py, nxt, px[i], py[i])) ? 1 : 0;
+      __syncthreads();
+      if (tid < 32) {
+        for (int g0 = 0; g0 < SEL_THREADS && c0 + g0 < n; g0 += 32) {
+          const int j = c0 + g0 + lane;
+          bool p = j < n && pend[g0 + lane];
+          if (!__any_sync(0xffffffffu, p)) continue;
+          const int x = j < n ? px[j] : 0, y = j < n ? py[j] : 0;
+          if (p && g0 > 0) p = !sel_conflict(g, head, px, py, nxt, x, y);      // points kept earlier in this chunk
+          const unsigned M = __ballot_sync(0xffffffffu, p);
+          unsigned cm = 0;
+          for (int b = 0; b < 32; b++) {
+            const int xb = __shfl_sync(0xffffffffu, x, b), yb = __shfl_sync(0xffffffffu, y, b);
+            const int dx = xb - x, dy = yb - y;
+            if (b < lane && ((M >> b) & 1u) && dx <= g.w && dx >= -g.w && dy <= g.w && dy >= -g.w) cm |= 1u << b;
+          }
+          unsigned km = 0;
+          for (int b = 0; b < 32; b++) {
+            const unsigned cb = __shfl_sync(0xffffffffu, cm, b);
+            if (((M >> b) & 1u) && !(cb & km)) km |= 1u << b;
+          }
+          if ((km >> lane) & 1u) {
+            sel[kept + __popc(km & ((1u << lane) - 1u))] = j;
+            nxt[j] = atomicExch(&head[((y - g.y0)/g.s)*g.nx + (x - g.x0)/g.s], j);
+          }
+          kept += __popc(km);
+          __syncwarp();
+        }
+        if (tid == 0) s_kept = kept;
+      }
+      __syncthreads();
+    }
+    if (tid == 0) {                                                // anms.cc:347-354
+      const unsigned r = (unsigned)s_kept;
+      s_done = 0;
+      if (r >= Kmin && r <= Kmax) s_done = 1;
+      else if (r < Kmin) high = s_width - 1;
+      else low = s_width + 1;
+      prevwidth = s_width;
+    }
+    __syncthreads();
+    if (s_done) break;
+  }
+  const int m = s_kept;
+  for (int r = tid; r < m; r += SEL_THREADS) sel[r] = porig[sel[r]];
+  if (tid == 0) nsel[l] = m;
+}
+
+// sampleDynamic after ANMS (FeatureTracker.cc:955-1015): list offsets and the number of corners needed per object
+__global__ void sd_prepare_kernel(int nobj, const int* tot, const int* num_track, int max_features, int* off, int* kneed) {
+  if (threadIdx.x != 0) return;
+  int run = 0;
+  for (int o = 0; o < nobj; o++) { off[o] = run; run += tot[o]; kneed[o] = max(max_features - num_track[o], 0); }
+}
+// one CTA per object: the selected candidate pixels become features, packed object after object in the given order
+__global__ void sd_construct_kernel(const int* __restrict__ off, const int* __restrict__ nsel, const int* __restrict__ sel, const int* __restrict__ idx,
+                                    const float* __restrict__ flow, int W, const int* __restrict__ objs, long long base_id, double* __restrict__ out /*[S][6]*/,
+                                    long long* __restrict__ otid, int32_t* __restrict__ olab) {
+  const int o = blockIdx.x;
+  int base = 0;
+  for (int q = 0; q < o; q++) base += nsel[q];
+  for (int r = threadIdx.x; r < nsel[o]; r += blockDim.x) {
+    const int p = idx[off[o] + sel[off[o] + r]], x = p % W, y = p / W, d = base + r;
+    const double fx = (double)flow[2*(size_t)p], fy = (double)flow[2*(size_t)p + 1];
+    out[6*(size_t)d] = x; out[6*(size_t)d + 1] = y; out[6*(size_t)d + 2] = fx; out[6*(size_t)d + 3] = fy;
+    out[6*(size_t)d + 4] = x + fx; out[6*(size_t)d + 5] = y + fy;     // Feature::CalculatePredictedKeypoint
+    otid[d] = base_id + d; olab[d] = objs[o];
   }
 }
 
@@ -663,6 +841,142 @@ int dynofront_sample_candidates(dynofront_handle h, int32_t nobj, const int32_t*
     FCK(cudaStreamSynchronize(h->s));
   }
   FCK(cudaGetLastError());
+  return 0;
+}
+
+static int ensure_selection(dynofront_ctx* h, size_t points, int lists) {
+  if (points > (size_t)h->sel_cap) {
+    const size_t cap = std::max<size_t>(points, (size_t)h->W*h->H);
+    if (cap > 0x7fffffff) { h->err = "too many key-points"; return -1; }
+    int rc = 0;
+    rc |= falloc(h, &h->sel_xy, 2*cap); rc |= falloc(h, &h->sel_px, cap); rc |= falloc(h, &h->sel_py, cap); rc |= falloc(h, &h->sel_orig, cap);
+    rc |= falloc(h, &h->sel_next, cap); rc |= falloc(h, &h->sel_out, cap);
+    if (rc) return -3;
+    h->sel_cap = (int)cap;
+  }
+  if (lists > h->sel_lists) {
+    const int cap = std::max(lists, ST_MAXOBJ);
+    int rc = 0;
+    rc |= falloc(h, &h->sel_off, cap); rc |= falloc(h, &h->sel_cnt, cap); rc |= falloc(h, &h->sel_k, cap); rc |= falloc(h, &h->sel_n, cap); rc |= falloc(h, &h->sel_tol, cap);
+    if (rc) return -3;
+    h->sel_lists = cap;
+  }
+  return 0;
+}
+
+int dynofront_anms_range_tree(dynofront_handle h, int32_t n_lists, const int32_t* offsets, const int32_t* xy, const int32_t* k_needed,
+                              const float* tolerance, int32_t cols, int32_t rows, int32_t* selected, int32_t* n_selected, float* ms_device) {
+  if (!h || n_lists < 0 || (n_lists && (!offsets || !k_needed || !tolerance || !n_selected)) || cols <= 0 || rows <= 0) return -1;
+  cudaSetDevice(h->dev);
+  if (n_lists == 0) return 0;
+  if (offsets[0] != 0) { h->err = "offsets[0] must be 0"; return -1; }
+  std::vector<int> cnt(n_lists);
+  for (int l = 0; l < n_lists; l++) {
+    cnt[l] = offsets[l + 1] - offsets[l];
+    if (cnt[l] < 0) { h->err = "offsets must not decrease"; return -1; }
+    if (k_needed[l] < 0) { h->err = "k_needed must be >= 0"; return -1; }
+  }
+  const size_t total = (size_t)offsets[n_lists];
+  if (total && (!xy || !selected)) return -1;
+  for (size_t i = 0; i < 2*total; i++) if (xy[i] < 0 || xy[i] > 65535) { h->err = "key-point coordinates must be in [0, 65535]"; return -1; }
+  for (int l = 0; l < n_lists; l++) {        // the reference's u16 range tree wraps x + width above 65535: reject instead of diverging
+    if (cnt[l] == 0 || k_needed[l] < 2) continue;
+    int cmax = 0;
+    for (int i = 2*offsets[l]; i < 2*offsets[l + 1]; i++) cmax = std::max(cmax, (int)xy[i]);
+    if ((long long)cmax + std::max(anms_high(k_needed[l], cols, rows), 0) > 65535) { h->err = "key-point coordinate + search width exceeds 65535 (u16 range tree)"; return -1; }
+  }
+  if (ensure_selection(h, total, n_lists)) return -3;
+  FCK(cudaEventRecord(h->e0, h->s));
+  FCK(cudaMemcpyAsync(h->sel_off, offsets, (size_t)n_lists*4, cudaMemcpyHostToDevice, h->s));
+  FCK(cudaMemcpyAsync(h->sel_cnt, cnt.data(), (size_t)n_lists*4, cudaMemcpyHostToDevice, h->s));
+  FCK(cudaMemcpyAsync(h->sel_k, k_needed, (size_t)n_lists*4, cudaMemcpyHostToDevice, h->s));
+  FCK(cudaMemcpyAsync(h->sel_tol, tolerance, (size_t)n_lists*4, cudaMemcpyHostToDevice, h->s));
+  if (total) FCK(cudaMemcpyAsync(h->sel_xy, xy, 2*total*4, cudaMemcpyHostToDevice, h->s));
+  anms_range_tree_kernel<<<n_lists, SEL_THREADS, 0, h->s>>>(h->sel_off, h->sel_cnt, h->sel_k, h->sel_tol, 0.f, nullptr, h->sel_xy, 0, cols, rows,
+                                                            h->sel_px, h->sel_py, h->sel_orig, h->sel_next, h->sel_out, h->sel_n);
+  FCK(cudaGetLastError());
+  if (total) FCK(cudaMemcpyAsync(selected, h->sel_out, total*4, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(n_selected, h->sel_n, (size_t)n_lists*4, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+
+int dynofront_sample_dynamic(dynofront_handle h, int32_t nobj, const int32_t* objects, const int32_t* num_track, int32_t max_features,
+                             const dynofront_track_params* prm, int64_t* next_tracklet_id, int32_t* counts, int32_t* num_sampled, int32_t* zero_flow,
+                             int32_t capacity, double* keypoint, double* flow_out, double* predicted, int64_t* tracklet, int32_t* label,
+                             int32_t* n_features, float* ms_device) {
+  if (!h || !prm || nobj < 0 || nobj > ST_MAXOBJ || capacity < 0 || !next_tracklet_id || !num_sampled || !n_features) return -1;
+  if (nobj && (!objects || !num_track)) return -1;
+  if (capacity && (!keypoint || !flow_out || !predicted || !tracklet)) { h->err = "null feature array"; return -1; }
+  {                                          // no width of the search may wrap the reference's u16 coordinates (see dynofront_anms_range_tree)
+    int hmax = 0;
+    for (int k = 2; k <= max_features; k++) hmax = std::max(hmax, anms_high(k, h->W, h->H));
+    if ((long long)std::max(h->W, h->H) - 1 + hmax > 65535) { h->err = "image too large for the u16 range tree of the reference"; return -1; }
+  }
+  cudaSetDevice(h->dev);
+  const size_t npx = (size_t)h->W*h->H; const int ntiles = (int)((npx + ST_TILE - 1)/ST_TILE);
+  if (ensure_selection(h, npx, ST_MAXOBJ)) return -3;
+  if (!h->sd_idx) {
+    int rc = 0;
+    rc |= falloc(h, &h->sd_idx, npx); rc |= falloc(h, &h->sd_off, ST_MAXOBJ); rc |= falloc(h, &h->sd_k, ST_MAXOBJ); rc |= falloc(h, &h->sd_ntrack, ST_MAXOBJ);
+    if (rc) return -3;
+  }
+  FCK(cudaEventRecord(h->e0, h->s));
+  if (!h->det_work_valid) prepare_det_work(h);
+  *n_features = 0;
+  std::vector<int> tot(std::max(nobj, 1)), zc(std::max(nobj, 1)), ns(std::max(nobj, 1));
+  if (nobj > 0) {
+    FCK(cudaMemcpyAsync(h->d_objs, objects, (size_t)nobj*4, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->sd_ntrack, num_track, (size_t)nobj*4, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemsetAsync(h->d_zero, 0, ST_MAXOBJ*4, h->s));
+    // (1) the candidate scan of dynofront_sample_candidates, its compaction kept on the device
+    sc_count_kernel<<<ntiles, ST_TILE, 0, h->s>>>(npx, h->W, h->H, h->det_work, h->mask, h->flow, h->d_objs, nobj, *prm, h->tile_cnt, h->d_zero);
+    sc_scan_kernel<<<1, ST_MAXOBJ, 0, h->s>>>(ntiles, nobj, h->tile_cnt, h->obj_tot);
+    sd_prepare_kernel<<<1, 32, 0, h->s>>>(nobj, h->obj_tot, h->sd_ntrack, max_features, h->sd_off, h->sd_k);
+    sc_scatter_kernel<<<ntiles, ST_TILE, 0, h->s>>>(npx, h->W, h->H, h->det_work, h->mask, h->flow, h->d_objs, nobj, *prm, h->tile_cnt, h->sd_off,
+                                                    h->sd_idx, (long long)npx);
+    // (2) + (3) P_n and the range-tree ANMS per object, K = max(max_features - num_track, 0), tolerance 0.01 (FeatureTracker.cc:955-980)
+    anms_range_tree_kernel<<<nobj, SEL_THREADS, 0, h->s>>>(h->sd_off, h->obj_tot, h->sd_k, nullptr, 0.01f, h->sd_idx, nullptr, h->W, h->W, h->H,
+                                                           h->sel_px, h->sel_py, h->sel_orig, h->sel_next, h->sel_out, h->sel_n);
+    FCK(cudaGetLastError());
+    FCK(cudaMemcpyAsync(tot.data(), h->obj_tot, (size_t)nobj*4, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(zc.data(), h->d_zero, (size_t)nobj*4, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(ns.data(), h->sel_n, (size_t)nobj*4, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaStreamSynchronize(h->s));
+  }
+  int S = 0;
+  for (int o = 0; o < nobj; o++) { if (counts) counts[o] = tot[o]; if (zero_flow) zero_flow[o] = zc[o]; num_sampled[o] = ns[o]; S += ns[o]; }
+  if (S > h->sd_cap) {
+    const int cap = std::max(S, 4096);
+    if (falloc(h, &h->sd_out, 6*(size_t)cap) || falloc(h, &h->sd_tid, cap) || falloc(h, &h->sd_lab, cap)) return -3;
+    h->sd_cap = cap;
+  }
+  const long long base_id = *next_tracklet_id;
+  const int ncopy = std::min(S, capacity);
+  std::vector<double> out6(6*(size_t)ncopy);
+  if (S > 0) {
+    // (4) the features, tracklet ids in object order then ANMS order
+    sd_construct_kernel<<<nobj, 128, 0, h->s>>>(h->sd_off, h->sel_n, h->sel_out, h->sd_idx, h->flow, h->W, h->d_objs, base_id, h->sd_out, h->sd_tid, h->sd_lab);
+    FCK(cudaGetLastError());
+    if (ncopy) {
+      FCK(cudaMemcpyAsync(out6.data(), h->sd_out, out6.size()*8, cudaMemcpyDeviceToHost, h->s));
+      FCK(cudaMemcpyAsync(tracklet, h->sd_tid, (size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
+      if (label) FCK(cudaMemcpyAsync(label, h->sd_lab, (size_t)ncopy*4, cudaMemcpyDeviceToHost, h->s));
+    }
+  }
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  FCK(cudaGetLastError());
+  for (int d = 0; d < ncopy; d++) {
+    keypoint[2*d] = out6[6*(size_t)d]; keypoint[2*d + 1] = out6[6*(size_t)d + 1];
+    flow_out[2*d] = out6[6*(size_t)d + 2]; flow_out[2*d + 1] = out6[6*(size_t)d + 3];
+    predicted[2*d] = out6[6*(size_t)d + 4]; predicted[2*d + 1] = out6[6*(size_t)d + 5];
+  }
+  *next_tracklet_id = base_id + S;
+  *n_features = S;
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
   return 0;
 }
 

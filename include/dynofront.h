@@ -5,6 +5,8 @@
  * Replaces, with the same inputs / outputs and the same ordering semantics:
  *   dynofront_track_dynamic     FeatureTracker::trackDynamic        dynosam/src/frontend/vision/FeatureTracker.cc:339-498
  *   dynofront_sample_candidates FeatureTracker::sampleDynamic scan  FeatureTracker.cc:864-953
+ *   dynofront_sample_dynamic    FeatureTracker::sampleDynamic: scan + range-tree ANMS + new features  FeatureTracker.cc:864-1015
+ *   dynofront_anms_range_tree   AdaptiveNonMaximumSuppression::suppressNonMax(RangeTree), batched  anms.cc:278-362
  *   dynofront_propagate_mask    FeatureTracker::propogateMask       FeatureTracker.cc:1212-1359
  *   dynofront_track_static_flow ExternalFlowFeatureTracker::trackStatic / constructStaticFeature  StaticFeatureTracker.cc:70-220
  *   dynofront_klt_track_fb      KltFeatureTracker::trackPoints: forward + backward LK, round-trip test, label / border / age checks (:486-592)
@@ -65,6 +67,39 @@ int dynofront_track_dynamic(dynofront_handle h, int32_t n, const double* prev_pr
  * object skipped because a flow component is exactly 0.  capacity = size of indices. */
 int dynofront_sample_candidates(dynofront_handle h, int32_t n_objects, const int32_t* objects, const dynofront_track_params* prm,
                                 int32_t* counts, int32_t* offsets, int32_t* zero_flow, int32_t* indices, int64_t capacity);
+
+/* AdaptiveNonMaximumSuppression::suppressNonMax with AnmsAlgorithmType::RangeTree (NonMaximumSupression.cc:33-116,
+ * anms.cc:278-362) on n_lists key-point lists in one launch.  List l holds the integer key-points xy[offsets[l] ..
+ * offsets[l+1])[2] (pixel column, row in [0, 65535]), all with response 0 as at both reference call sites: they are
+ * visited in the order cv::sortIdx(SORT_DESCENDING) gives all-equal keys (a fixed permutation of the input), and the
+ * binary search over the square half-width keeps those with no earlier kept point in the inclusive square, aiming at
+ * k_needed[l] within tolerance[l] (float, as the reference).  selected + offsets[l] receives the indices (within list l)
+ * of the n_selected[l] kept points in selection order; the search can end on more than k_needed (1 + tolerance) points
+ * but never on more than the list holds, so the list's own range of selected is always large enough.
+ * Defined where the reference is not: k_needed = 0 selects nothing, k_needed = 1 the first point in visiting order.
+ * The reference's range tree stores u16 coordinates and so wraps a search bound x + width above 65535; a list whose
+ * largest coordinate plus the largest width the search can try (its quadratic-formula upper bound) exceeds 65535 is
+ * refused with -1 instead of giving a different result (at 1242x375 the widest width is 497 px: far from it). */
+int dynofront_anms_range_tree(dynofront_handle h, int32_t n_lists, const int32_t* offsets /*[n_lists+1]*/, const int32_t* xy,
+                              const int32_t* k_needed, const float* tolerance, int32_t cols, int32_t rows, int32_t* selected,
+                              int32_t* n_selected, float* ms_device);
+
+/* FeatureTracker::sampleDynamic completed on the device (FeatureTracker.cc:864-1015): the candidate scan of
+ * dynofront_sample_candidates (same detection mask), then per object the range-tree ANMS above with tolerance 0.01 and
+ * k = max(max_features - num_track[o], 0) (max_dynamic_features_per_frame, params/FrontendParams.yaml), then the new
+ * features.  Candidates never leave the device.  Per object: counts[o] candidates, num_sampled[o] features kept
+ * (the reference's num_sampled after ANMS), zero_flow[o] (counts / zero_flow may be NULL).  Features are packed object
+ * after object in the order of objects, each in ANMS order: key-point (col, row), measured flow (float flow as double),
+ * predicted key-point (key-point + flow), tracklet id counting up from *next_tracklet_id (updated), label (may be NULL).
+ * *n_features = how many there are; the first min(n_features, capacity) are written (ids are handed out for all).
+ * Images whose side plus the widest search width exceeds 65535 are refused (see dynofront_anms_range_tree).
+ * Tracklet id order: the reference fills its candidate lists inside a tbb::parallel_for and hands out ids inside a
+ * tbb::parallel_for_each over objects, so its order depends on scheduling; the order here is the one a single-threaded
+ * run of the reference produces. */
+int dynofront_sample_dynamic(dynofront_handle h, int32_t n_objects, const int32_t* objects, const int32_t* num_track,
+                             int32_t max_features, const dynofront_track_params* prm, int64_t* next_tracklet_id, int32_t* counts,
+                             int32_t* num_sampled, int32_t* zero_flow, int32_t capacity, double* keypoint, double* flow,
+                             double* predicted_keypoint, int64_t* tracklet, int32_t* label, int32_t* n_features, float* ms_device);
 
 /* propogateMask: previous-frame features (predicted key-point, label), previous mask / flow, current mask (in/out).
  * All three images NULL: streaming mode, the resident previous frame votes into the resident current motion mask in place. */
