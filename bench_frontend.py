@@ -141,6 +141,7 @@ def run_dynoba(n, warmup, streaming=True):
                    f"({dense_bytes/1e6:.1f} MB) would take {dense_bytes/3.35e12*1e6:.1f} us at the H100 data-sheet HBM rate (3.35 TB/s)"}
     if streaming:
         out.update(full_frame(t, frames, static_pts, feats, n, warmup))
+        out.update(static_detection(t, frames, static_pts, n, warmup))
     out.update(card())
     return out
 
@@ -169,8 +170,35 @@ def full_frame(t, frames, static_pts, feats, n, warmup):
         ms, s = one(k); sd.append(ms); sampled.append(s)
     dt = time.perf_counter() - t0
     return {"full_frame_fps": n/dt, "sample_dynamic_ms": float(np.mean(sd)), "sampled_per_frame": float(np.mean(sampled)),
-            "full_frame_note": "streaming loop with dynofront_sample_dynamic in place of dynofront_sample_candidates; "
-                               "static feature detection is not on the device yet and is not part of the loop"}
+            "full_frame_note": "streaming loop with dynofront_sample_dynamic in place of dynofront_sample_candidates; static "
+                               "feature detection (dynofront_detect_static) runs on the device but is timed in its own loop "
+                               "(detect_static_ms), not in this one"}
+
+
+def static_detection(t, frames, static_pts, n, warmup):
+    """KltFeatureTracker::detectFeatures on the device over the streaming frames: after the forward-backward KLT, the kept
+    static tracks are the current features (n_cur = the keep count), as on the reference's trigger path; plus the first-frame
+    case n_cur = 0.  detect_static_ms is the device time of one call (CUDA events), detected_per_frame the new features."""
+    from dynosam_b200.frontend import DetectParams, TrackParams
+    prm = DetectParams(); tprm = TrackParams(); static_age = np.zeros(N_STATIC, np.int32)
+    t.next_frame(frames[0][0], frames[0][2], frames[0][1])
+
+    def one(k):
+        g1, m1, f1 = frames[k]
+        t.next_frame(g1, f1, m1)
+        p1, st, back, keep = t.klt_track_fb(None, None, static_pts, tprm, static_age, 25)
+        kp, tid, _, _ = t.detect_static(None, p1[keep.astype(bool)], prm, 0)
+        return t.last_ms, len(kp)
+    for k in range(1, warmup + 1):
+        one(k)
+    ms, det = [], []
+    for k in range(1, n + 1):
+        a, b = one(k); ms.append(a); det.append(b)
+    first = []
+    for k in range(1, min(n, 20) + 1):
+        t.detect_static(None, np.zeros((0, 2)), prm, 0); first.append(t.last_ms)
+    return {"detect_static_ms": float(np.mean(ms)), "detected_per_frame": float(np.mean(det)),
+            "detect_static_first_frame_ms": float(np.mean(first)), "detected_first_frame": len(t.detect_static(None, np.zeros((0, 2)), prm, 0)[0])}
 
 
 def card():

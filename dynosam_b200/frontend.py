@@ -13,7 +13,8 @@ LIB_PATH = os.path.join(_HERE, "libdynofront.so")
 EXPORTS = ["dynofront_create", "dynofront_destroy", "dynofront_last_error", "dynofront_set_frame", "dynofront_track_dynamic",
            "dynofront_sample_candidates", "dynofront_propagate_mask", "dynofront_klt_track", "dynofront_klt_track_fb",
            "dynofront_klt_last_min_eig", "dynofront_stereo_track", "dynofront_track_static_flow", "dynofront_next_frame", "dynofront_pin_host", "dynofront_unpin_host",
-           "dynofront_get_motion_mask", "dynofront_get_pyramid_level", "dynofront_anms_range_tree", "dynofront_sample_dynamic"]
+           "dynofront_get_motion_mask", "dynofront_get_pyramid_level", "dynofront_anms_range_tree", "dynofront_sample_dynamic",
+           "dynofront_detect_static", "dynofront_detect_last_stages"]
 
 
 class TrackParamsC(C.Structure):
@@ -36,6 +37,37 @@ class KltFbParamsC(C.Structure):
                 ("win_back", C.c_int32), ("max_level_back", C.c_int32), ("max_count_back", C.c_int32), ("epsilon_back", C.c_double),
                 ("use_initial_flow", C.c_int32), ("min_eig_threshold", C.c_double), ("max_fb_distance", C.c_double),
                 ("check_static", C.c_int32), ("max_feature_track_age", C.c_int32), ("track", TrackParamsC)]
+
+
+class DetectParamsC(C.Structure):
+    _fields_ = [("use_clahe", C.c_int32), ("use_anms", C.c_int32), ("use_subpix", C.c_int32), ("max_corners", C.c_int32),
+                ("quality_level", C.c_double), ("block_size", C.c_int32), ("use_harris", C.c_int32), ("min_distance", C.c_int32),
+                ("max_features", C.c_int32), ("subpix_win", C.c_int32), ("subpix_max_iter", C.c_int32), ("subpix_eps", C.c_double),
+                ("track", TrackParamsC)]
+
+
+@dataclass
+class DetectParams:
+    """KltFeatureTracker::detectFeatures parameters: TrackerParams defaults, params/FrontendParams.yaml where it sets them."""
+    use_clahe: bool = True
+    use_anms: bool = True
+    use_subpix: bool = True
+    max_corners: int = 1000          # max_nr_keypoints_before_anms
+    quality_level: float = 0.001
+    block_size: int = 3
+    use_harris: bool = False
+    min_distance: int = 15           # min_distance_btw_tracked_and_detected_static_features
+    max_features: int = 800          # max_features_per_frame
+    subpix_win: int = 5
+    subpix_max_iter: int = 40
+    subpix_eps: float = 0.001
+    shrink_row: int = 0
+    shrink_col: int = 0
+
+    def c(self):
+        return DetectParamsC(int(self.use_clahe), int(self.use_anms), int(self.use_subpix), self.max_corners, float(self.quality_level), self.block_size,
+                             int(self.use_harris), self.min_distance, self.max_features, self.subpix_win, self.subpix_max_iter, float(self.subpix_eps),
+                             TrackParamsC(0, 0, self.shrink_row, self.shrink_col))
 
 
 _LIB = None
@@ -71,6 +103,9 @@ def load():
         L.dynofront_anms_range_tree.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p]*4 + [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)]
         L.dynofront_sample_dynamic.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(TrackParamsC), C.POINTER(C.c_int64),
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p]*5 + [C.POINTER(C.c_int32), C.POINTER(C.c_float)]
+        L.dynofront_detect_static.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(DetectParamsC), C.POINTER(C.c_int64), C.c_int32,
+                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float)]
+        L.dynofront_detect_last_stages.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
         L.dynofront_get_pyramid_level.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]
         _LIB = L
     return _LIB
@@ -191,6 +226,30 @@ class FeatureTrackerGPU:
         s = nf.value
         return dict(counts=counts, num_sampled=ns, zero_flow=zero, keypoint=kp[:s], flow=fl[:s], predicted=pk[:s], tracklet=tid[:s], label=lab[:s],
                     next_tracklet_id=nid.value)
+
+    def detect_static(self, gray, cur_kp, prm: DetectParams, next_tracklet_id: int, capacity=None):
+        """KltFeatureTracker::detectFeatures on the device: detection mask, CLAHE, good-features-to-track, range-tree ANMS,
+        cornerSubPix and the new static features.  gray=None: the resident current frame of next_frame.  Uses the motion mask
+        and boundary mask of the current frame.  Returns (keypoints [n][2], tracklet ids, next_tracklet_id, n_corners)."""
+        g = None if gray is None else np.ascontiguousarray(gray, dtype=np.uint8)
+        kp = np.ascontiguousarray(cur_kp, dtype=np.float64).reshape(-1, 2); n = kp.shape[0]
+        cap = int(capacity if capacity is not None else max(prm.max_features, 1) + 64)
+        out = np.zeros((cap, 2)); tid = np.zeros(cap, np.int64)
+        nid = C.c_int64(int(next_tracklet_id)); nf = C.c_int32(); nc = C.c_int32(); ms = C.c_float(); pc = prm.c()
+        self._ck(self.lib.dynofront_detect_static(self.h, _p(g), n, _p(kp), C.byref(pc), C.byref(nid), cap, _p(out), _p(tid), C.byref(nf), C.byref(nc),
+                                                  C.byref(ms)))
+        self.last_ms = ms.value
+        if nf.value > cap:                                        # more than the guess: run again with room for all
+            return self.detect_static(gray, cur_kp, prm, next_tracklet_id, nf.value)
+        return out[:nf.value], tid[:nf.value], nid.value, nc.value
+
+    def detect_stages(self):
+        """the last detect_static's CLAHE image, minimum-eigenvalue image and GFTT corners before ANMS ([n][2] x, y)"""
+        nc = C.c_int32()
+        self._ck(self.lib.dynofront_detect_last_stages(self.h, None, None, None, C.byref(nc)))
+        cl = np.zeros((self.H, self.W), np.uint8); eig = np.zeros((self.H, self.W), np.float32); xy = np.zeros((max(nc.value, 1), 2), np.int32)
+        self._ck(self.lib.dynofront_detect_last_stages(self.h, _p(cl), _p(eig), _p(xy), C.byref(nc)))
+        return cl, eig, xy[:nc.value]
 
     def propagate_mask(self, prev_pred_kp, prev_label, prev_mask, prev_flow, current_mask, prm: TrackParams, min_votes=150):
         kp = np.ascontiguousarray(prev_pred_kp, dtype=np.float64).reshape(-1, 2)

@@ -47,6 +47,10 @@ struct dynofront_ctx {
   int *sel_off = nullptr, *sel_cnt = nullptr, *sel_k = nullptr, *sel_n = nullptr; float* sel_tol = nullptr;
   int* sd_idx = nullptr; int *sd_off = nullptr, *sd_k = nullptr, *sd_ntrack = nullptr; int sd_cap = 0; double* sd_out = nullptr;
   long long* sd_tid = nullptr; int32_t* sd_lab = nullptr;
+  // static detection (dynofront_detect_static); dt_int: candidates, corners, 0, K, ANMS count, -, features, max key
+  uint8_t *dt_gray = nullptr, *dt_mask = nullptr, *dt_clahe = nullptr, *dt_lut = nullptr; float *dt_dx = nullptr, *dt_dy = nullptr, *dt_box = nullptr, *dt_eig = nullptr;
+  unsigned long long* dt_keys = nullptr; int dt_keycap = 0; int *dt_corners = nullptr, *dt_int = nullptr; float *dt_pts = nullptr, *dt_resp = nullptr;
+  double* dt_kp = nullptr; long long* dt_tid = nullptr; bool dt_valid = false;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   std::vector<void*> allocs;
 };
@@ -272,16 +276,75 @@ __host__ __device__ inline int anms_high(int K, int cols, int rows) {
   return (int)(sol1 > sol2 ? sol1 : sol2);
 }
 struct SelGrid { int x0, y0, s, nx, ny, w; };
+// Two metrics share the ordered resolver: the range tree's inclusive square |dx|, |dy| <= w, and goodFeaturesToTrack's
+// strict disc dx^2 + dy^2 < w^2 (its minDistance test).
+template <bool EUCLID> __device__ __forceinline__ bool sel_near(int dx, int dy, int w) {
+  return EUCLID ? dx*dx + dy*dy < w*w : (dx <= w && dx >= -w && dy <= w && dy >= -w);
+}
+template <bool EUCLID>
 __device__ __forceinline__ bool sel_conflict(const SelGrid& g, const int* head, const int* px, const int* py, const int* nxt, int x, int y) {
   const int cx0 = max(x - g.w - g.x0, 0)/g.s, cx1 = min((x + g.w - g.x0)/g.s, g.nx - 1);
   const int cy0 = max(y - g.w - g.y0, 0)/g.s, cy1 = min((y + g.w - g.y0)/g.s, g.ny - 1);
   for (int cy = cy0; cy <= cy1; cy++)
     for (int cx = cx0; cx <= cx1; cx++)
-      for (int q = head[cy*g.nx + cx]; q >= 0; q = nxt[q]) {
-        const int dx = px[q] - x, dy = py[q] - y;
-        if (dx <= g.w && dx >= -g.w && dy <= g.w && dy >= -g.w) return true;
-      }
+      for (int q = head[cy*g.nx + cx]; q >= 0; q = nxt[q])
+        if (sel_near<EUCLID>(px[q] - x, py[q] - y, g.w)) return true;
   return false;
+}
+// The ordered greedy of one CTA over points 0..n-1 of px / py: a point is kept when no earlier kept point is near it, and
+// the pass stops once `limit` points are kept.  sel[0..) receives the kept positions in order; returns how many (the value
+// is also in *s_kept, for every thread).
+template <bool EUCLID>
+__device__ int sel_greedy(const SelGrid& g, int n, int limit, const int* px, const int* py, int* nxt, int* sel, int* head, uint8_t* pend, int* s_kept) {
+  const int tid = threadIdx.x, lane = tid & 31;
+  for (int c = tid; c < g.nx*g.ny; c += SEL_THREADS) head[c] = -1;
+  if (tid == 0) *s_kept = 0;
+  __syncthreads();
+  int kept = 0;                                                  // (warp 0's running count)
+  for (int c0 = 0; c0 < n; c0 += SEL_THREADS) {
+    const int i = c0 + tid;
+    pend[tid] = (i < n && !sel_conflict<EUCLID>(g, head, px, py, nxt, px[i], py[i])) ? 1 : 0;
+    __syncthreads();
+    if (tid < 32) {
+      for (int g0 = 0; g0 < SEL_THREADS && c0 + g0 < n && kept < limit; g0 += 32) {
+        const int j = c0 + g0 + lane;
+        bool p = j < n && pend[g0 + lane];
+        if (!__any_sync(0xffffffffu, p)) continue;
+        const int x = j < n ? px[j] : 0, y = j < n ? py[j] : 0;
+        if (p && g0 > 0) p = !sel_conflict<EUCLID>(g, head, px, py, nxt, x, y);      // points kept earlier in this chunk
+        const unsigned M = __ballot_sync(0xffffffffu, p);
+        unsigned cm = 0;
+        for (int b = 0; b < 32; b++) {
+          const int xb = __shfl_sync(0xffffffffu, x, b), yb = __shfl_sync(0xffffffffu, y, b);
+          if (b < lane && ((M >> b) & 1u) && sel_near<EUCLID>(xb - x, yb - y, g.w)) cm |= 1u << b;
+        }
+        unsigned km = 0;
+        for (int b = 0; b < 32; b++) {
+          const unsigned cb = __shfl_sync(0xffffffffu, cm, b);
+          if (((M >> b) & 1u) && !(cb & km)) km |= 1u << b;
+        }
+        while (__popc(km) > limit - kept) km &= ~(1u << (31 - __clz(km)));     // the count limit: later points are not reached
+        if ((km >> lane) & 1u) {
+          sel[kept + __popc(km & ((1u << lane) - 1u))] = j;
+          nxt[j] = atomicExch(&head[((y - g.y0)/g.s)*g.nx + (x - g.x0)/g.s], j);
+        }
+        kept += __popc(km);
+        __syncwarp();
+      }
+      if (tid == 0) *s_kept = kept;
+    }
+    __syncthreads();
+    if (*s_kept >= limit) break;
+  }
+  return *s_kept;
+}
+__host__ __device__ inline SelGrid sel_make_grid(int width, int bx0, int by0, int bx1, int by1) {
+  SelGrid g; g.w = width; g.x0 = bx0; g.y0 = by0;
+  const int bw = bx1 - bx0 + 1, bh = by1 - by0 + 1;
+  g.s = max(max(width, 1), (int)sqrt((double)bw*bh/SEL_GRID));
+  while ((long long)((bw + g.s - 1)/g.s)*((bh + g.s - 1)/g.s) > SEL_GRID) g.s++;
+  g.nx = (bw + g.s - 1)/g.s; g.ny = (bh + g.s - 1)/g.s;
+  return g;
 }
 // Points of list l: pixel (lin % W, lin / W) of lin[off + e] when lin is given, else xy[off + e].  Work arrays px / py /
 // porig / nxt and the result sel are indexed like the input (off + position).  sel[off + r] = index within the list of
@@ -294,7 +357,7 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) anms_range_tree_kernel(const i
   __shared__ uint8_t pend[SEL_THREADS];
   __shared__ int s_bb[4], s_kept, s_width, s_stop, s_done;   // (two flags: no thread rewrites one that a slow warp may still read)
   __shared__ SelGrid s_g;
-  const int l = blockIdx.x, o = off[l], n = cnt[l], K = kneed[l], tid = threadIdx.x, lane = tid & 31;
+  const int l = blockIdx.x, o = off[l], n = cnt[l], K = kneed[l], tid = threadIdx.x;
   if (n <= 0 || K <= 0) { if (tid == 0) nsel[l] = 0; return; }
   px += o; py += o; porig += o; nxt += o; sel += o;
   if (tid == 0) { s_bb[0] = s_bb[1] = 0x7fffffff; s_bb[2] = s_bb[3] = -1; }
@@ -323,55 +386,11 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) anms_range_tree_kernel(const i
     if (tid == 0) {
       const int width = low + (high - low)/2;
       s_stop = (width == prevwidth || low > high) ? 1 : 0;         // keep the last computed result
-      if (!s_stop) {
-        SelGrid g; g.w = width; g.x0 = s_bb[0]; g.y0 = s_bb[1];
-        const int bw = s_bb[2] - s_bb[0] + 1, bh = s_bb[3] - s_bb[1] + 1;
-        g.s = max(max(width, 1), (int)sqrt((double)bw*bh/SEL_GRID));
-        while ((long long)((bw + g.s - 1)/g.s)*((bh + g.s - 1)/g.s) > SEL_GRID) g.s++;
-        g.nx = (bw + g.s - 1)/g.s; g.ny = (bh + g.s - 1)/g.s;
-        s_g = g; s_width = width;
-      }
+      if (!s_stop) { s_g = sel_make_grid(width, s_bb[0], s_bb[1], s_bb[2], s_bb[3]); s_width = width; }
     }
     __syncthreads();
     if (s_stop) break;
-    const SelGrid g = s_g;
-    for (int c = tid; c < g.nx*g.ny; c += SEL_THREADS) head[c] = -1;
-    __syncthreads();
-    int kept = 0;                                                  // (warp 0's running count)
-    for (int c0 = 0; c0 < n; c0 += SEL_THREADS) {
-      const int i = c0 + tid;
-      pend[tid] = (i < n && !sel_conflict(g, head, px, py, nxt, px[i], py[i])) ? 1 : 0;
-      __syncthreads();
-      if (tid < 32) {
-        for (int g0 = 0; g0 < SEL_THREADS && c0 + g0 < n; g0 += 32) {
-          const int j = c0 + g0 + lane;
-          bool p = j < n && pend[g0 + lane];
-          if (!__any_sync(0xffffffffu, p)) continue;
-          const int x = j < n ? px[j] : 0, y = j < n ? py[j] : 0;
-          if (p && g0 > 0) p = !sel_conflict(g, head, px, py, nxt, x, y);      // points kept earlier in this chunk
-          const unsigned M = __ballot_sync(0xffffffffu, p);
-          unsigned cm = 0;
-          for (int b = 0; b < 32; b++) {
-            const int xb = __shfl_sync(0xffffffffu, x, b), yb = __shfl_sync(0xffffffffu, y, b);
-            const int dx = xb - x, dy = yb - y;
-            if (b < lane && ((M >> b) & 1u) && dx <= g.w && dx >= -g.w && dy <= g.w && dy >= -g.w) cm |= 1u << b;
-          }
-          unsigned km = 0;
-          for (int b = 0; b < 32; b++) {
-            const unsigned cb = __shfl_sync(0xffffffffu, cm, b);
-            if (((M >> b) & 1u) && !(cb & km)) km |= 1u << b;
-          }
-          if ((km >> lane) & 1u) {
-            sel[kept + __popc(km & ((1u << lane) - 1u))] = j;
-            nxt[j] = atomicExch(&head[((y - g.y0)/g.s)*g.nx + (x - g.x0)/g.s], j);
-          }
-          kept += __popc(km);
-          __syncwarp();
-        }
-        if (tid == 0) s_kept = kept;
-      }
-      __syncthreads();
-    }
+    sel_greedy<false>(s_g, n, 0x7fffffff, px, py, nxt, sel, head, pend, &s_kept);
     if (tid == 0) {                                                // anms.cc:347-354
       const unsigned r = (unsigned)s_kept;
       s_done = 0;
@@ -683,6 +702,307 @@ __global__ void __launch_bounds__(1024) sf_det_resolve_kernel(int n, const int* 
   if (threadIdx.x == 0) *cnt_det = min(s_base, room);
 }
 
+// ---------------------------------------------------------------------------------------------------- KltFeatureTracker::detectFeatures
+// StaticFeatureTracker.cc:330-418 and SparseFeatureDetector::detect (FeatureDetector.cc:187-239) with the CPU OpenCV routines
+// they call (TrackerParams defaults: cv::GFTTDetector, not cv::cuda's).  Every float result reproduces cv2 bit for bit; the
+// orders below were pinned against it (opencv-python 4.x on x86-64 with AVX2 dispatch):
+//  * CLAHE: tiles on the BORDER_REFLECT_101-extended image when W or H is not a multiple of 8 (both sides are then padded by
+//    8 - side % 8), clip max(int(2.0 * area / 256), 1), tile coordinates as y * (1.f / tile_h) - 0.5f;
+//  * Sobel (scale 1 / (4 * 3 * 255) folded into the smoothing tap): the x derivative is fma(r[-1] + r[+1], s, r[0] * 2s) over
+//    the exact row differences; the y derivative's row pass is the SIMD fma chain for x < (W / 32) * 32 and the scalar
+//    sequential sum on the remaining columns, then the exact column difference;
+//  * the unnormalised 3x3 box sum of the products: rows as (c[-1] + c[0]) + c[+1] in double, then a running double sum that
+//    slides down each column (add the entering row, subtract the leaving one), rounded to float;
+//  * (a + c) - sqrt((a - c)^2 + b^2) in float without FMA.
+constexpr int DT_SORT_TILE = 2048, DT_TILES = 8;
+__device__ __forceinline__ uint32_t f32_order(float v) { const uint32_t u = __float_as_uint(v); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
+__device__ __forceinline__ float f32_unorder(uint32_t u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
+
+// detection mask: the caller's boundary mask (255 without one) AND background, then a filled cv::circle of radius r around
+// every current feature, centred on cvRound of the float key-point (cv::Point2f -> cv::Point: round half to even)
+__global__ void dt_mask_kernel(size_t npx, const uint8_t* __restrict__ det, const int32_t* __restrict__ mask, uint8_t* __restrict__ out) {
+  const size_t p = (size_t)blockIdx.x*blockDim.x + threadIdx.x;
+  if (p < npx) out[p] = (mask[p] == 0) ? (det ? det[p] : 255) : 0;
+}
+__global__ void dt_circles_kernel(int n, const double* __restrict__ kp, Disc disc, int W, int H, uint8_t* out) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int cx = __float2int_rn((float)kp[2*i]), cy = __float2int_rn((float)kp[2*i + 1]);
+  for (int dy = -disc.r; dy <= disc.r; dy++) {
+    const int yy = cy + dy; if (yy < 0 || yy >= H) continue;
+    const int hw = disc.hw[dy < 0 ? -dy : dy];
+    for (int dx = -hw; dx <= hw; dx++) { const int xx = cx + dx; if (xx >= 0 && xx < W) out[(size_t)yy*W + xx] = 0; }
+  }
+}
+// CLAHE(2.0, 8x8), one CTA per tile: histogram, clip, redistribution, LUT (clahe.cpp CLAHE_CalcLut_Body)
+__global__ void __launch_bounds__(256) clahe_lut_kernel(const uint8_t* __restrict__ img, int W, int H, int tw, int th, int clip, float lut_scale,
+                                                        uint8_t* __restrict__ lut) {
+  __shared__ int hist[256];
+  const int tx = blockIdx.x, ty = blockIdx.y;
+  hist[threadIdx.x] = 0;
+  __syncthreads();
+  for (int q = threadIdx.x; q < tw*th; q += blockDim.x) {
+    int x = tx*tw + q % tw, y = ty*th + q / tw;
+    if (x >= W) x = 2*W - 2 - x;                                 // the BORDER_REFLECT_101 extension (right / bottom only)
+    if (y >= H) y = 2*H - 2 - y;
+    atomicAdd(&hist[img[(size_t)y*W + x]], 1);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (clip > 0) {
+      int clipped = 0;
+      for (int i = 0; i < 256; i++) if (hist[i] > clip) { clipped += hist[i] - clip; hist[i] = clip; }
+      const int batch = clipped/256; int residual = clipped - batch*256;
+      for (int i = 0; i < 256; i++) hist[i] += batch;
+      if (residual != 0) { const int step = max(256/residual, 1); for (int i = 0; i < 256 && residual > 0; i += step, residual--) hist[i]++; }
+    }
+    int sum = 0; uint8_t* L = lut + (ty*DT_TILES + tx)*256;
+    for (int i = 0; i < 256; i++) { sum += hist[i]; L[i] = (uint8_t)min(max(__float2int_rn((float)sum*lut_scale), 0), 255); }
+  }
+}
+__global__ void clahe_apply_kernel(const uint8_t* __restrict__ img, int W, int H, float inv_tw, float inv_th, const uint8_t* __restrict__ lut,
+                                   uint8_t* __restrict__ out) {
+  const int x = blockIdx.x*blockDim.x + threadIdx.x, y = blockIdx.y*blockDim.y + threadIdx.y;
+  if (x >= W || y >= H) return;
+  const float tyf = (float)y*inv_th - 0.5f, txf = (float)x*inv_tw - 0.5f;
+  int ty1 = (int)floorf(tyf), ty2 = ty1 + 1, tx1 = (int)floorf(txf), tx2 = tx1 + 1;
+  const float ya = tyf - (float)ty1, ya1 = 1.0f - ya, xa = txf - (float)tx1, xa1 = 1.0f - xa;
+  ty1 = max(ty1, 0); ty2 = min(ty2, DT_TILES - 1); tx1 = max(tx1, 0); tx2 = min(tx2, DT_TILES - 1);
+  const int v = img[(size_t)y*W + x];
+  const uint8_t *L1 = lut + ty1*DT_TILES*256, *L2 = lut + ty2*DT_TILES*256;
+  const float res = ((float)L1[tx1*256 + v]*xa1 + (float)L1[tx2*256 + v]*xa)*ya1 + ((float)L2[tx1*256 + v]*xa1 + (float)L2[tx2*256 + v]*xa)*ya;
+  out[(size_t)y*W + x] = (uint8_t)min(max(__float2int_rn(res), 0), 255);
+}
+// Sobel 3x3 of cornerEigenValsVecs (see the orders above)
+__global__ void dt_sobel_kernel(const uint8_t* __restrict__ img, int W, int H, float* __restrict__ dx, float* __restrict__ dy) {
+  const int x = blockIdx.x*blockDim.x + threadIdx.x, y = blockIdx.y*blockDim.y + threadIdx.y;
+  if (x >= W || y >= H) return;
+  const double s = 1.0/(4*3*255.0);
+  const float f1 = (float)s, f0 = (float)(2*s);
+  const int xm = reflect101(x - 1, W), xp = reflect101(x + 1, W), ym = reflect101(y - 1, H), yp = reflect101(y + 1, H);
+  auto at = [&](int yy, int xx) { return (float)img[(size_t)yy*W + xx]; };
+  auto rd = [&](int yy) { return at(yy, xp) - at(yy, xm); };
+  const bool simd = x < (W/32)*32;
+  auto rs = [&](int yy) { const float L = at(yy, xm), M = at(yy, x), R = at(yy, xp);
+    return simd ? __fmaf_rn(R, f1, __fmaf_rn(M, f0, L*f1)) : (f1*L + f0*M) + f1*R; };
+  dx[(size_t)y*W + x] = __fmaf_rn(rd(ym) + rd(yp), f1, rd(y)*f0);
+  dy[(size_t)y*W + x] = rs(yp) - rs(ym);
+}
+// the unnormalised 3x3 box sum of one product channel (0: Ix Ix, 1: Ix Iy, 2: Iy Iy), one thread per (column, channel)
+// sliding down the column as ColumnSum<double, float> does; box is [3][H][W]
+__global__ void __launch_bounds__(32) dt_box_kernel(const float* __restrict__ dx, const float* __restrict__ dy, int W, int H, float* __restrict__ box) {
+  const int t = blockIdx.x*blockDim.x + threadIdx.x;
+  if (t >= 3*W) return;
+  const int c = t / W, x = t - c*W;
+  const int xm = reflect101(x - 1, W), xp = reflect101(x + 1, W);
+  const float* U = c == 2 ? dy : dx; const float* V = c == 0 ? dx : dy;
+  auto row = [&](int yy) {
+    const size_t r = (size_t)reflect101(yy, H)*W;
+    return ((double)(U[r + xm]*V[r + xm]) + (double)(U[r + x]*V[r + x])) + (double)(U[r + xp]*V[r + xp]);
+  };
+  float* out = box + (size_t)c*W*H + x;
+  double rm = row(-1), r0 = row(0), rp = row(1), S = (0.0 + rm) + r0;
+  for (int y = 0; y < H; y++) {
+    const double rn = y + 2 <= H ? row(y + 2) : 0.0;            // the next row is loaded while this one is summed
+    const double s0 = S + rp;
+    out[(size_t)y*W] = (float)s0; S = s0 - rm;
+    rm = r0; r0 = rp; rp = rn;
+  }
+}
+// the minimum eigenvalue per pixel and the maximum of the eigen image under the detection mask (minMaxLoc), as an
+// order-preserving u32
+__global__ void dt_eig_kernel(const float* __restrict__ box, size_t npx, const uint8_t* __restrict__ mask, float* __restrict__ eig, unsigned* __restrict__ maxv) {
+  const size_t p = (size_t)blockIdx.x*blockDim.x + threadIdx.x;
+  uint32_t best = 0;
+  if (p < npx) {
+    const float a = box[p]*0.5f, b = box[npx + p], cc = box[2*npx + p]*0.5f;
+    const float e = (a + cc) - sqrtf((a - cc)*(a - cc) + b*b);
+    eig[p] = e;
+    if (mask[p]) best = f32_order(e);
+  }
+  for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
+  if ((threadIdx.x & 31) == 0 && best) atomicMax(maxv, best);
+}
+// goodFeaturesToTrack candidates: THRESH_TOZERO at (float)(maxVal * quality), 3x3 local maxima (dilate) that are non-zero
+// and inside the mask, the 1-px border excluded.  Key = value (order-preserving) << 32 | pixel address, sorted descending:
+// greaterThanPtr (larger value first, ties: larger address first).
+__global__ void dt_cand_kernel(const float* __restrict__ eig, int W, int H, const uint8_t* __restrict__ mask, const unsigned* __restrict__ maxv,
+                               double quality, unsigned long long* __restrict__ keys, int* __restrict__ count) {
+  const int x = blockIdx.x*blockDim.x + threadIdx.x, y = blockIdx.y*blockDim.y + threadIdx.y;
+  if (x < 1 || y < 1 || x >= W - 1 || y >= H - 1) return;
+  const float mx = *maxv ? f32_unorder(*maxv) : 0.f;             // minMaxLoc over an empty mask leaves maxVal = 0
+  const float thr = (float)((double)mx*quality);
+  auto tz = [&](int xx, int yy) { const float v = eig[(size_t)yy*W + xx]; return v > thr ? v : 0.f; };
+  const float v = tz(x, y);
+  if (v == 0.f || !mask[(size_t)y*W + x]) return;
+  float d = v;
+  for (int j = -1; j <= 1; j++) for (int i = -1; i <= 1; i++) d = fmaxf(d, tz(x + i, y + j));
+  if (v != d) return;
+  const int k = atomicAdd(count, 1);
+  keys[k] = ((unsigned long long)f32_order(v) << 32) | (unsigned)(y*W + x);
+}
+// bitonic sort (descending) of keys[0 .. npad), npad = max(next power of two >= *count, DT_SORT_TILE); every launch reads the
+// count on the device and the stages above npad return at once, so the host plans for the largest size without a readback
+__device__ __forceinline__ int dt_npad(const int* count) { int n = DT_SORT_TILE; while (n < *count) n <<= 1; return n; }
+__global__ void dt_sort_pad_kernel(unsigned long long* keys, const int* count, int cap) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x, n = dt_npad(count);
+  if (i >= *count && i < n && i < cap) keys[i] = 0ull;
+}
+__device__ __forceinline__ void dt_cmpx(unsigned long long* a, unsigned long long* b, bool desc) {
+  const unsigned long long x = *a, y = *b;
+  if ((x < y) == desc) { *a = y; *b = x; }
+}
+__global__ void __launch_bounds__(DT_SORT_TILE/2) dt_sort_local_kernel(unsigned long long* keys, const int* count, int k_first, int k_last) {
+  __shared__ unsigned long long s[DT_SORT_TILE];
+  const int n = dt_npad(count), base = blockIdx.x*DT_SORT_TILE;
+  if (base >= n || k_last > n) return;
+  s[threadIdx.x] = keys[base + threadIdx.x]; s[threadIdx.x + DT_SORT_TILE/2] = keys[base + threadIdx.x + DT_SORT_TILE/2];
+  __syncthreads();
+  for (int k = k_first; k <= k_last; k <<= 1)
+    for (int j = min(k, DT_SORT_TILE)/2; j > 0; j >>= 1) {
+      const int t = threadIdx.x, i = (t/j)*2*j + (t % j);
+      dt_cmpx(&s[i], &s[i + j], ((base + i) & k) == 0);
+      __syncthreads();
+    }
+  keys[base + threadIdx.x] = s[threadIdx.x]; keys[base + threadIdx.x + DT_SORT_TILE/2] = s[threadIdx.x + DT_SORT_TILE/2];
+}
+__global__ void dt_sort_global_kernel(unsigned long long* keys, const int* count, int k, int j) {
+  const int n = dt_npad(count), t = blockIdx.x*blockDim.x + threadIdx.x;
+  if (k > n || t >= n/2) return;
+  const int i = (t/j)*2*j + (t % j);
+  dt_cmpx(&keys[i], &keys[i + j], (i & k) == 0);
+}
+// the greedy minDistance filter with the maxCorners stop (goodFeaturesToTrack), one CTA, through the ordered resolver of
+// the ANMS with the strict Euclidean metric.  corners[2*c] = (x, y) in output order, *n_corners; resp = the first value.
+__global__ void __launch_bounds__(SEL_THREADS, 1) dt_gftt_select_kernel(const unsigned long long* __restrict__ keys, const int* __restrict__ count, int W, int H,
+                                                                      int min_dist, int max_corners, int* px, int* py, int* nxt, int* sel,
+                                                                      int* __restrict__ corners, int* __restrict__ n_corners, float* __restrict__ resp) {
+  __shared__ int head[SEL_GRID];
+  __shared__ uint8_t pend[SEL_THREADS];
+  __shared__ int s_kept;
+  __shared__ SelGrid s_g;
+  const int n = *count, tid = threadIdx.x;
+  if (n == 0) { if (tid == 0) { *n_corners = 0; *resp = 0.f; } return; }
+  for (int e = tid; e < n; e += SEL_THREADS) { const unsigned a = (unsigned)keys[e]; px[e] = (int)(a % W); py[e] = (int)(a / W); }
+  if (tid == 0) s_g = sel_make_grid(min_dist, 0, 0, W - 1, H - 1);
+  __syncthreads();
+  const int m = sel_greedy<true>(s_g, n, max_corners > 0 ? max_corners : 0x7fffffff, px, py, nxt, sel, head, pend, &s_kept);
+  for (int r = tid; r < m; r += SEL_THREADS) { corners[2*r] = px[sel[r]]; corners[2*r + 1] = py[sel[r]]; }
+  if (tid == 0) { *n_corners = m; *resp = f32_unorder((unsigned)(keys[0] >> 32)); }
+}
+// cv::getRectSubPix(img, 13x13, centre, CV_32F) as cornerSubPix calls it.  Inside the image: the four float weights, summed
+// as (p a11 + q a12) + (u a21 + v a22); near the border: adjustRect's clamped rectangle (columns outside the image repeat
+// the vertical interpolation of the edge column, rows outside repeat the edge row), which gives cv2's values up to the last
+// bit of some entries (cv2 runs Intel IPP there; DESIGN section 4).
+constexpr int SP_WIN = 5, SP_W = 2*SP_WIN + 1, SP_P = SP_W + 2;
+struct SubpixMask { float m[SP_W*SP_W]; };
+__device__ void dt_rect_subpix(const uint8_t* __restrict__ img, int W, int H, float cx0, float cy0, float* patch) {
+  const float cx = cx0 - (SP_P - 1)*0.5f, cy = cy0 - (SP_P - 1)*0.5f;
+  const int ix = (int)floorf(cx), iy = (int)floorf(cy);
+  const float a = cx - (float)ix, b = cy - (float)iy;
+  const float a11 = (1.f - a)*(1.f - b), a12 = a*(1.f - b), a21 = (1.f - a)*b, a22 = a*b, b1 = 1.f - b, b2 = b;
+  auto px = [&](int y, int x) { return (float)img[(size_t)y*W + x]; };
+  if (0 <= ix && ix < W - SP_P && 0 <= iy && iy < H - SP_P) {
+    for (int i = 0; i < SP_P; i++)
+      for (int j = 0; j < SP_P; j++)
+        patch[i*SP_P + j] = (px(iy + i, ix + j)*a11 + px(iy + i, ix + j + 1)*a12) + (px(iy + i + 1, ix + j)*a21 + px(iy + i + 1, ix + j + 1)*a22);
+    return;
+  }
+  int col = 0, row = 0, rx, rw, ry, rh;                          // adjustRect (imgwarp.cpp)
+  if (ix >= 0) { col += ix; rx = 0; } else { rx = min(-ix, SP_P); }
+  if (ix < W - SP_P) rw = SP_P; else { rw = W - ix - 1; if (rw < 0) { col += rw; rw = 0; } }
+  if (iy >= 0) { row += iy; ry = 0; } else ry = -iy;
+  if (iy < H - SP_P) rh = SP_P; else { rh = H - iy - 1; if (rh < 0) { row += rh; rh = 0; } }
+  col -= rx;
+  for (int i = 0; i < SP_P; i++) {
+    int r2 = row + 1;
+    if (i < ry || i >= rh) r2 -= 1;
+    // rows above the image that are cut on the right repeat column W - 2, not W - 1 (what cv2's getRectSubPix returns there)
+    const int cr = (i < ry && rw < SP_P) ? col + rw - 1 : col + rw;
+    const float s0 = px(row, col + rx)*b1 + px(r2, col + rx)*b2, s1 = px(row, cr)*b1 + px(r2, cr)*b2;
+    for (int j = 0; j < rx; j++) patch[i*SP_P + j] = s0;
+    for (int j = rw; j < SP_P; j++) patch[i*SP_P + j] = s1;
+    for (int j = rx; j < rw; j++) {
+      const float p = px(row, col + j), q = px(row, col + j + 1);
+      patch[i*SP_P + j] = r2 != row ? (p*a11 + q*a12) + (px(r2, col + j)*a21 + px(r2, col + j + 1)*a22) : p*(1.f - a) + q*a;
+    }
+    if (i < rh) row = r2;
+  }
+}
+// cv::cornerSubPix(img, pts, (5,5), (-1,-1), EPS+COUNT): one thread per point, OpenCV's sequential double sums over the
+// 11x11 window (the eps^2 test sees them, so their order is kept), the det <= DBL_EPSILON^2 and leave-the-image breaks, and
+// the reset to the start when the point moved more than the window.  The Gaussian weights come from the host (std::exp).
+// Point r is corner sel[r] (corner r without ANMS, sel == NULL), r < *cnt.
+__global__ void dt_subpix_kernel(int m, const int* __restrict__ corners, const int* __restrict__ sel, const int* __restrict__ cnt,
+                                 const uint8_t* __restrict__ img, int W, int H, SubpixMask mask, int max_iters, double eps2, float* __restrict__ pts) {
+  const int r = blockIdx.x*blockDim.x + threadIdx.x;
+  if (r >= m || r >= *cnt) return;
+  const int c = sel ? sel[r] : r;
+  const float tx = (float)corners[2*c], ty = (float)corners[2*c + 1];
+  float ix = tx, iy = ty;
+  float patch[SP_P*SP_P];
+  int iter = 0; double err = 0;
+  do {
+    dt_rect_subpix(img, W, H, ix, iy, patch);
+    double a = 0, b = 0, cc = 0, bb1 = 0, bb2 = 0;
+    for (int i = 0, k = 0; i < SP_W; i++) {
+      const double py = i - SP_WIN;
+      const float* sp = patch + (i + 1)*SP_P + 1;
+      for (int j = 0; j < SP_W; j++, k++) {
+        const double mk = mask.m[k];
+        const double tgx = sp[j + 1] - sp[j - 1], tgy = sp[j + SP_P] - sp[j - SP_P];
+        const double gxx = tgx*tgx*mk, gxy = tgx*tgy*mk, gyy = tgy*tgy*mk, pxd = j - SP_WIN;
+        a += gxx; b += gxy; cc += gyy;
+        bb1 += gxx*pxd + gxy*py; bb2 += gxy*pxd + gyy*py;
+      }
+    }
+    const double det = a*cc - b*b;
+    if (fabs(det) <= 2.220446049250313e-16*2.220446049250313e-16) break;
+    const double scale = 1.0/det;
+    const float nx = (float)(ix + cc*scale*bb1 - b*scale*bb2), ny = (float)(iy - b*scale*bb1 + a*scale*bb2);
+    err = (nx - ix)*(nx - ix) + (ny - iy)*(ny - iy);
+    ix = nx; iy = ny;
+    if (ix < 0 || ix >= W || iy < 0 || iy >= H) break;
+  } while (++iter < max_iters && err > eps2);
+  if (fabsf(ix - tx) > SP_WIN || fabsf(iy - ty) > SP_WIN) { ix = tx; iy = ty; }
+  pts[2*r] = ix; pts[2*r + 1] = iy;
+}
+// the detected points in ANMS order become features (StaticFeatureTracker.cc:393-415): contained, inside the shrunken
+// image, background at the truncated pixel; in-order prefix count, tracklet ids from base_id in that order.  One CTA.
+__global__ void __launch_bounds__(1024) dt_construct_kernel(const float* __restrict__ pts, const int* __restrict__ cnt, const int32_t* __restrict__ mask,
+                                                            int W, int H, dynofront_track_params prm, long long base_id, double* __restrict__ kp,
+                                                            long long* __restrict__ tid, int* __restrict__ n_out) {
+  __shared__ int s_scan[1024]; __shared__ int s_base;
+  const int n = *cnt;
+  if (threadIdx.x == 0) s_base = 0;
+  __syncthreads();
+  for (int j0 = 0; j0 < n; j0 += 1024) {
+    const int j = j0 + threadIdx.x;
+    double kx = 0, ky = 0; int a = 0;
+    if (j < n) {
+      kx = (double)pts[2*j]; ky = (double)pts[2*j + 1];
+      const bool contained = kx >= 0.0 && kx < (double)W && ky >= 0.0 && ky < (double)H;
+      a = (contained && within_shrunken(kx, ky, H, W, prm.shrink_row, prm.shrink_col) && mask[(size_t)((int)ky)*W + (int)kx] == 0) ? 1 : 0;
+    }
+    s_scan[threadIdx.x] = a;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) { const int v = threadIdx.x >= o ? s_scan[threadIdx.x - o] : 0; __syncthreads(); s_scan[threadIdx.x] += v; __syncthreads(); }
+    const int rank = s_base + s_scan[threadIdx.x] - a;
+    if (a) { kp[2*(size_t)rank] = kx; kp[2*(size_t)rank + 1] = ky; tid[rank] = base_id + rank; }
+    __syncthreads();
+    if (threadIdx.x == 1023) s_base += s_scan[1023];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *n_out = s_base;
+}
+// the points cornerSubPix would refine when it is off: the integer corners as floats, in selection order
+__global__ void dt_points_kernel(int m, const int* __restrict__ corners, const int* __restrict__ sel, const int* __restrict__ cnt, float* __restrict__ pts) {
+  const int r = blockIdx.x*blockDim.x + threadIdx.x;
+  if (r >= m || r >= *cnt) return;
+  const int c = sel ? sel[r] : r;
+  pts[2*r] = (float)corners[2*c]; pts[2*r + 1] = (float)corners[2*c + 1];
+}
+
 // ---------------------------------------------------------------------------------------------------- host API
 extern "C" {
 
@@ -977,6 +1297,122 @@ int dynofront_sample_dynamic(dynofront_handle h, int32_t nobj, const int32_t* ob
   *next_tracklet_id = base_id + S;
   *n_features = S;
   if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+
+int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_cur, const double* cur_kp, const dynofront_detect_params* prm,
+                            int64_t* next_tracklet_id, int32_t capacity, double* keypoint, int64_t* tracklet, int32_t* n_features,
+                            int32_t* n_corners, float* ms_device) {
+  if (!h || !prm || !next_tracklet_id || !n_features || n_cur < 0 || capacity < 0 || (n_cur && !cur_kp)) return -1;
+  if (capacity && (!keypoint || !tracklet)) { h->err = "null feature array"; return -1; }
+  if (prm->use_harris) { h->err = "the Harris response is not supported (TrackerParams: use_harris_corner_detector = false)"; return -1; }
+  if (prm->block_size != 3) { h->err = "block_size must be 3"; return -1; }
+  if (prm->min_distance < 0 || prm->min_distance > 15) { h->err = "min_distance must be in [0,15]"; return -1; }
+  if (prm->use_subpix && prm->subpix_win != SP_WIN) { h->err = "subpix_win must be 5"; return -1; }
+  if (!(prm->quality_level > 0.0)) { h->err = "quality_level must be > 0"; return -1; }
+  const int W = h->W, H = h->H; const size_t npx = (size_t)W*H;
+  if (W < SP_P + 2 || H < SP_P + 2) { h->err = "image smaller than the cornerSubPix window"; return -1; }
+  const int K = std::max(prm->max_features - n_cur, 0);
+  if (prm->use_anms && K >= 2 && (long long)std::max(W, H) - 1 + std::max(anms_high(K, W, H), 0) > 65535) { h->err = "image too large for the u16 range tree of the reference"; return -1; }
+  if (!gray && !h->have_pyr_cur) { h->err = "no current frame on the device"; return -2; }
+  cudaSetDevice(h->dev);
+  if (!h->dt_int) {
+    int keycap = DT_SORT_TILE; while ((size_t)keycap < npx) keycap <<= 1;
+    int rc = 0;
+    rc |= falloc(h, &h->dt_gray, npx); rc |= falloc(h, &h->dt_mask, npx); rc |= falloc(h, &h->dt_clahe, npx); rc |= falloc(h, &h->dt_lut, DT_TILES*DT_TILES*256);
+    rc |= falloc(h, &h->dt_dx, npx); rc |= falloc(h, &h->dt_dy, npx); rc |= falloc(h, &h->dt_box, 3*npx); rc |= falloc(h, &h->dt_eig, npx); rc |= falloc(h, &h->dt_keys, keycap);
+    rc |= falloc(h, &h->dt_corners, 2*npx); rc |= falloc(h, &h->dt_int, 8); rc |= falloc(h, &h->dt_pts, 2*npx); rc |= falloc(h, &h->dt_resp, 1);
+    rc |= falloc(h, &h->dt_kp, 2*npx); rc |= falloc(h, &h->dt_tid, npx);
+    if (rc) return -3;
+    h->dt_keycap = keycap;
+  }
+  if (ensure_selection(h, npx, 1) || ensure_features(h, n_cur)) return -3;
+  FCK(cudaEventRecord(h->e0, h->s));
+  const uint8_t* img = gray ? h->dt_gray : h->pyr[1][0];
+  if (gray) FCK(cudaMemcpyAsync(h->dt_gray, gray, npx, cudaMemcpyHostToDevice, h->s));
+  if (n_cur) FCK(cudaMemcpyAsync(h->f_kp, cur_kp, 2*(size_t)n_cur*8, cudaMemcpyHostToDevice, h->s));
+  int init[8] = {0, 0, 0, K, 0, 0, 0, 0};
+  FCK(cudaMemcpyAsync(h->dt_int, init, sizeof(init), cudaMemcpyHostToDevice, h->s));
+  const unsigned g1 = (unsigned)((npx + 255)/256); const dim3 blk(32, 8), grd((W + 31)/32, (H + 7)/8);
+  // (1) detection mask: boundary mask AND background, circles around the current features
+  dt_mask_kernel<<<g1, 256, 0, h->s>>>(npx, h->has_det ? h->det : nullptr, h->mask, h->dt_mask);
+  if (n_cur) dt_circles_kernel<<<(n_cur + 127)/128, 128, 0, h->s>>>(n_cur, h->f_kp, make_disc(prm->min_distance), W, H, h->dt_mask);
+  // (2) CLAHE(2.0, 8x8) on the plain mono image
+  if (prm->use_clahe) {
+    const bool exact = W % DT_TILES == 0 && H % DT_TILES == 0;
+    const int tw = exact ? W/DT_TILES : (W + DT_TILES - W % DT_TILES)/DT_TILES, th = exact ? H/DT_TILES : (H + DT_TILES - H % DT_TILES)/DT_TILES;
+    const int area = tw*th, clip = std::max((int)(2.0*area/256), 1);
+    clahe_lut_kernel<<<dim3(DT_TILES, DT_TILES), 256, 0, h->s>>>(img, W, H, tw, th, clip, 255.0f/(float)area, h->dt_lut);
+    clahe_apply_kernel<<<grd, blk, 0, h->s>>>(img, W, H, 1.0f/(float)tw, 1.0f/(float)th, h->dt_lut, h->dt_clahe);
+  } else FCK(cudaMemcpyAsync(h->dt_clahe, img, npx, cudaMemcpyDeviceToDevice, h->s));
+  // (3) cornerMinEigenVal(3, 3), its maximum under the mask, the candidates, their order, the minDistance / maxCorners filter
+  dt_sobel_kernel<<<grd, blk, 0, h->s>>>(h->dt_clahe, W, H, h->dt_dx, h->dt_dy);
+  dt_box_kernel<<<(3*W + 31)/32, 32, 0, h->s>>>(h->dt_dx, h->dt_dy, W, H, h->dt_box);
+  dt_eig_kernel<<<g1, 256, 0, h->s>>>(h->dt_box, npx, h->dt_mask, h->dt_eig, (unsigned*)(h->dt_int + 7));
+  dt_cand_kernel<<<grd, blk, 0, h->s>>>(h->dt_eig, W, H, h->dt_mask, (const unsigned*)(h->dt_int + 7), prm->quality_level, h->dt_keys, h->dt_int);
+  const int cap = h->dt_keycap, nb = cap/DT_SORT_TILE;
+  dt_sort_pad_kernel<<<(cap + 255)/256, 256, 0, h->s>>>(h->dt_keys, h->dt_int, cap);
+  dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(h->dt_keys, h->dt_int, 2, DT_SORT_TILE);
+  for (int k = 2*DT_SORT_TILE; k <= cap; k <<= 1) {
+    for (int j = k/2; j >= DT_SORT_TILE; j >>= 1) dt_sort_global_kernel<<<(cap/2 + 255)/256, 256, 0, h->s>>>(h->dt_keys, h->dt_int, k, j);
+    dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(h->dt_keys, h->dt_int, k, k);
+  }
+  dt_gftt_select_kernel<<<1, SEL_THREADS, 0, h->s>>>(h->dt_keys, h->dt_int, W, H, prm->min_distance, prm->max_corners, h->sel_px, h->sel_py, h->sel_next,
+                                                     h->sel_orig, h->dt_corners, h->dt_int + 1, h->dt_resp);
+  // (4) range-tree ANMS, K = max(max_features - n_cur, 0), tolerance 0.1 (FeatureDetector.cc:206-224)
+  const int* sel = nullptr; const int* cnt = h->dt_int + 1;
+  if (prm->use_anms) {
+    anms_range_tree_kernel<<<1, SEL_THREADS, 0, h->s>>>(h->dt_int + 2, h->dt_int + 1, h->dt_int + 3, nullptr, 0.1f, nullptr, h->dt_corners, 0, W, H,
+                                                         h->sel_px, h->sel_py, h->sel_orig, h->sel_next, h->sel_out, h->dt_int + 4);
+    sel = h->sel_out; cnt = h->dt_int + 4;
+  }
+  // (5) cornerSubPix in ANMS order, (6) the features
+  const int mcap = prm->max_corners > 0 ? (int)std::min<size_t>((size_t)prm->max_corners, npx) : (int)npx;
+  if (prm->use_subpix) {
+    SubpixMask sm;                                            // cornersubpix.cpp: the Gaussian weights, std::exp in float
+    for (int i = 0; i < SP_W; i++) {
+      const float y = (float)(i - SP_WIN)/SP_WIN, vy = std::exp(-y*y);
+      for (int j = 0; j < SP_W; j++) { const float x = (float)(j - SP_WIN)/SP_WIN; sm.m[i*SP_W + j] = (float)(vy*std::exp(-x*x)); }
+    }
+    const int iters = std::min(std::max(prm->subpix_max_iter, 1), 100); const double eps = std::max(prm->subpix_eps, 0.0);
+    dt_subpix_kernel<<<(mcap + 127)/128, 128, 0, h->s>>>(mcap, h->dt_corners, sel, cnt, h->dt_clahe, W, H, sm, iters, eps*eps, h->dt_pts);
+  } else dt_points_kernel<<<(mcap + 255)/256, 256, 0, h->s>>>(mcap, h->dt_corners, sel, cnt, h->dt_pts);
+  const long long base_id = *next_tracklet_id;
+  dt_construct_kernel<<<1, 1024, 0, h->s>>>(h->dt_pts, cnt, h->mask, W, H, prm->track, base_id, h->dt_kp, h->dt_tid, h->dt_int + 6);
+  FCK(cudaGetLastError());
+  int res[8]; float resp = 0.f;
+  FCK(cudaMemcpyAsync(res, h->dt_int, sizeof(res), cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(&resp, h->dt_resp, 4, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  h->dt_valid = true;
+  // suppressNonMax truncates the responses to int (NonMaximumSupression.cc:47-53); the visiting order P_n assumes they are
+  // all 0.  For blockSize 3 on 8-bit input |Ix|, |Iy| <= 1/3 after OpenCV's scale, so a, c <= 9 * (1/9) / 2 and the minimum
+  // eigenvalue (a + c) - sqrt((a - c)^2 + b^2) <= 2 min(a, c) <= 1, with equality impossible (a step that is maximal in x
+  // and in y over the whole 3x3 window would need its corner pixel to be 0 and 255).  Checked rather than assumed.
+  if (prm->use_anms && res[1] > 0 && resp >= 1.0f) { h->err = "a GFTT response >= 1.0: the ANMS order of the reference would differ"; return -1; }
+  const int total = res[6], ncopy = std::min(total, capacity);
+  if (ncopy) {
+    FCK(cudaMemcpyAsync(keypoint, h->dt_kp, 2*(size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(tracklet, h->dt_tid, (size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
+  }
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  *next_tracklet_id = base_id + total; *n_features = total;
+  if (n_corners) *n_corners = res[1];
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+int dynofront_detect_last_stages(dynofront_handle h, uint8_t* clahe, float* eig, int32_t* corners_xy, int32_t* n_corners) {
+  if (!h || !n_corners) return -1;
+  if (!h->dt_valid) { h->err = "no detection on this handle yet"; return -2; }
+  cudaSetDevice(h->dev);
+  const size_t npx = (size_t)h->W*h->H;
+  int nc = 0;
+  FCK(cudaMemcpy(&nc, h->dt_int + 1, 4, cudaMemcpyDeviceToHost));
+  if (clahe) FCK(cudaMemcpy(clahe, h->dt_clahe, npx, cudaMemcpyDeviceToHost));
+  if (eig) FCK(cudaMemcpy(eig, h->dt_eig, npx*4, cudaMemcpyDeviceToHost));
+  if (corners_xy && nc) FCK(cudaMemcpy(corners_xy, h->dt_corners, 2*(size_t)nc*4, cudaMemcpyDeviceToHost));
+  *n_corners = nc;
   return 0;
 }
 

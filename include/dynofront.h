@@ -10,6 +10,7 @@
  *   dynofront_propagate_mask    FeatureTracker::propogateMask       FeatureTracker.cc:1212-1359
  *   dynofront_track_static_flow ExternalFlowFeatureTracker::trackStatic / constructStaticFeature  StaticFeatureTracker.cc:70-220
  *   dynofront_klt_track_fb      KltFeatureTracker::trackPoints: forward + backward LK, round-trip test, label / border / age checks (:486-592)
+ *   dynofront_detect_static     KltFeatureTracker::detectFeatures: mask, CLAHE, GFTT, range-tree ANMS, cornerSubPix  StaticFeatureTracker.cc:330-418
  *   dynofront_stereo_track      FeatureTracker::stereoTrack: left -> right LK + disparity / depth test  FeatureTracker.cc:194-337
  *   dynofront_klt_track         cv::calcOpticalFlowPyrLK as called by KltFeatureTracker::trackPoints
  *                               (StaticFeatureTracker.cc:420-625) and FeatureTracker::trackDynamicKLT (FeatureTracker.cc:500-862)
@@ -153,6 +154,45 @@ int dynofront_track_static_flow(dynofront_handle h, int32_t n_prev, const double
                                 int32_t max_features, int64_t* next_tracklet_id, uint8_t* acc_prev, double* flow_prev,
                                 double* pred_prev, int32_t* age_out, uint8_t* acc_det, double* flow_det, double* pred_det,
                                 int64_t* tracklet_det, int32_t* n_tracked, int32_t* n_detected);
+
+/* KltFeatureTracker::detectFeatures (StaticFeatureTracker.cc:330-418) with SparseFeatureDetector::detect
+ * (FeatureDetector.cc:187-239) in ONE call, CPU OpenCV semantics (cv::GFTTDetector, the TrackerParams default and the
+ * reference's fall-back without OpenCV CUDA):
+ *   detection mask = the boundary mask given to dynofront_set_frame / dynofront_next_frame (255 without one; never the copy
+ *   dynofront_track_dynamic drew into) AND motion_mask == 0, then a filled cv::circle of radius min_distance around each of
+ *   the n_cur current static features cur_kp[n_cur][2], centred on cvRound of the float key-point;
+ *   CLAHE(2.0, 8x8) of the mono image (use_clahe); goodFeaturesToTrack(max_corners, quality_level, min_distance, mask,
+ *   block_size 3, gradient 3, no Harris); range-tree ANMS (use_anms) with K = max(max_features - n_cur, 0) and tolerance 0.1,
+ *   under the conventions of dynofront_anms_range_tree (K = 0: nothing, K = 1: the first point in visiting order);
+ *   cornerSubPix (use_subpix) on the CLAHE image, window (subpix_win, subpix_win), zero zone (-1, -1), EPS+COUNT criteria, in
+ *   ANMS order; then the points contained in the image, inside the shrunken image (track.shrink_row / shrink_col) and on the
+ *   background at their truncated pixel become new static features (age 0, label 0), tracklet ids counting up from
+ *   *next_tracklet_id (updated).
+ * gray == NULL: the resident current frame of dynofront_next_frame (nothing is uploaded).  Nothing returns to the host
+ * between the stages.  *n_features = how many new features there are; the first min(n_features, capacity) key-points
+ * [capacity][2] (the refined floats as double) and tracklet ids are written (ids are handed out for all).  *n_corners (may
+ * be NULL) = the GFTT output count before ANMS.
+ * Refused with -1: Harris, block_size != 3, min_distance outside [0, 15], subpix_win != 5, an image whose side plus the
+ * widest ANMS width exceeds 65535 (see dynofront_anms_range_tree), and -- after the fact, nothing written -- a largest GFTT
+ * response >= 1.0, where the reference's int-truncated ANMS keys would stop being all equal (it cannot happen for block
+ * size 3 on 8-bit input). */
+typedef struct {
+  int32_t use_clahe, use_anms, use_subpix;                 /* TrackerParams defaults: 1, 1, 1 */
+  int32_t max_corners;                                     /* max_nr_keypoints_before_anms (yaml 1000) */
+  double quality_level; int32_t block_size, use_harris;    /* 0.001, 3, 0 */
+  int32_t min_distance;                                    /* min_distance_btw_tracked_and_detected_static_features (yaml 15): GFTT
+                                                              minDistance and circle radius */
+  int32_t max_features;                                    /* max_features_per_frame (yaml 800) */
+  int32_t subpix_win, subpix_max_iter; double subpix_eps;  /* 5, 40, 0.001 */
+  dynofront_track_params track;                            /* shrink margins */
+} dynofront_detect_params;
+int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_cur, const double* cur_kp, const dynofront_detect_params* prm,
+                            int64_t* next_tracklet_id, int32_t capacity, double* keypoint, int64_t* tracklet, int32_t* n_features,
+                            int32_t* n_corners, float* ms_device);
+/* parity hook: the CLAHE image (u8[H][W], the input itself without CLAHE), the minimum-eigenvalue image (f32[H][W]) and the
+ * GFTT corners before ANMS ([n_corners][2] (x, y), in GFTT order) of the last dynofront_detect_static; any output may be
+ * NULL, *n_corners is always set. */
+int dynofront_detect_last_stages(dynofront_handle h, uint8_t* clahe, float* eig, int32_t* corners_xy, int32_t* n_corners);
 
 /* parity hooks: pyramid level / Scharr derivative of the last prev image (level l): sizes via w,h out */
 int dynofront_get_pyramid_level(dynofront_handle h, int32_t which /*0 prev,1 cur*/, int32_t level, int32_t* w, int32_t* hgt,
