@@ -20,44 +20,68 @@
 
 #define FCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return -3; } } while (0)
 
+// A grow-only device array that owns its allocation.  Growing waits for the work queued on the stream (it may still read
+// the old array), frees the old array and allocates the new one; when the array is large enough, ensure() does nothing, so
+// the steady state neither synchronises nor frees.
+template <class T> struct DevBuf {
+  T* p = nullptr; size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+  ~DevBuf() { cudaFree(p); }
+  operator T*() const { return p; }
+  cudaError_t ensure(size_t n, cudaStream_t s) {
+    if (n <= cap) return cudaSuccess;
+    if (p) {
+      const cudaError_t e = cudaStreamSynchronize(s);
+      if (e != cudaSuccess) return e;
+      cudaFree(p); p = nullptr; cap = 0;
+    }
+    const cudaError_t e = cudaMalloc((void**)&p, n*sizeof(T));
+    if (e != cudaSuccess) { p = nullptr; return e; }
+    cap = n; return cudaSuccess;
+  }
+};
+// the counters of dynofront_detect_static; (anms_off, corners, K) is the one list anms_range_tree_kernel reads, anms its count
+struct DetectCounters { int candidates, corners, anms_off, K, anms, unused, features; unsigned max_eig; };
+
 struct dynofront_ctx {
   int dev = 0, W = 0, H = 0; cudaStream_t s = nullptr; std::string err; bool have_prev = false, have_cur = false, have_pyr = false, have_pyr_cur = false;
-  float* flow = nullptr; int32_t* mask = nullptr; uint8_t* det = nullptr; bool has_det = false;
-  uint8_t* det_work = nullptr; uint8_t* trk = nullptr; int* trk_idx = nullptr; bool det_work_valid = false;
-  // feature scratch (capacity cap)
-  int cap = 0; double* f_kp = nullptr; int32_t *f_lab = nullptr, *f_age = nullptr; int64_t* f_tid = nullptr;
-  int *f_x = nullptr, *f_y = nullptr, *f_state = nullptr, *f_next = nullptr; double* f_out = nullptr; int32_t* f_oage = nullptr; int64_t* f_otid = nullptr;
-  int32_t* f_olab = nullptr; uint8_t* f_acc = nullptr; int* cell = nullptr; long long* nextid = nullptr;
+  DevBuf<float> flow; DevBuf<int32_t> mask; DevBuf<uint8_t> det; bool has_det = false;
+  DevBuf<uint8_t> det_work, trk; DevBuf<int> trk_idx; bool det_work_valid = false;
+  // feature scratch
+  DevBuf<double> f_kp, f_pred, f_flow; DevBuf<int32_t> f_lab, f_age, f_oage, f_olab; DevBuf<int64_t> f_tid, f_otid;
+  DevBuf<int> f_x, f_y, f_state, f_next, cell; DevBuf<uint8_t> f_acc; DevBuf<long long> nextid;
   // sampling scratch
-  int* tile_cnt = nullptr; int* obj_tot = nullptr; int* d_objs = nullptr; int* d_zero = nullptr; int* d_idx = nullptr; size_t idx_cap = 0;
+  DevBuf<int> tile_cnt, obj_tot, d_objs, d_zero, d_idx;
   // propagate scratch
-  int32_t* pmask = nullptr; float* pflow = nullptr; int32_t* cmask = nullptr; int* pflag = nullptr;
-  // KLT
-  std::vector<uint8_t*> pyr[2]; std::vector<short*> der; std::vector<int> lw, lh;
-  float *k_prev = nullptr, *k_next = nullptr, *k_err = nullptr; uint8_t* k_st = nullptr; int k_cap = 0;
-  float *k_back = nullptr, *k_eig = nullptr; uint8_t *k_st2 = nullptr, *k_keep = nullptr; int32_t* k_age = nullptr; int* k_count = nullptr;   // forward-backward tracker
-  double* st_depth = nullptr; int st_cap = 0;     // stereoTrack
-  std::vector<short*> der2;                       // Scharr derivatives of the CURRENT image (backward pass)
+  DevBuf<int32_t> pmask, cmask; DevBuf<float> pflow; DevBuf<int> pflag;
+  // KLT; der2: Scharr derivatives of the CURRENT image (backward pass)
+  std::vector<DevBuf<uint8_t>> pyr[2]; std::vector<DevBuf<short>> der, der2; std::vector<int> lw, lh;
+  DevBuf<float> k_prev, k_next, k_err, k_back, k_eig; DevBuf<uint8_t> k_st, k_st2, k_keep; DevBuf<int32_t> k_age; DevBuf<int> k_count;
+  DevBuf<double> st_depth;                        // stereoTrack
   // external-flow static tracker scratch
-  int sf_cap = 0, sf_cells = 0; double* sf_kp = nullptr; int32_t* sf_age = nullptr; uint8_t* sf_use = nullptr; int32_t* sf_det = nullptr;
-  int *sf_cell = nullptr, *sf_win = nullptr, *sf_win2 = nullptr, *sf_cnt = nullptr; uint8_t* sf_pass = nullptr; uint8_t* sf_acc = nullptr; double* sf_out = nullptr;
-  int32_t* sf_oage = nullptr; long long* sf_otid = nullptr;
-  // ANMS work arrays (grow-only: points, lists) and sampleDynamic selection scratch
-  int sel_cap = 0, sel_lists = 0; int *sel_xy = nullptr, *sel_px = nullptr, *sel_py = nullptr, *sel_orig = nullptr, *sel_next = nullptr, *sel_out = nullptr;
-  int *sel_off = nullptr, *sel_cnt = nullptr, *sel_k = nullptr, *sel_n = nullptr; float* sel_tol = nullptr;
-  int* sd_idx = nullptr; int *sd_off = nullptr, *sd_k = nullptr, *sd_ntrack = nullptr; int sd_cap = 0; double* sd_out = nullptr;
-  long long* sd_tid = nullptr; int32_t* sd_lab = nullptr;
-  // static detection (dynofront_detect_static); dt_int: candidates, corners, 0, K, ANMS count, -, features, max key
-  uint8_t *dt_gray = nullptr, *dt_mask = nullptr, *dt_clahe = nullptr, *dt_lut = nullptr; float *dt_dx = nullptr, *dt_dy = nullptr, *dt_box = nullptr, *dt_eig = nullptr;
-  unsigned long long* dt_keys = nullptr; int dt_keycap = 0; int *dt_corners = nullptr, *dt_int = nullptr; float *dt_pts = nullptr, *dt_resp = nullptr;
-  double* dt_kp = nullptr; long long* dt_tid = nullptr; bool dt_valid = false;
+  DevBuf<double> sf_kp, sf_flow, sf_pred; DevBuf<int32_t> sf_age, sf_det, sf_oage; DevBuf<uint8_t> sf_use, sf_pass, sf_acc;
+  DevBuf<int> sf_cell, sf_win, sf_win2, sf_cnt; DevBuf<long long> sf_otid;
+  // ANMS work arrays and lists, sampleDynamic selection scratch
+  DevBuf<int> sel_xy, sel_px, sel_py, sel_orig, sel_next, sel_out, sel_off, sel_cnt, sel_k, sel_n; DevBuf<float> sel_tol;
+  DevBuf<int> sd_idx, sd_ntrack, sd_counts; DevBuf<double> sd_kp, sd_flow, sd_pred; DevBuf<long long> sd_tid; DevBuf<int32_t> sd_lab;
+  // static detection (dynofront_detect_static)
+  DevBuf<uint8_t> dt_gray, dt_mask, dt_clahe, dt_lut; DevBuf<float> dt_dx, dt_dy, dt_box, dt_eig, dt_pts, dt_resp;
+  DevBuf<unsigned long long> dt_keys; DevBuf<int> dt_corners; DevBuf<DetectCounters> dt_cnt;
+  DevBuf<double> dt_kp; DevBuf<long long> dt_tid; bool dt_valid = false;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
-  std::vector<void*> allocs;
 };
-template <class T> static int falloc(dynofront_ctx* h, T** p, size_t n) {
-  *p = nullptr; if (n == 0) n = 1;
-  FCK(cudaMalloc((void**)p, n*sizeof(T))); h->allocs.push_back((void*)*p); return 0;
+// grows each (buffer, element count) pair in turn; 0, or -3 with the error at the first allocation that fails
+static int grow(dynofront_ctx*) { return 0; }
+template <class T, class... R> static int grow(dynofront_ctx* h, DevBuf<T>& b, size_t n, R&&... rest) {
+  const cudaError_t e = b.ensure(n, h->s);
+  if (e != cudaSuccess) { h->err = std::string("device allocation: ") + cudaGetErrorString(e); return -3; }
+  return grow(h, rest...);
 }
+// feature arrays are sized for at least this many features, so that small changes of the count do not reallocate
+static size_t feature_cap(int n) { return (size_t)std::max(n, 4096); }
 
 // ---------------------------------------------------------------------------------------------------- trackDynamic
 struct Disc { int r; int hw[16]; };   // half width of the filled cv::circle per |dy|
@@ -72,9 +96,14 @@ static Disc make_disc(int r) {       // OpenCV drawing.cpp Circle(): midpoint al
   }
   return d;
 }
-__device__ __forceinline__ bool disc_covers(const Disc& d, int dxp, int dyp) {
-  const int ay = dyp < 0 ? -dyp : dyp, ax = dxp < 0 ? -dxp : dxp;
-  return ay <= d.r && ax <= d.hw[ay];
+// visits the pixels (x, y) of the filled disc around (cx, cy) that lie inside the W x H image, rows top to bottom, each row
+// left to right; stops after the first pixel for which visit returns true
+template <class F> __device__ __forceinline__ void disc_walk(const Disc& d, int cx, int cy, int W, int H, F visit) {
+  for (int dy = -d.r; dy <= d.r; dy++) {
+    const int yy = cy + dy; if (yy < 0 || yy >= H) continue;
+    const int hw = d.hw[dy < 0 ? -dy : dy];
+    for (int dx = -hw; dx <= hw; dx++) { const int xx = cx + dx; if (xx >= 0 && xx < W && visit(xx, yy)) return; }
+  }
 }
 __device__ __forceinline__ bool within_shrunken(double kx, double ky, int rows, int cols, int sr, int sc) {
   const int pc = (int)kx, pr = (int)ky;     // static_cast<int>
@@ -83,14 +112,14 @@ __device__ __forceinline__ bool within_shrunken(double kx, double ky, int rows, 
 
 __global__ void td_candidate_kernel(int n, const double* __restrict__ kp, const int32_t* __restrict__ plab, const int32_t* __restrict__ page,
                                     const float* __restrict__ flow, const int32_t* __restrict__ mask, const uint8_t* __restrict__ det, int W, int H,
-                                    dynofront_track_params prm, int* fx, int* fy, int* state, double* out /*[n][4]*/, int32_t* oage, int32_t* olab) {
+                                    dynofront_track_params prm, int* fx, int* fy, int* state, double* pred, double* oflow, int32_t* oage, int32_t* olab) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x;
   if (i >= n) return;
   const double kx = kp[2*i], ky = kp[2*i + 1];
   const int x = (int)kx, y = (int)ky;
   fx[i] = x; fy[i] = y;
   int st = 2;   // 0 unknown (candidate), 1 accepted, 2 rejected
-  out[4*i] = out[4*i+1] = out[4*i+2] = out[4*i+3] = 0.0; oage[i] = 0; olab[i] = 0;
+  pred[2*i] = pred[2*i+1] = oflow[2*i] = oflow[2*i+1] = 0.0; oage[i] = 0; olab[i] = 0;
   if (x >= 0 && x < W && y >= 0 && y < H) {
     const int lab = mask[(size_t)y*W + x];
     const bool det_ok = det ? det[(size_t)y*W + x] != 0 : true;
@@ -100,7 +129,7 @@ __global__ void td_candidate_kernel(int n, const double* __restrict__ kp, const 
       const double px = kx + fxe, py = ky + fye;
       if (within_shrunken(px, py, H, W, prm.shrink_row, prm.shrink_col) && !(fxe == 0 || fye == 0)) {
         st = 0;
-        out[4*i] = px; out[4*i+1] = py; out[4*i+2] = fxe; out[4*i+3] = fye;
+        pred[2*i] = px; pred[2*i+1] = py; oflow[2*i] = fxe; oflow[2*i+1] = fye;
         oage[i] = page[i] + 1; olab[i] = lab;
       }
     }
@@ -123,19 +152,15 @@ __global__ void __launch_bounds__(1024) td_resolve_kernel(int n, const int* fx, 
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
       if (state[i] != 0) continue;
       bool any_acc = false, any_unknown = false;
-      for (int dy = -disc.r; dy <= disc.r && !any_acc; dy++) {
-        const int yy = fy[i] + dy; if (yy < 0 || yy >= H) continue;
-        const int hw = disc.hw[dy < 0 ? -dy : dy];
-        for (int dx = -hw; dx <= hw && !any_acc; dx++) {
-          const int xx = fx[i] + dx; if (xx < 0 || xx >= W) continue;
-          for (int j = cell[(size_t)yy*W + xx]; j >= 0; j = next[j]) {
-            if (j >= i) continue;
-            const int sj = ((volatile int*)state)[j];
-            if (sj == 1) { any_acc = true; break; }
-            if (sj == 0) any_unknown = true;
-          }
+      disc_walk(disc, fx[i], fy[i], W, H, [&](int xx, int yy) {
+        for (int j = cell[(size_t)yy*W + xx]; j >= 0; j = next[j]) {
+          if (j >= i) continue;
+          const int sj = ((volatile int*)state)[j];
+          if (sj == 1) { any_acc = true; break; }
+          if (sj == 0) any_unknown = true;
         }
-      }
+        return any_acc;
+      });
       if (any_acc) state[i] = 2;
       else if (!any_unknown) state[i] = 1;
       else atomicAdd(&remaining, 1);
@@ -154,23 +179,19 @@ __global__ void __launch_bounds__(1024) td_resolve_kernel(int n, const int* fx, 
     *nextid = id;
   }
 }
-__global__ void td_clear_rejected_kernel(int n, const uint8_t* acc, double* out, int32_t* olab) {
+__global__ void td_clear_rejected_kernel(int n, const uint8_t* acc, double* pred, double* oflow, int32_t* olab) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x;
   if (i >= n || acc[i]) return;
-  out[4*i] = out[4*i+1] = out[4*i+2] = out[4*i+3] = 0.0; olab[i] = 0;
+  pred[2*i] = pred[2*i+1] = oflow[2*i] = oflow[2*i+1] = 0.0; olab[i] = 0;
 }
 __global__ void td_masks_kernel(int n, const int* fx, const int* fy, const uint8_t* acc, int W, int H, Disc disc, uint8_t* det, int* trk_idx) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x;
   if (i >= n || !acc[i]) return;
-  for (int dy = -disc.r; dy <= disc.r; dy++) {
-    const int yy = fy[i] + dy; if (yy < 0 || yy >= H) continue;
-    const int hw = disc.hw[dy < 0 ? -dy : dy];
-    for (int dx = -hw; dx <= hw; dx++) {
-      const int xx = fx[i] + dx; if (xx < 0 || xx >= W) continue;
-      det[(size_t)yy*W + xx] = 0;
-      atomicMax(&trk_idx[(size_t)yy*W + xx], i + 1);     // last writer (largest index) wins
-    }
-  }
+  disc_walk(disc, fx[i], fy[i], W, H, [&](int xx, int yy) {
+    det[(size_t)yy*W + xx] = 0;
+    atomicMax(&trk_idx[(size_t)yy*W + xx], i + 1);     // last writer (largest index) wins
+    return false;
+  });
 }
 __global__ void td_trk_final_kernel(size_t npx, const int* trk_idx, const int32_t* olab, uint8_t* trk) {
   const size_t p = (size_t)blockIdx.x*blockDim.x + threadIdx.x;
@@ -274,6 +295,11 @@ __host__ __device__ inline int anms_high(int K, int cols, int rows) {
   const double exp3 = sqrt((double)exp2), exp4 = K - 1;
   const double sol1 = -round((exp1 + exp3)/exp4), sol2 = -round((exp1 - exp3)/exp4);
   return (int)(sol1 > sol2 ? sol1 : sol2);
+}
+// the reference's u16 range tree wraps coordinate + width above 65535: true when a list with K >= 2 whose largest coordinate
+// is max_coord could reach that, so that the call is refused rather than answered differently
+static bool anms_u16_wraps(long long max_coord, int K, int cols, int rows) {
+  return max_coord + std::max(anms_high(K, cols, rows), 0) > 65535;
 }
 struct SelGrid { int x0, y0, s, nx, ny, w; };
 // Two metrics share the ordered resolver: the range tree's inclusive square |dx|, |dy| <= w, and goodFeaturesToTrack's
@@ -415,16 +441,16 @@ __global__ void sd_prepare_kernel(int nobj, const int* tot, const int* num_track
 }
 // one CTA per object: the selected candidate pixels become features, packed object after object in the given order
 __global__ void sd_construct_kernel(const int* __restrict__ off, const int* __restrict__ nsel, const int* __restrict__ sel, const int* __restrict__ idx,
-                                    const float* __restrict__ flow, int W, const int* __restrict__ objs, long long base_id, double* __restrict__ out /*[S][6]*/,
-                                    long long* __restrict__ otid, int32_t* __restrict__ olab) {
+                                    const float* __restrict__ flow, int W, const int* __restrict__ objs, long long base_id, double* __restrict__ okp,
+                                    double* __restrict__ oflow, double* __restrict__ opred, long long* __restrict__ otid, int32_t* __restrict__ olab) {
   const int o = blockIdx.x;
   int base = 0;
   for (int q = 0; q < o; q++) base += nsel[q];
   for (int r = threadIdx.x; r < nsel[o]; r += blockDim.x) {
     const int p = idx[off[o] + sel[off[o] + r]], x = p % W, y = p / W, d = base + r;
     const double fx = (double)flow[2*(size_t)p], fy = (double)flow[2*(size_t)p + 1];
-    out[6*(size_t)d] = x; out[6*(size_t)d + 1] = y; out[6*(size_t)d + 2] = fx; out[6*(size_t)d + 3] = fy;
-    out[6*(size_t)d + 4] = x + fx; out[6*(size_t)d + 5] = y + fy;     // Feature::CalculatePredictedKeypoint
+    okp[2*(size_t)d] = x; okp[2*(size_t)d + 1] = y; oflow[2*(size_t)d] = fx; oflow[2*(size_t)d + 1] = fy;
+    opred[2*(size_t)d] = x + fx; opred[2*(size_t)d + 1] = y + fy;     // Feature::CalculatePredictedKeypoint
     otid[d] = base_id + d; olab[d] = objs[o];
   }
 }
@@ -629,17 +655,23 @@ __global__ void count_status_kernel(int n, const uint8_t* st, int* count) {
 // successful constructions): in parallel, the passing feature with the smallest index per cell wins (atomicMin).  New
 // detections do the same among the cells the tracked features left free, in detection order, until the frame holds
 // max_features (a prefix count); tracklet ids are handed out in that order.
-__device__ __forceinline__ bool sf_construct(const float* flow, const int32_t* mask, int W, int H, int x, int y, double kx, double ky, double* out) {
+// feature i: flow and predicted key-point at oflow[2i] / pred[2i]
+__device__ __forceinline__ bool sf_construct(const float* flow, const int32_t* mask, int W, int H, int x, int y, double kx, double ky, int i,
+                                             double* oflow, double* pred) {
   if (mask[(size_t)y*W + x] != 0) return false;
   const double fx = (double)flow[2*((size_t)y*W + x)], fy = (double)flow[2*((size_t)y*W + x) + 1];
   if (!(fx != 0 && fy != 0)) return false;
   const double px = kx + fx, py = ky + fy;
   if (!(px >= 0.0 && px < (double)W && py >= 0.0 && py < (double)H)) return false;
-  out[0] = fx; out[1] = fy; out[2] = px; out[3] = py;
+  oflow[2*(size_t)i] = fx; oflow[2*(size_t)i + 1] = fy; pred[2*(size_t)i] = px; pred[2*(size_t)i + 1] = py;
   return true;
 }
+__device__ __forceinline__ void sf_clear(int i, double* oflow, double* pred) {
+  oflow[2*(size_t)i] = oflow[2*(size_t)i + 1] = pred[2*(size_t)i] = pred[2*(size_t)i + 1] = 0.0;
+}
 __global__ void sf_prev_kernel(int n, const double* __restrict__ kp, const uint8_t* __restrict__ usable, const float* flow, const int32_t* mask, int W, int H,
-                               int cell_size, int ncols, int* __restrict__ cell, uint8_t* __restrict__ pass, double* __restrict__ out, int* __restrict__ win) {
+                               int cell_size, int ncols, int* __restrict__ cell, uint8_t* __restrict__ pass, double* __restrict__ oflow,
+                               double* __restrict__ pred, int* __restrict__ win) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x;
   if (i >= n) return;
   const double kx = kp[2*i], ky = kp[2*i + 1];
@@ -649,20 +681,22 @@ __global__ void sf_prev_kernel(int n, const double* __restrict__ kp, const uint8
   const int c = (int)floor(ky/cell_size)*ncols + (int)floor(kx/cell_size);
   cell[i] = c;
   if (!usable[i]) return;
-  if (!sf_construct(flow, mask, W, H, x, y, kx, ky, out + 4*(size_t)i)) return;
+  if (!sf_construct(flow, mask, W, H, x, y, kx, ky, i, oflow, pred)) return;
   pass[i] = 1;
   atomicMin(win + c, i);
 }
-__global__ void sf_prev_resolve_kernel(int n, const int* cell, const uint8_t* pass, const int* win, const int32_t* age, uint8_t* acc, double* out, int32_t* oage, int* cnt) {
+__global__ void sf_prev_resolve_kernel(int n, const int* cell, const uint8_t* pass, const int* win, const int32_t* age, uint8_t* acc, double* oflow,
+                                       double* pred, int32_t* oage, int* cnt) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x;
   if (i >= n) return;
   const bool a = pass[i] && win[cell[i]] == i;
   acc[i] = a ? 1 : 0; oage[i] = a ? age[i] + 1 : 0;
-  if (!a) { out[4*(size_t)i] = out[4*(size_t)i + 1] = out[4*(size_t)i + 2] = out[4*(size_t)i + 3] = 0.0; }
+  if (!a) sf_clear(i, oflow, pred);
   else atomicAdd(cnt, 1);
 }
 __global__ void sf_det_kernel(int n, const int32_t* __restrict__ xy, const float* flow, const int32_t* mask, int W, int H, int cell_size, int ncols,
-                              const int* __restrict__ win_prev, int* __restrict__ cell, uint8_t* __restrict__ pass, double* __restrict__ out, int* __restrict__ win) {
+                              const int* __restrict__ win_prev, int* __restrict__ cell, uint8_t* __restrict__ pass, double* __restrict__ oflow,
+                              double* __restrict__ pred, int* __restrict__ win) {
   const int j = blockIdx.x*blockDim.x + threadIdx.x;
   if (j >= n) return;
   const int x = xy[2*j], y = xy[2*j + 1];
@@ -672,34 +706,39 @@ __global__ void sf_det_kernel(int n, const int32_t* __restrict__ xy, const float
   const int c = (int)floor((double)y/cell_size)*ncols + (int)floor((double)x/cell_size);
   cell[j] = c;
   if (win_prev[c] != 0x7fffffff) return;                       // cell taken by a tracked feature
-  if (!sf_construct(flow, mask, W, H, x, y, (double)x, (double)y, out + 4*(size_t)j)) return;
+  if (!sf_construct(flow, mask, W, H, x, y, (double)x, (double)y, j, oflow, pred)) return;
   pass[j] = 1;
   atomicMin(win + c, j);
 }
+// In-order compaction inside one CTA of 1024 threads that walks a list in 1024-wide chunks, every thread calling this once
+// per chunk: returns how many flags before this thread's are set, in this chunk and the earlier ones, and adds the chunk's
+// flags to the running count `base` (the same in every thread).
+__device__ __forceinline__ int cta_rank(int flag, int& base) {
+  __shared__ int s_scan[1024];
+  s_scan[threadIdx.x] = flag;
+  __syncthreads();
+  for (int o = 1; o < 1024; o <<= 1) { const int v = threadIdx.x >= o ? s_scan[threadIdx.x - o] : 0; __syncthreads(); s_scan[threadIdx.x] += v; __syncthreads(); }
+  const int rank = base + s_scan[threadIdx.x] - flag;
+  base += s_scan[1023];
+  __syncthreads();
+  return rank;
+}
 // one CTA: in-order prefix count of the accepted detections, truncated at `room`; tracklet ids follow the order
 __global__ void __launch_bounds__(1024) sf_det_resolve_kernel(int n, const int* cell, const uint8_t* pass, const int* win, const int* cnt_prev, int max_features,
-                                                              long long base_id, uint8_t* acc, double* out, long long* otid, int* cnt_det) {
-  __shared__ int s_scan[1024]; __shared__ int s_base;
+                                                              long long base_id, uint8_t* acc, double* oflow, double* pred, long long* otid, int* cnt_det) {
   const int room = max(0, max_features - *cnt_prev);
-  if (threadIdx.x == 0) s_base = 0;
-  __syncthreads();
+  int base = 0;
   for (int j0 = 0; j0 < n; j0 += 1024) {
     const int j = j0 + threadIdx.x;
     const int a = (j < n && pass[j] && win[cell[j]] == j) ? 1 : 0;
-    s_scan[threadIdx.x] = a;
-    __syncthreads();
-    for (int o = 1; o < 1024; o <<= 1) { const int v = threadIdx.x >= o ? s_scan[threadIdx.x - o] : 0; __syncthreads(); s_scan[threadIdx.x] += v; __syncthreads(); }
-    const int rank = s_base + s_scan[threadIdx.x] - a;           // accepted detections before j
+    const int rank = cta_rank(a, base);                          // accepted detections before j
     if (j < n) {
       const bool fin = a && rank < room;
       acc[j] = fin ? 1 : 0; otid[j] = fin ? base_id + rank : 0;
-      if (!fin) { out[4*(size_t)j] = out[4*(size_t)j + 1] = out[4*(size_t)j + 2] = out[4*(size_t)j + 3] = 0.0; }
+      if (!fin) sf_clear(j, oflow, pred);
     }
-    __syncthreads();
-    if (threadIdx.x == 1023) s_base += s_scan[1023];
-    __syncthreads();
   }
-  if (threadIdx.x == 0) *cnt_det = min(s_base, room);
+  if (threadIdx.x == 0) *cnt_det = min(base, room);
 }
 
 // ---------------------------------------------------------------------------------------------------- KltFeatureTracker::detectFeatures
@@ -728,11 +767,7 @@ __global__ void dt_circles_kernel(int n, const double* __restrict__ kp, Disc dis
   const int i = blockIdx.x*blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int cx = __float2int_rn((float)kp[2*i]), cy = __float2int_rn((float)kp[2*i + 1]);
-  for (int dy = -disc.r; dy <= disc.r; dy++) {
-    const int yy = cy + dy; if (yy < 0 || yy >= H) continue;
-    const int hw = disc.hw[dy < 0 ? -dy : dy];
-    for (int dx = -hw; dx <= hw; dx++) { const int xx = cx + dx; if (xx >= 0 && xx < W) out[(size_t)yy*W + xx] = 0; }
-  }
+  disc_walk(disc, cx, cy, W, H, [&](int xx, int yy) { out[(size_t)yy*W + xx] = 0; return false; });
 }
 // CLAHE(2.0, 8x8), one CTA per tile: histogram, clip, redistribution, LUT (clahe.cpp CLAHE_CalcLut_Body)
 __global__ void __launch_bounds__(256) clahe_lut_kernel(const uint8_t* __restrict__ img, int W, int H, int tw, int th, int clip, float lut_scale,
@@ -972,10 +1007,8 @@ __global__ void dt_subpix_kernel(int m, const int* __restrict__ corners, const i
 __global__ void __launch_bounds__(1024) dt_construct_kernel(const float* __restrict__ pts, const int* __restrict__ cnt, const int32_t* __restrict__ mask,
                                                             int W, int H, dynofront_track_params prm, long long base_id, double* __restrict__ kp,
                                                             long long* __restrict__ tid, int* __restrict__ n_out) {
-  __shared__ int s_scan[1024]; __shared__ int s_base;
   const int n = *cnt;
-  if (threadIdx.x == 0) s_base = 0;
-  __syncthreads();
+  int base = 0;
   for (int j0 = 0; j0 < n; j0 += 1024) {
     const int j = j0 + threadIdx.x;
     double kx = 0, ky = 0; int a = 0;
@@ -984,16 +1017,10 @@ __global__ void __launch_bounds__(1024) dt_construct_kernel(const float* __restr
       const bool contained = kx >= 0.0 && kx < (double)W && ky >= 0.0 && ky < (double)H;
       a = (contained && within_shrunken(kx, ky, H, W, prm.shrink_row, prm.shrink_col) && mask[(size_t)((int)ky)*W + (int)kx] == 0) ? 1 : 0;
     }
-    s_scan[threadIdx.x] = a;
-    __syncthreads();
-    for (int o = 1; o < 1024; o <<= 1) { const int v = threadIdx.x >= o ? s_scan[threadIdx.x - o] : 0; __syncthreads(); s_scan[threadIdx.x] += v; __syncthreads(); }
-    const int rank = s_base + s_scan[threadIdx.x] - a;
+    const int rank = cta_rank(a, base);
     if (a) { kp[2*(size_t)rank] = kx; kp[2*(size_t)rank + 1] = ky; tid[rank] = base_id + rank; }
-    __syncthreads();
-    if (threadIdx.x == 1023) s_base += s_scan[1023];
-    __syncthreads();
   }
-  if (threadIdx.x == 0) *n_out = s_base;
+  if (threadIdx.x == 0) *n_out = base;
 }
 // the points cornerSubPix would refine when it is off: the integer corners as floats, in selection order
 __global__ void dt_points_kernel(int m, const int* __restrict__ corners, const int* __restrict__ sel, const int* __restrict__ cnt, float* __restrict__ pts) {
@@ -1019,23 +1046,18 @@ int dynofront_create(int device, int width, int height, dynofront_handle* out) {
   if (cudaStreamCreateWithFlags(&h->s, cudaStreamNonBlocking) != cudaSuccess) { delete h; return -3; }
   cudaEventCreate(&h->e0); cudaEventCreate(&h->e1);
   const size_t npx = (size_t)width*height;
-  int rc = 0;
-  rc |= falloc(h, &h->flow, 2*npx); rc |= falloc(h, &h->mask, npx); rc |= falloc(h, &h->det, npx); rc |= falloc(h, &h->det_work, npx);
-  rc |= falloc(h, &h->trk, npx); rc |= falloc(h, &h->trk_idx, npx); rc |= falloc(h, &h->cell, npx); rc |= falloc(h, &h->nextid, 1);
-  rc |= falloc(h, &h->tile_cnt, ((npx + ST_TILE - 1)/ST_TILE)*ST_MAXOBJ); rc |= falloc(h, &h->obj_tot, ST_MAXOBJ);
-  rc |= falloc(h, &h->d_objs, ST_MAXOBJ); rc |= falloc(h, &h->d_zero, ST_MAXOBJ);
-  rc |= falloc(h, &h->pmask, npx); rc |= falloc(h, &h->pflow, 2*npx); rc |= falloc(h, &h->cmask, npx); rc |= falloc(h, &h->pflag, 1);
-  if (rc) { dynofront_destroy(h); return -3; }
+  if (grow(h, h->flow, 2*npx, h->mask, npx, h->det, npx, h->det_work, npx, h->trk, npx, h->trk_idx, npx, h->cell, npx, h->nextid, 1,
+           h->tile_cnt, ((npx + ST_TILE - 1)/ST_TILE)*ST_MAXOBJ, h->obj_tot, ST_MAXOBJ, h->d_objs, ST_MAXOBJ, h->d_zero, ST_MAXOBJ,
+           h->pmask, npx, h->pflow, 2*npx, h->cmask, npx, h->pflag, 1)) { dynofront_destroy(h); return -3; }
   *out = h;
   return 0;
 }
 int dynofront_destroy(dynofront_handle h) {
   if (!h) return -1;
   cudaSetDevice(h->dev);
-  for (void* p : h->allocs) cudaFree(p);
   if (h->e0) cudaEventDestroy(h->e0); if (h->e1) cudaEventDestroy(h->e1);
   if (h->s) cudaStreamDestroy(h->s);
-  delete h; return 0;
+  delete h; return 0;                                           // (the buffers free their device memory)
 }
 int dynofront_set_frame(dynofront_handle h, const float* flow, const int32_t* motion_mask, const uint8_t* detection_mask) {
   if (!h) return -1; cudaSetDevice(h->dev);
@@ -1067,17 +1089,6 @@ int dynofront_next_frame(dynofront_handle h, const uint8_t* gray, const float* f
   if (build_pyramid(h, 1, gray, 5, 21, true)) return -3;       // (levels that are too small for a window are simply never read)
   return 0;                                                     // no synchronisation: the next call's work is ordered behind on the stream
 }
-static int ensure_features(dynofront_ctx* h, int n) {
-  if (n <= h->cap) return 0;
-  const int cap = std::max(n, 4096);
-  int rc = 0;
-  rc |= falloc(h, &h->f_kp, 2*(size_t)cap); rc |= falloc(h, &h->f_lab, cap); rc |= falloc(h, &h->f_age, cap); rc |= falloc(h, &h->f_tid, cap);
-  rc |= falloc(h, &h->f_x, cap); rc |= falloc(h, &h->f_y, cap); rc |= falloc(h, &h->f_state, cap); rc |= falloc(h, &h->f_next, cap);
-  rc |= falloc(h, &h->f_out, 4*(size_t)cap); rc |= falloc(h, &h->f_oage, cap); rc |= falloc(h, &h->f_otid, cap); rc |= falloc(h, &h->f_olab, cap);
-  rc |= falloc(h, &h->f_acc, cap);
-  if (rc) return -3;
-  h->cap = cap; return 0;
-}
 static void prepare_det_work(dynofront_ctx* h) {
   const size_t npx = (size_t)h->W*h->H;
   if (h->has_det) cudaMemcpyAsync(h->det_work, h->det, npx, cudaMemcpyDeviceToDevice, h->s);
@@ -1091,7 +1102,9 @@ int dynofront_track_dynamic(dynofront_handle h, int32_t n, const double* kp, con
   if (!h || !prm || n < 0 || !next_tracklet_id) return -1;
   if (prm->min_distance < 0 || prm->min_distance > 15) { h->err = "min_distance must be in [0,15]"; return -1; }
   cudaSetDevice(h->dev);
-  if (ensure_features(h, n)) return -3;
+  const size_t cap = feature_cap(n);
+  if (grow(h, h->f_kp, 2*cap, h->f_lab, cap, h->f_age, cap, h->f_tid, cap, h->f_x, cap, h->f_y, cap, h->f_state, cap, h->f_next, cap,
+           h->f_pred, 2*cap, h->f_flow, 2*cap, h->f_oage, cap, h->f_otid, cap, h->f_olab, cap, h->f_acc, cap)) return -3;
   const size_t npx = (size_t)h->W*h->H; const int W = h->W, H = h->H;
   const Disc disc = make_disc(prm->min_distance);
   FCK(cudaMemcpyAsync(h->f_kp, kp, 2*(size_t)n*8, cudaMemcpyHostToDevice, h->s));
@@ -1105,18 +1118,18 @@ int dynofront_track_dynamic(dynofront_handle h, int32_t n, const double* kp, con
   fill_i32_kernel<<<(unsigned)((npx + 255)/256), 256, 0, h->s>>>(h->trk_idx, npx, 0);
   if (n > 0) {
     const int g = (n + 127)/128;
-    td_candidate_kernel<<<g, 128, 0, h->s>>>(n, h->f_kp, h->f_lab, h->f_age, h->flow, h->mask, h->has_det ? h->det : nullptr, W, H, *prm,
-                                             h->f_x, h->f_y, h->f_state, h->f_out, h->f_oage, h->f_olab);
+    td_candidate_kernel<<<g, 128, 0, h->s>>>(n, h->f_kp, h->f_lab, h->f_age, h->flow, h->mask, h->has_det ? h->det.p : nullptr, W, H, *prm,
+                                             h->f_x, h->f_y, h->f_state, h->f_pred, h->f_flow, h->f_oage, h->f_olab);
     td_link_kernel<<<g, 128, 0, h->s>>>(n, h->f_x, h->f_y, h->f_state, W, h->cell, h->f_next);
     td_resolve_kernel<<<1, 1024, 0, h->s>>>(n, h->f_x, h->f_y, h->f_state, h->cell, h->f_next, W, H, disc, prm->max_dynamic_feature_age,
-                                            (const int64_t*)h->f_tid, h->f_oage, h->f_otid, h->f_acc, h->nextid);
-    td_clear_rejected_kernel<<<g, 128, 0, h->s>>>(n, h->f_acc, h->f_out, h->f_olab);
+                                            h->f_tid, h->f_oage, h->f_otid, h->f_acc, h->nextid);
+    td_clear_rejected_kernel<<<g, 128, 0, h->s>>>(n, h->f_acc, h->f_pred, h->f_flow, h->f_olab);
     td_masks_kernel<<<g, 128, 0, h->s>>>(n, h->f_x, h->f_y, h->f_acc, W, H, disc, h->det_work, h->trk_idx);
   }
   td_trk_final_kernel<<<(unsigned)((npx + 255)/256), 256, 0, h->s>>>(npx, h->trk_idx, h->f_olab, h->trk);
-  std::vector<double> out4((size_t)4*n);
   if (n) {
-    FCK(cudaMemcpyAsync(out4.data(), h->f_out, out4.size()*8, cudaMemcpyDeviceToHost, h->s));
+    if (pred_kp) FCK(cudaMemcpyAsync(pred_kp, h->f_pred, 2*(size_t)n*8, cudaMemcpyDeviceToHost, h->s));
+    if (flow_out) FCK(cudaMemcpyAsync(flow_out, h->f_flow, 2*(size_t)n*8, cudaMemcpyDeviceToHost, h->s));
     if (accepted) FCK(cudaMemcpyAsync(accepted, h->f_acc, n, cudaMemcpyDeviceToHost, h->s));
     if (oage) FCK(cudaMemcpyAsync(oage, h->f_oage, (size_t)n*4, cudaMemcpyDeviceToHost, h->s));
     if (otid) FCK(cudaMemcpyAsync(otid, h->f_otid, (size_t)n*8, cudaMemcpyDeviceToHost, h->s));
@@ -1128,10 +1141,6 @@ int dynofront_track_dynamic(dynofront_handle h, int32_t n, const double* kp, con
   FCK(cudaStreamSynchronize(h->s));
   FCK(cudaGetLastError());
   *next_tracklet_id = nid;
-  for (int i = 0; i < n; i++) {
-    if (pred_kp) { pred_kp[2*i] = out4[4*i]; pred_kp[2*i+1] = out4[4*i+1]; }
-    if (flow_out) { flow_out[2*i] = out4[4*i+2]; flow_out[2*i+1] = out4[4*i+3]; }
-  }
   return 0;
 }
 
@@ -1141,7 +1150,7 @@ int dynofront_sample_candidates(dynofront_handle h, int32_t nobj, const int32_t*
   cudaSetDevice(h->dev);
   const size_t npx = (size_t)h->W*h->H; const int ntiles = (int)((npx + ST_TILE - 1)/ST_TILE);
   if (!h->det_work_valid) prepare_det_work(h);
-  if ((size_t)capacity > h->idx_cap) { if (falloc(h, &h->d_idx, (size_t)capacity)) return -3; h->idx_cap = (size_t)capacity; }
+  if (grow(h, h->d_idx, (size_t)capacity)) return -3;
   FCK(cudaMemcpyAsync(h->d_objs, objects, (size_t)nobj*4, cudaMemcpyHostToDevice, h->s));
   FCK(cudaMemsetAsync(h->d_zero, 0, ST_MAXOBJ*4, h->s));
   sc_count_kernel<<<ntiles, ST_TILE, 0, h->s>>>(npx, h->W, h->H, h->det_work, h->mask, h->flow, h->d_objs, nobj, *prm, h->tile_cnt, h->d_zero);
@@ -1164,24 +1173,12 @@ int dynofront_sample_candidates(dynofront_handle h, int32_t nobj, const int32_t*
   return 0;
 }
 
-static int ensure_selection(dynofront_ctx* h, size_t points, int lists) {
-  if (points > (size_t)h->sel_cap) {
-    const size_t cap = std::max<size_t>(points, (size_t)h->W*h->H);
-    if (cap > 0x7fffffff) { h->err = "too many key-points"; return -1; }
-    int rc = 0;
-    rc |= falloc(h, &h->sel_xy, 2*cap); rc |= falloc(h, &h->sel_px, cap); rc |= falloc(h, &h->sel_py, cap); rc |= falloc(h, &h->sel_orig, cap);
-    rc |= falloc(h, &h->sel_next, cap); rc |= falloc(h, &h->sel_out, cap);
-    if (rc) return -3;
-    h->sel_cap = (int)cap;
-  }
-  if (lists > h->sel_lists) {
-    const int cap = std::max(lists, ST_MAXOBJ);
-    int rc = 0;
-    rc |= falloc(h, &h->sel_off, cap); rc |= falloc(h, &h->sel_cnt, cap); rc |= falloc(h, &h->sel_k, cap); rc |= falloc(h, &h->sel_n, cap); rc |= falloc(h, &h->sel_tol, cap);
-    if (rc) return -3;
-    h->sel_lists = cap;
-  }
-  return 0;
+// the work arrays of the ordered resolver (anms_range_tree_kernel, dt_gftt_select_kernel) hold at least a frame of points,
+// indexed by int
+static int grow_resolver(dynofront_ctx* h, size_t points) {
+  const size_t cap = std::max(points, (size_t)h->W*h->H);
+  if (cap > 0x7fffffff) { h->err = "too many key-points"; return -3; }
+  return grow(h, h->sel_px, cap, h->sel_py, cap, h->sel_orig, cap, h->sel_next, cap, h->sel_out, cap);
 }
 
 int dynofront_anms_range_tree(dynofront_handle h, int32_t n_lists, const int32_t* offsets, const int32_t* xy, const int32_t* k_needed,
@@ -1199,13 +1196,15 @@ int dynofront_anms_range_tree(dynofront_handle h, int32_t n_lists, const int32_t
   const size_t total = (size_t)offsets[n_lists];
   if (total && (!xy || !selected)) return -1;
   for (size_t i = 0; i < 2*total; i++) if (xy[i] < 0 || xy[i] > 65535) { h->err = "key-point coordinates must be in [0, 65535]"; return -1; }
-  for (int l = 0; l < n_lists; l++) {        // the reference's u16 range tree wraps x + width above 65535: reject instead of diverging
+  for (int l = 0; l < n_lists; l++) {
     if (cnt[l] == 0 || k_needed[l] < 2) continue;
     int cmax = 0;
     for (int i = 2*offsets[l]; i < 2*offsets[l + 1]; i++) cmax = std::max(cmax, (int)xy[i]);
-    if ((long long)cmax + std::max(anms_high(k_needed[l], cols, rows), 0) > 65535) { h->err = "key-point coordinate + search width exceeds 65535 (u16 range tree)"; return -1; }
+    if (anms_u16_wraps(cmax, k_needed[l], cols, rows)) { h->err = "key-point coordinate + search width exceeds 65535 (u16 range tree)"; return -1; }
   }
-  if (ensure_selection(h, total, n_lists)) return -3;
+  const size_t lists = std::max(n_lists, ST_MAXOBJ);
+  if (grow_resolver(h, total) || grow(h, h->sel_xy, 2*std::max(total, (size_t)h->W*h->H), h->sel_off, lists, h->sel_cnt, lists, h->sel_k, lists,
+                                      h->sel_n, lists, h->sel_tol, lists)) return -3;
   FCK(cudaEventRecord(h->e0, h->s));
   FCK(cudaMemcpyAsync(h->sel_off, offsets, (size_t)n_lists*4, cudaMemcpyHostToDevice, h->s));
   FCK(cudaMemcpyAsync(h->sel_cnt, cnt.data(), (size_t)n_lists*4, cudaMemcpyHostToDevice, h->s));
@@ -1230,58 +1229,50 @@ int dynofront_sample_dynamic(dynofront_handle h, int32_t nobj, const int32_t* ob
   if (!h || !prm || nobj < 0 || nobj > ST_MAXOBJ || capacity < 0 || !next_tracklet_id || !num_sampled || !n_features) return -1;
   if (nobj && (!objects || !num_track)) return -1;
   if (capacity && (!keypoint || !flow_out || !predicted || !tracklet)) { h->err = "null feature array"; return -1; }
-  {                                          // no width of the search may wrap the reference's u16 coordinates (see dynofront_anms_range_tree)
-    int hmax = 0;
-    for (int k = 2; k <= max_features; k++) hmax = std::max(hmax, anms_high(k, h->W, h->H));
-    if ((long long)std::max(h->W, h->H) - 1 + hmax > 65535) { h->err = "image too large for the u16 range tree of the reference"; return -1; }
-  }
+  const long long cmax = std::max(h->W, h->H) - 1;       // no width of the search, for any K the objects can need, may wrap
+  bool wraps = cmax > 65535;
+  for (int k = 2; k <= max_features && !wraps; k++) wraps = anms_u16_wraps(cmax, k, h->W, h->H);
+  if (wraps) { h->err = "image too large for the u16 range tree of the reference"; return -1; }
   cudaSetDevice(h->dev);
   const size_t npx = (size_t)h->W*h->H; const int ntiles = (int)((npx + ST_TILE - 1)/ST_TILE);
-  if (ensure_selection(h, npx, ST_MAXOBJ)) return -3;
-  if (!h->sd_idx) {
-    int rc = 0;
-    rc |= falloc(h, &h->sd_idx, npx); rc |= falloc(h, &h->sd_off, ST_MAXOBJ); rc |= falloc(h, &h->sd_k, ST_MAXOBJ); rc |= falloc(h, &h->sd_ntrack, ST_MAXOBJ);
-    if (rc) return -3;
-  }
+  if (grow_resolver(h, npx) || grow(h, h->sel_off, ST_MAXOBJ, h->sel_k, ST_MAXOBJ, h->sd_idx, npx, h->sd_ntrack, ST_MAXOBJ, h->sd_counts, 3*ST_MAXOBJ)) return -3;
   FCK(cudaEventRecord(h->e0, h->s));
   if (!h->det_work_valid) prepare_det_work(h);
   *n_features = 0;
-  std::vector<int> tot(std::max(nobj, 1)), zc(std::max(nobj, 1)), ns(std::max(nobj, 1));
+  int oc[3][ST_MAXOBJ] = {};                              // per object: candidates, zero-flow pixels, selected (sd_counts)
+  int* const d_tot = h->sd_counts; int* const d_zero = d_tot + ST_MAXOBJ; int* const d_nsel = d_tot + 2*ST_MAXOBJ;
   if (nobj > 0) {
     FCK(cudaMemcpyAsync(h->d_objs, objects, (size_t)nobj*4, cudaMemcpyHostToDevice, h->s));
     FCK(cudaMemcpyAsync(h->sd_ntrack, num_track, (size_t)nobj*4, cudaMemcpyHostToDevice, h->s));
-    FCK(cudaMemsetAsync(h->d_zero, 0, ST_MAXOBJ*4, h->s));
+    FCK(cudaMemsetAsync(d_zero, 0, ST_MAXOBJ*4, h->s));
     // (1) the candidate scan of dynofront_sample_candidates, its compaction kept on the device
-    sc_count_kernel<<<ntiles, ST_TILE, 0, h->s>>>(npx, h->W, h->H, h->det_work, h->mask, h->flow, h->d_objs, nobj, *prm, h->tile_cnt, h->d_zero);
-    sc_scan_kernel<<<1, ST_MAXOBJ, 0, h->s>>>(ntiles, nobj, h->tile_cnt, h->obj_tot);
-    sd_prepare_kernel<<<1, 32, 0, h->s>>>(nobj, h->obj_tot, h->sd_ntrack, max_features, h->sd_off, h->sd_k);
-    sc_scatter_kernel<<<ntiles, ST_TILE, 0, h->s>>>(npx, h->W, h->H, h->det_work, h->mask, h->flow, h->d_objs, nobj, *prm, h->tile_cnt, h->sd_off,
+    sc_count_kernel<<<ntiles, ST_TILE, 0, h->s>>>(npx, h->W, h->H, h->det_work, h->mask, h->flow, h->d_objs, nobj, *prm, h->tile_cnt, d_zero);
+    sc_scan_kernel<<<1, ST_MAXOBJ, 0, h->s>>>(ntiles, nobj, h->tile_cnt, d_tot);
+    sd_prepare_kernel<<<1, 32, 0, h->s>>>(nobj, d_tot, h->sd_ntrack, max_features, h->sel_off, h->sel_k);
+    sc_scatter_kernel<<<ntiles, ST_TILE, 0, h->s>>>(npx, h->W, h->H, h->det_work, h->mask, h->flow, h->d_objs, nobj, *prm, h->tile_cnt, h->sel_off,
                                                     h->sd_idx, (long long)npx);
     // (2) + (3) P_n and the range-tree ANMS per object, K = max(max_features - num_track, 0), tolerance 0.01 (FeatureTracker.cc:955-980)
-    anms_range_tree_kernel<<<nobj, SEL_THREADS, 0, h->s>>>(h->sd_off, h->obj_tot, h->sd_k, nullptr, 0.01f, h->sd_idx, nullptr, h->W, h->W, h->H,
-                                                           h->sel_px, h->sel_py, h->sel_orig, h->sel_next, h->sel_out, h->sel_n);
+    anms_range_tree_kernel<<<nobj, SEL_THREADS, 0, h->s>>>(h->sel_off, d_tot, h->sel_k, nullptr, 0.01f, h->sd_idx, nullptr, h->W, h->W, h->H,
+                                                           h->sel_px, h->sel_py, h->sel_orig, h->sel_next, h->sel_out, d_nsel);
     FCK(cudaGetLastError());
-    FCK(cudaMemcpyAsync(tot.data(), h->obj_tot, (size_t)nobj*4, cudaMemcpyDeviceToHost, h->s));
-    FCK(cudaMemcpyAsync(zc.data(), h->d_zero, (size_t)nobj*4, cudaMemcpyDeviceToHost, h->s));
-    FCK(cudaMemcpyAsync(ns.data(), h->sel_n, (size_t)nobj*4, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(oc, h->sd_counts, sizeof(oc), cudaMemcpyDeviceToHost, h->s));
     FCK(cudaStreamSynchronize(h->s));
   }
   int S = 0;
-  for (int o = 0; o < nobj; o++) { if (counts) counts[o] = tot[o]; if (zero_flow) zero_flow[o] = zc[o]; num_sampled[o] = ns[o]; S += ns[o]; }
-  if (S > h->sd_cap) {
-    const int cap = std::max(S, 4096);
-    if (falloc(h, &h->sd_out, 6*(size_t)cap) || falloc(h, &h->sd_tid, cap) || falloc(h, &h->sd_lab, cap)) return -3;
-    h->sd_cap = cap;
-  }
+  for (int o = 0; o < nobj; o++) { if (counts) counts[o] = oc[0][o]; if (zero_flow) zero_flow[o] = oc[1][o]; num_sampled[o] = oc[2][o]; S += oc[2][o]; }
+  const size_t cap = feature_cap(S);
+  if (grow(h, h->sd_kp, 2*cap, h->sd_flow, 2*cap, h->sd_pred, 2*cap, h->sd_tid, cap, h->sd_lab, cap)) return -3;
   const long long base_id = *next_tracklet_id;
   const int ncopy = std::min(S, capacity);
-  std::vector<double> out6(6*(size_t)ncopy);
   if (S > 0) {
     // (4) the features, tracklet ids in object order then ANMS order
-    sd_construct_kernel<<<nobj, 128, 0, h->s>>>(h->sd_off, h->sel_n, h->sel_out, h->sd_idx, h->flow, h->W, h->d_objs, base_id, h->sd_out, h->sd_tid, h->sd_lab);
+    sd_construct_kernel<<<nobj, 128, 0, h->s>>>(h->sel_off, d_nsel, h->sel_out, h->sd_idx, h->flow, h->W, h->d_objs, base_id, h->sd_kp, h->sd_flow,
+                                                h->sd_pred, h->sd_tid, h->sd_lab);
     FCK(cudaGetLastError());
     if (ncopy) {
-      FCK(cudaMemcpyAsync(out6.data(), h->sd_out, out6.size()*8, cudaMemcpyDeviceToHost, h->s));
+      FCK(cudaMemcpyAsync(keypoint, h->sd_kp, 2*(size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
+      FCK(cudaMemcpyAsync(flow_out, h->sd_flow, 2*(size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
+      FCK(cudaMemcpyAsync(predicted, h->sd_pred, 2*(size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
       FCK(cudaMemcpyAsync(tracklet, h->sd_tid, (size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
       if (label) FCK(cudaMemcpyAsync(label, h->sd_lab, (size_t)ncopy*4, cudaMemcpyDeviceToHost, h->s));
     }
@@ -1289,11 +1280,6 @@ int dynofront_sample_dynamic(dynofront_handle h, int32_t nobj, const int32_t* ob
   FCK(cudaEventRecord(h->e1, h->s));
   FCK(cudaStreamSynchronize(h->s));
   FCK(cudaGetLastError());
-  for (int d = 0; d < ncopy; d++) {
-    keypoint[2*d] = out6[6*(size_t)d]; keypoint[2*d + 1] = out6[6*(size_t)d + 1];
-    flow_out[2*d] = out6[6*(size_t)d + 2]; flow_out[2*d + 1] = out6[6*(size_t)d + 3];
-    predicted[2*d] = out6[6*(size_t)d + 4]; predicted[2*d + 1] = out6[6*(size_t)d + 5];
-  }
   *next_tracklet_id = base_id + S;
   *n_features = S;
   if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
@@ -1313,29 +1299,23 @@ int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_c
   const int W = h->W, H = h->H; const size_t npx = (size_t)W*H;
   if (W < SP_P + 2 || H < SP_P + 2) { h->err = "image smaller than the cornerSubPix window"; return -1; }
   const int K = std::max(prm->max_features - n_cur, 0);
-  if (prm->use_anms && K >= 2 && (long long)std::max(W, H) - 1 + std::max(anms_high(K, W, H), 0) > 65535) { h->err = "image too large for the u16 range tree of the reference"; return -1; }
+  if (prm->use_anms && K >= 2 && anms_u16_wraps(std::max(W, H) - 1, K, W, H)) { h->err = "image too large for the u16 range tree of the reference"; return -1; }
   if (!gray && !h->have_pyr_cur) { h->err = "no current frame on the device"; return -2; }
   cudaSetDevice(h->dev);
-  if (!h->dt_int) {
-    int keycap = DT_SORT_TILE; while ((size_t)keycap < npx) keycap <<= 1;
-    int rc = 0;
-    rc |= falloc(h, &h->dt_gray, npx); rc |= falloc(h, &h->dt_mask, npx); rc |= falloc(h, &h->dt_clahe, npx); rc |= falloc(h, &h->dt_lut, DT_TILES*DT_TILES*256);
-    rc |= falloc(h, &h->dt_dx, npx); rc |= falloc(h, &h->dt_dy, npx); rc |= falloc(h, &h->dt_box, 3*npx); rc |= falloc(h, &h->dt_eig, npx); rc |= falloc(h, &h->dt_keys, keycap);
-    rc |= falloc(h, &h->dt_corners, 2*npx); rc |= falloc(h, &h->dt_int, 8); rc |= falloc(h, &h->dt_pts, 2*npx); rc |= falloc(h, &h->dt_resp, 1);
-    rc |= falloc(h, &h->dt_kp, 2*npx); rc |= falloc(h, &h->dt_tid, npx);
-    if (rc) return -3;
-    h->dt_keycap = keycap;
-  }
-  if (ensure_selection(h, npx, 1) || ensure_features(h, n_cur)) return -3;
+  size_t keycap = DT_SORT_TILE; while (keycap < npx) keycap <<= 1;
+  if (grow(h, h->dt_gray, npx, h->dt_mask, npx, h->dt_clahe, npx, h->dt_lut, DT_TILES*DT_TILES*256, h->dt_dx, npx, h->dt_dy, npx, h->dt_box, 3*npx,
+           h->dt_eig, npx, h->dt_keys, keycap, h->dt_corners, 2*npx, h->dt_cnt, 1, h->dt_pts, 2*npx, h->dt_resp, 1, h->dt_kp, 2*npx, h->dt_tid, npx,
+           h->f_kp, 2*feature_cap(n_cur)) || grow_resolver(h, npx)) return -3;
   FCK(cudaEventRecord(h->e0, h->s));
   const uint8_t* img = gray ? h->dt_gray : h->pyr[1][0];
   if (gray) FCK(cudaMemcpyAsync(h->dt_gray, gray, npx, cudaMemcpyHostToDevice, h->s));
   if (n_cur) FCK(cudaMemcpyAsync(h->f_kp, cur_kp, 2*(size_t)n_cur*8, cudaMemcpyHostToDevice, h->s));
-  int init[8] = {0, 0, 0, K, 0, 0, 0, 0};
-  FCK(cudaMemcpyAsync(h->dt_int, init, sizeof(init), cudaMemcpyHostToDevice, h->s));
+  DetectCounters init = {}; init.K = K;
+  FCK(cudaMemcpyAsync(h->dt_cnt, &init, sizeof(init), cudaMemcpyHostToDevice, h->s));
+  DetectCounters* const c = h->dt_cnt;                          // (device addresses of the counters)
   const unsigned g1 = (unsigned)((npx + 255)/256); const dim3 blk(32, 8), grd((W + 31)/32, (H + 7)/8);
   // (1) detection mask: boundary mask AND background, circles around the current features
-  dt_mask_kernel<<<g1, 256, 0, h->s>>>(npx, h->has_det ? h->det : nullptr, h->mask, h->dt_mask);
+  dt_mask_kernel<<<g1, 256, 0, h->s>>>(npx, h->has_det ? h->det.p : nullptr, h->mask, h->dt_mask);
   if (n_cur) dt_circles_kernel<<<(n_cur + 127)/128, 128, 0, h->s>>>(n_cur, h->f_kp, make_disc(prm->min_distance), W, H, h->dt_mask);
   // (2) CLAHE(2.0, 8x8) on the plain mono image
   if (prm->use_clahe) {
@@ -1348,23 +1328,23 @@ int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_c
   // (3) cornerMinEigenVal(3, 3), its maximum under the mask, the candidates, their order, the minDistance / maxCorners filter
   dt_sobel_kernel<<<grd, blk, 0, h->s>>>(h->dt_clahe, W, H, h->dt_dx, h->dt_dy);
   dt_box_kernel<<<(3*W + 31)/32, 32, 0, h->s>>>(h->dt_dx, h->dt_dy, W, H, h->dt_box);
-  dt_eig_kernel<<<g1, 256, 0, h->s>>>(h->dt_box, npx, h->dt_mask, h->dt_eig, (unsigned*)(h->dt_int + 7));
-  dt_cand_kernel<<<grd, blk, 0, h->s>>>(h->dt_eig, W, H, h->dt_mask, (const unsigned*)(h->dt_int + 7), prm->quality_level, h->dt_keys, h->dt_int);
-  const int cap = h->dt_keycap, nb = cap/DT_SORT_TILE;
-  dt_sort_pad_kernel<<<(cap + 255)/256, 256, 0, h->s>>>(h->dt_keys, h->dt_int, cap);
-  dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(h->dt_keys, h->dt_int, 2, DT_SORT_TILE);
+  dt_eig_kernel<<<g1, 256, 0, h->s>>>(h->dt_box, npx, h->dt_mask, h->dt_eig, &c->max_eig);
+  dt_cand_kernel<<<grd, blk, 0, h->s>>>(h->dt_eig, W, H, h->dt_mask, &c->max_eig, prm->quality_level, h->dt_keys, &c->candidates);
+  const int cap = (int)keycap, nb = cap/DT_SORT_TILE;
+  dt_sort_pad_kernel<<<(cap + 255)/256, 256, 0, h->s>>>(h->dt_keys, &c->candidates, cap);
+  dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(h->dt_keys, &c->candidates, 2, DT_SORT_TILE);
   for (int k = 2*DT_SORT_TILE; k <= cap; k <<= 1) {
-    for (int j = k/2; j >= DT_SORT_TILE; j >>= 1) dt_sort_global_kernel<<<(cap/2 + 255)/256, 256, 0, h->s>>>(h->dt_keys, h->dt_int, k, j);
-    dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(h->dt_keys, h->dt_int, k, k);
+    for (int j = k/2; j >= DT_SORT_TILE; j >>= 1) dt_sort_global_kernel<<<(cap/2 + 255)/256, 256, 0, h->s>>>(h->dt_keys, &c->candidates, k, j);
+    dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(h->dt_keys, &c->candidates, k, k);
   }
-  dt_gftt_select_kernel<<<1, SEL_THREADS, 0, h->s>>>(h->dt_keys, h->dt_int, W, H, prm->min_distance, prm->max_corners, h->sel_px, h->sel_py, h->sel_next,
-                                                     h->sel_orig, h->dt_corners, h->dt_int + 1, h->dt_resp);
+  dt_gftt_select_kernel<<<1, SEL_THREADS, 0, h->s>>>(h->dt_keys, &c->candidates, W, H, prm->min_distance, prm->max_corners, h->sel_px, h->sel_py, h->sel_next,
+                                                     h->sel_orig, h->dt_corners, &c->corners, h->dt_resp);
   // (4) range-tree ANMS, K = max(max_features - n_cur, 0), tolerance 0.1 (FeatureDetector.cc:206-224)
-  const int* sel = nullptr; const int* cnt = h->dt_int + 1;
+  const int* sel = nullptr; const int* cnt = &c->corners;
   if (prm->use_anms) {
-    anms_range_tree_kernel<<<1, SEL_THREADS, 0, h->s>>>(h->dt_int + 2, h->dt_int + 1, h->dt_int + 3, nullptr, 0.1f, nullptr, h->dt_corners, 0, W, H,
-                                                         h->sel_px, h->sel_py, h->sel_orig, h->sel_next, h->sel_out, h->dt_int + 4);
-    sel = h->sel_out; cnt = h->dt_int + 4;
+    anms_range_tree_kernel<<<1, SEL_THREADS, 0, h->s>>>(&c->anms_off, &c->corners, &c->K, nullptr, 0.1f, nullptr, h->dt_corners, 0, W, H,
+                                                         h->sel_px, h->sel_py, h->sel_orig, h->sel_next, h->sel_out, &c->anms);
+    sel = h->sel_out; cnt = &c->anms;
   }
   // (5) cornerSubPix in ANMS order, (6) the features
   const int mcap = prm->max_corners > 0 ? (int)std::min<size_t>((size_t)prm->max_corners, npx) : (int)npx;
@@ -1378,10 +1358,10 @@ int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_c
     dt_subpix_kernel<<<(mcap + 127)/128, 128, 0, h->s>>>(mcap, h->dt_corners, sel, cnt, h->dt_clahe, W, H, sm, iters, eps*eps, h->dt_pts);
   } else dt_points_kernel<<<(mcap + 255)/256, 256, 0, h->s>>>(mcap, h->dt_corners, sel, cnt, h->dt_pts);
   const long long base_id = *next_tracklet_id;
-  dt_construct_kernel<<<1, 1024, 0, h->s>>>(h->dt_pts, cnt, h->mask, W, H, prm->track, base_id, h->dt_kp, h->dt_tid, h->dt_int + 6);
+  dt_construct_kernel<<<1, 1024, 0, h->s>>>(h->dt_pts, cnt, h->mask, W, H, prm->track, base_id, h->dt_kp, h->dt_tid, &c->features);
   FCK(cudaGetLastError());
-  int res[8]; float resp = 0.f;
-  FCK(cudaMemcpyAsync(res, h->dt_int, sizeof(res), cudaMemcpyDeviceToHost, h->s));
+  DetectCounters res; float resp = 0.f;
+  FCK(cudaMemcpyAsync(&res, c, sizeof(res), cudaMemcpyDeviceToHost, h->s));
   FCK(cudaMemcpyAsync(&resp, h->dt_resp, 4, cudaMemcpyDeviceToHost, h->s));
   FCK(cudaStreamSynchronize(h->s));
   h->dt_valid = true;
@@ -1389,8 +1369,8 @@ int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_c
   // all 0.  For blockSize 3 on 8-bit input |Ix|, |Iy| <= 1/3 after OpenCV's scale, so a, c <= 9 * (1/9) / 2 and the minimum
   // eigenvalue (a + c) - sqrt((a - c)^2 + b^2) <= 2 min(a, c) <= 1, with equality impossible (a step that is maximal in x
   // and in y over the whole 3x3 window would need its corner pixel to be 0 and 255).  Checked rather than assumed.
-  if (prm->use_anms && res[1] > 0 && resp >= 1.0f) { h->err = "a GFTT response >= 1.0: the ANMS order of the reference would differ"; return -1; }
-  const int total = res[6], ncopy = std::min(total, capacity);
+  if (prm->use_anms && res.corners > 0 && resp >= 1.0f) { h->err = "a GFTT response >= 1.0: the ANMS order of the reference would differ"; return -1; }
+  const int total = res.features, ncopy = std::min(total, capacity);
   if (ncopy) {
     FCK(cudaMemcpyAsync(keypoint, h->dt_kp, 2*(size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
     FCK(cudaMemcpyAsync(tracklet, h->dt_tid, (size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
@@ -1398,7 +1378,7 @@ int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_c
   FCK(cudaEventRecord(h->e1, h->s));
   FCK(cudaStreamSynchronize(h->s));
   *next_tracklet_id = base_id + total; *n_features = total;
-  if (n_corners) *n_corners = res[1];
+  if (n_corners) *n_corners = res.corners;
   if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
   return 0;
 }
@@ -1408,7 +1388,7 @@ int dynofront_detect_last_stages(dynofront_handle h, uint8_t* clahe, float* eig,
   cudaSetDevice(h->dev);
   const size_t npx = (size_t)h->W*h->H;
   int nc = 0;
-  FCK(cudaMemcpy(&nc, h->dt_int + 1, 4, cudaMemcpyDeviceToHost));
+  FCK(cudaMemcpy(&nc, &h->dt_cnt.p->corners, 4, cudaMemcpyDeviceToHost));
   if (clahe) FCK(cudaMemcpy(clahe, h->dt_clahe, npx, cudaMemcpyDeviceToHost));
   if (eig) FCK(cudaMemcpy(eig, h->dt_eig, npx*4, cudaMemcpyDeviceToHost));
   if (corners_xy && nc) FCK(cudaMemcpy(corners_xy, h->dt_corners, 2*(size_t)nc*4, cudaMemcpyDeviceToHost));
@@ -1423,7 +1403,7 @@ int dynofront_propagate_mask(dynofront_handle h, int32_t n, const double* kp, co
   if (!resident && (!prev_mask || !prev_flow || !current_mask)) { h->err = "pass all three images, or none for the resident frames"; return -1; }
   if (resident && !h->have_prev) { h->err = "no previous frame on the device"; return -2; }
   cudaSetDevice(h->dev);
-  if (ensure_features(h, n)) return -3;
+  if (grow(h, h->f_kp, 2*feature_cap(n), h->f_lab, feature_cap(n))) return -3;
   const size_t npx = (size_t)h->W*h->H;
   FCK(cudaMemcpyAsync(h->f_kp, kp, 2*(size_t)n*8, cudaMemcpyHostToDevice, h->s));
   FCK(cudaMemcpyAsync(h->f_lab, lab, (size_t)n*4, cudaMemcpyHostToDevice, h->s));
@@ -1463,25 +1443,20 @@ int dynofront_unpin_host(dynofront_handle h, void* ptr) {
   FCK(cudaHostUnregister(ptr));
   return 0;
 }
-static int klt_scratch(dynofront_ctx* h, int cap) {
-  if (falloc(h, &h->k_prev, 2*(size_t)cap) || falloc(h, &h->k_next, 2*(size_t)cap) || falloc(h, &h->k_err, cap) || falloc(h, &h->k_st, cap) ||
-      falloc(h, &h->k_back, 2*(size_t)cap) || falloc(h, &h->k_eig, 2*(size_t)cap) || falloc(h, &h->k_st2, cap) || falloc(h, &h->k_keep, cap) ||
-      falloc(h, &h->k_age, cap) || falloc(h, &h->k_count, 2)) return -3;
-  h->k_cap = cap; return 0;
-}
 static int build_pyramid(dynofront_ctx* h, int which, const uint8_t* host_img, int max_level, int win, bool with_deriv) {
   const int W = h->W, H = h->H;
   if (h->lw.empty()) {
-    int w = W, hh = H;
-    for (int l = 0; l < 8; l++) {
+    for (int l = 0, w = W, hh = H; l < 8; l++) {
       h->lw.push_back(w); h->lh.push_back(hh);
-      uint8_t *a, *b; short* d;
-      if (falloc(h, &a, (size_t)w*hh) || falloc(h, &b, (size_t)w*hh) || falloc(h, &d, 2*(size_t)w*hh)) return -3;
-      h->pyr[0].push_back(a); h->pyr[1].push_back(b); h->der.push_back(d);
-      short* d2; if (falloc(h, &d2, 2*(size_t)w*hh)) return -3; h->der2.push_back(d2);
       w = (w + 1)/2; hh = (hh + 1)/2;
       if (w < 2 || hh < 2) break;
     }
+    const size_t L = h->lw.size();
+    h->pyr[0].resize(L); h->pyr[1].resize(L); h->der.resize(L); h->der2.resize(L);
+  }
+  for (size_t l = 0; l < h->lw.size(); l++) {
+    const size_t n = (size_t)h->lw[l]*h->lh[l];
+    if (grow(h, h->pyr[0][l], n, h->pyr[1][l], n, h->der[l], 2*n, h->der2[l], 2*n)) return -3;
   }
   FCK(cudaMemcpyAsync(h->pyr[which][0], host_img, (size_t)W*H, cudaMemcpyHostToDevice, h->s));
   const dim3 blk(32, 8);
@@ -1493,30 +1468,49 @@ static int build_pyramid(dynofront_ctx* h, int which, const uint8_t* host_img, i
   return 0;
 }
 
+// buildOpticalFlowPyramid's top level: stop when a level is not larger than the window (lkpyramid.cpp)
+static int klt_top_level(const dynofront_ctx* h, int max_level, int win) {
+  int levels = 0, w = h->W, hh = h->H;
+  for (int l = 0; l <= max_level && l < 8; l++) {
+    levels = l;
+    if (l < max_level) { const int w2 = (w + 1)/2, h2 = (hh + 1)/2; if (w2 <= win || h2 <= win) break; w = w2; hh = h2; }
+  }
+  return levels;
+}
+// levels 0..top of one direction: I = pyramid `from` with its derivatives (der for pyramid 0, der2 for pyramid 1), J = the other
+static KltLevels klt_levels(const dynofront_ctx* h, int top, int from) {
+  KltLevels L; L.nlev = top + 1;
+  for (int l = 0; l <= top; l++) {
+    L.I[l] = h->pyr[from][l]; L.J[l] = h->pyr[1 - from][l]; L.D[l] = from == 0 ? h->der[l] : h->der2[l]; L.w[l] = h->lw[l]; L.h[l] = h->lh[l];
+  }
+  return L;
+}
+// cv::calcOpticalFlowPyrLK's criteria (max_count clamped to [0, 100], epsilon to [0, 10]), one warp per point; errors to k_err
+static void klt_launch(dynofront_ctx* h, const KltLevels& L, int n, const float* from, float* to, uint8_t* st, int win, int max_count, double epsilon,
+                       int use_initial, float min_eig, float* eig) {
+  if (n == 0) return;
+  const int mc = std::min(std::max(max_count, 0), 100);
+  double eps = std::min(std::max(epsilon, 0.0), 10.0); eps *= eps;
+  klt_kernel<<<(n + KLT_WARPS - 1)/KLT_WARPS, KLT_WARPS*32, (size_t)KLT_WARPS*win*win*3*sizeof(short), h->s>>>(L, n, from, to, st, h->k_err, win, mc,
+                                                                                                              (float)eps, use_initial, min_eig, eig);
+}
+
 int dynofront_klt_track(dynofront_handle h, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n, const float* prev_pts, float* next_pts,
                         uint8_t* status, float* err, int32_t win, int32_t max_level, int32_t max_count, double epsilon, int32_t use_initial,
                         double min_eig, float* ms_device) {
   if (!h || !prev_gray || !cur_gray || n < 0 || !prev_pts || !next_pts || !status) return -1;
   if (win < 3 || win > KLT_MAXWIN || max_level < 0) { h->err = "win must be in [3,31]"; return -1; }
   cudaSetDevice(h->dev);
-  // buildOpticalFlowPyramid: stop when a level is not larger than the window (lkpyramid.cpp)
-  int levels = 0; { int w = h->W, hh = h->H; for (int l = 0; l <= max_level && l < 8; l++) { levels = l; if (l < max_level) { const int w2 = (w + 1)/2, h2 = (hh + 1)/2; if (w2 <= win || h2 <= win) break; w = w2; hh = h2; } } }
-  if (n > h->k_cap) { const int cap = std::max(n, 4096); if (klt_scratch(h, cap)) return -3; }
+  const int levels = klt_top_level(h, max_level, win);
+  const size_t cap = feature_cap(n);
+  if (grow(h, h->k_prev, 2*cap, h->k_next, 2*cap, h->k_st, cap, h->k_err, cap, h->k_eig, 2*cap)) return -3;
   FCK(cudaEventRecord(h->e0, h->s));
   if (build_pyramid(h, 0, prev_gray, levels, win, true)) return -3;
   if (build_pyramid(h, 1, cur_gray, levels, win, false)) return -3;
   h->have_pyr = h->have_pyr_cur = false;      // (the resident pyramids of the streaming mode were overwritten)
   FCK(cudaMemcpyAsync(h->k_prev, prev_pts, 2*(size_t)n*4, cudaMemcpyHostToDevice, h->s));
   FCK(cudaMemcpyAsync(h->k_next, use_initial ? next_pts : prev_pts, 2*(size_t)n*4, cudaMemcpyHostToDevice, h->s));
-  KltLevels L; L.nlev = levels + 1;
-  for (int l = 0; l <= levels; l++) { L.I[l] = h->pyr[0][l]; L.J[l] = h->pyr[1][l]; L.D[l] = h->der[l]; L.w[l] = h->lw[l]; L.h[l] = h->lh[l]; }
-  max_count = std::min(std::max(max_count, 0), 100);
-  double eps = std::min(std::max(epsilon, 0.0), 10.0); eps *= eps;
-  if (n > 0) {
-    const size_t smem = (size_t)KLT_WARPS*win*win*3*sizeof(short);
-    klt_kernel<<<(n + KLT_WARPS - 1)/KLT_WARPS, KLT_WARPS*32, smem, h->s>>>(L, n, h->k_prev, h->k_next, h->k_st, h->k_err, win, max_count, (float)eps,
-                                                                            use_initial, (float)min_eig, h->k_eig);
-  }
+  klt_launch(h, klt_levels(h, levels, 0), n, h->k_prev, h->k_next, h->k_st, win, max_count, epsilon, use_initial, (float)min_eig, h->k_eig);
   FCK(cudaMemcpyAsync(next_pts, h->k_next, 2*(size_t)n*4, cudaMemcpyDeviceToHost, h->s));
   FCK(cudaMemcpyAsync(status, h->k_st, n, cudaMemcpyDeviceToHost, h->s));
   if (err) FCK(cudaMemcpyAsync(err, h->k_err, (size_t)n*4, cudaMemcpyDeviceToHost, h->s));
@@ -1537,10 +1531,10 @@ int dynofront_klt_track_fb(dynofront_handle h, const uint8_t* prev_gray, const u
   if (P->win < 3 || P->win > KLT_MAXWIN || P->win_back < 3 || P->win_back > KLT_MAXWIN || P->max_level < 0 || P->max_level_back < 0) { h->err = "win must be in [3,31]"; return -1; }
   if (P->check_static && (!prev_age || !keep)) { h->err = "check_static needs prev_age and keep"; return -1; }
   cudaSetDevice(h->dev);
-  auto nlevels = [&](int max_level, int win) { int levels = 0; int w = h->W, hh = h->H;
-    for (int l = 0; l <= max_level && l < 8; l++) { levels = l; if (l < max_level) { const int w2 = (w + 1)/2, h2 = (hh + 1)/2; if (w2 <= win || h2 <= win) break; w = w2; hh = h2; } } return levels; };
-  const int lf = nlevels(P->max_level, P->win), lb = nlevels(P->max_level_back, P->win_back), lmax = std::max(lf, lb);
-  if (n > h->k_cap) { if (klt_scratch(h, std::max(n, 4096))) return -3; }
+  const int lf = klt_top_level(h, P->max_level, P->win), lb = klt_top_level(h, P->max_level_back, P->win_back), lmax = std::max(lf, lb);
+  const size_t cap = feature_cap(n);
+  if (grow(h, h->k_prev, 2*cap, h->k_next, 2*cap, h->k_back, 2*cap, h->k_st, cap, h->k_st2, cap, h->k_keep, cap, h->k_err, cap, h->k_eig, 2*cap,
+           h->k_age, cap, h->k_count, 2)) return -3;
   FCK(cudaEventRecord(h->e0, h->s));
   if (!resident) {
     if (build_pyramid(h, 0, prev_gray, lmax, P->win, true)) return -3;      // both images with derivatives: each is "previous" once
@@ -1551,25 +1545,22 @@ int dynofront_klt_track_fb(dynofront_handle h, const uint8_t* prev_gray, const u
   FCK(cudaMemcpyAsync(h->k_next, P->use_initial_flow ? next_pts : prev_pts, 2*(size_t)n*4, cudaMemcpyHostToDevice, h->s));
   if (P->check_static) FCK(cudaMemcpyAsync(h->k_age, prev_age, (size_t)n*4, cudaMemcpyHostToDevice, h->s));
   FCK(cudaMemsetAsync(h->k_count, 0, 2*sizeof(int), h->s));
-  auto levels_of = [&](int nl, int fwd) { KltLevels L; L.nlev = nl + 1;
-    for (int l = 0; l <= nl; l++) { L.I[l] = h->pyr[fwd ? 0 : 1][l]; L.J[l] = h->pyr[fwd ? 1 : 0][l]; L.D[l] = fwd ? h->der[l] : h->der2[l]; L.w[l] = h->lw[l]; L.h[l] = h->lh[l]; } return L; };
-  auto run = [&](const KltLevels& L, const float* from, float* to, uint8_t* st, int win, int max_count, double epsilon, int use_initial, float* eig) {
-    const int mc = std::min(std::max(max_count, 0), 100); double eps = std::min(std::max(epsilon, 0.0), 10.0); eps *= eps;
-    if (n > 0) klt_kernel<<<(n + KLT_WARPS - 1)/KLT_WARPS, KLT_WARPS*32, (size_t)KLT_WARPS*win*win*3*sizeof(short), h->s>>>(L, n, from, to, st, h->k_err, win, mc, (float)eps,
-                                                                                                                        use_initial, (float)P->min_eig_threshold, eig);
-  };
-  const KltLevels LF = levels_of(lf, 1), LB = levels_of(lb, 0);
-  run(LF, h->k_prev, h->k_next, h->k_st, P->win, P->max_count, P->epsilon, P->use_initial_flow, h->k_eig);
+  const KltLevels LF = klt_levels(h, lf, 0), LB = klt_levels(h, lb, 1);
+  const float min_eig = (float)P->min_eig_threshold;
+  klt_launch(h, LF, n, h->k_prev, h->k_next, h->k_st, P->win, P->max_count, P->epsilon, P->use_initial_flow, min_eig, h->k_eig);
   if (P->use_initial_flow && n > 0) {
     // StaticFeatureTracker.cc:491-503: with OPTFLOW_USE_INITIAL_FLOW fewer than 10 successes -> track again from scratch
     int succ = 0;
     count_status_kernel<<<(n + 255)/256, 256, 0, h->s>>>(n, h->k_st, h->k_count);
     FCK(cudaMemcpyAsync(&succ, h->k_count, sizeof(int), cudaMemcpyDeviceToHost, h->s)); FCK(cudaStreamSynchronize(h->s));
     FCK(cudaMemsetAsync(h->k_count, 0, 2*sizeof(int), h->s));
-    if (succ < 10) { FCK(cudaMemcpyAsync(h->k_next, h->k_prev, 2*(size_t)n*4, cudaMemcpyDeviceToDevice, h->s)); run(LF, h->k_prev, h->k_next, h->k_st, P->win, P->max_count, P->epsilon, 0, h->k_eig); }
+    if (succ < 10) {
+      FCK(cudaMemcpyAsync(h->k_next, h->k_prev, 2*(size_t)n*4, cudaMemcpyDeviceToDevice, h->s));
+      klt_launch(h, LF, n, h->k_prev, h->k_next, h->k_st, P->win, P->max_count, P->epsilon, 0, min_eig, h->k_eig);
+    }
   }
   FCK(cudaMemcpyAsync(h->k_back, h->k_next, 2*(size_t)n*4, cudaMemcpyDeviceToDevice, h->s));       // flags = 0: the backward search starts at the forward result
-  run(LB, h->k_next, h->k_back, h->k_st2, P->win_back, P->max_count_back, P->epsilon_back, 0, nullptr);
+  klt_launch(h, LB, n, h->k_next, h->k_back, h->k_st2, P->win_back, P->max_count_back, P->epsilon_back, 0, min_eig, nullptr);
   if (n > 0) klt_fb_filter_kernel<<<(n + 255)/256, 256, 0, h->s>>>(n, h->k_prev, h->k_next, h->k_back, h->k_st, h->k_st2, (float)P->max_fb_distance, h->k_st,
                                                                   P->check_static, h->mask, h->W, h->H, P->track, h->k_age, P->max_feature_track_age, h->k_keep, h->k_count);
   int counts[2] = {0, 0};
@@ -1604,28 +1595,20 @@ int dynofront_stereo_track(dynofront_handle h, const uint8_t* left_gray, const u
                            uint8_t* status, double fx, double baseline, double* depth, uint8_t* valid, float* ms_device) {
   if (!h || !left_gray || !right_gray || n < 0 || !left_pts || !right_pts || !status || !depth || !valid) return -1;
   cudaSetDevice(h->dev);
-  const int win = 21, max_level = 5;
-  int levels = 0; { int w = h->W, hh = h->H; for (int l = 0; l <= max_level && l < 8; l++) { levels = l; if (l < max_level) { const int w2 = (w + 1)/2, h2 = (hh + 1)/2; if (w2 <= win || h2 <= win) break; w = w2; hh = h2; } } }
-  if (n > h->k_cap) { if (klt_scratch(h, std::max(n, 4096))) return -3; }
-  double* d_depth = nullptr;
-  if (n > h->st_cap) { if (falloc(h, &h->st_depth, (size_t)std::max(n, 4096))) return -3; h->st_cap = std::max(n, 4096); }
-  d_depth = h->st_depth;
+  const int win = 21, levels = klt_top_level(h, 5, win);
+  const size_t cap = feature_cap(n);
+  if (grow(h, h->k_prev, 2*cap, h->k_next, 2*cap, h->k_st, cap, h->k_keep, cap, h->k_err, cap, h->k_eig, 2*cap, h->st_depth, cap)) return -3;
   FCK(cudaEventRecord(h->e0, h->s));
   if (build_pyramid(h, 0, left_gray, levels, win, true)) return -3;
   if (build_pyramid(h, 1, right_gray, levels, win, false)) return -3;
   h->have_pyr = h->have_pyr_cur = false;
   FCK(cudaMemcpyAsync(h->k_prev, left_pts, 2*(size_t)n*4, cudaMemcpyHostToDevice, h->s));
   FCK(cudaMemcpyAsync(h->k_next, left_pts, 2*(size_t)n*4, cudaMemcpyHostToDevice, h->s));
-  KltLevels L; L.nlev = levels + 1;
-  for (int l = 0; l <= levels; l++) { L.I[l] = h->pyr[0][l]; L.J[l] = h->pyr[1][l]; L.D[l] = h->der[l]; L.w[l] = h->lw[l]; L.h[l] = h->lh[l]; }
-  if (n > 0) {
-    klt_kernel<<<(n + KLT_WARPS - 1)/KLT_WARPS, KLT_WARPS*32, (size_t)KLT_WARPS*win*win*3*sizeof(short), h->s>>>(L, n, h->k_prev, h->k_next, h->k_st, h->k_err, win, 30, 0.01f*0.01f,
-                                                                                                                0, 1e-4f, h->k_eig);
-    stereo_post_kernel<<<(n + 255)/256, 256, 0, h->s>>>(n, h->k_prev, h->k_next, h->k_st, fx, baseline, d_depth, h->k_keep);
-  }
+  klt_launch(h, klt_levels(h, levels, 0), n, h->k_prev, h->k_next, h->k_st, win, 30, 0.01, 0, 1e-4f, h->k_eig);
+  if (n > 0) stereo_post_kernel<<<(n + 255)/256, 256, 0, h->s>>>(n, h->k_prev, h->k_next, h->k_st, fx, baseline, h->st_depth, h->k_keep);
   FCK(cudaMemcpyAsync(right_pts, h->k_next, 2*(size_t)n*4, cudaMemcpyDeviceToHost, h->s));
   FCK(cudaMemcpyAsync(status, h->k_st, n, cudaMemcpyDeviceToHost, h->s));
-  FCK(cudaMemcpyAsync(depth, d_depth, (size_t)n*8, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(depth, h->st_depth, (size_t)n*8, cudaMemcpyDeviceToHost, h->s));
   FCK(cudaMemcpyAsync(valid, h->k_keep, n, cudaMemcpyDeviceToHost, h->s));
   FCK(cudaEventRecord(h->e1, h->s));
   FCK(cudaStreamSynchronize(h->s));
@@ -1635,7 +1618,7 @@ int dynofront_stereo_track(dynofront_handle h, const uint8_t* left_gray, const u
 }
 
 int dynofront_klt_last_min_eig(dynofront_handle h, int32_t n, float* out) {
-  if (!h || !out || n < 0 || n > h->k_cap || !h->k_eig) return -1;
+  if (!h || !out || n < 0 || !h->k_eig.p || 2*(size_t)n > h->k_eig.cap) return -1;
   cudaSetDevice(h->dev);
   FCK(cudaMemcpy(out, h->k_eig, 2*(size_t)n*4, cudaMemcpyDeviceToHost));
   return 0;
@@ -1650,43 +1633,36 @@ int dynofront_track_static_flow(dynofront_handle h, int32_t n_prev, const double
       (n_det && (!det_xy || !acc_det || !flow_det || !pred_det || !tracklet_det))) { h->err = "null array"; return -1; }
   cudaSetDevice(h->dev);
   const int ncols = (int)std::ceil((double)h->W/cell_size), nrows = (int)std::ceil((double)h->H/cell_size), ncell = ncols*nrows;
-  const int nmax = std::max(std::max(n_prev, n_det), 1);
-  if (nmax > h->sf_cap || ncell > h->sf_cells) {
-    const int cap = std::max(nmax, 4096), cells = std::max(ncell, h->sf_cells);
-    int rc = 0;
-    rc |= falloc(h, &h->sf_kp, 2*(size_t)cap); rc |= falloc(h, &h->sf_age, cap); rc |= falloc(h, &h->sf_use, cap); rc |= falloc(h, &h->sf_det, 2*(size_t)cap);
-    rc |= falloc(h, &h->sf_cell, cap); rc |= falloc(h, &h->sf_win, cells); rc |= falloc(h, &h->sf_win2, cells); rc |= falloc(h, &h->sf_cnt, 2);
-    rc |= falloc(h, &h->sf_pass, cap); rc |= falloc(h, &h->sf_acc, cap); rc |= falloc(h, &h->sf_out, 4*(size_t)cap); rc |= falloc(h, &h->sf_oage, cap); rc |= falloc(h, &h->sf_otid, cap);
-    if (rc) return -3;
-    h->sf_cap = cap; h->sf_cells = cells;
-  }
+  const size_t cap = feature_cap(std::max(n_prev, n_det));
+  if (grow(h, h->sf_kp, 2*cap, h->sf_age, cap, h->sf_use, cap, h->sf_det, 2*cap, h->sf_cell, cap, h->sf_win, ncell, h->sf_win2, ncell, h->sf_cnt, 2,
+           h->sf_pass, cap, h->sf_acc, cap, h->sf_flow, 2*cap, h->sf_pred, 2*cap, h->sf_oage, cap, h->sf_otid, cap)) return -3;
   fill_i32_kernel<<<(ncell + 255)/256, 256, 0, h->s>>>(h->sf_win, ncell, 0x7fffffff);
   fill_i32_kernel<<<(ncell + 255)/256, 256, 0, h->s>>>(h->sf_win2, ncell, 0x7fffffff);
   FCK(cudaMemsetAsync(h->sf_cnt, 0, 2*sizeof(int), h->s));
-  std::vector<double> o4; std::vector<uint8_t> acc; int cnt[2] = {0, 0};
-  if (n_prev) {
+  int cnt[2] = {0, 0};
+  if (n_prev) {          // (the copies out are ordered before the detections reuse sf_acc / sf_flow / sf_pred)
     FCK(cudaMemcpyAsync(h->sf_kp, prev_pred_kp, 2*(size_t)n_prev*8, cudaMemcpyHostToDevice, h->s));
     FCK(cudaMemcpyAsync(h->sf_age, prev_age, (size_t)n_prev*4, cudaMemcpyHostToDevice, h->s));
     FCK(cudaMemcpyAsync(h->sf_use, prev_usable, (size_t)n_prev, cudaMemcpyHostToDevice, h->s));
-    sf_prev_kernel<<<(n_prev + 255)/256, 256, 0, h->s>>>(n_prev, h->sf_kp, h->sf_use, h->flow, h->mask, h->W, h->H, cell_size, ncols, h->sf_cell, h->sf_pass, h->sf_out, h->sf_win);
-    sf_prev_resolve_kernel<<<(n_prev + 255)/256, 256, 0, h->s>>>(n_prev, h->sf_cell, h->sf_pass, h->sf_win, h->sf_age, h->sf_acc, h->sf_out, h->sf_oage, h->sf_cnt);
-    o4.resize(4*(size_t)n_prev);
+    sf_prev_kernel<<<(n_prev + 255)/256, 256, 0, h->s>>>(n_prev, h->sf_kp, h->sf_use, h->flow, h->mask, h->W, h->H, cell_size, ncols, h->sf_cell, h->sf_pass,
+                                                         h->sf_flow, h->sf_pred, h->sf_win);
+    sf_prev_resolve_kernel<<<(n_prev + 255)/256, 256, 0, h->s>>>(n_prev, h->sf_cell, h->sf_pass, h->sf_win, h->sf_age, h->sf_acc, h->sf_flow, h->sf_pred,
+                                                                 h->sf_oage, h->sf_cnt);
     FCK(cudaMemcpyAsync(acc_prev, h->sf_acc, n_prev, cudaMemcpyDeviceToHost, h->s));
-    FCK(cudaMemcpyAsync(o4.data(), h->sf_out, o4.size()*8, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(flow_prev, h->sf_flow, 2*(size_t)n_prev*8, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(pred_prev, h->sf_pred, 2*(size_t)n_prev*8, cudaMemcpyDeviceToHost, h->s));
     FCK(cudaMemcpyAsync(age_out, h->sf_oage, (size_t)n_prev*4, cudaMemcpyDeviceToHost, h->s));
-    FCK(cudaStreamSynchronize(h->s));
-    for (int i = 0; i < n_prev; i++) { flow_prev[2*i] = o4[4*(size_t)i]; flow_prev[2*i + 1] = o4[4*(size_t)i + 1]; pred_prev[2*i] = o4[4*(size_t)i + 2]; pred_prev[2*i + 1] = o4[4*(size_t)i + 3]; }
   }
   if (n_det) {
     FCK(cudaMemcpyAsync(h->sf_det, det_xy, 2*(size_t)n_det*4, cudaMemcpyHostToDevice, h->s));
-    sf_det_kernel<<<(n_det + 255)/256, 256, 0, h->s>>>(n_det, h->sf_det, h->flow, h->mask, h->W, h->H, cell_size, ncols, h->sf_win, h->sf_cell, h->sf_pass, h->sf_out, h->sf_win2);
-    sf_det_resolve_kernel<<<1, 1024, 0, h->s>>>(n_det, h->sf_cell, h->sf_pass, h->sf_win2, h->sf_cnt, max_features, (long long)*next_tracklet_id, h->sf_acc, h->sf_out, h->sf_otid, h->sf_cnt + 1);
-    o4.resize(4*(size_t)n_det);
+    sf_det_kernel<<<(n_det + 255)/256, 256, 0, h->s>>>(n_det, h->sf_det, h->flow, h->mask, h->W, h->H, cell_size, ncols, h->sf_win, h->sf_cell, h->sf_pass,
+                                                       h->sf_flow, h->sf_pred, h->sf_win2);
+    sf_det_resolve_kernel<<<1, 1024, 0, h->s>>>(n_det, h->sf_cell, h->sf_pass, h->sf_win2, h->sf_cnt, max_features, (long long)*next_tracklet_id, h->sf_acc,
+                                                h->sf_flow, h->sf_pred, h->sf_otid, h->sf_cnt + 1);
     FCK(cudaMemcpyAsync(acc_det, h->sf_acc, n_det, cudaMemcpyDeviceToHost, h->s));
-    FCK(cudaMemcpyAsync(o4.data(), h->sf_out, o4.size()*8, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(flow_det, h->sf_flow, 2*(size_t)n_det*8, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(pred_det, h->sf_pred, 2*(size_t)n_det*8, cudaMemcpyDeviceToHost, h->s));
     FCK(cudaMemcpyAsync(tracklet_det, h->sf_otid, (size_t)n_det*8, cudaMemcpyDeviceToHost, h->s));
-    FCK(cudaStreamSynchronize(h->s));
-    for (int j = 0; j < n_det; j++) { flow_det[2*j] = o4[4*(size_t)j]; flow_det[2*j + 1] = o4[4*(size_t)j + 1]; pred_det[2*j] = o4[4*(size_t)j + 2]; pred_det[2*j + 1] = o4[4*(size_t)j + 3]; }
   }
   FCK(cudaMemcpyAsync(cnt, h->sf_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, h->s)); FCK(cudaStreamSynchronize(h->s));
   FCK(cudaGetLastError());

@@ -4,12 +4,20 @@ Bar (north_star): bit-exact on track / association indices (accept flags, ages, 
 index sets, KLT status flags); KLT sub-pixel positions within 1e-2 px of cv2 (OpenCV accumulates the 21x21 sums in
 float with a SIMD lane order we do not replicate; our sums are exact integers).
 """
+import os
+import re
+import shlex
+import shutil
+import subprocess
+import tempfile
+
 import numpy as np
 import pytest
 
 from dynosam_b200.synth_frames import SyntheticStream
 
 W, H = 1242, 375
+CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "dynosam_b200", "frontend_csrc")
 
 
 def _features_from_mask(rng, mask, flow, per_object=200, jitter=True):
@@ -74,6 +82,25 @@ def test_c_abi_frontend_exports():
         assert hasattr(lib, s), s
 
 
+def test_frontend_kernels_compile_without_spills():
+    """Every kernel of libdynofront, compiled with the Makefile's code-generation flags, keeps its values in registers:
+    ptxas reports 0 bytes of spill stores and loads (a stack frame alone, such as a local patch array, is not a spill)."""
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    nvcc = nvcc if os.path.exists(nvcc) else shutil.which("nvcc")
+    if nvcc is None:
+        pytest.skip("nvcc not available")
+    with open(os.path.join(CSRC, "Makefile")) as f:
+        flags = shlex.split(re.search(r"^NVFLAGS\s*:=(.*)$", f.read(), re.M).group(1))
+    with tempfile.TemporaryDirectory() as d:
+        r = subprocess.run([nvcc, *flags, "-Xptxas", "-v", "-cubin", "-o", os.path.join(d, "f.cubin"), os.path.join(CSRC, "frontend.cu")],
+                           capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr[-2000:]
+    props = re.findall(r"Function properties for (\S+)\n\s+\d+ bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", r.stderr)
+    assert len(props) >= 30, len(props)
+    spills = [(name, int(st), int(ld)) for name, st, ld in props if int(st) or int(ld)]
+    assert not spills, spills
+
+
 # ------------------------------------------------------------------------------------------------ GPU parity
 @pytest.mark.gpu
 @pytest.mark.parametrize("with_det,min_dist", [(False, 2), (True, 3), (True, 0)])
@@ -97,6 +124,28 @@ def test_track_dynamic_bit_exact(with_det, min_dist):
     assert np.array_equal(a, ra) and np.array_equal(oa, roa) and np.array_equal(ot, rot) and np.array_equal(ol, rol) and nid == rnid
     assert np.array_equal(pk, rpk) and np.array_equal(fl, rfl)          # fp32 -> fp64 adds are exact on both sides
     assert np.array_equal(dm, rdm) and np.array_equal(tm, rtm)
+
+
+@pytest.mark.gpu
+def test_growing_feature_count_reuses_device_memory():
+    """A stream whose feature count creeps upward: each growth of the scratch buffers frees the old ones, so the device's
+    free memory falls by about the final buffers (~30 MB at 300 000 features), not by every size seen on the way."""
+    import torch
+    from dynosam_b200.frontend import FeatureTrackerGPU, TrackParams
+    rng = np.random.default_rng(8)
+    _, m, f = SyntheticStream(n_objects=4, seed=1).frame(1)
+    t = FeatureTrackerGPU(W, H); t.set_frame(f, m, None)
+
+    def call(n):
+        kp = np.stack([rng.uniform(0, W, n), rng.uniform(0, H, n)], 1)
+        t.track_dynamic(kp, np.zeros(n, np.int32), np.zeros(n, np.int32), np.arange(n, dtype=np.int64), TrackParams(), 0, want_masks=False)
+    call(100)                                                 # module load and the first buffers
+    torch.cuda.synchronize(); free0, _ = torch.cuda.mem_get_info()
+    for n in np.linspace(4097, 300000, 64).astype(int):
+        call(int(n))
+    torch.cuda.synchronize(); free1, _ = torch.cuda.mem_get_info()
+    t.close()
+    assert free0 - free1 < 200e6, (free0 - free1)/1e6
 
 
 @pytest.mark.gpu

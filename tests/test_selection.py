@@ -2,18 +2,14 @@
 
 CPU: the oracle's visiting order equals cv2.sortIdx on all-equal keys, and its range-tree ANMS equals a second
 implementation that shares no code with it (cv2.sortIdx for the order, a scipy cKDTree Chebyshev ball query for the
-square search, Decimal rounding for the bounds).  The new kernels build for sm_90a without spills.
+square search, Decimal rounding for the bounds).  That the kernels build for sm_90a without spills is checked for the whole
+library in tests/test_frontend.py.
 GPU (tests/test_selection_gpu.py): the batched kernel and sample_dynamic bit-exact against the oracle.
 """
 import os
-import re
-import shutil
-import subprocess
-import tempfile
 from decimal import ROUND_HALF_UP, Decimal
 
 import numpy as np
-import pytest
 
 import selection_oracle as SO
 
@@ -112,20 +108,3 @@ def test_selection_exports():
     lib = frontend.load()
     for s in ("dynofront_anms_range_tree", "dynofront_sample_dynamic"):
         assert s in frontend.EXPORTS and hasattr(lib, s), s
-
-
-def test_selection_kernels_compile_without_spills():
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not os.path.exists(nvcc) and shutil.which("nvcc") is None:
-        pytest.skip("nvcc not available")
-    nvcc = nvcc if os.path.exists(nvcc) else shutil.which("nvcc")
-    src = os.path.join(ROOT, "dynosam_b200", "frontend_csrc", "frontend.cu")
-    with tempfile.TemporaryDirectory() as d:
-        r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-fmad=false", "-Xptxas", "-v",
-                            "-cubin", "-o", os.path.join(d, "f.cubin"), src], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-2000:]
-    props = re.findall(r"Function properties for (\S+)\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", r.stderr)
-    new = {name: (int(a), int(b), int(c)) for name, a, b, c in props if any(k in name for k in ("anms_range_tree", "sd_prepare", "sd_construct"))}
-    assert len(new) == 3, new
-    for name, (stack, st, ld) in new.items():
-        assert st == 0 and ld == 0, (name, st, ld)
