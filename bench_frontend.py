@@ -142,6 +142,7 @@ def run_dynoba(n, warmup, streaming=True):
     if streaming:
         out.update(full_frame(t, frames, static_pts, feats, n, warmup))
         out.update(static_detection(t, frames, static_pts, n, warmup))
+        out.update(depth_stage(t, frames, static_pts, feats, n, warmup))
     out.update(card())
     return out
 
@@ -199,6 +200,41 @@ def static_detection(t, frames, static_pts, n, warmup):
         t.detect_static(None, np.zeros((0, 2)), prm, 0); first.append(t.last_ms)
     return {"detect_static_ms": float(np.mean(ms)), "detected_per_frame": float(np.mean(det)),
             "detect_static_first_frame_ms": float(np.mean(first)), "detected_first_frame": len(t.detect_static(None, np.zeros((0, 2)), prm, 0)[0])}
+
+
+def depth_stage(t, frames, static_pts, feats, n, warmup):
+    """Depth and back-projection on the device over the streaming frames (Frame::updateDepths, the per-feature half of
+    fillOutputPacketWithTracks, Frame::projectToDenseCloud): after next_frame the frame's depth image (float64, from pinned host
+    memory) is uploaded with set_depth, then update_depths runs over the 800 static points and the dynamic features, back_project
+    over what it kept (RGB-D right key-points, KITTI-like intrinsics) and dense_cloud over the whole image, its four planar
+    outputs copied to the host.  The *_ms keys are the device time of one call (CUDA events, including its copies)."""
+    cal, baseline = (718.856, 718.856, 0.0, 607.1928, 185.2157), 0.537
+    stream = SyntheticStream(n_objects=10, seed=42)             # the stream make_inputs draws its frames from
+    bufs = [np.empty((H, W)), np.empty((H, W))]
+    for b in bufs:
+        t.pin(b)
+    t.next_frame(frames[0][0], frames[0][2], frames[0][1])
+
+    def one(k):
+        g1, m1, f1 = frames[k]
+        kp, lab, _, _ = feats[k-1]
+        buf = bufs[k % 2]; np.copyto(buf, stream.depth(k))    # (the other buffer's copy finished inside the previous frame's calls)
+        t.next_frame(g1, f1, m1)
+        t.set_depth(buf)
+        allkp = np.concatenate([static_pts.astype(np.float64), kp]); alllab = np.concatenate([np.zeros(N_STATIC, np.int32), lab])
+        d, v, _, _ = t.update_depths(allkp, alllab); ud = t.last_ms
+        r = t.back_project(allkp, d, v, cal, baseline, True); bp = t.last_ms
+        nv = t.dense_cloud(cal)[4]
+        return ud, bp, t.last_ms, len(allkp), r["m"], nv
+    for k in range(1, warmup + 1):
+        one(k)
+    rows = np.array([one(k) for k in range(1, n + 1)], np.float64)
+    for b in bufs:
+        t.unpin(b)
+    return {"depth_update_ms": float(rows[:, 0].mean()), "back_project_ms": float(rows[:, 1].mean()), "dense_cloud_ms": float(rows[:, 2].mean()),
+            "depth_h2d_bytes_per_frame": int(8*W*H), "dense_cloud_d2h_bytes_per_frame": int(W*H*(12 + 3 + 4 + 1)),
+            "depth_features_per_frame": float(rows[:, 3].mean()), "measurements_per_frame": float(rows[:, 4].mean()),
+            "dense_points_per_frame": float(rows[:, 5].mean())}
 
 
 def card():

@@ -14,7 +14,8 @@ EXPORTS = ["dynofront_create", "dynofront_destroy", "dynofront_last_error", "dyn
            "dynofront_sample_candidates", "dynofront_propagate_mask", "dynofront_klt_track", "dynofront_klt_track_fb",
            "dynofront_klt_last_min_eig", "dynofront_stereo_track", "dynofront_track_static_flow", "dynofront_next_frame", "dynofront_pin_host", "dynofront_unpin_host",
            "dynofront_get_motion_mask", "dynofront_get_pyramid_level", "dynofront_anms_range_tree", "dynofront_sample_dynamic",
-           "dynofront_detect_static", "dynofront_detect_last_stages"]
+           "dynofront_detect_static", "dynofront_detect_last_stages", "dynofront_set_depth", "dynofront_update_depths",
+           "dynofront_back_project", "dynofront_dense_cloud"]
 
 
 class TrackParamsC(C.Structure):
@@ -106,6 +107,12 @@ def load():
         L.dynofront_detect_static.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(DetectParamsC), C.POINTER(C.c_int64), C.c_int32,
                                               C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float)]
         L.dynofront_detect_last_stages.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
+        L.dynofront_set_depth.argtypes = [C.c_void_p, C.c_void_p]
+        L.dynofront_update_depths.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_void_p,
+                                              C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float)]
+        L.dynofront_back_project.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p]*5 + [C.c_double, C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p]*4 + \
+                                            [C.POINTER(C.c_int32), C.POINTER(C.c_float)]
+        L.dynofront_dense_cloud.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_double] + [C.c_void_p]*4 + [C.POINTER(C.c_int32), C.POINTER(C.c_float)]
         L.dynofront_get_pyramid_level.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]
         _LIB = L
     return _LIB
@@ -117,6 +124,17 @@ def _p(a):
 
 class FrontendError(RuntimeError):
     pass
+
+
+def builder_measurements(bp, tracklet, object_id):
+    """Turns FeatureTrackerGPU.back_project output into graph-builder arguments: the measurements that have a point, split into
+    static (object 0) and dynamic ones.  tracklet / object_id are per input feature.  Returns ((tracklet, z), (tracklet, object,
+    z)) for dynoba_builder_add_static / dynoba_builder_add_dynamic (dynosam_b200.builder.GraphBuilder.add_static / add_dynamic)."""
+    idx = np.asarray(bp["index"]); z = np.asarray(bp["point"]).reshape(-1, 3)
+    has = ~np.isnan(z[:, 2]); idx = idx[has]; z = z[has]
+    tid = np.asarray(tracklet, np.int64)[idx]; obj = np.asarray(object_id, np.int32)[idx]
+    st = obj == 0
+    return (tid[st], z[st]), (tid[~st], obj[~st], z[~st])
 
 
 class FeatureTrackerGPU:
@@ -297,6 +315,53 @@ class FeatureTrackerGPU:
         self._ck(self.lib.dynofront_stereo_track(self.h, _p(lg), _p(rg), n, _p(p0), _p(rp), _p(st), float(fx), float(baseline), _p(depth), _p(valid), C.byref(ms)))
         self.last_ms = ms.value
         return rp, st, depth, valid
+
+    # ---- depth and back-projection
+    def set_depth(self, depth):
+        """upload the current frame's depth image (float64 [H][W]); call after set_frame / next_frame, which mark it stale.
+        A C-contiguous float64 array is passed as is (pin it for an asynchronous copy and keep it untouched until the next call)."""
+        d = np.ascontiguousarray(depth, dtype=np.float64)
+        assert d.shape == (self.H, self.W)
+        self._keep_depth = d                                     # the copy may still be in flight when this returns
+        self._ck(self.lib.dynofront_set_depth(self.h, _p(d)))
+
+    def update_depths(self, kp, label, max_background_depth=200.0, max_object_depth=30.0):
+        """Frame::updateDepths on features kp[n][2] with labels (0 = static): returns (depth, valid, n_invalid, n_outside)"""
+        k = np.ascontiguousarray(kp, dtype=np.float64).reshape(-1, 2); n = k.shape[0]
+        lab = np.ascontiguousarray(np.broadcast_to(np.asarray(label, np.int32), (n,)))
+        d = np.zeros(n); v = np.zeros(n, np.uint8); ni = C.c_int32(); no = C.c_int32(); ms = C.c_float()
+        self._ck(self.lib.dynofront_update_depths(self.h, n, _p(k), _p(lab), float(max_background_depth), float(max_object_depth), _p(d), _p(v),
+                                                  C.byref(ni), C.byref(no), C.byref(ms)))
+        self.last_ms = ms.value
+        return d, v, ni.value, no.value
+
+    def back_project(self, kp, depth, usable, calib5, baseline=0.0, rgbd=False, right_u=None, X_world=None, capacity=None):
+        """fillOutputPacketWithTracks per feature: returns a dict with index [m], point [m][3], stereo [m][3] (uL, uR, v),
+        outlier [n] and m (the first min(m, capacity) rows are filled when a capacity is given)"""
+        k = np.ascontiguousarray(kp, dtype=np.float64).reshape(-1, 2); n = k.shape[0]
+        d = np.ascontiguousarray(depth, dtype=np.float64); u = np.ascontiguousarray(usable, dtype=np.uint8)
+        r = None if right_u is None else np.ascontiguousarray(right_u, dtype=np.float64)
+        X = None if X_world is None else np.ascontiguousarray(X_world, dtype=np.float64).reshape(12)
+        cal = np.ascontiguousarray(calib5, dtype=np.float64).reshape(5)
+        cap = int(n if capacity is None else capacity)
+        idx = np.zeros(max(cap, 1), np.int32); pt = np.zeros((max(cap, 1), 3)); st = np.zeros((max(cap, 1), 3)); out = np.zeros(n, np.uint8)
+        m = C.c_int32(); ms = C.c_float()
+        self._ck(self.lib.dynofront_back_project(self.h, n, _p(k), _p(d), _p(u), _p(r), _p(cal), float(baseline), int(bool(rgbd)), _p(X), cap, _p(idx),
+                                                 _p(pt), _p(st), _p(out), C.byref(m), C.byref(ms)))
+        self.last_ms = ms.value
+        s = min(m.value, cap)
+        return dict(index=idx[:s], point=pt[:s], stereo=st[:s], outlier=out, m=m.value)
+
+    def dense_cloud(self, calib5, max_background_depth=200.0, max_object_depth=30.0):
+        """Frame::projectToDenseCloud on the resident depth / motion mask / boundary mask: (xyz f32[H][W][3], rgb u8[H][W][3],
+        label u32[H][W], valid u8[H][W], n_valid)"""
+        cal = np.ascontiguousarray(calib5, dtype=np.float64).reshape(5)
+        xyz = np.zeros((self.H, self.W, 3), np.float32); rgb = np.zeros((self.H, self.W, 3), np.uint8)
+        lab = np.zeros((self.H, self.W), np.uint32); val = np.zeros((self.H, self.W), np.uint8); nv = C.c_int32(); ms = C.c_float()
+        self._ck(self.lib.dynofront_dense_cloud(self.h, _p(cal), float(max_background_depth), float(max_object_depth), _p(xyz), _p(rgb), _p(lab), _p(val),
+                                                C.byref(nv), C.byref(ms)))
+        self.last_ms = ms.value
+        return xyz, rgb, lab, val, nv.value
 
     def klt_last_min_eig(self, n):
         out = np.zeros((n, 2), np.float32)

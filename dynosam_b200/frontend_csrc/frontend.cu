@@ -9,6 +9,7 @@
 //  * new tracklet ids are handed out in iteration order: prefix count over the accepted features;
 //  * propogateMask processes objects one after the other, each vote seeing the previous object's writes.
 #include <cuda_runtime.h>
+#include <math_constants.h>
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -71,6 +72,10 @@ struct dynofront_ctx {
   DevBuf<uint8_t> dt_gray, dt_mask, dt_clahe, dt_lut; DevBuf<float> dt_dx, dt_dy, dt_box, dt_eig, dt_pts, dt_resp;
   DevBuf<unsigned long long> dt_keys; DevBuf<int> dt_corners; DevBuf<DetectCounters> dt_cnt;
   DevBuf<double> dt_kp; DevBuf<long long> dt_tid; bool dt_valid = false;
+  // depth and back-projection: the current frame's depth image (stale after set_frame / next_frame until set_depth)
+  DevBuf<double> depth; bool has_frame = false, has_depth = false;
+  DevBuf<double> dp_kp, dp_depth, dp_right, dp_point, dp_stereo; DevBuf<int32_t> dp_lab, dp_index; DevBuf<uint8_t> dp_flag, dp_out; DevBuf<int> dp_cnt;
+  DevBuf<float> dc_xyz; DevBuf<uint8_t> dc_rgb, dc_valid; DevBuf<uint32_t> dc_label;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
 };
 // grows each (buffer, element count) pair in turn; 0, or -3 with the error at the first allocation that fails
@@ -1030,6 +1035,124 @@ __global__ void dt_points_kernel(int m, const int* __restrict__ corners, const i
   pts[2*r] = (float)corners[2*c]; pts[2*r + 1] = (float)corners[2*c + 1];
 }
 
+// ---------------------------------------------------------------------------------------------------- depth and back-projection
+// Frame::updateDepths (Frame.cc:241-251,430-467), the per-feature half of RGBDInstanceFrontendModule::fillOutputPacketWithTracks
+// (:391-486) and Frame::projectToDenseCloud (Frame.cc:172-238).  The camera is gtsam::PinholeCamera<Cal3_S2> at the identity
+// pose (Camera.cc:39-46), calib = fx fy s u0 v0.  Every double / float operation below is one IEEE operation in the order of
+// the reference (the library is built with -fmad=false, so nothing is contracted into an FMA).
+struct Calib5 { double fx, fy, s, u0, v0; };
+struct Pose12 { double m[12]; };     // row-major R, then t
+// Cal3_S2::calibrate in GTSAM 4.2's operation order, then PinholeBase::BackprojectFromCamera (x d, y d, d)
+__device__ __forceinline__ void backproject_cam(const Calib5& K, double u, double v, double d, double* p) {
+  const double du = u - K.u0, dv = v - K.v0;
+  const double inv_fx = 1.0/K.fx, inv_fy = 1.0/K.fy;
+  const double ify_dv = inv_fy*dv;
+  const double x = inv_fx*(du - K.s*ify_dv), y = ify_dv;
+  p[0] = x*d; p[1] = y*d; p[2] = d;
+}
+// Pose3::transformFrom: q_i = ((R_i0 p0 + R_i1 p1) + R_i2 p2) + t_i
+__device__ __forceinline__ void transform_from(const Pose12& X, double* p) {
+  double q[3];
+  for (int r = 0; r < 3; r++) q[r] = ((X.m[3*r]*p[0] + X.m[3*r + 1]*p[1]) + X.m[3*r + 2]*p[2]) + X.m[9 + r];
+  p[0] = q[0]; p[1] = q[1]; p[2] = q[2];
+}
+// Color::uniqueId(size_t(label), 0.5f, 0.95f) (Colour.cc:178-185) through Color::fromHSV / rgbFromChromaHue (:73-100), with
+// the reference's mix of float and double: fmod(float, int) and the terms around it are double, x is rounded to float
+__device__ __forceinline__ void unique_id_rgb(int32_t label, uint8_t* rgb) {
+  const float phi = (float)((1.0 + sqrt(5.0))/2.0);
+  const float t = (float)(unsigned long long)(long long)label*phi;
+  const float n = t - floorf(t);
+  float hue = (float)(floor((double)n*256.0)/255.0);
+  hue = fminf(fmaxf(hue, 0.0f), 1.0f);
+  const float value = 0.95f, chroma = value*0.5f;
+  const float hp = hue*6.0f;
+  const float x = (float)((double)chroma*(1.0 - fabs(fmod((double)hp, 2.0) - 1.0)));
+  float r1 = chroma, g1 = 0.0f, b1 = x;
+  if (hp < 1.0f) { r1 = chroma; g1 = x; b1 = 0.0f; }
+  else if (hp < 2.0f) { r1 = x; g1 = chroma; b1 = 0.0f; }
+  else if (hp < 3.0f) { r1 = 0.0f; g1 = chroma; b1 = x; }
+  else if (hp < 4.0f) { r1 = 0.0f; g1 = x; b1 = chroma; }
+  else if (hp < 5.0f) { r1 = x; g1 = 0.0f; b1 = chroma; }
+  const float m = value - chroma;
+  rgb[0] = (uint8_t)((r1 + m)*255.0f); rgb[1] = (uint8_t)((g1 + m)*255.0f); rgb[2] = (uint8_t)((b1 + m)*255.0f);
+}
+// updateDepthsFeatureContainer: d = depth(int(v), int(u)); invalid (NaN depth) when d > max || d <= 0, so a NaN depth stays
+// valid without depth.  A truncated pixel outside the image (undefined in the reference) is invalid with NaN depth; the test
+// -1 < u < W is the truncation test without converting an out-of-range double to int.  cnt[0] invalid, cnt[1] outside.
+__global__ void ud_kernel(int n, const double* __restrict__ kp, const int32_t* __restrict__ lab, const double* __restrict__ depth, int W, int H,
+                          double max_bg, double max_obj, double* __restrict__ dout, uint8_t* __restrict__ valid, int* cnt) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double kx = kp[2*i], ky = kp[2*i + 1];
+  const bool inside = kx > -1.0 && kx < (double)W && ky > -1.0 && ky < (double)H;
+  const double mx = lab[i] == 0 ? max_bg : max_obj;
+  const double d = inside ? depth[(size_t)(int)ky*W + (int)kx] : 0.0;
+  const bool ok = inside && !(d > mx || d <= 0.0);
+  dout[i] = ok ? d : CUDART_NAN;
+  valid[i] = ok ? 1 : 0;
+  if (!ok) atomicAdd(&cnt[0], 1);
+  if (!inside) atomicAdd(&cnt[1], 1);
+}
+// fill_camera_measurements over the usable features in input order, one CTA: landmark when the depth is not NaN (hasDepth),
+// stereo (uL, uR, v) from the given right key-point, else with rgbd and depth uR = uL - fx b / d, an outlier (dropped) when
+// uR < 0 || uR > W.  Emitted measurements are compacted in input order; the first `capacity` are written, *m counts all.
+__global__ void __launch_bounds__(1024) bp_kernel(int n, const double* __restrict__ kp, const double* __restrict__ depth, const uint8_t* __restrict__ usable,
+                                                  const double* __restrict__ right_u, Calib5 K, double fx_b, int rgbd, int W, Pose12 X, int use_X, int capacity,
+                                                  int32_t* index, double* point, double* stereo, uint8_t* outlier, int* m) {
+  int base = 0;
+  for (int i0 = 0; i0 < n; i0 += 1024) {
+    const int i = i0 + threadIdx.x;
+    int emit = 0; uint8_t out = 0;
+    double p[3] = {CUDART_NAN, CUDART_NAN, CUDART_NAN}, st[3] = {CUDART_NAN, CUDART_NAN, CUDART_NAN};
+    if (i < n && usable[i]) {
+      const double u = kp[2*i], v = kp[2*i + 1], d = depth[i];
+      const bool has_depth = !isnan(d);
+      if (has_depth) { backproject_cam(K, u, v, d, p); if (use_X) transform_from(X, p); }
+      const double ur_given = right_u ? right_u[i] : CUDART_NAN;
+      if (!isnan(ur_given)) { st[0] = u; st[1] = ur_given; st[2] = v; }
+      else if (rgbd && has_depth) {
+        const double ur = u - fx_b/d;
+        if (ur < 0.0 || ur > (double)W) out = 1;
+        else { st[0] = u; st[1] = ur; st[2] = v; }
+      }
+      emit = !out;
+    }
+    if (i < n) outlier[i] = out;
+    const int rank = cta_rank(emit, base);
+    if (emit && rank < capacity) {
+      index[rank] = i;
+      for (int c = 0; c < 3; c++) { point[3*(size_t)rank + c] = p[c]; stereo[3*(size_t)rank + c] = st[c]; }
+    }
+  }
+  if (threadIdx.x == 0) *m = base;
+}
+// projectToDenseCloud, one thread per pixel: pixels outside the boundary mask, or with depth > thresh || depth <= 0 || !finite
+// (thresh by background / object label) are zero; the others hold the camera-frame point rounded to float, black (background)
+// or Color::uniqueId(label), the label and valid = 1.  *count = number of valid pixels.
+__global__ void dc_kernel(size_t npx, int W, const double* __restrict__ depth, const int32_t* __restrict__ mask, const uint8_t* __restrict__ det,
+                          Calib5 K, double max_bg, double max_obj, float* xyz, uint8_t* rgb, uint32_t* label, uint8_t* valid, int* count) {
+  const size_t p = (size_t)blockIdx.x*blockDim.x + threadIdx.x;
+  bool ok = false;
+  if (p < npx) {
+    float q[3] = {0.f, 0.f, 0.f}; uint8_t c[3] = {0, 0, 0}; uint32_t l = 0;
+    if (!det || det[p] != 0) {
+      const int32_t oid = mask[p]; const double d = depth[p];
+      const double thresh = oid == 0 ? max_bg : max_obj;
+      if (!(d > thresh || d <= 0.0 || !isfinite(d))) {
+        double pt[3];
+        backproject_cam(K, (double)(int)(p % W), (double)(int)(p / W), d, pt);
+        q[0] = (float)pt[0]; q[1] = (float)pt[1]; q[2] = (float)pt[2];
+        if (oid != 0) unique_id_rgb(oid, c);
+        l = (uint32_t)oid; ok = true;
+      }
+    }
+    for (int k = 0; k < 3; k++) { xyz[3*p + k] = q[k]; rgb[3*p + k] = c[k]; }
+    label[p] = l; valid[p] = ok ? 1 : 0;
+  }
+  const int nv = __syncthreads_count(ok);
+  if (threadIdx.x == 0 && nv) atomicAdd(count, nv);
+}
+
 // ---------------------------------------------------------------------------------------------------- host API
 extern "C" {
 
@@ -1067,6 +1190,7 @@ int dynofront_set_frame(dynofront_handle h, const float* flow, const int32_t* mo
   if (detection_mask) { FCK(cudaMemcpyAsync(h->det, detection_mask, npx, cudaMemcpyHostToDevice, h->s)); h->has_det = true; }
   else h->has_det = false;
   h->det_work_valid = false;
+  h->has_depth = false; h->has_frame = h->has_frame || motion_mask;
   FCK(cudaStreamSynchronize(h->s));
   return 0;
 }
@@ -1083,6 +1207,7 @@ int dynofront_next_frame(dynofront_handle h, const uint8_t* gray, const float* f
   FCK(cudaMemcpyAsync(h->mask, motion_mask, npx*sizeof(int32_t), cudaMemcpyHostToDevice, h->s));
   if (detection_mask) { FCK(cudaMemcpyAsync(h->det, detection_mask, npx, cudaMemcpyHostToDevice, h->s)); h->has_det = true; } else h->has_det = false;
   h->det_work_valid = false;
+  h->has_depth = false; h->has_frame = true;
   h->have_prev = h->have_cur; h->have_cur = true;
   if (!h->lw.empty()) { std::swap(h->pyr[0], h->pyr[1]); std::swap(h->der, h->der2); }
   h->have_pyr = h->have_pyr_cur; h->have_pyr_cur = true;
@@ -1678,6 +1803,118 @@ int dynofront_get_pyramid_level(dynofront_handle h, int32_t which, int32_t level
   const size_t n = (size_t)h->lw[level]*h->lh[level];
   if (img) FCK(cudaMemcpy(img, h->pyr[which][level], n, cudaMemcpyDeviceToHost));
   if (deriv) FCK(cudaMemcpy(deriv, h->der[level], 2*n*sizeof(short), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// ---- depth and back-projection
+int dynofront_set_depth(dynofront_handle h, const double* depth) {
+  if (!h || !depth) return -1;
+  if (!h->has_frame) { h->err = "no frame on the device: call dynofront_set_frame or dynofront_next_frame first"; return -1; }
+  cudaSetDevice(h->dev);
+  const size_t npx = (size_t)h->W*h->H;
+  if (grow(h, h->depth, npx)) return -3;
+  FCK(cudaMemcpyAsync(h->depth, depth, npx*sizeof(double), cudaMemcpyHostToDevice, h->s));
+  h->has_depth = true;
+  return 0;                                                     // no synchronisation, as dynofront_next_frame
+}
+static int depth_args(dynofront_ctx* h, double max_bg, double max_obj) {
+  if (!(max_bg > 0.0) || !(max_obj > 0.0)) { h->err = "depth thresholds must be > 0 (Frame::setMaxBackgroundDepth / setMaxObjectDepth)"; return -1; }
+  if (!h->has_depth) { h->err = "no depth for the current frame: call dynofront_set_depth after dynofront_set_frame / dynofront_next_frame"; return -1; }
+  return 0;
+}
+static Calib5 calib_of(const double* c) { return Calib5{c[0], c[1], c[2], c[3], c[4]}; }
+
+int dynofront_update_depths(dynofront_handle h, int32_t n, const double* kp, const int32_t* label, double max_background_depth,
+                            double max_object_depth, double* depth_out, uint8_t* valid_out, int32_t* n_invalid, int32_t* n_outside, float* ms_device) {
+  if (!h || n < 0 || (n && (!kp || !label || !depth_out || !valid_out))) return -1;
+  if (depth_args(h, max_background_depth, max_object_depth)) return -1;
+  cudaSetDevice(h->dev);
+  const size_t cap = feature_cap(n);
+  if (grow(h, h->dp_kp, 2*cap, h->dp_lab, cap, h->dp_depth, cap, h->dp_flag, cap, h->dp_cnt, 2)) return -3;
+  FCK(cudaEventRecord(h->e0, h->s));
+  FCK(cudaMemsetAsync(h->dp_cnt, 0, 2*sizeof(int), h->s));
+  int cnt[2] = {0, 0};
+  if (n) {
+    FCK(cudaMemcpyAsync(h->dp_kp, kp, 2*(size_t)n*8, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->dp_lab, label, (size_t)n*4, cudaMemcpyHostToDevice, h->s));
+    ud_kernel<<<(n + 255)/256, 256, 0, h->s>>>(n, h->dp_kp, h->dp_lab, h->depth, h->W, h->H, max_background_depth, max_object_depth, h->dp_depth,
+                                               h->dp_flag, h->dp_cnt);
+    FCK(cudaGetLastError());
+    FCK(cudaMemcpyAsync(depth_out, h->dp_depth, (size_t)n*8, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(valid_out, h->dp_flag, (size_t)n, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(cnt, h->dp_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, h->s));
+  }
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  if (n_invalid) *n_invalid = cnt[0];
+  if (n_outside) *n_outside = cnt[1];
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+
+int dynofront_back_project(dynofront_handle h, int32_t n, const double* kp, const double* depth, const uint8_t* usable, const double* right_u,
+                           const double* calib5, double baseline, int32_t rgbd, const double* X_world, int32_t capacity, int32_t* index,
+                           double* point, double* stereo, uint8_t* outlier, int32_t* m, float* ms_device) {
+  if (!h || n < 0 || capacity < 0 || !calib5 || !m || (n && (!kp || !depth || !usable))) return -1;
+  if (capacity && (!index || !point || !stereo)) { h->err = "null measurement array"; return -1; }
+  if (right_u)
+    for (int i = 0; i < n; i++)
+      if (usable[i] && !std::isnan(right_u[i]) && std::isnan(depth[i])) { h->err = "a usable feature has a right key-point but no depth"; return -1; }
+  cudaSetDevice(h->dev);
+  const size_t cap = feature_cap(n);
+  if (grow(h, h->dp_kp, 2*cap, h->dp_depth, cap, h->dp_flag, cap, h->dp_right, cap, h->dp_out, cap, h->dp_index, cap, h->dp_point, 3*cap,
+           h->dp_stereo, 3*cap, h->dp_cnt, 2)) return -3;
+  Pose12 X{}; if (X_world) std::memcpy(X.m, X_world, sizeof(X.m));
+  FCK(cudaEventRecord(h->e0, h->s));
+  if (n) {
+    FCK(cudaMemcpyAsync(h->dp_kp, kp, 2*(size_t)n*8, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->dp_depth, depth, (size_t)n*8, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->dp_flag, usable, (size_t)n, cudaMemcpyHostToDevice, h->s));
+    if (right_u) FCK(cudaMemcpyAsync(h->dp_right, right_u, (size_t)n*8, cudaMemcpyHostToDevice, h->s));
+  }
+  const double fx_b = calib5[0]*baseline;                       // RGBDCamera::fx_b_
+  bp_kernel<<<1, 1024, 0, h->s>>>(n, h->dp_kp, h->dp_depth, h->dp_flag, right_u ? h->dp_right.p : nullptr, calib_of(calib5), fx_b, rgbd ? 1 : 0, h->W, X,
+                                  X_world ? 1 : 0, std::min(capacity, n), h->dp_index, h->dp_point, h->dp_stereo, h->dp_out, h->dp_cnt);
+  FCK(cudaGetLastError());
+  int total = 0;
+  FCK(cudaMemcpyAsync(&total, h->dp_cnt, sizeof(int), cudaMemcpyDeviceToHost, h->s));
+  if (n && outlier) FCK(cudaMemcpyAsync(outlier, h->dp_out, (size_t)n, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  const int ncopy = std::min(total, capacity);
+  if (ncopy) {
+    FCK(cudaMemcpyAsync(index, h->dp_index, (size_t)ncopy*4, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(point, h->dp_point, 3*(size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(stereo, h->dp_stereo, 3*(size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
+  }
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  *m = total;
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+
+int dynofront_dense_cloud(dynofront_handle h, const double* calib5, double max_background_depth, double max_object_depth, float* xyz, uint8_t* rgb,
+                          uint32_t* label, uint8_t* valid, int32_t* n_valid, float* ms_device) {
+  if (!h || !calib5) return -1;
+  if (depth_args(h, max_background_depth, max_object_depth)) return -1;
+  cudaSetDevice(h->dev);
+  const size_t npx = (size_t)h->W*h->H;
+  if (grow(h, h->dc_xyz, 3*npx, h->dc_rgb, 3*npx, h->dc_label, npx, h->dc_valid, npx, h->dp_cnt, 2)) return -3;
+  FCK(cudaEventRecord(h->e0, h->s));
+  FCK(cudaMemsetAsync(h->dp_cnt, 0, sizeof(int), h->s));
+  dc_kernel<<<(unsigned)((npx + 255)/256), 256, 0, h->s>>>(npx, h->W, h->depth, h->mask, h->has_det ? h->det.p : nullptr, calib_of(calib5),
+                                                           max_background_depth, max_object_depth, h->dc_xyz, h->dc_rgb, h->dc_label, h->dc_valid, h->dp_cnt);
+  FCK(cudaGetLastError());
+  int cnt = 0;
+  FCK(cudaMemcpyAsync(&cnt, h->dp_cnt, sizeof(int), cudaMemcpyDeviceToHost, h->s));
+  if (xyz) FCK(cudaMemcpyAsync(xyz, h->dc_xyz, 3*npx*4, cudaMemcpyDeviceToHost, h->s));
+  if (rgb) FCK(cudaMemcpyAsync(rgb, h->dc_rgb, 3*npx, cudaMemcpyDeviceToHost, h->s));
+  if (label) FCK(cudaMemcpyAsync(label, h->dc_label, npx*4, cudaMemcpyDeviceToHost, h->s));
+  if (valid) FCK(cudaMemcpyAsync(valid, h->dc_valid, npx, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  if (n_valid) *n_valid = cnt;
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
   return 0;
 }
 

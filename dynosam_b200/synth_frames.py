@@ -17,7 +17,7 @@ def _value_noise(rng, h, w, cells):
 
 class SyntheticStream:
     def __init__(self, n_objects=10, seed=42, width=W, height=H):
-        self.rng = np.random.default_rng(seed); self.W, self.H = width, height
+        self.rng = np.random.default_rng(seed); self.W, self.H = width, height; self.seed = seed
         rng = self.rng
         self.bg = (0.5*_value_noise(rng, height, width + 400, 8) + 0.3*_value_noise(rng, height, width + 400, 3)
                    + 0.2*rng.uniform(0, 255, (height, width + 400)))
@@ -50,3 +50,30 @@ class SyntheticStream:
             mask[y0:y1, x0:x1] = o["label"]
             flow[y0:y1, x0:x1, 0] = o["vx"]; flow[y0:y1, x0:x1, 1] = o["vy"] if o["vy"] != 0 else 1e-3
         return np.clip(gray, 0, 255).astype(np.uint8), mask, flow
+
+    # fixed pixels of depth(k) that hold the values updateDepths / projectToDenseCloud treat specially (d == 30 and d == 200 are
+    # the yaml thresholds max_object_depth / max_background_depth, kept by both)
+    DEPTH_EDGE_VALUES = (0.0, -1.5, np.nan, np.inf, -np.inf, 30.0, 200.0)
+
+    def depth_edge_pixels(self):
+        """{value index: (rows, cols)} of the edge pixels of depth(k), the same in every frame"""
+        t = np.arange(8)
+        return {j: ((7 + 37*t + 3*j) % self.H, (11 + 131*j + 17*t) % self.W) for j in range(len(self.DEPTH_EDGE_VALUES))}
+
+    def depth(self, k):
+        """depth float64[H,W] in metres (CV_64F) for frame k, drawn from generators of its own (frame(k) is unchanged).
+        Background 5-263 m, nearer towards the bottom rows; each object at its own depth in 8-60 m plus a small slope, so both
+        classes lie on both sides of 30 m and 200 m.  The pixels of depth_edge_pixels() hold 0, -1.5, NaN, +-inf, 30 and 200."""
+        _, mask, _ = self.frame(k)
+        rng = np.random.default_rng([self.seed, 0x6465707468, k])
+        r = (np.arange(self.H)/max(self.H - 1, 1))[:, None]; c = (np.arange(self.W)/max(self.W - 1, 1))[None, :]
+        d = 8.0 + 252.0*(1.0 - r)**2 + 3.0*np.sin(2*np.pi*(c + 0.01*k)) + rng.normal(0.0, 0.05, (self.H, self.W))
+        for o in self.obj:
+            sel = mask == o["label"]
+            if sel.any():
+                base = np.random.default_rng([self.seed, 0x6f626a, o["label"]]).uniform(8.0, 60.0)
+                ys, xs = np.nonzero(sel)
+                d[ys, xs] = base + 0.08*(xs - xs.min()) + rng.normal(0.0, 0.02, len(ys))
+        for j, (ys, xs) in self.depth_edge_pixels().items():
+            d[ys, xs] = self.DEPTH_EDGE_VALUES[j]
+        return d
