@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <mutex>
 #include <vector>
 #include "factors.cuh"
 
@@ -282,5 +283,27 @@ int launch_pose_delta_norm(const DevBand& B, double lambda, double* partials, cu
 int pose_norm_grid(int n);
 int launch_retract(const DevVars& cur, const DevVars& cand, const DevBand& B, const double* dl_point,
                    const double* dl_flow, cudaStream_t s);
+
+// ---- per-frame batch entry points (kernels_star.cu, kernels_ransac.cu).  Per-device state kept between calls (these entry
+// points run every frame): one stream and one grow-only workspace, so a call costs copies + one launch -- no cudaMalloc /
+// cudaFree / stream creation on the per-frame path.  Calls on one device serialise on mu; dynoba_batch_release frees it.
+struct StarContext { std::mutex mu; cudaStream_t stream = nullptr; char* base = nullptr; size_t cap = 0; };
+StarContext& star_context(int device);          // device in [0, 64)
+int star_device_ready(int device);              // sm_90 check, cudaSetDevice, stream creation (call with mu held)
+// a bump allocator over the workspace, 16-byte granules; with base == nullptr it only measures
+struct DeviceBlock {
+  char* base = nullptr; size_t used = 0;
+  template <class T> T* take(size_t count) { T* p = base ? (T*)(base + used) : nullptr; used += (count*sizeof(T) + 15) & ~(size_t)15; return p; }
+  bool allocate(StarContext& c) {
+    const size_t need = used + 256; used = 0;
+    if (need > c.cap) {
+      if (c.base) { cudaFree(c.base); c.base = nullptr; c.cap = 0; }
+      const size_t cap = need + need/2;
+      if (cudaMalloc((void**)&c.base, cap) != cudaSuccess) { c.base = nullptr; return false; }
+      c.cap = cap;
+    }
+    base = c.base; return true;
+  }
+};
 
 }  // namespace dynoba

@@ -544,26 +544,9 @@ __global__ void __launch_bounds__(STAR_THREADS) motion_refine_kernel(MotionBatch
   }
 }
 
-// Per-device state kept between calls (these entry points run every frame): one stream and one grow-only workspace, so a call
-// costs copies + one launch -- no cudaMalloc / cudaFree / stream creation on the per-frame path.  Calls on one device serialise.
-struct StarContext { std::mutex mu; cudaStream_t stream = nullptr; char* base = nullptr; size_t cap = 0; };
 static StarContext g_star[64];
-// a bump allocator over the workspace, 16-byte granules; with base == nullptr it only measures
-struct DeviceBlock {
-  char* base = nullptr; size_t used = 0;
-  template <class T> T* take(size_t count) { T* p = base ? (T*)(base + used) : nullptr; used += (count*sizeof(T) + 15) & ~(size_t)15; return p; }
-  bool allocate(StarContext& c) {
-    const size_t need = used + 256; used = 0;
-    if (need > c.cap) {
-      if (c.base) { cudaFree(c.base); c.base = nullptr; c.cap = 0; }
-      const size_t cap = need + need/2;
-      if (cudaMalloc((void**)&c.base, cap) != cudaSuccess) { c.base = nullptr; return false; }
-      c.cap = cap;
-    }
-    base = c.base; return true;
-  }
-};
-static int star_device_ready(int device) {
+StarContext& star_context(int device) { return g_star[device]; }
+int star_device_ready(int device) {
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return DYNOBA_ERR_CUDA;     // no CPU fallback
   cudaDeviceProp prop;
@@ -698,7 +681,7 @@ int dynoba_motion_refine_batch(int device, int32_t n_problems, const int32_t* of
   return (e1 == cudaSuccess && e2 == cudaSuccess) ? DYNOBA_OK : DYNOBA_ERR_CUDA;
 }
 
-// frees the per-device workspace and stream the two batch entry points keep between calls
+// frees the per-device workspace and stream the batch entry points (these two and dynoba_pnp_ransac_batch) keep between calls
 int dynoba_batch_release(int device) {
   if (device < 0 || device >= 64) return DYNOBA_ERR_BAD_ARG;
   StarContext& c = g_star[device];

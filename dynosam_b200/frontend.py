@@ -137,6 +137,33 @@ def builder_measurements(bp, tracklet, object_id):
     return (tid[st], z[st]), (tid[~st], obj[~st], z[~st])
 
 
+def pnp_correspondences(tracklet_prev, usable_prev, label_prev, bp_prev, tracklet_cur, usable_cur, label_cur, kp_cur, calib5):
+    """The 3D-2D problems of a frame for binding.pnp_ransac_batch: what Frame::getCorrespondences gathers for
+    EgoMotionSolver::geometricOutlierRejection3d2d (camera, label 0) and for every object (Frame-inl.hpp:38-64,
+    VisionTools.cc:75-98).  Frame k's features are visited in container order; a feature enters when it is usable, its tracklet
+    is in frame k-1, usable there with the same label.  Its reference is the world point of the k-1 feature, from
+    FeatureTrackerGPU.back_project(..., X_world=pose_k-1) of frame k-1 (bp_prev: index / point); a feature without one raises
+    ValueError, as the reference throws when the previous feature has no depth (Frame.cc:280-285).  Returns the camera problem
+    first, then one problem per object in ascending label: dicts with label, tracklet [m], points [m,3], kp [m,2], calib [5]."""
+    t0 = np.asarray(tracklet_prev, np.int64); u0 = np.asarray(usable_prev, bool); l0 = np.asarray(label_prev, np.int64)
+    t1 = np.asarray(tracklet_cur, np.int64); u1 = np.asarray(usable_cur, bool); l1 = np.asarray(label_cur, np.int64)
+    kp = np.asarray(kp_cur, np.float64).reshape(-1, 2)
+    pw = np.full((len(t0), 3), np.nan)
+    pw[np.asarray(bp_prev["index"], np.int64)] = np.asarray(bp_prev["point"], np.float64).reshape(-1, 3)
+    order = np.argsort(t0, kind="stable")
+    j = np.searchsorted(t0[order], t1).clip(0, max(len(t0) - 1, 0))
+    j = order[j] if len(t0) else np.zeros(len(t1), np.int64)
+    take = u1 & (t0[j] == t1) & u0[j] & (l0[j] == l1) if len(t0) else np.zeros(len(t1), bool)
+    if np.isnan(pw[j[take]]).any():
+        raise ValueError("pnp_correspondences: a previous feature has no world point (no depth)")
+    cal = np.asarray(calib5, np.float64).reshape(5)
+    out = []
+    for lab in [0] + sorted(set(int(x) for x in l1[take]) - {0}):
+        s = take & (l1 == lab)
+        out.append(dict(label=lab, tracklet=t1[s], points=pw[j[s]], kp=kp[s], calib=cal.copy()))
+    return out
+
+
 class FeatureTrackerGPU:
     """One handle per camera stream (image size fixed at construction)."""
 

@@ -77,3 +77,51 @@ def motion_set():
     rng = np.random.default_rng(31)
     sizes = [6, 7, 20, 64, 100, 255, 256, 257] + list(rng.integers(10, 120, 6))
     return [make_motion_problem(rng, int(n), outliers=0.1 if i % 2 else 0.0) for i, n in enumerate(sizes)]
+
+
+IMAGE_W, IMAGE_H = 1242, 375                                    # the image K5 belongs to
+
+
+def make_pnp_problem(rng, n, noise_px=0.5, outliers=0.0, collinear=0, duplicate=0, calib=K5):
+    """a 3D-2D absolute-pose problem (what geometricOutlierRejection3d2d reads, MotionSolver.cc:234-265): world points in front of
+    a camera at the ground-truth pose, their key-points with Gaussian noise; round(outliers n) of them get a key-point drawn
+    uniformly over the image instead (gross outliers), the first `collinear` points lie on one world line, and the last
+    `duplicate` points repeat earlier ones exactly.  Returns calib, points [n,3], kp [n,2], gt (camera pose in the world, 12) and
+    outlier [n] (bool)."""
+    K = np.asarray(calib, dtype=np.float64)
+    X = lie.se3_exp(np.concatenate([rng.normal(0, 0.2, 3), rng.normal(0, 2.0, 3)])[None])[0]
+    u = rng.uniform(0, IMAGE_W, n); v = rng.uniform(0, IMAGE_H, n); z = rng.uniform(3.0, 40.0, n)
+    y = (v - K[4])/K[1]
+    pc = np.stack([((u - K[3]) - K[2]*y)/K[0]*z, y*z, z], 1)
+    pw = lie.transform_from(np.tile(X, (n, 1)), pc) if n else np.zeros((0, 3))
+    c = min(collinear, n)
+    if c:          # exactly collinear in the world: equal y and z, so every cross product of differences is exactly zero
+        pw[:c, 1] = pw[0, 1]; pw[:c, 2] = pw[0, 2]; pw[:c, 0] = pw[0, 0] + np.linspace(-1.0, 1.0, c)
+    if duplicate and n > duplicate:
+        pw[n - duplicate:] = pw[:duplicate]
+    q = lie.transform_to(np.tile(X, (n, 1)), pw) if n else np.zeros((0, 3))
+    kp = np.stack([K[0]*q[:, 0]/q[:, 2] + K[2]*q[:, 1]/q[:, 2] + K[3], K[1]*q[:, 1]/q[:, 2] + K[4]], 1) if n else np.zeros((0, 2))
+    kp = kp + rng.normal(0, noise_px, (n, 2)) if noise_px > 0 else kp
+    bad = np.zeros(n, bool)
+    nb = int(round(outliers*n))
+    if nb:
+        bad[rng.permutation(n)[:nb]] = True
+        kp[bad] = np.stack([rng.uniform(0, IMAGE_W, nb), rng.uniform(0, IMAGE_H, nb)], 1)
+    if duplicate and n > duplicate:
+        kp[n - duplicate:] = kp[:duplicate]; bad[n - duplicate:] = bad[:duplicate]
+    return dict(calib=K.copy(), points=pw, kp=kp, gt=X, outlier=bad)
+
+
+def pnp_parity_set():
+    """problems of 0 .. 20 000 correspondences: below the five-match minimum, warp and tile boundaries, the camera's sizes,
+    0 - 70 % gross outliers, collinear and duplicated subsets, an all-collinear problem"""
+    rng = np.random.default_rng(41)
+    sizes = [0, 4, 5, 6, 7, 31, 32, 33, 255, 256, 257, 800, 2700, 20000]
+    fracs = [0.0, 0.1, 0.3, 0.5, 0.7]
+    probs = [make_pnp_problem(rng, n, noise_px=0.5 if i % 4 else 0.0, outliers=fracs[i % 5] if n >= 5 else 0.0,
+                              collinear=8 if i % 3 == 1 and n > 40 else 0, duplicate=5 if i % 3 == 2 and n > 40 else 0)
+             for i, n in enumerate(sizes)]
+    probs.append(make_pnp_problem(rng, 60, noise_px=0.0, collinear=60))                       # every triple collinear
+    probs.append(make_pnp_problem(rng, 300, noise_px=0.5, outliers=0.7))
+    probs.append(make_pnp_problem(rng, 1500, noise_px=0.5, outliers=0.1))
+    return probs
