@@ -15,7 +15,8 @@ EXPORTS = ["dynofront_create", "dynofront_destroy", "dynofront_last_error", "dyn
            "dynofront_klt_last_min_eig", "dynofront_stereo_track", "dynofront_track_static_flow", "dynofront_next_frame", "dynofront_pin_host", "dynofront_unpin_host",
            "dynofront_get_motion_mask", "dynofront_get_pyramid_level", "dynofront_anms_range_tree", "dynofront_sample_dynamic",
            "dynofront_detect_static", "dynofront_detect_last_stages", "dynofront_set_depth", "dynofront_update_depths",
-           "dynofront_back_project", "dynofront_dense_cloud"]
+           "dynofront_back_project", "dynofront_dense_cloud", "dynofront_homography_default_params", "dynofront_find_homography_batch",
+           "dynofront_homography_last_trace", "dynofront_homography_record_counts", "dynofront_klt_track_points"]
 
 
 class TrackParamsC(C.Structure):
@@ -71,6 +72,26 @@ class DetectParams:
                              TrackParamsC(0, 0, self.shrink_row, self.shrink_col))
 
 
+class HomographyParamsC(C.Structure):
+    _fields_ = [("threshold_px", C.c_double), ("confidence", C.c_double), ("max_iters", C.c_int32), ("refine", C.c_int32)]
+
+
+@dataclass
+class HomographyParams:
+    """cv::findHomography(src, dst, RANSAC, threshold_px, mask, max_iters, confidence) as geometricVerification calls it;
+    refine=False returns the RANSAC model and mask instead of the refined ones."""
+    threshold_px: float = 5.0
+    confidence: float = 0.995
+    max_iters: int = 2000
+    refine: bool = True
+
+    def c(self):
+        return HomographyParamsC(float(self.threshold_px), float(self.confidence), int(self.max_iters), int(bool(self.refine)))
+
+
+HOM_OK, HOM_TOO_FEW, HOM_FOUR_POINT, HOM_RANSAC_FAILED = 0, 1, 2, 3     # dynofront_find_homography_batch status
+
+
 _LIB = None
 
 
@@ -113,6 +134,15 @@ def load():
         L.dynofront_back_project.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p]*5 + [C.c_double, C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p]*4 + \
                                             [C.POINTER(C.c_int32), C.POINTER(C.c_float)]
         L.dynofront_dense_cloud.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_double] + [C.c_void_p]*4 + [C.POINTER(C.c_int32), C.POINTER(C.c_float)]
+        L.dynofront_homography_default_params.argtypes = [C.POINTER(HomographyParamsC)]
+        L.dynofront_homography_default_params.restype = None
+        L.dynofront_find_homography_batch.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(HomographyParamsC)] + \
+                                                     [C.c_void_p]*5 + [C.POINTER(C.c_float)]
+        L.dynofront_homography_last_trace.argtypes = [C.c_void_p] + [C.c_void_p]*4 + [C.c_int32, C.c_void_p, C.POINTER(C.c_int32)]
+        L.dynofront_homography_record_counts.argtypes = [C.c_void_p, C.c_int32]
+        L.dynofront_klt_track_points.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.POINTER(KltFbParamsC), C.POINTER(HomographyParamsC)] + [C.c_void_p]*4 + \
+                                                [C.POINTER(C.c_int32)]*4 + [C.POINTER(C.c_float)]
         L.dynofront_get_pyramid_level.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]
         _LIB = L
     return _LIB
@@ -333,6 +363,66 @@ class FeatureTrackerGPU:
                                                  C.byref(ns), C.byref(nk), C.byref(ms)))
         self.last_ms = ms.value; self.last_counts = (ns.value, nk.value)
         return nxt, st, back, (keep if check else None)
+
+    def klt_track_points(self, prev_gray, cur_gray, prev_pts, prm: TrackParams | None = None, prev_age=None, max_feature_track_age=25,
+                         hom: HomographyParams | None = None, win=21, max_level=3, max_count=30, eps=0.03, initial=None, min_eig=1e-4,
+                         max_fb_distance=0.5):
+        """KltFeatureTracker::trackPoints steps 1-4 in one call: klt_track_fb's stages, then cv::findHomography(RANSAC) over the
+        points that passed the round trip, in order, then the checks.  Returns (next, status, verified, keep, H); keep is None
+        without prev_age, H is None when the homography has none.  self.last_counts = (n_status, n_verified, n_keep),
+        self.last_hom_status = the homography's HOM_* status."""
+        pg = None if prev_gray is None else np.ascontiguousarray(prev_gray, dtype=np.uint8)     # None, None: the resident frame pair
+        cg = None if cur_gray is None else np.ascontiguousarray(cur_gray, dtype=np.uint8)
+        p0 = np.ascontiguousarray(prev_pts, dtype=np.float32).reshape(-1, 2); n = p0.shape[0]
+        nxt = np.ascontiguousarray(initial, dtype=np.float32).reshape(-1, 2).copy() if initial is not None else np.zeros((n, 2), np.float32)
+        st = np.zeros(n, np.uint8); ver = np.zeros(n, np.uint8); keep = np.zeros(n, np.uint8); H = np.zeros(9); ms = C.c_float()
+        check = prev_age is not None
+        age = np.ascontiguousarray(prev_age, dtype=np.int32) if check else None
+        pc = KltFbParamsC(win, max_level, max_count, float(eps), 21, 5, 30, 0.01, 1 if initial is not None else 0, float(min_eig), float(max_fb_distance),
+                          1 if check else 0, int(max_feature_track_age), (prm or TrackParams()).c())
+        hc = (hom or HomographyParams()).c()
+        hs = C.c_int32(); ns = C.c_int32(); nv = C.c_int32(); nk = C.c_int32()
+        self._ck(self.lib.dynofront_klt_track_points(self.h, _p(pg), _p(cg), n, _p(p0), _p(nxt), _p(st), C.byref(pc), C.byref(hc), _p(age), _p(ver),
+                                                     _p(keep), _p(H), C.byref(hs), C.byref(ns), C.byref(nv), C.byref(nk), C.byref(ms)))
+        self.last_ms = ms.value; self.last_counts = (ns.value, nv.value, nk.value); self.last_hom_status = hs.value
+        return nxt, st, ver, (keep if check else None), (H.reshape(3, 3) if hs.value in (HOM_OK, HOM_FOUR_POINT) and H.any() else None)
+
+    def find_homography_batch(self, problems, prm: HomographyParams | None = None):
+        """cv::findHomography(src, dst, RANSAC, ...) on every problem in one launch.  problems: sequence of (src [n][2], dst [n][2]).
+        Returns a dict: H [P][3][3] (0 where there is none), masks (one u8 array per problem), n_inliers, status, iterations."""
+        srcs = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1, 2) for a, _ in problems]
+        dsts = [np.ascontiguousarray(b, dtype=np.float32).reshape(-1, 2) for _, b in problems]
+        P = len(srcs)
+        off = np.zeros(P + 1, np.int32); off[1:] = np.cumsum([len(a) for a in srcs])
+        src = np.ascontiguousarray(np.concatenate(srcs) if P else np.zeros((0, 2), np.float32))
+        dst = np.ascontiguousarray(np.concatenate(dsts) if P else np.zeros((0, 2), np.float32))
+        if src.shape != dst.shape:
+            raise ValueError("find_homography_batch: src and dst of a problem must have the same length")
+        H = np.zeros((max(P, 1), 9)); mask = np.zeros(max(int(off[-1]), 1), np.uint8)
+        ninl = np.zeros(max(P, 1), np.int32); st = np.zeros(max(P, 1), np.int32); it = np.zeros(max(P, 1), np.int32); ms = C.c_float()
+        pc = (prm or HomographyParams()).c()
+        self._ck(self.lib.dynofront_find_homography_batch(self.h, P, _p(off), _p(src), _p(dst), C.byref(pc), _p(H), _p(mask), _p(ninl), _p(st), _p(it),
+                                                          C.byref(ms)))
+        self.last_ms = ms.value
+        return dict(H=H[:P].reshape(P, 3, 3), masks=[mask[off[p]:off[p + 1]].copy() for p in range(P)], n_inliers=ninl[:P], status=st[:P],
+                    iterations=it[:P])
+
+    def homography_record_counts(self, counts_cap):
+        """record the inlier count of each of the first counts_cap iterations in the following calls (0: none, the default)"""
+        self._ck(self.lib.dynofront_homography_record_counts(self.h, int(counts_cap)))
+
+    def homography_trace(self, counts_cap=0):
+        """the draw trace of the last find_homography_batch / klt_track_points: status, groups, rejected, best (iteration of the
+        best model) per problem, and counts [P][counts_cap] (inlier count per iteration as recorded after
+        homography_record_counts; -1 without a model, past the end or not recorded)"""
+        npb = C.c_int32()
+        self._ck(self.lib.dynofront_homography_last_trace(self.h, None, None, None, None, 0, None, C.byref(npb)))
+        P = npb.value; m = max(P, 1)
+        st = np.zeros(m, np.int32); g = np.zeros(m, np.int32); rj = np.zeros(m, np.int32); b = np.zeros(m, np.int32)
+        cnt = np.zeros((m, max(counts_cap, 1)), np.int32)
+        self._ck(self.lib.dynofront_homography_last_trace(self.h, _p(st), _p(g), _p(rj), _p(b), int(counts_cap), _p(cnt) if counts_cap else None,
+                                                          C.byref(npb)))
+        return dict(status=st[:P], groups=g[:P], rejected=rj[:P], best=b[:P], counts=cnt[:P, :counts_cap])
 
     def stereo_track(self, left_gray, right_gray, left_pts, fx, baseline):
         """FeatureTracker::stereoTrack without its RANSAC: (right_pts, status, depth, valid)"""

@@ -11,6 +11,7 @@
 #include <cuda_runtime.h>
 #include <math_constants.h>
 #include <algorithm>
+#include <cfloat>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -76,6 +77,9 @@ struct dynofront_ctx {
   DevBuf<double> depth; bool has_frame = false, has_depth = false;
   DevBuf<double> dp_kp, dp_depth, dp_right, dp_point, dp_stereo; DevBuf<int32_t> dp_lab, dp_index; DevBuf<uint8_t> dp_flag, dp_out; DevBuf<int> dp_cnt;
   DevBuf<float> dc_xyz; DevBuf<uint8_t> dc_rgb, dc_valid; DevBuf<uint32_t> dc_label;
+  // homography RANSAC: inputs, point / inlier lists, outputs, per-problem statistics (6 arrays of hm_np) and per-iteration counts
+  DevBuf<int> hm_off, hm_cidx, hm_lidx, hm_stat, hm_counts; DevBuf<float> hm_src, hm_dst; DevBuf<float4> hm_inl; DevBuf<double> hm_H; DevBuf<uint8_t> hm_mask;
+  int hm_np = 0, hm_cap = 0, hm_record = 0;       // problems and recorded iterations of the last call; iterations to record
   cudaEvent_t e0 = nullptr, e1 = nullptr;
 };
 // grows each (buffer, element count) pair in turn; 0, or -3 with the error at the first allocation that fails
@@ -1153,6 +1157,454 @@ __global__ void dc_kernel(size_t npx, int W, const double* __restrict__ depth, c
   if (threadIdx.x == 0 && nv) atomicAdd(count, nv);
 }
 
+// ---------------------------------------------------------------------------------------------------- homography RANSAC
+// cv::findHomography(src, dst, RANSAC, thr, mask, max_iters, confidence) as KltFeatureTracker::geometricVerification calls it
+// (StaticFeatureTracker.cc:627-639), one persistent CTA per problem.  OpenCV's orders, pinned against cv2 by tests/test_homography.py
+// (tests/homography_oracle.py restates them):
+//  * draws: cv::RNG((uint64)-1) (multiply-with-carry), uniform(0, n) = next() % n, groups of 4 distinct indices with duplicates
+//    re-drawn at once.  The split of the stream into groups does not depend on the subset test, so one lane cuts a chunk of
+//    groups and the subset tests and 4-point models run in parallel, one thread per group;
+//  * an iteration takes groups until one passes checkSubset; 10 000 rejections in a row end the loop (fail it in iteration 0);
+//  * model: runKernel (centroid / mean absolute deviation normalisation, LtL summed in point order, OpenCV's Jacobi, the
+//    eigenvector of the smallest eigenvalue, invHnorm * H0 * Hnorm2, times 1 / H22); error in float with H cast to float;
+//  * thread 0 replays the sequential best-model / RANSACUpdateNumIters loop over each chunk's counts, so nothing depends on the
+//    chunk size (32, 64, 128, then 256 groups);
+//  * after RANSAC: in-order compaction of the inliers, runKernel over them (each of the 4 centroid / deviation sums and the 45 LtL
+//    sums sequential in point order on one lane), OpenCV 4's 10-step Levenberg-Marquardt control over the 8 free entries (normal
+//    equations by a fixed-order block reduction, a Cholesky solve, lambda from the host's C library), H / H22, and the returned
+//    mask recomputed as err(H) <= thr^2 over all points.
+// The problem's points are the rows of [off[p], off[p+1]) whose sel is non-zero (all rows without sel), in row order; the mask is
+// written at the rows (0 on unselected rows).
+#define HOM_THREADS 256
+#define HOM_WARPS (HOM_THREADS/32)
+#define HOM_CHUNK 256
+#define HOM_MAX_ATTEMPTS 10000
+#define HOM_NRED 45                      // 36 entries of the upper triangle of J^T J, 8 of J^T r, S
+enum { HOM_OK = 0, HOM_TOO_FEW = 1, HOM_FOUR_POINT = 2, HOM_RANSAC_FAILED = 3 };
+
+struct HomBatch {
+  const int* off; const float* src; const float* dst; const uint8_t* sel;
+  int* cidx; int* lidx;                  // per row: the problem's point list (row of each rank), then its inlier list (ranks)
+  float4* inl;                           // per row: the inliers gathered in order (src x, src y, dst x, dst y)
+  float thr2; double conf; int max_iters, refine;
+  double* H; uint8_t* mask; int* n_inl; int* status; int* iters; int* groups; int* rejected; int* best;
+  int* counts; int counts_cap;           // per-iteration inlier counts (parity hook), the first counts_cap iterations; NULL: none
+  double lam[33];                        // the LM's lambda = exp(lg * log(10.)), lg = -16 .. 16, from the host's C library as OpenCV
+};
+
+__device__ __forceinline__ double cv_hypot(double a, double b) {      // OpenCV lapack.cpp hypot
+  a = fabs(a); b = fabs(b);
+  if (a > b) { b /= a; return a*sqrt(1 + b*b); }
+  if (b > 0) { a /= b; return b*sqrt(1 + a*a); }
+  return 0;
+}
+// cv::eigen of the symmetric 9x9 A (upper triangle read, destroyed) by JacobiImpl_; returns the row of V holding the eigenvector of
+// the smallest eigenvalue after OpenCV's descending selection sort (tracked as a permutation instead of swapping rows).
+__device__ int cv_jacobi9(double* A, double* V) {
+  const int n = 9; double W[9]; int indR[9], indC[9];
+  for (int i = 0; i < n; i++) for (int j = 0; j < n; j++) V[i*n + j] = i == j ? 1.0 : 0.0;
+  for (int k = 0; k < n; k++) {
+    W[k] = A[(n + 1)*k];
+    if (k < n - 1) { int m = k + 1; double mv = fabs(A[n*k + m]); for (int i = k + 2; i < n; i++) { const double v = fabs(A[n*k + i]); if (mv < v) mv = v, m = i; } indR[k] = m; }
+    if (k > 0) { int m = 0; double mv = fabs(A[k]); for (int i = 1; i < k; i++) { const double v = fabs(A[n*i + k]); if (mv < v) mv = v, m = i; } indC[k] = m; }
+  }
+  for (int iters = 0; iters < n*n*30; iters++) {
+    int k = 0; double mv = fabs(A[indR[0]]);
+    for (int i = 1; i < n - 1; i++) { const double v = fabs(A[n*i + indR[i]]); if (mv < v) mv = v, k = i; }
+    int l = indR[k];
+    for (int i = 1; i < n; i++) { const double v = fabs(A[n*indC[i] + i]); if (mv < v) mv = v, k = indC[i], l = i; }
+    const double p = A[n*k + l];
+    if (fabs(p) <= DBL_EPSILON) break;
+    const double y = (W[l] - W[k])*0.5;
+    double t = fabs(y) + cv_hypot(p, y);
+    double s = cv_hypot(p, t);
+    const double c = t/s;
+    s = p/s; t = (p/t)*p;
+    if (y < 0) s = -s, t = -t;
+    A[n*k + l] = 0;
+    W[k] -= t; W[l] += t;
+    double a0, b0;
+#define HOM_ROT(v0, v1) a0 = v0, b0 = v1, v0 = a0*c - b0*s, v1 = a0*s + b0*c
+    for (int i = 0; i < k; i++) HOM_ROT(A[n*i + k], A[n*i + l]);
+    for (int i = k + 1; i < l; i++) HOM_ROT(A[n*k + i], A[n*i + l]);
+    for (int i = l + 1; i < n; i++) HOM_ROT(A[n*k + i], A[n*l + i]);
+    for (int i = 0; i < n; i++) HOM_ROT(V[n*k + i], V[n*l + i]);
+#undef HOM_ROT
+    for (int j = 0; j < 2; j++) {
+      const int idx = j == 0 ? k : l;
+      if (idx < n - 1) { int m = idx + 1; double mv2 = fabs(A[n*idx + m]); for (int i = idx + 2; i < n; i++) { const double v = fabs(A[n*idx + i]); if (mv2 < v) mv2 = v, m = i; } indR[idx] = m; }
+      if (idx > 0) { int m = 0; double mv2 = fabs(A[idx]); for (int i = 1; i < idx; i++) { const double v = fabs(A[n*i + idx]); if (mv2 < v) mv2 = v, m = i; } indC[idx] = m; }
+    }
+  }
+  int perm[9]; for (int i = 0; i < n; i++) perm[i] = i;
+  for (int k = 0; k < n - 1; k++) {
+    int m = k; for (int i = k + 1; i < n; i++) if (W[m] < W[i]) m = i;
+    if (k != m) { const double w = W[m]; W[m] = W[k]; W[k] = w; const int q = perm[m]; perm[m] = perm[k]; perm[k] = q; }
+  }
+  return perm[n - 1];
+}
+// the tail of runKernel: Jacobi on LtL (upper triangle), H = invHnorm * H0 * Hnorm2, times 1 / H22
+__device__ void hom_from_ltl(double* L, const double c[4], const double s[4], double* H) {
+  // c = (cm.x, cm.y, cM.x, cM.y), s = (sm.x, sm.y, sM.x, sM.y) after s = count / sum
+  double V[81];
+  const int r = cv_jacobi9(L, V);
+  const double* H0 = V + 9*r;
+  const double inv[9] = {1./s[0], 0, c[0], 0, 1./s[1], c[1], 0, 0, 1};
+  const double h2[9] = {s[2], 0, -c[2]*s[2], 0, s[3], -c[3]*s[3], 0, 0, 1};
+  double T[9];
+  for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) T[3*i + j] = (inv[3*i]*H0[j] + inv[3*i + 1]*H0[3 + j]) + inv[3*i + 2]*H0[6 + j];
+  double R[9];
+  for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) R[3*i + j] = (T[3*i]*h2[j] + T[3*i + 1]*h2[3 + j]) + T[3*i + 2]*h2[6 + j];
+  const double sc = 1./R[8];
+  for (int e = 0; e < 9; e++) H[e] = R[e]*sc;
+}
+__device__ __forceinline__ void hom_ltl_add(double* L, double x, double y, double X, double Y) {
+  const double Lx[9] = {X, Y, 1, 0, 0, 0, -x*X, -x*Y, -x}, Ly[9] = {0, 0, 0, X, Y, 1, -y*X, -y*Y, -y};
+  for (int j = 0; j < 9; j++) for (int k = j; k < 9; k++) L[9*j + k] += Lx[j]*Lx[k] + Ly[j]*Ly[k];
+}
+// runKernel on 4 correspondences (one thread); false = no model
+__device__ bool hom_kernel4(const float* Ms, const float* ms, double* H) {
+  double c[4] = {0, 0, 0, 0}, s[4] = {0, 0, 0, 0};
+  for (int i = 0; i < 4; i++) { c[0] += ms[2*i]; c[1] += ms[2*i + 1]; c[2] += Ms[2*i]; c[3] += Ms[2*i + 1]; }
+  for (int e = 0; e < 4; e++) c[e] /= 4;
+  for (int i = 0; i < 4; i++) {
+    s[0] += fabs(ms[2*i] - c[0]); s[1] += fabs(ms[2*i + 1] - c[1]); s[2] += fabs(Ms[2*i] - c[2]); s[3] += fabs(Ms[2*i + 1] - c[3]);
+  }
+  for (int e = 0; e < 4; e++) if (fabs(s[e]) < DBL_EPSILON) return false;
+  for (int e = 0; e < 4; e++) s[e] = 4/s[e];
+  double L[81];
+  for (int e = 0; e < 81; e++) L[e] = 0;
+  for (int i = 0; i < 4; i++)
+    hom_ltl_add(L, (ms[2*i] - c[0])*s[0], (ms[2*i + 1] - c[1])*s[1], (Ms[2*i] - c[2])*s[2], (Ms[2*i + 1] - c[3])*s[3]);
+  hom_from_ltl(L, c, s, H);
+  return true;
+}
+__device__ bool hom_collinear(const float* p) {       // haveCollinearPoints(ms, 4): float differences, double products
+  for (int j = 0; j < 3; j++) {
+    const double dx1 = p[2*j] - p[6], dy1 = p[2*j + 1] - p[7];
+    for (int k = 0; k < j; k++) {
+      const double dx2 = p[2*k] - p[6], dy2 = p[2*k + 1] - p[7];
+      if (fabs(dx2*dy1 - dy2*dx1) <= FLT_EPSILON*(fabs(dx1) + fabs(dy1) + fabs(dx2) + fabs(dy2))) return true;
+    }
+  }
+  return false;
+}
+__device__ __forceinline__ double hom_det3(const float* p, int a, int b, int c) {   // determinant(Matx33d) of rows (x, y, 1)
+  const double a00 = p[2*a], a01 = p[2*a + 1], a10 = p[2*b], a11 = p[2*b + 1], a20 = p[2*c], a21 = p[2*c + 1];
+  return a00*(a11*1.0 - a21*1.0) - a01*(a10*1.0 - a20*1.0) + 1.0*(a10*a21 - a20*a11);
+}
+__device__ bool hom_check_subset(const float* S, const float* D) {
+  if (hom_collinear(S) || hom_collinear(D)) return false;
+  const int tt[4][3] = {{0, 1, 2}, {1, 2, 3}, {0, 2, 3}, {0, 1, 3}};
+  int neg = 0;
+  for (int i = 0; i < 4; i++) neg += hom_det3(S, tt[i][0], tt[i][1], tt[i][2])*hom_det3(D, tt[i][0], tt[i][1], tt[i][2]) < 0;
+  return neg == 0 || neg == 4;
+}
+__device__ __forceinline__ float hom_err(const float* Hf, float x, float y, float u, float v) {   // computeError
+  const float ww = 1.f/(Hf[6]*x + Hf[7]*y + 1.f);
+  const float dx = (Hf[0]*x + Hf[1]*y + Hf[2])*ww - u, dy = (Hf[3]*x + Hf[4]*y + Hf[5])*ww - v;
+  return dx*dx + dy*dy;
+}
+// RANSACUpdateNumIters(p, ep, 4, niters)
+__device__ int hom_update_iters(double p, double ep, int max_iters) {
+  p = fmin(fmax(p, 0.), 1.); ep = fmin(fmax(ep, 0.), 1.);
+  double num = fmax(1. - p, DBL_MIN), denom = 1. - pow(1. - ep, 4.0);
+  if (denom < DBL_MIN) return 0;
+  num = log(num); denom = log(denom);
+  return denom >= 0 || -num >= max_iters*(-denom) ? max_iters : __double2int_rn(num/denom);
+}
+// HomographyRefineCallback::compute for one correspondence: residuals (2) and, with J, the two Jacobian rows
+__device__ __forceinline__ void hom_resid(const double* h, double Mx, double My, double mx, double my, double* r, double* J) {
+  double ww = h[6]*Mx + h[7]*My + 1.;
+  ww = fabs(ww) > DBL_EPSILON ? 1./ww : 0;
+  const double xi = (h[0]*Mx + h[1]*My + h[2])*ww, yi = (h[3]*Mx + h[4]*My + h[5])*ww;
+  r[0] = xi - mx; r[1] = yi - my;
+  if (J) {
+    J[0] = Mx*ww; J[1] = My*ww; J[2] = ww; J[3] = J[4] = J[5] = 0.; J[6] = -Mx*ww*xi; J[7] = -My*ww*xi;
+    J[8] = J[9] = J[10] = 0.; J[11] = Mx*ww; J[12] = My*ww; J[13] = ww; J[14] = -Mx*ww*yi; J[15] = -My*ww*yi;
+  }
+}
+// block-wide sum of NV doubles per thread in a fixed order (warp butterflies, then warps in order on thread 0) into out
+template <int NV> __device__ void hom_block_sum(double* v, double (*red)[HOM_NRED], double* out) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int e = 0; e < NV; e++) {
+    double x = v[e];
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    v[e] = x;
+  }
+  if (lane == 0) for (int e = 0; e < NV; e++) red[warp][e] = v[e];
+  __syncthreads();
+  if (threadIdx.x == 0) for (int e = 0; e < NV; e++) { double x = red[0][e]; for (int w = 1; w < HOM_WARPS; w++) x += red[w][e]; out[e] = x; }
+  __syncthreads();
+}
+// in-order compaction inside the CTA: out[k] = value(i) of the k-th i in [0, n) with flag(i); returns the count (all threads)
+template <class F, class G> __device__ int hom_compact(int n, F flag, G value, int* out, int* sh_wcnt) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int base = 0;
+  for (int i0 = 0; i0 < n; i0 += HOM_THREADS) {
+    const int i = i0 + threadIdx.x;
+    const bool f = i < n && flag(i);
+    const unsigned b = __ballot_sync(0xffffffffu, f);
+    if (lane == 0) sh_wcnt[warp] = __popc(b);
+    __syncthreads();
+    int before = base;
+    for (int w = 0; w < warp; w++) before += sh_wcnt[w];
+    if (f) out[before + __popc(b & ((1u << lane) - 1))] = value(i);
+    int tot = 0; for (int w = 0; w < HOM_WARPS; w++) tot += sh_wcnt[w];
+    base += tot;
+    __syncthreads();
+  }
+  return base;
+}
+
+__global__ void __launch_bounds__(HOM_THREADS) hom_ransac_kernel(HomBatch B) {
+  __shared__ int sh_grp[HOM_CHUNK][4];
+  __shared__ int sh_cnt[HOM_CHUNK];              // -2: rejected by the subset test, -1: no model, else the inlier count
+  __shared__ double sh_H[HOM_CHUNK][9];
+  __shared__ float4 sh_tile[HOM_THREADS];        // (src x, src y, dst x, dst y)
+  __shared__ double sh_red[HOM_WARPS][HOM_NRED];
+  __shared__ double sh_best[9], sh_x[9], sh_xd[9], sh_sum[HOM_NRED], sh_A[64], sh_v[8], sh_S, sh_Sd, sh_c[4], sh_s[4], sh_L[81];
+  __shared__ int sh_wcnt[HOM_WARPS];
+  __shared__ unsigned long long sh_rng;
+  __shared__ int sh_it, sh_niters, sh_best_cnt, sh_best_it, sh_groups, sh_rej, sh_run, sh_done, sh_fail, sh_ninl, sh_ok, sh_lm_go;
+  const int pb = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int r0 = B.off[pb], nrows = B.off[pb + 1] - r0;
+  int* cidx = B.cidx + r0; int* lidx = B.lidx + r0;
+  const float2* src = reinterpret_cast<const float2*>(B.src); const float2* dst = reinterpret_cast<const float2*>(B.dst);
+  for (int i = t; i < nrows; i += HOM_THREADS) B.mask[r0 + i] = 0;
+  const uint8_t* sel = B.sel;
+  const int n = sel ? hom_compact(nrows, [&](int i) { return sel[r0 + i] != 0; }, [&](int i) { return r0 + i; }, cidx, sh_wcnt)
+                    : hom_compact(nrows, [&](int) { return true; }, [&](int i) { return r0 + i; }, cidx, sh_wcnt);
+  double* Hout = B.H + 9*(size_t)pb;
+  if (n < 4) {                                   // geometricVerification: fewer than 4 points are all inliers
+    for (int i = t; i < n; i += HOM_THREADS) B.mask[cidx[i]] = 1;
+    if (t < 9) Hout[t] = 0;
+    if (t == 0) { B.status[pb] = HOM_TOO_FEW; B.n_inl[pb] = n; B.iters[pb] = 0; B.groups[pb] = 0; B.rejected[pb] = 0; B.best[pb] = -1; }
+    return;
+  }
+  if (n == 4) {                                  // findHomography: runKernel only, no RANSAC and no refinement
+    if (t == 0) {
+      float Ms[8], ms[8];
+      for (int i = 0; i < 4; i++) { const float2 a = src[cidx[i]], b = dst[cidx[i]]; Ms[2*i] = a.x; Ms[2*i + 1] = a.y; ms[2*i] = b.x; ms[2*i + 1] = b.y; }
+      double H[9]; const bool ok = hom_kernel4(Ms, ms, H);
+      for (int e = 0; e < 9; e++) Hout[e] = ok ? H[e] : 0;
+      for (int i = 0; i < 4; i++) B.mask[cidx[i]] = ok ? 1 : 0;
+      B.status[pb] = HOM_FOUR_POINT; B.n_inl[pb] = ok ? 4 : 0; B.iters[pb] = 0; B.groups[pb] = 0; B.rejected[pb] = 0; B.best[pb] = -1;
+    }
+    return;
+  }
+  if (t == 0) {
+    sh_rng = ~0ull; sh_it = 0; sh_niters = max(B.max_iters, 1); sh_best_cnt = 0; sh_best_it = -1; sh_groups = 0; sh_rej = 0; sh_run = 0;
+    sh_done = 0; sh_fail = 0;
+  }
+  __syncthreads();
+  int* counts = B.counts ? B.counts + (size_t)pb*B.counts_cap : nullptr;
+  for (int c = 0; !sh_done; c++) {
+    const int nch = min(HOM_CHUNK, 32 << min(c, 3));
+    if (t == 0) {                                // the draw stream, cut into groups of 4 distinct indices
+      unsigned long long st = sh_rng;
+      for (int g = 0; g < nch; g++)
+        for (int i = 0; i < 4;) {
+          st = (unsigned long long)(unsigned)st*4164903690ull + (st >> 32);
+          const int k = (int)((unsigned)st % (unsigned)n);
+          bool dup = false; for (int j = 0; j < i; j++) dup |= sh_grp[g][j] == k;
+          if (!dup) sh_grp[g][i++] = k;
+        }
+      sh_rng = st;
+    }
+    __syncthreads();
+    if (t < nch) {                               // subset test and 4-point model, one thread per group
+      float Ms[8], ms[8];
+      for (int i = 0; i < 4; i++) { const int r = cidx[sh_grp[t][i]]; const float2 a = src[r], b = dst[r]; Ms[2*i] = a.x; Ms[2*i + 1] = a.y; ms[2*i] = b.x; ms[2*i + 1] = b.y; }
+      int cnt = -2;
+      if (hom_check_subset(Ms, ms)) cnt = hom_kernel4(Ms, ms, sh_H[t]) ? 0 : -1;
+      sh_cnt[t] = cnt;
+    }
+    for (int tile0 = 0; tile0 < n; tile0 += HOM_THREADS) {    // inlier counts, points staged through shared memory
+      const int tn = min(HOM_THREADS, n - tile0);
+      __syncthreads();
+      if (t < tn) { const int r = cidx[tile0 + t]; const float2 a = src[r], b = dst[r]; sh_tile[t] = make_float4(a.x, a.y, b.x, b.y); }
+      __syncthreads();
+      for (int m = warp; m < nch; m += HOM_WARPS) {
+        if (sh_cnt[m] < 0) continue;
+        float Hf[8]; for (int e = 0; e < 8; e++) Hf[e] = (float)sh_H[m][e];
+        int cnt = 0;
+        for (int j0 = 0; j0 < tn; j0 += 32) {
+          const int j = j0 + lane;
+          bool in = false;
+          if (j < tn) { const float4 q = sh_tile[j]; in = hom_err(Hf, q.x, q.y, q.z, q.w) <= B.thr2; }
+          cnt += __popc(__ballot_sync(0xffffffffu, in));
+        }
+        if (lane == 0) sh_cnt[m] += cnt;
+      }
+    }
+    __syncthreads();
+    if (t == 0) {                                // the sequential loop of RANSACPointSetRegistrator::run over this chunk
+      int it = sh_it, niters = sh_niters, best = sh_best_cnt, run = sh_run, groups = sh_groups, rej = sh_rej;
+      bool done = false;
+      for (int m = 0; m < nch; m++) {
+        groups++;
+        if (sh_cnt[m] == -2) {
+          rej++;
+          if (++run >= HOM_MAX_ATTEMPTS) { done = true; if (it == 0) sh_fail = 1; break; }
+          continue;
+        }
+        run = 0;
+        const int cnt = sh_cnt[m];
+        if (counts && it < B.counts_cap) counts[it] = cnt;
+        if (cnt > max(best, 3)) {
+          best = cnt; sh_best_it = it;
+          for (int e = 0; e < 9; e++) sh_best[e] = sh_H[m][e];
+          niters = hom_update_iters(B.conf, (double)(n - cnt)/n, niters);
+        }
+        if (++it >= niters) { done = true; break; }
+      }
+      sh_it = it; sh_niters = niters; sh_best_cnt = best; sh_run = run; sh_groups = groups; sh_rej = rej; sh_done = done;
+    }
+    __syncthreads();
+  }
+  const bool model = !sh_fail && sh_best_cnt > 0;
+  if (!model) {                                  // RANSAC failed: no H, all zeros
+    if (t < 9) Hout[t] = 0;
+    if (t == 0) { B.status[pb] = HOM_RANSAC_FAILED; B.n_inl[pb] = 0; B.iters[pb] = sh_fail ? 0 : sh_it; B.groups[pb] = sh_groups; B.rejected[pb] = sh_rej; B.best[pb] = -1; }
+    return;
+  }
+  if (B.refine) {
+    // the RANSAC mask, compacted in order (ranks)
+    float Hb[8]; for (int e = 0; e < 8; e++) Hb[e] = (float)sh_best[e];
+    const int m = hom_compact(n, [&](int i) { const float2 a = src[cidx[i]], b = dst[cidx[i]]; return hom_err(Hb, a.x, a.y, b.x, b.y) <= B.thr2; },
+                              [&](int i) { return i; }, lidx, sh_wcnt);
+    float4* Q = B.inl + r0;                     // the inliers, gathered in order: the sequential sums below read them contiguously
+    for (int i = t; i < m; i += HOM_THREADS) { const int r = cidx[lidx[i]]; const float2 a = src[r], b = dst[r]; Q[i] = make_float4(a.x, a.y, b.x, b.y); }
+    __syncthreads();
+    // runKernel over the inliers: 4 centroid sums, 4 deviation sums, then the 45 LtL sums, each sequential in point order on one lane
+    auto coord = [](const float4& q, int e) { return e == 0 ? q.z : e == 1 ? q.w : e == 2 ? q.x : q.y; };   // (m.x, m.y, M.x, M.y)
+    if (t < 4) {
+      double a = 0;
+      for (int i = 0; i < m; i++) a += coord(Q[i], t);
+      sh_c[t] = a/m;
+    }
+    __syncthreads();
+    if (t < 4) {
+      double a = 0; const double cc = sh_c[t];
+      for (int i = 0; i < m; i++) a += fabs(coord(Q[i], t) - cc);
+      sh_s[t] = a;
+    }
+    __syncthreads();
+    const bool ok = fabs(sh_s[0]) >= DBL_EPSILON && fabs(sh_s[1]) >= DBL_EPSILON && fabs(sh_s[2]) >= DBL_EPSILON && fabs(sh_s[3]) >= DBL_EPSILON;
+    if (ok) {
+      double s[4]; for (int e = 0; e < 4; e++) s[e] = m/sh_s[e];
+      if (t < HOM_NRED) {
+        int j = 0, k = t; while (k >= 9 - j) { k -= 9 - j; j++; } k += j;        // t -> (j, k), k >= j
+        double a = 0;
+        for (int i = 0; i < m; i++) {
+          const float4 q = Q[i];
+          const double x = (q.z - sh_c[0])*s[0], y = (q.w - sh_c[1])*s[1], X = (q.x - sh_c[2])*s[2], Y = (q.y - sh_c[3])*s[3];
+          const double Lx[9] = {X, Y, 1, 0, 0, 0, -x*X, -x*Y, -x}, Ly[9] = {0, 0, 0, X, Y, 1, -y*X, -y*Y, -y};
+          a += Lx[j]*Lx[k] + Ly[j]*Ly[k];
+        }
+        sh_L[9*j + k] = a;
+      }
+      __syncthreads();
+      if (t == 0) { double c4[4] = {sh_c[0], sh_c[1], sh_c[2], sh_c[3]}; hom_from_ltl(sh_L, c4, s, sh_x); }
+    } else if (t < 9) sh_x[t] = sh_best[t];       // (runKernel's result is not checked: H stays the RANSAC model)
+    __syncthreads();
+    // Levenberg-Marquardt over H[0..7] (OpenCV 4 LMSolver, 10 steps): J^T J, J^T r and S by a fixed-order block reduction
+    int lg = -3, it = 0;
+    auto normal_eq = [&](const double* h) {
+      double acc[HOM_NRED]; for (int e = 0; e < HOM_NRED; e++) acc[e] = 0;
+      for (int i = t; i < m; i += HOM_THREADS) {
+        const float4 q = Q[i];
+        double rr[2], J[16]; hom_resid(h, q.x, q.y, q.z, q.w, rr, J);
+        for (int row = 0; row < 2; row++) {
+          const double* Jr = J + 8*row; int e = 0;
+          for (int a = 0; a < 8; a++) for (int b = a; b < 8; b++) acc[e++] += Jr[a]*Jr[b];
+          for (int a = 0; a < 8; a++) acc[36 + a] += Jr[a]*rr[row];
+          acc[44] += rr[row]*rr[row];
+        }
+      }
+      hom_block_sum<HOM_NRED>(acc, sh_red, sh_sum);
+      if (t == 0) {
+        int e = 0;
+        for (int a = 0; a < 8; a++) for (int b = a; b < 8; b++) { sh_A[8*a + b] = sh_sum[e]; sh_A[8*b + a] = sh_sum[e]; e++; }
+        for (int a = 0; a < 8; a++) sh_v[a] = sh_sum[36 + a];
+        sh_S = sh_sum[44];
+      }
+      __syncthreads();
+    };
+    normal_eq(sh_x);
+    for (;;) {
+      double dmax = 0;
+      if (t == 0) {                              // (A + lambda diag A) d = v by Cholesky, xd = x - d
+        const double lambda = B.lam[lg + 16];
+        double Ap[64], d[8];
+        for (int e = 0; e < 64; e++) Ap[e] = sh_A[e];
+        for (int a = 0; a < 8; a++) Ap[9*a] *= 1 + lambda;
+        for (int j = 0; j < 8; j++) {
+          double s = Ap[9*j]; for (int k = 0; k < j; k++) s -= Ap[8*j + k]*Ap[8*j + k];
+          const double lj = sqrt(fmax(s, 0.0)); Ap[9*j] = lj;
+          for (int i = j + 1; i < 8; i++) { double q = Ap[8*i + j]; for (int k = 0; k < j; k++) q -= Ap[8*i + k]*Ap[8*j + k]; Ap[8*i + j] = lj > 0 ? q/lj : 0; }
+        }
+        for (int i = 0; i < 8; i++) { double q = sh_v[i]; for (int k = 0; k < i; k++) q -= Ap[8*i + k]*d[k]; d[i] = Ap[9*i] > 0 ? q/Ap[9*i] : 0; }
+        for (int i = 7; i >= 0; i--) { double q = d[i]; for (int k = i + 1; k < 8; k++) q -= Ap[8*k + i]*d[k]; d[i] = Ap[9*i] > 0 ? q/Ap[9*i] : 0; }
+        for (int e = 0; e < 8; e++) { sh_xd[e] = sh_x[e] - d[e]; dmax = fmax(dmax, fabs(d[e])); }
+        sh_xd[8] = sh_x[8];
+      }
+      __syncthreads();
+      {
+        double acc[1] = {0};
+        for (int i = t; i < m; i += HOM_THREADS) {
+          const float4 q = Q[i];
+          double rr[2]; hom_resid(sh_xd, q.x, q.y, q.z, q.w, rr, nullptr);
+          acc[0] += rr[0]*rr[0]; acc[0] += rr[1]*rr[1];
+        }
+        hom_block_sum<1>(acc, sh_red, &sh_Sd);
+      }
+      bool better = false;
+      if (t == 0) {
+        better = sh_Sd < sh_S;
+        if (better) { lg = max(lg - 1, -16); it++; for (int e = 0; e < 9; e++) sh_x[e] = sh_xd[e]; }
+        else { it += lg == 16; lg = min(lg + 1, 16); }
+        sh_ok = better;
+      }
+      __syncthreads();
+      if (sh_ok) normal_eq(sh_x);                // (S becomes Sd)
+      if (t == 0) sh_lm_go = it < 10 && dmax >= FLT_EPSILON && sh_S >= (double)FLT_EPSILON*FLT_EPSILON;
+      __syncthreads();
+      if (!sh_lm_go) break;
+    }
+    if (t == 0) {
+      const double sc = fabs(sh_x[8]) > FLT_EPSILON ? 1./sh_x[8] : 1.;
+      for (int e = 0; e < 9; e++) sh_best[e] = sh_x[e]*sc;
+    }
+    __syncthreads();
+  }
+  // the returned mask: err(H) <= thr^2 over all points
+  if (t == 0) sh_ninl = 0;
+  __syncthreads();
+  float Hf[8]; for (int e = 0; e < 8; e++) Hf[e] = (float)sh_best[e];
+  int cnt = 0;
+  for (int i = t; i < n; i += HOM_THREADS) {
+    const int r = cidx[i]; const float2 a = src[r], b = dst[r];
+    const bool in = hom_err(Hf, a.x, a.y, b.x, b.y) <= B.thr2;
+    B.mask[r] = in; cnt += in;
+  }
+  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if (lane == 0) atomicAdd(&sh_ninl, cnt);
+  __syncthreads();
+  if (t < 9) Hout[t] = sh_best[t];
+  if (t == 0) { B.status[pb] = HOM_OK; B.n_inl[pb] = sh_ninl; B.iters[pb] = sh_it; B.groups[pb] = sh_groups; B.rejected[pb] = sh_rej; B.best[pb] = sh_best_it; }
+}
+// klt_track_points: verified = the homography mask (0 on rows the forward-backward test dropped), keep = keep && verified
+__global__ void ktp_post_kernel(int n, const uint8_t* __restrict__ verified, uint8_t* __restrict__ keep, int check, int* __restrict__ count) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const bool v = verified[i] != 0;
+  if (check) keep[i] = keep[i] && v;
+  if (v) atomicAdd(count, 1);
+  if (check && keep[i]) atomicAdd(count + 1, 1);
+}
+
 // ---------------------------------------------------------------------------------------------------- host API
 extern "C" {
 
@@ -1646,6 +2098,8 @@ int dynofront_klt_track(dynofront_handle h, const uint8_t* prev_gray, const uint
   return 0;
 }
 
+static int klt_fb_stages(dynofront_ctx* h, bool resident, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n, const float* prev_pts,
+                         const float* next_pts, const dynofront_klt_fb_params* P, const int32_t* prev_age);
 int dynofront_klt_track_fb(dynofront_handle h, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n, const float* prev_pts, float* next_pts,
                            uint8_t* status, float* back_pts, const dynofront_klt_fb_params* P, const int32_t* prev_age, uint8_t* keep,
                            int32_t* n_status, int32_t* n_keep, float* ms_device) {
@@ -1655,6 +2109,24 @@ int dynofront_klt_track_fb(dynofront_handle h, const uint8_t* prev_gray, const u
   if (resident && !(h->have_pyr && h->have_pyr_cur)) { h->err = "two frames are needed on the device"; return -2; }
   if (P->win < 3 || P->win > KLT_MAXWIN || P->win_back < 3 || P->win_back > KLT_MAXWIN || P->max_level < 0 || P->max_level_back < 0) { h->err = "win must be in [3,31]"; return -1; }
   if (P->check_static && (!prev_age || !keep)) { h->err = "check_static needs prev_age and keep"; return -1; }
+  if (int rc = klt_fb_stages(h, resident, prev_gray, cur_gray, n, prev_pts, next_pts, P, prev_age)) return rc;
+  int counts[2] = {0, 0};
+  FCK(cudaMemcpyAsync(next_pts, h->k_next, 2*(size_t)n*4, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(status, h->k_st, n, cudaMemcpyDeviceToHost, h->s));
+  if (back_pts) FCK(cudaMemcpyAsync(back_pts, h->k_back, 2*(size_t)n*4, cudaMemcpyDeviceToHost, h->s));
+  if (keep) FCK(cudaMemcpyAsync(keep, h->k_keep, n, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(counts, h->k_count, sizeof(counts), cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  FCK(cudaGetLastError());
+  if (n_status) *n_status = counts[0]; if (n_keep) *n_keep = counts[1];
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+
+// the device stages of dynofront_klt_track_fb, queued from event e0 on: status in k_st, keep in k_keep, counts in k_count
+static int klt_fb_stages(dynofront_ctx* h, bool resident, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n, const float* prev_pts,
+                         const float* next_pts, const dynofront_klt_fb_params* P, const int32_t* prev_age) {
   cudaSetDevice(h->dev);
   const int lf = klt_top_level(h, P->max_level, P->win), lb = klt_top_level(h, P->max_level_back, P->win_back), lmax = std::max(lf, lb);
   const size_t cap = feature_cap(n);
@@ -1688,16 +2160,130 @@ int dynofront_klt_track_fb(dynofront_handle h, const uint8_t* prev_gray, const u
   klt_launch(h, LB, n, h->k_next, h->k_back, h->k_st2, P->win_back, P->max_count_back, P->epsilon_back, 0, min_eig, nullptr);
   if (n > 0) klt_fb_filter_kernel<<<(n + 255)/256, 256, 0, h->s>>>(n, h->k_prev, h->k_next, h->k_back, h->k_st, h->k_st2, (float)P->max_fb_distance, h->k_st,
                                                                   P->check_static, h->mask, h->W, h->H, P->track, h->k_age, P->max_feature_track_age, h->k_keep, h->k_count);
-  int counts[2] = {0, 0};
+  return 0;
+}
+
+// ---- homography RANSAC
+void dynofront_homography_default_params(dynofront_homography_params* p) {
+  if (!p) return;
+  p->threshold_px = 5.0; p->confidence = 0.995; p->max_iters = 2000; p->refine = 1;      // StaticFeatureTracker.cc:632, OpenCV defaults
+}
+static int hom_check_params(dynofront_ctx* h, const dynofront_homography_params& P) {
+  if (!(P.threshold_px > 0) || !std::isfinite(P.threshold_px) || !(P.confidence > 0 && P.confidence < 1) || P.max_iters > (1 << 20)) {
+    h->err = "homography params: threshold_px > 0, 0 < confidence < 1, max_iters <= 2^20"; return -1;
+  }
+  return 0;
+}
+// one CTA per problem over rows [off[p], off[p+1]) of src / dst (device), rows with sel == 0 left out when sel is given
+static int hom_launch(dynofront_ctx* h, int np, const int* d_off, const float* src, const float* dst, const uint8_t* sel, size_t rows,
+                      const dynofront_homography_params& P) {
+  const int cap = h->hm_record > 0 ? std::min(h->hm_record, std::max(P.max_iters, 1)) : 0;
+  const size_t nr = std::max(rows, (size_t)1);
+  if (grow(h, h->hm_cidx, nr, h->hm_lidx, nr, h->hm_inl, nr, h->hm_mask, nr, h->hm_H, 9*(size_t)np, h->hm_stat, 6*(size_t)np)) return -3;
+  if (cap && grow(h, h->hm_counts, (size_t)np*cap)) return -3;
+  if (cap) FCK(cudaMemsetAsync(h->hm_counts, 0xff, 4*(size_t)np*cap, h->s));      // -1 past the last iteration
+  HomBatch B{};
+  B.off = d_off; B.src = src; B.dst = dst; B.sel = sel; B.cidx = h->hm_cidx; B.lidx = h->hm_lidx; B.inl = h->hm_inl;
+  B.thr2 = (float)(P.threshold_px*P.threshold_px); B.conf = P.confidence; B.max_iters = P.max_iters; B.refine = P.refine != 0;
+  B.H = h->hm_H; B.mask = h->hm_mask; int* st = h->hm_stat;
+  B.n_inl = st; B.status = st + np; B.iters = st + 2*np; B.groups = st + 3*np; B.rejected = st + 4*np; B.best = st + 5*np;
+  B.counts = cap ? (int*)h->hm_counts : nullptr; B.counts_cap = cap;
+  for (int lg = -16; lg <= 16; lg++) B.lam[lg + 16] = std::exp(lg*std::log(10.));
+  if (np > 0) hom_ransac_kernel<<<np, HOM_THREADS, 0, h->s>>>(B);
+  h->hm_np = np; h->hm_cap = cap;
+  return 0;
+}
+int dynofront_homography_record_counts(dynofront_handle h, int32_t counts_cap) {
+  if (!h || counts_cap < 0) return -1;
+  h->hm_record = counts_cap; return 0;
+}
+int dynofront_find_homography_batch(dynofront_handle h, int32_t n_problems, const int32_t* offsets, const float* src, const float* dst,
+                                    const dynofront_homography_params* prm, double* H, uint8_t* mask, int32_t* n_inliers, int32_t* status,
+                                    int32_t* iterations, float* ms_device) {
+  if (!h || n_problems < 0 || !offsets || !H || !n_inliers || !status) return -1;
+  dynofront_homography_params P; if (prm) P = *prm; else dynofront_homography_default_params(&P);
+  if (hom_check_params(h, P)) return -1;
+  if (offsets[0] != 0) { h->err = "offsets[0] must be 0"; return -1; }
+  for (int p = 0; p < n_problems; p++) if (offsets[p + 1] < offsets[p]) { h->err = "offsets must not decrease"; return -1; }
+  const size_t rows = (size_t)offsets[n_problems];
+  if (rows > 0 && (!src || !dst || !mask)) return -1;
+  for (size_t i = 0; i < 2*rows; i++) if (!std::isfinite(src[i]) || !std::isfinite(dst[i])) { h->err = "non-finite point"; return -1; }
+  cudaSetDevice(h->dev);
+  const size_t nr = std::max(rows, (size_t)1);
+  if (grow(h, h->hm_off, (size_t)n_problems + 1, h->hm_src, 2*nr, h->hm_dst, 2*nr)) return -3;
+  FCK(cudaEventRecord(h->e0, h->s));
+  FCK(cudaMemcpyAsync(h->hm_off, offsets, 4*((size_t)n_problems + 1), cudaMemcpyHostToDevice, h->s));
+  if (rows) {
+    FCK(cudaMemcpyAsync(h->hm_src, src, 8*rows, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->hm_dst, dst, 8*rows, cudaMemcpyHostToDevice, h->s));
+  }
+  if (int rc = hom_launch(h, n_problems, h->hm_off, h->hm_src, h->hm_dst, nullptr, rows, P)) return rc;
+  const size_t np = (size_t)n_problems;
+  if (np) {
+    FCK(cudaMemcpyAsync(H, h->hm_H, 72*np, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(n_inliers, h->hm_stat, 4*np, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(status, h->hm_stat + np, 4*np, cudaMemcpyDeviceToHost, h->s));
+    if (iterations) FCK(cudaMemcpyAsync(iterations, h->hm_stat + 2*np, 4*np, cudaMemcpyDeviceToHost, h->s));
+  }
+  if (rows) FCK(cudaMemcpyAsync(mask, h->hm_mask, rows, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  FCK(cudaGetLastError());
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+int dynofront_homography_last_trace(dynofront_handle h, int32_t* status, int32_t* groups, int32_t* rejected, int32_t* best, int32_t counts_cap,
+                                    int32_t* counts, int32_t* n_problems) {
+  if (!h || !n_problems) return -1;
+  cudaSetDevice(h->dev);
+  const size_t np = (size_t)h->hm_np;
+  *n_problems = h->hm_np;
+  if (np == 0) return 0;
+  if (status) FCK(cudaMemcpy(status, h->hm_stat + np, 4*np, cudaMemcpyDeviceToHost));
+  if (groups) FCK(cudaMemcpy(groups, h->hm_stat + 3*np, 4*np, cudaMemcpyDeviceToHost));
+  if (rejected) FCK(cudaMemcpy(rejected, h->hm_stat + 4*np, 4*np, cudaMemcpyDeviceToHost));
+  if (best) FCK(cudaMemcpy(best, h->hm_stat + 5*np, 4*np, cudaMemcpyDeviceToHost));
+  if (counts && counts_cap > 0) {
+    std::fill(counts, counts + (size_t)counts_cap*np, -1);        // iterations that were not recorded
+    const int w = std::min(counts_cap, h->hm_cap);
+    if (w > 0)
+    FCK(cudaMemcpy2D(counts, 4*(size_t)counts_cap, h->hm_counts, 4*(size_t)h->hm_cap, 4*(size_t)w, np, cudaMemcpyDeviceToHost));
+  }
+  return 0;
+}
+int dynofront_klt_track_points(dynofront_handle h, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n, const float* prev_pts,
+                               float* next_pts, uint8_t* status, const dynofront_klt_fb_params* fb, const dynofront_homography_params* hom,
+                               const int32_t* prev_age, uint8_t* verified, uint8_t* keep, double* H, int32_t* hom_status, int32_t* n_status,
+                               int32_t* n_verified, int32_t* n_keep, float* ms_device) {
+  if (!h || n < 0 || !prev_pts || !next_pts || !status || !fb || !verified) return -1;
+  const bool resident = !prev_gray && !cur_gray;
+  if (!resident && (!prev_gray || !cur_gray)) { h->err = "pass both images, or none for the resident frames"; return -1; }
+  if (resident && !(h->have_pyr && h->have_pyr_cur)) { h->err = "two frames are needed on the device"; return -2; }
+  if (fb->win < 3 || fb->win > KLT_MAXWIN || fb->win_back < 3 || fb->win_back > KLT_MAXWIN || fb->max_level < 0 || fb->max_level_back < 0) { h->err = "win must be in [3,31]"; return -1; }
+  if (fb->check_static && (!prev_age || !keep)) { h->err = "check_static needs prev_age and keep"; return -1; }
+  dynofront_homography_params P; if (hom) P = *hom; else dynofront_homography_default_params(&P);
+  if (hom_check_params(h, P)) return -1;
+  if (int rc = klt_fb_stages(h, resident, prev_gray, cur_gray, n, prev_pts, next_pts, fb, prev_age)) return rc;
+  // one problem: the rows whose forward-backward status is set, in order -- trackPoints' good_previous / good_current
+  const int off[2] = {0, n};
+  if (grow(h, h->hm_off, 2)) return -3;
+  FCK(cudaMemcpyAsync(h->hm_off, off, sizeof(off), cudaMemcpyHostToDevice, h->s));
+  if (int rc = hom_launch(h, 1, h->hm_off, h->k_prev, h->k_next, h->k_st, (size_t)n, P)) return rc;
+  FCK(cudaMemsetAsync(h->k_count, 0, 2*sizeof(int), h->s));       // (k_count[0] is reported from the status copy below)
+  int counts[2] = {0, 0}, stat[2] = {0, 0};
+  if (n > 0) ktp_post_kernel<<<(n + 255)/256, 256, 0, h->s>>>(n, h->hm_mask, h->k_keep, fb->check_static, h->k_count);
   FCK(cudaMemcpyAsync(next_pts, h->k_next, 2*(size_t)n*4, cudaMemcpyDeviceToHost, h->s));
   FCK(cudaMemcpyAsync(status, h->k_st, n, cudaMemcpyDeviceToHost, h->s));
-  if (back_pts) FCK(cudaMemcpyAsync(back_pts, h->k_back, 2*(size_t)n*4, cudaMemcpyDeviceToHost, h->s));
-  if (keep) FCK(cudaMemcpyAsync(keep, h->k_keep, n, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(verified, h->hm_mask, n, cudaMemcpyDeviceToHost, h->s));
+  if (fb->check_static) FCK(cudaMemcpyAsync(keep, h->k_keep, n, cudaMemcpyDeviceToHost, h->s));
+  if (H) FCK(cudaMemcpyAsync(H, h->hm_H, 72, cudaMemcpyDeviceToHost, h->s));
+  if (hom_status) FCK(cudaMemcpyAsync(hom_status, h->hm_stat + 1, 4, cudaMemcpyDeviceToHost, h->s));
   FCK(cudaMemcpyAsync(counts, h->k_count, sizeof(counts), cudaMemcpyDeviceToHost, h->s));
   FCK(cudaEventRecord(h->e1, h->s));
   FCK(cudaStreamSynchronize(h->s));
   FCK(cudaGetLastError());
-  if (n_status) *n_status = counts[0]; if (n_keep) *n_keep = counts[1];
+  for (int i = 0; i < n; i++) stat[0] += status[i] != 0;
+  if (n_status) *n_status = stat[0]; if (n_verified) *n_verified = counts[0]; if (n_keep) *n_keep = counts[1];
   if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
   return 0;
 }

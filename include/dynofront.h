@@ -10,6 +10,8 @@
  *   dynofront_propagate_mask    FeatureTracker::propogateMask       FeatureTracker.cc:1212-1359
  *   dynofront_track_static_flow ExternalFlowFeatureTracker::trackStatic / constructStaticFeature  StaticFeatureTracker.cc:70-220
  *   dynofront_klt_track_fb      KltFeatureTracker::trackPoints: forward + backward LK, round-trip test, label / border / age checks (:486-592)
+ *   dynofront_klt_track_points  KltFeatureTracker::trackPoints steps 1-4: klt_track_fb + geometricVerification's cv::findHomography (:486-639)
+ *   dynofront_find_homography_batch  cv::findHomography(RANSAC) on many point sets in one launch
  *   dynofront_detect_static     KltFeatureTracker::detectFeatures: mask, CLAHE, GFTT, range-tree ANMS, cornerSubPix  StaticFeatureTracker.cc:330-418
  *   dynofront_stereo_track      FeatureTracker::stereoTrack: left -> right LK + disparity / depth test  FeatureTracker.cc:194-337
  *   dynofront_update_depths     Frame::updateDepths                 dynosam/src/frontend/vision/Frame.cc:241-251,430-467
@@ -120,7 +122,7 @@ int dynofront_klt_track(dynofront_handle h, const uint8_t* prev_gray, const uint
 /* KltFeatureTracker::trackPoints as ONE call (StaticFeatureTracker.cc:486-534,575-592): forward LK, the reference's
  * retry without the initial flow when fewer than 10 points survive, backward LK from the forward result, the
  * forward-backward test (both statuses good and the backward track within max_fb_distance of the start, float
- * arithmetic) and, with check_static, the per-point checks that follow the (host-side, out of scope) RANSAC:
+ * arithmetic) and, with check_static, the per-point checks that follow the RANSAC (dynofront_klt_track_points adds it):
  * background label at the truncated key-point of the motion mask given to dynofront_set_frame, inside the image and the
  * shrunken image, age + 1 <= max_feature_track_age.  Nothing returns to the host between the stages.
  * prev_gray == cur_gray == NULL: streaming mode, the two resident pyramids are used (nothing is uploaded or rebuilt).
@@ -136,6 +138,46 @@ typedef struct {
 int dynofront_klt_track_fb(dynofront_handle h, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n, const float* prev_pts,
                            float* next_pts, uint8_t* status, float* back_pts, const dynofront_klt_fb_params* prm,
                            const int32_t* prev_age, uint8_t* keep, int32_t* n_status, int32_t* n_keep, float* ms_device);
+/* ---- homography RANSAC: cv::findHomography(src, dst, cv::RANSAC, threshold_px, mask, max_iters, confidence) as
+ * KltFeatureTracker::geometricVerification calls it (StaticFeatureTracker.cc:627-639), with OpenCV's draw sequence (cv::RNG seeded
+ * with (uint64)-1 on every call), subset test, normalised DLT with OpenCV's Jacobi eigen solver, float reprojection error, stopping
+ * rule and, with refine = 1, its final DLT over the inliers, 10-step Levenberg-Marquardt refinement and the mask recomputed under
+ * the refined H.  refine = 0 returns the RANSAC model and its mask.  Per problem status:
+ *   DYNOFRONT_HOM_TOO_FEW      fewer than 4 points: all are inliers, H = 0 (geometricVerification's all-ones mask);
+ *   DYNOFRONT_HOM_FOUR_POINT   exactly 4: the DLT alone, mask all ones (all zeros and H = 0 when it has no solution);
+ *   DYNOFRONT_HOM_RANSAC_FAILED no subset passed the test in 10 000 draws, or no model had 4 inliers: H = 0, mask all zeros;
+ *   DYNOFRONT_HOM_OK           H (row-major, H22 = 1) and mask as cv::findHomography returns them. */
+enum { DYNOFRONT_HOM_OK = 0, DYNOFRONT_HOM_TOO_FEW = 1, DYNOFRONT_HOM_FOUR_POINT = 2, DYNOFRONT_HOM_RANSAC_FAILED = 3 };
+typedef struct {
+  double threshold_px;   /* 5.0 (StaticFeatureTracker.cc:632); refused <= 0 */
+  double confidence;     /* 0.995 */
+  int32_t max_iters;     /* 2000; values below 1 count as 1, as in OpenCV */
+  int32_t refine;        /* 1: findHomography's full behaviour; 0: the RANSAC model and mask */
+} dynofront_homography_params;
+void dynofront_homography_default_params(dynofront_homography_params* p);
+/* n_problems problems in one launch: problem p is src / dst rows [offsets[p], offsets[p+1]) ([row][2] float, (x, y)).
+ * H[n_problems][9], mask[offsets[n_problems]], n_inliers / status / iterations (may be NULL) [n_problems]. */
+int dynofront_find_homography_batch(dynofront_handle h, int32_t n_problems, const int32_t* offsets, const float* src, const float* dst,
+                                    const dynofront_homography_params* prm, double* H, uint8_t* mask, int32_t* n_inliers, int32_t* status,
+                                    int32_t* iterations, float* ms_device);
+/* parity hooks.  dynofront_homography_record_counts(h, cap): the following calls record the inlier count of each of the first
+ * cap iterations' models per problem (default 0: none are recorded, and no memory is set aside for them).
+ * dynofront_homography_last_trace, after dynofront_find_homography_batch or dynofront_klt_track_points: per problem the status,
+ * the groups of 4 indices drawn, those the subset test rejected, the iteration of the best model (-1: none), and
+ * counts[p][counts_cap] = the recorded counts (-1: no model, past the last iteration, or not recorded).  Any output may be NULL. */
+int dynofront_homography_record_counts(dynofront_handle h, int32_t counts_cap);
+int dynofront_homography_last_trace(dynofront_handle h, int32_t* status, int32_t* groups, int32_t* rejected, int32_t* best, int32_t counts_cap,
+                                    int32_t* counts, int32_t* n_problems);
+/* KltFeatureTracker::trackPoints steps 1-4 as ONE call (StaticFeatureTracker.cc:486-625): the stages of dynofront_klt_track_fb,
+ * then the homography above over the points whose status is set, in order (good_previous -> good_current), then
+ * verified[i] = status[i] && mask[rank of i] (so !verified is what determineOutlierIds reports) and, with fb->check_static,
+ * keep[i] = verified[i] && the label / border / age checks.  Nothing returns to the host between the stages.  H (may be NULL)
+ * receives the homography (0 when it has none), hom_status (may be NULL) its DYNOFRONT_HOM_* status.  NULL images: the
+ * resident frame pair. */
+int dynofront_klt_track_points(dynofront_handle h, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n, const float* prev_pts,
+                               float* next_pts, uint8_t* status, const dynofront_klt_fb_params* fb, const dynofront_homography_params* hom,
+                               const int32_t* prev_age, uint8_t* verified, uint8_t* keep, double* H, int32_t* hom_status, int32_t* n_status,
+                               int32_t* n_verified, int32_t* n_keep, float* ms_device);
 /* FeatureTracker::stereoTrack (FeatureTracker.cc:194-337): LK from the left to the right image (21x21, 5 levels, OpenCV default
  * criteria) and the per-point disparity test: valid[i] = status[i] && !(uL - uR <= 1 || uR < 0), depth[i] = fx * baseline /
  * (uL - uR) (0 where invalid).  The fundamental-matrix RANSAC the reference runs between the two is host code:
