@@ -143,6 +143,7 @@ def run_dynoba(n, warmup, streaming=True):
         out.update(full_frame(t, frames, static_pts, feats, n, warmup))
         out.update(static_detection(t, frames, static_pts, n, warmup))
         out.update(depth_stage(t, frames, static_pts, feats, n, warmup))
+        out.update(dynamic_klt(t, frames, n, warmup))
     out.update(card())
     return out
 
@@ -235,6 +236,56 @@ def depth_stage(t, frames, static_pts, feats, n, warmup):
             "depth_h2d_bytes_per_frame": int(8*W*H), "dense_cloud_d2h_bytes_per_frame": int(W*H*(12 + 3 + 4 + 1)),
             "depth_features_per_frame": float(rows[:, 3].mean()), "measurements_per_frame": float(rows[:, 4].mean()),
             "dense_points_per_frame": float(rows[:, 5].mean())}
+
+
+def _objects(m):
+    """objects_detected and inner bounding boxes (x, y, w, h) of a motion mask: each label's box shrunk by 2 px"""
+    objs, bb = [], []
+    for oid in range(1, 11):
+        ys, xs = np.nonzero(m == oid)
+        if len(ys):
+            x0, y0, x1, y1 = xs.min(), ys.min(), xs.max(), ys.max()
+            objs.append(oid); bb.append((x0 + 2, y0 + 2, max(x1 - x0 - 3, 1), max(y1 - y0 - 3, 1)))
+    return objs, np.array(bb, np.int32).reshape(-1, 4)
+
+
+def dynamic_klt(t, frames, n, warmup):
+    """FeatureTracker::trackDynamicKLT + requiresSampling on the device (dynofront_track_dynamic_klt) over the streaming frames, the
+    features carried from frame to frame as the reference does; track_dynamic_klt_ms is the device time of one call (CUDA events,
+    copies included).  Beside it, on the first frames, the host composition it replaces: dynofront_klt_track for the LK plus the
+    test oracle's cv2 / numpy stages (tests/dynamic_klt_oracle.py: per-feature loop, cv2.circle, requiresSampling,
+    cv2.goodFeaturesToTrack per sampled object, range-tree ANMS), wall clock on one host thread."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import dynamic_klt_oracle as KO
+    objs_of = [_objects(m) for _, m, _ in frames]
+    empty = (np.zeros((0, 2), np.float32), np.zeros(0, np.int32), np.zeros(0, np.int32), np.zeros(0, np.int64))
+    t.next_frame(frames[0][0], frames[0][2], frames[0][1])
+    state = {"prev": empty, "nid": 0}
+
+    def one(k):
+        g1, m1, f1 = frames[k]
+        t.next_frame(g1, f1, m1)
+        r = t.track_dynamic_klt(None, None, *state["prev"], *objs_of[k], state["nid"], want_masks=False)
+        state["prev"] = (r["keypoint"].astype(np.float32), r["label"], r["age"], r["tracklet"]); state["nid"] = r["next_tracklet_id"]
+        return t.last_ms, len(r["keypoint"]), int(r["tracked"].sum()), int(r["status"]["sampled"].sum())
+    for k in range(1, warmup + 1):
+        one(k)
+    state["prev"] = empty; state["nid"] = 0
+    rows = np.array([one(k) for k in range(1, n + 1)], np.float64)
+    # the host composition on the first frames, from the same carried-forward inputs
+    nb = min(n, 10); prev = empty; nid = 0; lk_ms = []; host_s = []
+    for k in range(1, nb + 1):
+        g0 = frames[k - 1][0]; g1, m1, _ = frames[k]; objs, bb = objs_of[k]
+        p1, st, _ = t.klt_track(g0, g1, prev[0], 21, 3, 30, 0.03); lk_ms.append(t.last_ms)
+        t0 = time.perf_counter()
+        r = KO.track_dynamic_klt(g1, m1, None, *prev, p1, st, objs, bb, KO.Params(), nid)
+        host_s.append(time.perf_counter() - t0)
+        prev = (r["keypoint"].astype(np.float32), r["label"], r["age"], r["tracklet"]); nid = r["next_tracklet_id"]
+    return {"track_dynamic_klt_ms": float(rows[:, 0].mean()), "track_dynamic_klt_features_per_frame": float(rows[:, 1].mean()),
+            "track_dynamic_klt_tracked_per_frame": float(rows[:, 2].mean()), "track_dynamic_klt_sampled_objects_per_frame": float(rows[:, 3].mean()),
+            "track_dynamic_klt_host_composition_ms": float(np.mean(lk_ms) + 1e3*np.mean(host_s)),
+            "track_dynamic_klt_host_composition_note": f"{nb} frames: dynofront_klt_track {np.mean(lk_ms):.3f} ms (device) + the oracle's "
+                                                       f"cv2 / numpy stages {1e3*np.mean(host_s):.1f} ms (one host thread, Python loops)"}
 
 
 def card():

@@ -16,7 +16,8 @@ EXPORTS = ["dynofront_create", "dynofront_destroy", "dynofront_last_error", "dyn
            "dynofront_get_motion_mask", "dynofront_get_pyramid_level", "dynofront_anms_range_tree", "dynofront_sample_dynamic",
            "dynofront_detect_static", "dynofront_detect_last_stages", "dynofront_set_depth", "dynofront_update_depths",
            "dynofront_back_project", "dynofront_dense_cloud", "dynofront_homography_default_params", "dynofront_find_homography_batch",
-           "dynofront_homography_last_trace", "dynofront_homography_record_counts", "dynofront_klt_track_points"]
+           "dynofront_homography_last_trace", "dynofront_homography_record_counts", "dynofront_klt_track_points",
+           "dynofront_klt_dynamic_default_params", "dynofront_track_dynamic_klt"]
 
 
 class TrackParamsC(C.Structure):
@@ -92,6 +93,47 @@ class HomographyParams:
 HOM_OK, HOM_TOO_FEW, HOM_FOUR_POINT, HOM_RANSAC_FAILED = 0, 1, 2, 3     # dynofront_find_homography_batch status
 
 
+class KltDynamicParamsC(C.Structure):
+    _fields_ = [("win", C.c_int32), ("max_level", C.c_int32), ("max_count", C.c_int32), ("epsilon", C.c_double), ("min_eig_threshold", C.c_double),
+                ("track", TrackParamsC), ("max_features", C.c_int32), ("quality_level", C.c_double), ("age_buffer", C.c_int32),
+                ("min_tracks", C.c_int32), ("min_iou", C.c_double)]
+
+
+@dataclass
+class KltDynamicParams:
+    """FeatureTracker::trackDynamicKLT + requiresSampling parameters: the LK criteria of the reference's CPU call
+    (FeatureTracker.cc:625-639) and params/FrontendParams.yaml."""
+    win: int = 21
+    max_level: int = 3
+    max_count: int = 30
+    epsilon: float = 0.03
+    min_eig_threshold: float = 1e-4
+    max_dynamic_feature_age: int = 20
+    min_distance: int = 2              # min_distance_btw_tracked_and_detected_dynamic_features
+    shrink_row: int = 0
+    shrink_col: int = 0
+    max_features: int = 200            # max_dynamic_features_per_frame
+    quality_level: float = 0.01
+    age_buffer: int = 3                # dynamic_feature_age_buffer
+    min_tracks: int = 20               # min_dynamic_tracks
+    min_iou: float = 0.1               # min_dynamic_mask_iou
+
+    def c(self):
+        return KltDynamicParamsC(self.win, self.max_level, self.max_count, float(self.epsilon), float(self.min_eig_threshold),
+                                 TrackParamsC(self.max_dynamic_feature_age, self.min_distance, self.shrink_row, self.shrink_col),
+                                 self.max_features, float(self.quality_level), self.age_buffer, self.min_tracks, float(self.min_iou))
+
+
+class ObjectStatusC(C.Structure):
+    _fields_ = [(f, C.c_int32) for f in ("object_id", "exists", "num_previous_track", "num_track", "num_outside_shrunken_image",
+                                         "num_tracked_with_different_label", "num_tracked_with_background_label", "object_new",
+                                         "object_resampled", "sampled", "num_sampled")]
+
+
+OBJECT_STATUS_FIELDS = [f for f, _ in ObjectStatusC._fields_]
+DKLT_TRACKED, DKLT_MASKED, DKLT_REJECTED, DKLT_OUTSIDE, DKLT_LOST = 1, 2, 3, 4, 5     # dynofront_track_dynamic_klt per-feature state
+
+
 _LIB = None
 
 
@@ -143,6 +185,12 @@ def load():
         L.dynofront_klt_track_points.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.POINTER(KltFbParamsC), C.POINTER(HomographyParamsC)] + [C.c_void_p]*4 + \
                                                 [C.POINTER(C.c_int32)]*4 + [C.POINTER(C.c_float)]
+        L.dynofront_klt_dynamic_default_params.argtypes = [C.POINTER(KltDynamicParamsC)]
+        L.dynofront_klt_dynamic_default_params.restype = None
+        L.dynofront_track_dynamic_klt.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p]*4 + [C.c_int32, C.c_void_p, C.c_void_p,
+                                                  C.POINTER(KltDynamicParamsC), C.POINTER(C.c_int64)] + [C.c_void_p]*4 + [C.c_int32] + \
+                                                 [C.c_void_p]*5 + [C.POINTER(C.c_int32), C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p,
+                                                  C.POINTER(C.c_float)]
         L.dynofront_get_pyramid_level.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p]
         _LIB = L
     return _LIB
@@ -386,6 +434,43 @@ class FeatureTrackerGPU:
                                                      _p(keep), _p(H), C.byref(hs), C.byref(ns), C.byref(nv), C.byref(nk), C.byref(ms)))
         self.last_ms = ms.value; self.last_counts = (ns.value, nv.value, nk.value); self.last_hom_status = hs.value
         return nxt, st, ver, (keep if check else None), (H.reshape(3, 3) if hs.value in (HOM_OK, HOM_FOUR_POINT) and H.any() else None)
+
+    def track_dynamic_klt(self, prev_gray, cur_gray, prev_kp, prev_label, prev_age, prev_tracklet, objects, inner_bb, next_tracklet_id: int,
+                          prm: KltDynamicParams | None = None, want_masks=True, capacity=None):
+        """FeatureTracker::trackDynamicKLT with requiresSampling in one call (dynofront_track_dynamic_klt).  prev_gray = cur_gray =
+        None: the resident frame pair of next_frame.  prev_kp [n][2] (float32, as toOpenCV gives it), labels, ages, tracklet ids of
+        the previous usable dynamic features; objects / inner_bb [m][4] (x, y, w, h) from the object boundary mask.  Uses the motion
+        mask and boundary mask of the current frame.  Returns a dict: per previous feature lk_pts, lk_status, state (DKLT_*),
+        tracked, measured_flow; the output features keypoint / age / tracklet / label / source (tracked ones first, by ascending
+        label, then the new ones in objects order); status (a dict of arrays over [label 0] + objects, OBJECT_STATUS_FIELDS);
+        n_outside_image, next_tracklet_id and, with want_masks, detection_mask / tracking_mask."""
+        pg = None if prev_gray is None else np.ascontiguousarray(prev_gray, dtype=np.uint8)
+        cg = None if cur_gray is None else np.ascontiguousarray(cur_gray, dtype=np.uint8)
+        kp = np.ascontiguousarray(prev_kp, dtype=np.float32).reshape(-1, 2); n = kp.shape[0]
+        lab = np.ascontiguousarray(prev_label, dtype=np.int32).reshape(n); age = np.ascontiguousarray(prev_age, dtype=np.int32).reshape(n)
+        tid = np.ascontiguousarray(prev_tracklet, dtype=np.int64).reshape(n)
+        objs = np.ascontiguousarray(objects, dtype=np.int32).reshape(-1); m = objs.shape[0]
+        bb = np.ascontiguousarray(inner_bb, dtype=np.int32).reshape(m, 4)
+        p = prm or KltDynamicParams()
+        cap = int(capacity if capacity is not None else n + m*max(p.max_features, 1))
+        lk = np.zeros((n, 2), np.float32); st = np.zeros(n, np.uint8); state = np.zeros(n, np.uint8); fl = np.zeros((n, 2))
+        okp = np.zeros((max(cap, 1), 2)); oage = np.zeros(max(cap, 1), np.int32); otid = np.zeros(max(cap, 1), np.int64)
+        olab = np.zeros(max(cap, 1), np.int32); osrc = np.zeros(max(cap, 1), np.int32)
+        rows = (ObjectStatusC*(m + 1))()
+        det = np.zeros((self.H, self.W), np.uint8) if want_masks else None
+        trk = np.zeros((self.H, self.W), np.uint8) if want_masks else None
+        nid = C.c_int64(int(next_tracklet_id)); nf = C.c_int32(); no = C.c_int32(); ms = C.c_float(); pc = p.c()
+        self._ck(self.lib.dynofront_track_dynamic_klt(self.h, _p(pg), _p(cg), n, _p(kp), _p(lab), _p(age), _p(tid), m, _p(objs), _p(bb), C.byref(pc),
+                                                      C.byref(nid), _p(lk), _p(st), _p(state), _p(fl), cap, _p(okp), _p(oage), _p(otid), _p(olab),
+                                                      _p(osrc), C.byref(nf), C.cast(rows, C.c_void_p), C.byref(no), _p(det), _p(trk), C.byref(ms)))
+        self.last_ms = ms.value
+        if nf.value > cap:                                        # more than the guess: the call is not repeatable (ids), so refuse
+            raise FrontendError(f"track_dynamic_klt: {nf.value} features exceed capacity {cap}")
+        s = nf.value
+        status = {f: np.array([getattr(r, f) for r in rows], np.int32) for f in OBJECT_STATUS_FIELDS}
+        return dict(lk_pts=lk, lk_status=st, state=state, tracked=(state == DKLT_TRACKED).astype(np.uint8), measured_flow=fl, keypoint=okp[:s],
+                    age=oage[:s], tracklet=otid[:s], label=olab[:s], source=osrc[:s], status=status, n_outside_image=no.value,
+                    next_tracklet_id=nid.value, detection_mask=det, tracking_mask=trk)
 
     def find_homography_batch(self, problems, prm: HomographyParams | None = None):
         """cv::findHomography(src, dst, RANSAC, ...) on every problem in one launch.  problems: sequence of (src [n][2], dst [n][2]).

@@ -80,6 +80,10 @@ struct dynofront_ctx {
   // homography RANSAC: inputs, point / inlier lists, outputs, per-problem statistics (6 arrays of hm_np) and per-iteration counts
   DevBuf<int> hm_off, hm_cidx, hm_lidx, hm_stat, hm_counts; DevBuf<float> hm_src, hm_dst; DevBuf<float4> hm_inl; DevBuf<double> hm_H; DevBuf<uint8_t> hm_mask;
   int hm_np = 0, hm_cap = 0, hm_record = 0;       // problems and recorded iterations of the last call; iterations to record
+  // trackDynamicKLT (also uses the trackDynamic, KLT, detection and ANMS scratch): status rows, counters, per-object lists (tk_int:
+  // bb[4][64], K, cand, off, corners, selected), tracked sort keys, eigen image, GFTT corners, output features
+  DevBuf<unsigned char> tk_rows, tk_cnt; DevBuf<int> tk_int, tk_corners; DevBuf<unsigned long long> tk_keys; DevBuf<float> tk_eig;
+  DevBuf<double> tk_kp; DevBuf<int32_t> tk_age, tk_lab, tk_src; DevBuf<long long> tk_tid;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
 };
 // grows each (buffer, element count) pair in turn; 0, or -3 with the error at the first allocation that fails
@@ -150,10 +154,10 @@ __global__ void td_link_kernel(int n, const int* fx, const int* fy, const int* s
   if (i >= n || state[i] != 0) return;
   next[i] = atomicExch(&cell[(size_t)fy[i]*W + fx[i]], i);
 }
-// greedy resolution + tracklet ids, one CTA
+// greedy resolution + tracklet ids, one CTA; a candidate covered by an earlier accepted one gets state `masked`
 __global__ void __launch_bounds__(1024) td_resolve_kernel(int n, const int* fx, const int* fy, int* state, const int* cell, const int* next,
                                                           int W, int H, Disc disc, int max_age, const int64_t* ptid, int32_t* oage, int64_t* otid,
-                                                          uint8_t* acc, long long* nextid) {
+                                                          uint8_t* acc, long long* nextid, int masked) {
   __shared__ int remaining;
   for (;;) {
     if (threadIdx.x == 0) remaining = 0;
@@ -170,7 +174,7 @@ __global__ void __launch_bounds__(1024) td_resolve_kernel(int n, const int* fx, 
         }
         return any_acc;
       });
-      if (any_acc) state[i] = 2;
+      if (any_acc) state[i] = masked;
       else if (!any_unknown) state[i] = 1;
       else atomicAdd(&remaining, 1);
     }
@@ -916,23 +920,27 @@ __global__ void dt_sort_global_kernel(unsigned long long* keys, const int* count
   const int i = (t/j)*2*j + (t % j);
   dt_cmpx(&keys[i], &keys[i + j], (i & k) == 0);
 }
-// the greedy minDistance filter with the maxCorners stop (goodFeaturesToTrack), one CTA, through the ordered resolver of
-// the ANMS with the strict Euclidean metric.  corners[2*c] = (x, y) in output order, *n_corners; resp = the first value.
-__global__ void __launch_bounds__(SEL_THREADS, 1) dt_gftt_select_kernel(const unsigned long long* __restrict__ keys, const int* __restrict__ count, int W, int H,
+// the greedy minDistance filter with the maxCorners stop (goodFeaturesToTrack), one CTA per sorted key list, through the
+// ordered resolver of the ANMS with the strict Euclidean metric.  List l is keys[off[l] .. off[l] + count[l]) (one list at 0
+// without off); the pixel address is key & addr_mask.  corners[2*(off[l] + c)] = (x, y) in output order, n_corners[l]; resp
+// (may be NULL) = the first value of a key whose value sits in the upper 32 bits.
+__global__ void __launch_bounds__(SEL_THREADS, 1) dt_gftt_select_kernel(const unsigned long long* __restrict__ keys, const int* __restrict__ off,
+                                                                      const int* __restrict__ count, unsigned addr_mask, int W, int H,
                                                                       int min_dist, int max_corners, int* px, int* py, int* nxt, int* sel,
                                                                       int* __restrict__ corners, int* __restrict__ n_corners, float* __restrict__ resp) {
   __shared__ int head[SEL_GRID];
   __shared__ uint8_t pend[SEL_THREADS];
   __shared__ int s_kept;
   __shared__ SelGrid s_g;
-  const int n = *count, tid = threadIdx.x;
-  if (n == 0) { if (tid == 0) { *n_corners = 0; *resp = 0.f; } return; }
-  for (int e = tid; e < n; e += SEL_THREADS) { const unsigned a = (unsigned)keys[e]; px[e] = (int)(a % W); py[e] = (int)(a / W); }
+  const int l = blockIdx.x, o = off ? off[l] : 0, n = count[l], tid = threadIdx.x;
+  if (n == 0) { if (tid == 0) { n_corners[l] = 0; if (resp) *resp = 0.f; } return; }
+  keys += o; px += o; py += o; nxt += o; sel += o; corners += 2*(size_t)o;
+  for (int e = tid; e < n; e += SEL_THREADS) { const unsigned a = (unsigned)keys[e] & addr_mask; px[e] = (int)(a % W); py[e] = (int)(a / W); }
   if (tid == 0) s_g = sel_make_grid(min_dist, 0, 0, W - 1, H - 1);
   __syncthreads();
   const int m = sel_greedy<true>(s_g, n, max_corners > 0 ? max_corners : 0x7fffffff, px, py, nxt, sel, head, pend, &s_kept);
   for (int r = tid; r < m; r += SEL_THREADS) { corners[2*r] = px[sel[r]]; corners[2*r + 1] = py[sel[r]]; }
-  if (tid == 0) { *n_corners = m; *resp = f32_unorder((unsigned)(keys[0] >> 32)); }
+  if (tid == 0) { n_corners[l] = m; if (resp) *resp = f32_unorder((unsigned)(keys[0] >> 32)); }
 }
 // cv::getRectSubPix(img, 13x13, centre, CV_32F) as cornerSubPix calls it.  Inside the image: the four float weights, summed
 // as (p a11 + q a12) + (u a21 + v a22); near the border: adjustRect's clamped rectangle (columns outside the image repeat
@@ -1605,6 +1613,231 @@ __global__ void ktp_post_kernel(int n, const uint8_t* __restrict__ verified, uin
   if (check && keep[i]) atomicAdd(count + 1, 1);
 }
 
+// ---------------------------------------------------------------------------------------------------- trackDynamicKLT
+// FeatureTracker::trackDynamicKLT with requiresSampling (FeatureTracker.cc:500-862,1018-1149) after the forward LK:
+//  * a status-good point whose truncated pixel is outside the image is dropped and counted apart (cv::Mat::at out of range in
+//    the reference);
+//  * the detection-mask test reads detection_mask_impl as the feature is visited: the boundary mask, then the discs of the EARLIER
+//    accepted features.  A point that would be accepted is a candidate of the greedy resolution of trackDynamic (td_link /
+//    td_resolve, which marks a covered candidate TK_MASKED); any other point is TK_PENDING until the resolution is known and
+//    then TK_MASKED when an earlier accepted disc covers its pixel, else TK_REJECTED.  Only TK_TRACKED and TK_REJECTED points are
+//    counted, under their predicted label (integer atomics: order-independent);
+//  * the tracked features leave ordered by (label, index) keys (tracks_per_object is an ordered map), through the bitonic sort;
+//  * requiresSampling: one thread per detected object, from the per-label counters, the geriatric count and the float bounding
+//    box (cv::boundingRect: floor of the extremes, width floor(max) - floor(min) + 1) against the inner bounding box (cv::Rect
+//    intersection, int areas, calculateIoU);
+//  * goodFeaturesToTrack(mono, max_features, quality, min_distance, (motion_mask == id) & detection_mask_impl) per sampled object:
+//    the eigen image is computed once (the stages of dynofront_detect_static, no CLAHE).  Under THRESH_TOZERO a pixel is a corner
+//    candidate iff it is a 3x3 local maximum of the raw eigen image above the object's threshold (the threshold is >= 0 whenever a
+//    masked pixel can pass it), so one local-maximum pass serves every object; the per-object parts are the masked maximum, the
+//    threshold and the candidate lists, sorted together with keys (object rank, value, address);
+//  * the minDistance / maxCorners filter one CTA per list, the range-tree ANMS of every sampled object in one launch (response 1
+//    for all, KeyPoint::convert: the visiting order is P_n), then the new features in objects order, each in ANMS order, the
+//    shrunken-image test before an id is taken.
+enum { TK_CAND = 0, TK_TRACKED = 1, TK_MASKED = 2, TK_REJECTED = 3, TK_OUTSIDE = 4, TK_LOST = 5, TK_PENDING = 6 };
+constexpr int TK_ADDR_BITS = 26;          // pixel address bits of the corner keys: images up to 2^26 pixels
+// one status row: rows[0] is label 0, rows[1 + o] objects[o]
+struct TkRow { int exists, prev, track, shrunk, diff, bg, geri; unsigned bx0, by0, bx1, by1, max_eig; int is_new, resampled, sampled, num_sampled; };
+struct TkCounters { int tracked, outside, cand, features; };
+struct TkParams {
+  dynofront_track_params track; int max_age, expiry, max_features, min_tracks; double quality, min_iou;
+};
+__device__ __forceinline__ int tk_slot(const int* objs, int nobj, int lab) {
+  for (int o = 0; o < nobj; o++) if (objs[o] == lab) return o;
+  return -1;
+}
+__global__ void tk_init_kernel(int nrows, TkRow* rows, TkCounters* cnt, int* cand) {
+  const int r = threadIdx.x;
+  if (r < nrows) { TkRow z = {}; z.bx0 = z.by0 = 0xffffffffu; rows[r] = z; }
+  if (r < ST_MAXOBJ) cand[r] = 0;
+  if (r == 0) *cnt = TkCounters{};
+}
+__global__ void tk_gather_kernel(int n, const float* __restrict__ next, const uint8_t* __restrict__ st, const int32_t* __restrict__ plab,
+                                 const int32_t* __restrict__ page, const int32_t* __restrict__ mask, const uint8_t* __restrict__ det, int W, int H,
+                                 TkParams P, int* fx, int* fy, int* state, int32_t* oage, int32_t* olab) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double kx = (double)next[2*i], ky = (double)next[2*i + 1];
+  int s = TK_LOST, x = 0, y = 0, lab = 0;
+  if (st[i]) {
+    s = TK_OUTSIDE;
+    if (kx > -1.0 && kx < (double)W && ky > -1.0 && ky < (double)H) {       // the truncated pixel is inside the image
+      x = (int)kx; y = (int)ky;
+      lab = mask[(size_t)y*W + x];
+      if (det && det[(size_t)y*W + x] == 0) s = TK_MASKED;                   // the boundary mask: not counted
+      else {
+        const bool contained = kx >= 0.0 && kx < (double)W && ky >= 0.0 && ky < (double)H;
+        const bool ok = contained && lab != 0 && lab == plab[i] && within_shrunken(kx, ky, H, W, P.track.shrink_row, P.track.shrink_col) &&
+                        page[i] + 1 <= P.max_age;
+        s = ok ? TK_CAND : TK_PENDING;
+      }
+    }
+  }
+  fx[i] = x; fy[i] = y; state[i] = s; oage[i] = page[i] + 1; olab[i] = lab;
+}
+// after td_resolve: the pending points learn whether an earlier accepted disc covers them, the counted points are counted, the
+// accepted ones get their sort key; measured flow = kp_current - keypoint in double
+__global__ void tk_count_kernel(int n, const float* __restrict__ prev, const float* __restrict__ next, const int* __restrict__ fx, const int* __restrict__ fy,
+                                int* state, const int* __restrict__ cell, const int* __restrict__ lnext, Disc disc, int W, int H,
+                                const int32_t* __restrict__ plab, const int32_t* __restrict__ oage, const int32_t* __restrict__ olab,
+                                const int* __restrict__ objs, int nobj, TkParams P, TkRow* rows, TkCounters* cnt, unsigned long long* keys, double* flow) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int s = state[i];
+  if (s == TK_PENDING) {
+    bool covered = false;
+    disc_walk(disc, fx[i], fy[i], W, H, [&](int xx, int yy) {
+      for (int j = cell[(size_t)yy*W + xx]; j >= 0; j = lnext[j]) if (j < i && state[j] == TK_TRACKED) { covered = true; break; }
+      return covered;
+    });
+    s = covered ? TK_MASKED : TK_REJECTED;
+    state[i] = s;
+  }
+  const double kx = (double)next[2*i], ky = (double)next[2*i + 1];
+  flow[2*i] = s == TK_TRACKED ? kx - (double)prev[2*i] : 0.0;
+  flow[2*i + 1] = s == TK_TRACKED ? ky - (double)prev[2*i + 1] : 0.0;
+  if (s == TK_OUTSIDE) atomicAdd(&cnt->outside, 1);
+  if (s != TK_TRACKED && s != TK_REJECTED) return;
+  const int lab = olab[i];
+  if (s == TK_TRACKED) {
+    const unsigned long long a = ((unsigned long long)((unsigned)lab ^ 0x80000000u) << 32) | (unsigned)i;   // ascending (label, index)
+    keys[atomicAdd(&cnt->tracked, 1)] = ~a;                                                                  // (the sort is descending)
+  }
+  const int o = lab == 0 ? -1 : tk_slot(objs, nobj, lab);
+  if (lab != 0 && o < 0) return;                                   // a label that is not listed has no row in the output
+  TkRow* r = rows + (o + 1);
+  const bool contained = kx >= 0.0 && kx < (double)W && ky >= 0.0 && ky < (double)H;
+  r->exists = 1;
+  atomicAdd(&r->prev, 1);
+  if (lab == 0) atomicAdd(&r->bg, 1);
+  if (lab != plab[i]) atomicAdd(&r->diff, 1);
+  if (contained && lab != 0 && lab == plab[i] && !within_shrunken(kx, ky, H, W, P.track.shrink_row, P.track.shrink_col)) atomicAdd(&r->shrunk, 1);
+  if (s == TK_TRACKED) {
+    atomicAdd(&r->track, 1);
+    if (oage[i] > P.expiry) atomicAdd(&r->geri, 1);
+    atomicMin(&r->bx0, f32_order(next[2*i])); atomicMax(&r->bx1, f32_order(next[2*i]));
+    atomicMin(&r->by0, f32_order(next[2*i + 1])); atomicMax(&r->by1, f32_order(next[2*i + 1]));
+  }
+}
+// requiresSampling, one thread per detected object in the given order; K[o] = corners needed (0: not sampled)
+__global__ void tk_decide_kernel(int nobj, const int* __restrict__ bb, TkParams P, TkRow* rows, int* K) {
+  const int o = threadIdx.x;
+  if (o >= nobj) return;
+  TkRow* r = rows + 1 + o;
+  bool sample;
+  if (!r->exists) { sample = true; r->exists = 1; r->is_new = 1; }          // getObjectStatus makes the row
+  else if (r->track == 0) sample = false;                                    // a row but no tracked feature: skipped
+  else {
+    const bool old = (double)r->geri/(double)r->track > 0.8;
+    const bool few = r->track < P.min_tracks;
+    const int tx = (int)floorf(f32_unorder(r->bx0)), ty = (int)floorf(f32_unorder(r->by0));
+    const int tw = (int)floorf(f32_unorder(r->bx1)) - tx + 1, th = (int)floorf(f32_unorder(r->by1)) - ty + 1;
+    const int ax = bb[4*o], ay = bb[4*o + 1], aw = bb[4*o + 2], ah = bb[4*o + 3];
+    int iw = 0, ih = 0;                                                      // cv::Rect operator& (empty: Rect())
+    if (aw > 0 && ah > 0 && tw > 0 && th > 0) {
+      iw = min(ax + aw, tx + tw) - max(ax, tx); ih = min(ay + ah, ty + th) - max(ay, ty);
+      if (iw <= 0 || ih <= 0) iw = ih = 0;
+    }
+    const double inter = (double)(iw*ih), uni = (double)(aw*ah + tw*th) - inter;
+    const double iou = uni == 0 ? 0.0 : inter/uni;
+    sample = old || few || iou < P.min_iou;
+  }
+  if (sample) r->resampled = 1;
+  r->sampled = sample ? 1 : 0;
+  K[o] = sample ? max(P.max_features - r->track, 0) : 0;
+}
+// the minimum eigenvalue per pixel and, per sampled object, its maximum under (motion_mask == id) & detection_mask_impl
+__global__ void tk_eig_kernel(const float* __restrict__ box, size_t npx, const int32_t* __restrict__ mask, const uint8_t* __restrict__ det,
+                              const int* __restrict__ objs, int nobj, TkRow* rows, float* __restrict__ eig) {
+  __shared__ int s_obj[ST_MAXOBJ]; __shared__ unsigned s_max[ST_MAXOBJ];
+  if (threadIdx.x < ST_MAXOBJ) { s_obj[threadIdx.x] = threadIdx.x < nobj && rows[1 + threadIdx.x].sampled ? objs[threadIdx.x] : 0; s_max[threadIdx.x] = 0; }
+  __syncthreads();
+  const size_t p = (size_t)blockIdx.x*blockDim.x + threadIdx.x;
+  if (p < npx) {
+    const float a = box[p]*0.5f, b = box[npx + p], cc = box[2*npx + p]*0.5f;
+    const float e = (a + cc) - sqrtf((a - cc)*(a - cc) + b*b);
+    eig[p] = e;
+    const int lab = mask[p];
+    const int o = (lab != 0 && det[p]) ? tk_slot(s_obj, nobj, lab) : -1;
+    if (o >= 0) atomicMax(&s_max[o], f32_order(e));
+  }
+  __syncthreads();
+  if ((int)threadIdx.x < nobj && s_max[threadIdx.x]) atomicMax(&rows[1 + threadIdx.x].max_eig, s_max[threadIdx.x]);
+}
+// the candidates of every sampled object: a masked 3x3 local maximum of the raw eigen image above (float)(maxVal * quality), the
+// 1-px border excluded; key = (63 - object rank) << 58 | value (order-preserving) << 26 | address, sorted descending
+__global__ void tk_cand_kernel(const float* __restrict__ eig, int W, int H, const int32_t* __restrict__ mask, const uint8_t* __restrict__ det,
+                               const int* __restrict__ objs, int nobj, const TkRow* __restrict__ rows, double quality, unsigned long long* __restrict__ keys,
+                               TkCounters* cnt, int* __restrict__ cand) {
+  __shared__ int s_obj[ST_MAXOBJ]; __shared__ float s_thr[ST_MAXOBJ];
+  const int t = threadIdx.y*blockDim.x + threadIdx.x;
+  if (t < ST_MAXOBJ) {
+    s_obj[t] = t < nobj && rows[1 + t].sampled ? objs[t] : 0;
+    const unsigned m = t < nobj ? rows[1 + t].max_eig : 0u;
+    s_thr[t] = (float)((double)(m ? f32_unorder(m) : 0.f)*quality);          // minMaxLoc over an empty mask leaves maxVal = 0
+  }
+  __syncthreads();
+  const int x = blockIdx.x*blockDim.x + threadIdx.x, y = blockIdx.y*blockDim.y + threadIdx.y;
+  if (x < 1 || y < 1 || x >= W - 1 || y >= H - 1) return;
+  const size_t p = (size_t)y*W + x;
+  const int lab = mask[p];
+  if (lab == 0 || !det[p]) return;
+  const int o = tk_slot(s_obj, nobj, lab);
+  if (o < 0) return;
+  const float v = eig[p];
+  if (!(v > s_thr[o])) return;
+  float d = v;
+  for (int j = -1; j <= 1; j++) for (int i = -1; i <= 1; i++) d = fmaxf(d, eig[(size_t)(y + j)*W + x + i]);
+  if (v != d) return;
+  atomicAdd(&cand[o], 1);
+  keys[atomicAdd(&cnt->cand, 1)] = ((unsigned long long)(63 - o) << 58) | ((unsigned long long)f32_order(v) << TK_ADDR_BITS) | (unsigned long long)p;
+}
+__global__ void tk_offsets_kernel(int nobj, const int* cand, int* off) {
+  if (threadIdx.x != 0) return;
+  int run = 0;
+  for (int o = 0; o < nobj; o++) { off[o] = run; run += cand[o]; }
+}
+// the output features, one CTA: the tracked ones in (label, index) order, then the new ones object after object in ANMS order,
+// the shrunken-image test before an id is taken; tracklet ids count up from base_id
+__global__ void __launch_bounds__(1024) tk_construct_kernel(const unsigned long long* __restrict__ tkeys, const float* __restrict__ next,
+                                                            const int32_t* __restrict__ oage, const int32_t* __restrict__ olab, const int64_t* __restrict__ ptid,
+                                                            const int* __restrict__ objs, int nobj, const int* __restrict__ off, const int* __restrict__ nsel,
+                                                            const int* __restrict__ sel, const int* __restrict__ corners, int W, int H, TkParams P,
+                                                            long long base_id, TkRow* rows, TkCounters* cnt, double* okp, int32_t* oage_out,
+                                                            long long* otid, int32_t* olab_out, int32_t* osrc) {
+  __shared__ int s_pre[ST_MAXOBJ + 1];
+  const int ntr = cnt->tracked;
+  for (int q = threadIdx.x; q < ntr; q += 1024) {
+    const int i = (int)~(unsigned)tkeys[q];
+    okp[2*(size_t)q] = (double)next[2*i]; okp[2*(size_t)q + 1] = (double)next[2*i + 1];
+    oage_out[q] = oage[i]; otid[q] = ptid[i]; olab_out[q] = olab[i]; osrc[q] = i;
+  }
+  if (threadIdx.x == 0) {
+    int run = 0;
+    for (int o = 0; o < nobj; o++) { s_pre[o] = run; run += nsel[o]; rows[1 + o].num_sampled = nsel[o]; }
+    s_pre[nobj] = run;
+  }
+  __syncthreads();
+  const int S = s_pre[nobj];
+  int base = 0;
+  for (int q0 = 0; q0 < S; q0 += 1024) {
+    const int q = q0 + threadIdx.x;
+    int a = 0, x = 0, y = 0, o = 0;
+    if (q < S) {
+      while (q >= s_pre[o + 1]) o++;
+      const int c = sel[off[o] + (q - s_pre[o])];
+      x = corners[2*(off[o] + c)]; y = corners[2*(off[o] + c) + 1];
+      a = within_shrunken((double)x, (double)y, H, W, P.track.shrink_row, P.track.shrink_col) ? 1 : 0;
+    }
+    const int rank = cta_rank(a, base);
+    if (a) {
+      const size_t d = (size_t)ntr + rank;
+      okp[2*d] = x; okp[2*d + 1] = y; oage_out[d] = 0; otid[d] = base_id + rank; olab_out[d] = objs[o]; osrc[d] = -1;
+    }
+  }
+  if (threadIdx.x == 0) cnt->features = ntr + base;
+}
+
 // ---------------------------------------------------------------------------------------------------- host API
 extern "C" {
 
@@ -1699,7 +1932,7 @@ int dynofront_track_dynamic(dynofront_handle h, int32_t n, const double* kp, con
                                              h->f_x, h->f_y, h->f_state, h->f_pred, h->f_flow, h->f_oage, h->f_olab);
     td_link_kernel<<<g, 128, 0, h->s>>>(n, h->f_x, h->f_y, h->f_state, W, h->cell, h->f_next);
     td_resolve_kernel<<<1, 1024, 0, h->s>>>(n, h->f_x, h->f_y, h->f_state, h->cell, h->f_next, W, H, disc, prm->max_dynamic_feature_age,
-                                            h->f_tid, h->f_oage, h->f_otid, h->f_acc, h->nextid);
+                                            h->f_tid, h->f_oage, h->f_otid, h->f_acc, h->nextid, 2);
     td_clear_rejected_kernel<<<g, 128, 0, h->s>>>(n, h->f_acc, h->f_pred, h->f_flow, h->f_olab);
     td_masks_kernel<<<g, 128, 0, h->s>>>(n, h->f_x, h->f_y, h->f_acc, W, H, disc, h->det_work, h->trk_idx);
   }
@@ -1863,6 +2096,19 @@ int dynofront_sample_dynamic(dynofront_handle h, int32_t nobj, const int32_t* ob
   return 0;
 }
 
+// the descending bitonic sort of keys[0 .. *count) (dt_sort_*), planned for cap keys (a power of two >= DT_SORT_TILE): every launch
+// reads the count on the device, so nothing is read back
+static void sort_keys_desc(dynofront_ctx* h, unsigned long long* keys, const int* count, size_t keycap) {
+  const int cap = (int)keycap, nb = cap/DT_SORT_TILE;
+  dt_sort_pad_kernel<<<(cap + 255)/256, 256, 0, h->s>>>(keys, count, cap);
+  dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(keys, count, 2, DT_SORT_TILE);
+  for (int k = 2*DT_SORT_TILE; k <= cap; k <<= 1) {
+    for (int j = k/2; j >= DT_SORT_TILE; j >>= 1) dt_sort_global_kernel<<<(cap/2 + 255)/256, 256, 0, h->s>>>(keys, count, k, j);
+    dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(keys, count, k, k);
+  }
+}
+static size_t sort_cap(size_t n) { size_t c = DT_SORT_TILE; while (c < n) c <<= 1; return c; }
+
 int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_cur, const double* cur_kp, const dynofront_detect_params* prm,
                             int64_t* next_tracklet_id, int32_t capacity, double* keypoint, int64_t* tracklet, int32_t* n_features,
                             int32_t* n_corners, float* ms_device) {
@@ -1879,7 +2125,7 @@ int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_c
   if (prm->use_anms && K >= 2 && anms_u16_wraps(std::max(W, H) - 1, K, W, H)) { h->err = "image too large for the u16 range tree of the reference"; return -1; }
   if (!gray && !h->have_pyr_cur) { h->err = "no current frame on the device"; return -2; }
   cudaSetDevice(h->dev);
-  size_t keycap = DT_SORT_TILE; while (keycap < npx) keycap <<= 1;
+  const size_t keycap = sort_cap(npx);
   if (grow(h, h->dt_gray, npx, h->dt_mask, npx, h->dt_clahe, npx, h->dt_lut, DT_TILES*DT_TILES*256, h->dt_dx, npx, h->dt_dy, npx, h->dt_box, 3*npx,
            h->dt_eig, npx, h->dt_keys, keycap, h->dt_corners, 2*npx, h->dt_cnt, 1, h->dt_pts, 2*npx, h->dt_resp, 1, h->dt_kp, 2*npx, h->dt_tid, npx,
            h->f_kp, 2*feature_cap(n_cur)) || grow_resolver(h, npx)) return -3;
@@ -1907,15 +2153,9 @@ int dynofront_detect_static(dynofront_handle h, const uint8_t* gray, int32_t n_c
   dt_box_kernel<<<(3*W + 31)/32, 32, 0, h->s>>>(h->dt_dx, h->dt_dy, W, H, h->dt_box);
   dt_eig_kernel<<<g1, 256, 0, h->s>>>(h->dt_box, npx, h->dt_mask, h->dt_eig, &c->max_eig);
   dt_cand_kernel<<<grd, blk, 0, h->s>>>(h->dt_eig, W, H, h->dt_mask, &c->max_eig, prm->quality_level, h->dt_keys, &c->candidates);
-  const int cap = (int)keycap, nb = cap/DT_SORT_TILE;
-  dt_sort_pad_kernel<<<(cap + 255)/256, 256, 0, h->s>>>(h->dt_keys, &c->candidates, cap);
-  dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(h->dt_keys, &c->candidates, 2, DT_SORT_TILE);
-  for (int k = 2*DT_SORT_TILE; k <= cap; k <<= 1) {
-    for (int j = k/2; j >= DT_SORT_TILE; j >>= 1) dt_sort_global_kernel<<<(cap/2 + 255)/256, 256, 0, h->s>>>(h->dt_keys, &c->candidates, k, j);
-    dt_sort_local_kernel<<<nb, DT_SORT_TILE/2, 0, h->s>>>(h->dt_keys, &c->candidates, k, k);
-  }
-  dt_gftt_select_kernel<<<1, SEL_THREADS, 0, h->s>>>(h->dt_keys, &c->candidates, W, H, prm->min_distance, prm->max_corners, h->sel_px, h->sel_py, h->sel_next,
-                                                     h->sel_orig, h->dt_corners, &c->corners, h->dt_resp);
+  sort_keys_desc(h, h->dt_keys, &c->candidates, keycap);
+  dt_gftt_select_kernel<<<1, SEL_THREADS, 0, h->s>>>(h->dt_keys, nullptr, &c->candidates, 0xffffffffu, W, H, prm->min_distance, prm->max_corners, h->sel_px,
+                                                     h->sel_py, h->sel_next, h->sel_orig, h->dt_corners, &c->corners, h->dt_resp);
   // (4) range-tree ANMS, K = max(max_features - n_cur, 0), tolerance 0.1 (FeatureDetector.cc:206-224)
   const int* sel = nullptr; const int* cnt = &c->corners;
   if (prm->use_anms) {
@@ -2500,6 +2740,162 @@ int dynofront_dense_cloud(dynofront_handle h, const double* calib5, double max_b
   FCK(cudaEventRecord(h->e1, h->s));
   FCK(cudaStreamSynchronize(h->s));
   if (n_valid) *n_valid = cnt;
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+
+// ---- trackDynamicKLT
+void dynofront_klt_dynamic_default_params(dynofront_klt_dynamic_params* p) {
+  if (!p) return;
+  p->win = 21; p->max_level = 3; p->max_count = 30; p->epsilon = 0.03; p->min_eig_threshold = 1e-4;      // FeatureTracker.cc:625-639
+  p->track.max_dynamic_feature_age = 20; p->track.min_distance = 2; p->track.shrink_row = 0; p->track.shrink_col = 0;
+  p->max_features = 200; p->quality_level = 0.01; p->age_buffer = 3; p->min_tracks = 20; p->min_iou = 0.1;   // params/FrontendParams.yaml
+}
+
+int dynofront_track_dynamic_klt(dynofront_handle h, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n, const float* prev_kp,
+                                const int32_t* prev_label, const int32_t* prev_age, const int64_t* prev_tracklet, int32_t n_objects,
+                                const int32_t* objects, const int32_t* inner_bb, const dynofront_klt_dynamic_params* prm, int64_t* next_tracklet_id,
+                                float* lk_pts, uint8_t* lk_status, uint8_t* state, double* measured_flow, int32_t capacity, double* keypoint,
+                                int32_t* age, int64_t* tracklet, int32_t* label, int32_t* source, int32_t* n_features,
+                                dynofront_object_status* status, int32_t* n_outside_image, uint8_t* detection_mask_out, uint8_t* tracking_mask_out,
+                                float* ms_device) {
+  if (!h || !prm || !next_tracklet_id || !n_features || !status || n < 0 || capacity < 0 || n_objects < 0) return -1;
+  if (n && (!prev_kp || !prev_label || !prev_age || !prev_tracklet)) { h->err = "null previous-feature array"; return -1; }
+  if (n_objects && (!objects || !inner_bb)) { h->err = "null object array"; return -1; }
+  if (capacity && (!keypoint || !age || !tracklet || !label || !source)) { h->err = "null feature array"; return -1; }
+  if (n_objects > ST_MAXOBJ) { h->err = "at most 64 objects"; return -1; }
+  for (int o = 0; o < n_objects; o++) {
+    if (objects[o] <= 0) { h->err = "object ids must be > 0 (0 is the background)"; return -1; }
+    for (int q = 0; q < o; q++) if (objects[q] == objects[o]) { h->err = "object ids must be distinct"; return -1; }
+    if (inner_bb[4*o + 2] < 0 || inner_bb[4*o + 3] < 0) { h->err = "bounding boxes must have width, height >= 0"; return -1; }
+  }
+  const dynofront_track_params& T = prm->track;
+  if (T.min_distance < 0 || T.min_distance > 15) { h->err = "min_distance must be in [0,15]"; return -1; }
+  if (prm->win < 3 || prm->win > KLT_MAXWIN || prm->max_level < 0) { h->err = "win must be in [3,31]"; return -1; }
+  const int expiry = T.max_dynamic_feature_age - std::max(3, prm->age_buffer);
+  if (expiry <= 0) { h->err = "max_dynamic_feature_age - max(3, age_buffer) must be > 0"; return -1; }
+  if (prm->min_tracks < 0 || prm->max_features < 0) { h->err = "min_tracks and max_features must be >= 0"; return -1; }
+  if (!(prm->quality_level > 0.0)) { h->err = "quality_level must be > 0"; return -1; }
+  const int W = h->W, H = h->H; const size_t npx = (size_t)W*H;
+  if (npx > ((size_t)1 << TK_ADDR_BITS)) { h->err = "image larger than 2^26 pixels"; return -1; }
+  {
+    const long long cmax = std::max(W, H) - 1;                   // no width of the search, for any K an object can need, may wrap
+    bool wraps = cmax > 65535;
+    for (int k = 2; k <= prm->max_features && !wraps; k++) wraps = anms_u16_wraps(cmax, k, W, H);
+    if (wraps) { h->err = "image too large for the u16 range tree of the reference"; return -1; }
+  }
+  const bool resident = !prev_gray && !cur_gray;
+  if (!resident && (!prev_gray || !cur_gray)) { h->err = "pass both images, or none for the resident frames"; return -1; }
+  if (resident && !(h->have_pyr && h->have_pyr_cur)) { h->err = "two frames are needed on the device"; return -2; }
+  if (!h->has_frame) { h->err = "no motion mask on the device"; return -2; }
+  const int top = klt_top_level(h, prm->max_level, prm->win);
+  if (resident && top > 5) { h->err = "the resident pyramids have 5 levels"; return -1; }
+  cudaSetDevice(h->dev);
+  const size_t cap = feature_cap(n), ocap = (size_t)n + (size_t)n_objects*std::max(prm->max_features, 1), tkeys = sort_cap(n), keycap = sort_cap(npx);
+  if (grow(h, h->k_prev, 2*cap, h->k_next, 2*cap, h->k_st, cap, h->k_err, cap, h->k_eig, 2*cap, h->f_lab, cap, h->f_age, cap, h->f_tid, cap,
+           h->f_x, cap, h->f_y, cap, h->f_state, cap, h->f_next, cap, h->f_flow, 2*cap, h->f_oage, cap, h->f_otid, cap, h->f_olab, cap, h->f_acc, cap,
+           h->tk_rows, (ST_MAXOBJ + 1)*sizeof(TkRow), h->tk_cnt, sizeof(TkCounters), h->tk_int, 9*ST_MAXOBJ, h->tk_keys, tkeys, h->tk_eig, npx,
+           h->tk_corners, 2*npx, h->dt_dx, npx, h->dt_dy, npx, h->dt_box, 3*npx, h->dt_keys, keycap, h->tk_kp, 2*ocap, h->tk_age, ocap,
+           h->tk_tid, ocap, h->tk_lab, ocap, h->tk_src, ocap) || grow_resolver(h, npx)) return -3;
+  TkRow* rows = reinterpret_cast<TkRow*>(h->tk_rows.p); TkCounters* cnt = reinterpret_cast<TkCounters*>(h->tk_cnt.p);
+  int* const d_bb = h->tk_int; int* const d_K = d_bb + 4*ST_MAXOBJ; int* const d_cand = d_K + ST_MAXOBJ; int* const d_off = d_cand + ST_MAXOBJ;
+  int* const d_ncorn = d_off + ST_MAXOBJ; int* const d_nsel = d_ncorn + ST_MAXOBJ;
+  TkParams P; P.track = T; P.max_age = T.max_dynamic_feature_age; P.expiry = expiry; P.max_features = prm->max_features;
+  P.min_tracks = prm->min_tracks; P.quality = prm->quality_level; P.min_iou = prm->min_iou;
+  const Disc disc = make_disc(T.min_distance);
+  FCK(cudaEventRecord(h->e0, h->s));
+  if (!resident) {                                               // as dynofront_klt_track: the resident pyramids are overwritten
+    if (build_pyramid(h, 0, prev_gray, top, prm->win, true)) return -3;
+    if (build_pyramid(h, 1, cur_gray, top, prm->win, false)) return -3;
+    h->have_pyr = h->have_pyr_cur = false;
+  }
+  if (n) {
+    FCK(cudaMemcpyAsync(h->k_prev, prev_kp, 2*(size_t)n*4, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->k_next, h->k_prev, 2*(size_t)n*4, cudaMemcpyDeviceToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->f_lab, prev_label, (size_t)n*4, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->f_age, prev_age, (size_t)n*4, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->f_tid, prev_tracklet, (size_t)n*8, cudaMemcpyHostToDevice, h->s));
+  }
+  if (n_objects) {
+    FCK(cudaMemcpyAsync(h->d_objs, objects, (size_t)n_objects*4, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(d_bb, inner_bb, (size_t)n_objects*16, cudaMemcpyHostToDevice, h->s));
+  }
+  prepare_det_work(h);                                          // detection_mask_impl starts as the boundary mask (255 without one)
+  const unsigned gp = (unsigned)((npx + 255)/256);
+  fill_i32_kernel<<<gp, 256, 0, h->s>>>(h->cell, npx, -1);
+  fill_i32_kernel<<<gp, 256, 0, h->s>>>(h->trk_idx, npx, 0);
+  tk_init_kernel<<<1, 128, 0, h->s>>>(n_objects + 1, rows, cnt, d_cand);
+  // (1) forward LK on levels 0..top (flags 0)
+  klt_launch(h, klt_levels(h, top, 0), n, h->k_prev, h->k_next, h->k_st, prm->win, prm->max_count, prm->epsilon, 0, (float)prm->min_eig_threshold, h->k_eig);
+  // (2) per feature: gather, greedy disc resolution, counters, sort keys of the tracked features; the two masks
+  if (n) {
+    const int g = (n + 127)/128;
+    tk_gather_kernel<<<g, 128, 0, h->s>>>(n, h->k_next, h->k_st, h->f_lab, h->f_age, h->mask, h->has_det ? h->det.p : nullptr, W, H, P, h->f_x, h->f_y,
+                                          h->f_state, h->f_oage, h->f_olab);
+    td_link_kernel<<<g, 128, 0, h->s>>>(n, h->f_x, h->f_y, h->f_state, W, h->cell, h->f_next);
+    td_resolve_kernel<<<1, 1024, 0, h->s>>>(n, h->f_x, h->f_y, h->f_state, h->cell, h->f_next, W, H, disc, T.max_dynamic_feature_age, h->f_tid,
+                                            h->f_oage, h->f_otid, h->f_acc, h->nextid, TK_MASKED);
+    tk_count_kernel<<<g, 128, 0, h->s>>>(n, h->k_prev, h->k_next, h->f_x, h->f_y, h->f_state, h->cell, h->f_next, disc, W, H, h->f_lab, h->f_oage,
+                                         h->f_olab, h->d_objs, n_objects, P, rows, cnt, h->tk_keys, h->f_flow);
+    td_masks_kernel<<<g, 128, 0, h->s>>>(n, h->f_x, h->f_y, h->f_acc, W, H, disc, h->det_work, h->trk_idx);
+    sort_keys_desc(h, h->tk_keys, &cnt->tracked, tkeys);
+  }
+  td_trk_final_kernel<<<gp, 256, 0, h->s>>>(npx, h->trk_idx, h->f_olab, h->trk);
+  // (3) requiresSampling, (4) goodFeaturesToTrack per sampled object on the mono image, (5) range-tree ANMS
+  if (n_objects) {
+    const uint8_t* mono = h->pyr[1][0];
+    const dim3 blk(32, 8), grd((W + 31)/32, (H + 7)/8);
+    tk_decide_kernel<<<1, ST_MAXOBJ, 0, h->s>>>(n_objects, d_bb, P, rows, d_K);
+    dt_sobel_kernel<<<grd, blk, 0, h->s>>>(mono, W, H, h->dt_dx, h->dt_dy);
+    dt_box_kernel<<<(3*W + 31)/32, 32, 0, h->s>>>(h->dt_dx, h->dt_dy, W, H, h->dt_box);
+    tk_eig_kernel<<<gp, 256, 0, h->s>>>(h->dt_box, npx, h->mask, h->det_work, h->d_objs, n_objects, rows, h->tk_eig);
+    tk_cand_kernel<<<grd, blk, 0, h->s>>>(h->tk_eig, W, H, h->mask, h->det_work, h->d_objs, n_objects, rows, prm->quality_level, h->dt_keys, cnt, d_cand);
+    sort_keys_desc(h, h->dt_keys, &cnt->cand, keycap);
+    tk_offsets_kernel<<<1, 32, 0, h->s>>>(n_objects, d_cand, d_off);
+    dt_gftt_select_kernel<<<n_objects, SEL_THREADS, 0, h->s>>>(h->dt_keys, d_off, d_cand, (1u << TK_ADDR_BITS) - 1u, W, H, T.min_distance, prm->max_features,
+                                                                h->sel_px, h->sel_py, h->sel_next, h->sel_orig, h->tk_corners, d_ncorn, nullptr);
+    anms_range_tree_kernel<<<n_objects, SEL_THREADS, 0, h->s>>>(d_off, d_ncorn, d_K, nullptr, 0.01f, nullptr, h->tk_corners, 0, W, H, h->sel_px, h->sel_py,
+                                                                 h->sel_orig, h->sel_next, h->sel_out, d_nsel);
+  }
+  // (6) the output features
+  const long long base_id = *next_tracklet_id;
+  tk_construct_kernel<<<1, 1024, 0, h->s>>>(h->tk_keys, h->k_next, h->f_oage, h->f_olab, h->f_tid, h->d_objs, n_objects, d_off, d_nsel, h->sel_out,
+                                            h->tk_corners, W, H, P, base_id, rows, cnt, h->tk_kp, h->tk_age, h->tk_tid, h->tk_lab, h->tk_src);
+  FCK(cudaGetLastError());
+  TkRow hr[ST_MAXOBJ + 1]; TkCounters hc;
+  FCK(cudaMemcpyAsync(hr, rows, (size_t)(n_objects + 1)*sizeof(TkRow), cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(&hc, cnt, sizeof(hc), cudaMemcpyDeviceToHost, h->s));
+  if (n) {
+    if (lk_pts) FCK(cudaMemcpyAsync(lk_pts, h->k_next, 2*(size_t)n*4, cudaMemcpyDeviceToHost, h->s));
+    if (lk_status) FCK(cudaMemcpyAsync(lk_status, h->k_st, n, cudaMemcpyDeviceToHost, h->s));
+    if (measured_flow) FCK(cudaMemcpyAsync(measured_flow, h->f_flow, 2*(size_t)n*8, cudaMemcpyDeviceToHost, h->s));
+  }
+  std::vector<int> st_host(state && n ? n : 0);
+  if (state && n) FCK(cudaMemcpyAsync(st_host.data(), h->f_state, (size_t)n*4, cudaMemcpyDeviceToHost, h->s));
+  if (detection_mask_out) FCK(cudaMemcpyAsync(detection_mask_out, h->det_work, npx, cudaMemcpyDeviceToHost, h->s));
+  if (tracking_mask_out) FCK(cudaMemcpyAsync(tracking_mask_out, h->trk, npx, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  const int total = hc.features, ncopy = std::min(total, capacity);
+  if (ncopy) {
+    FCK(cudaMemcpyAsync(keypoint, h->tk_kp, 2*(size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(age, h->tk_age, (size_t)ncopy*4, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(tracklet, h->tk_tid, (size_t)ncopy*8, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(label, h->tk_lab, (size_t)ncopy*4, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(source, h->tk_src, (size_t)ncopy*4, cudaMemcpyDeviceToHost, h->s));
+  }
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  FCK(cudaGetLastError());
+  for (int i = 0; i < (int)st_host.size(); i++) state[i] = (uint8_t)st_host[i];
+  for (int r = 0; r <= n_objects; r++) {
+    const TkRow& x = hr[r]; dynofront_object_status& s = status[r];
+    s.object_id = r ? objects[r - 1] : 0; s.exists = x.exists; s.num_previous_track = x.prev; s.num_track = x.track;
+    s.num_outside_shrunken_image = x.shrunk; s.num_tracked_with_different_label = x.diff; s.num_tracked_with_background_label = x.bg;
+    s.object_new = x.is_new; s.object_resampled = x.resampled; s.sampled = x.sampled; s.num_sampled = x.num_sampled;
+  }
+  const int n_new = total - hc.tracked;
+  *next_tracklet_id = base_id + n_new; *n_features = total;
+  if (n_outside_image) *n_outside_image = hc.outside;
   if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
   return 0;
 }

@@ -17,6 +17,7 @@
  *   dynofront_update_depths     Frame::updateDepths                 dynosam/src/frontend/vision/Frame.cc:241-251,430-467
  *   dynofront_back_project      RGBDInstanceFrontendModule::fillOutputPacketWithTracks, per feature  RGBDInstanceFrontendModule.cc:391-486
  *   dynofront_dense_cloud       Frame::projectToDenseCloud          Frame.cc:172-238
+ *   dynofront_track_dynamic_klt FeatureTracker::trackDynamicKLT + requiresSampling: LK, checks, circles, GFTT + ANMS per object  FeatureTracker.cc:500-862,1018-1149
  *   dynofront_klt_track         cv::calcOpticalFlowPyrLK as called by KltFeatureTracker::trackPoints
  *                               (StaticFeatureTracker.cc:420-625) and FeatureTracker::trackDynamicKLT (FeatureTracker.cc:500-862)
  * Images are row-major, tightly packed: flow float32[H][W][2] (CV_32FC2), masks int32[H][W] (CV_32S, ObjectId),
@@ -286,6 +287,80 @@ int dynofront_back_project(dynofront_handle h, int32_t n, const double* kp, cons
  * u32[H][W], valid u8[H][W] (any may be NULL); *n_valid (may be NULL) = the number of kept pixels. */
 int dynofront_dense_cloud(dynofront_handle h, const double* calib5, double max_background_depth, double max_object_depth, float* xyz, uint8_t* rgb,
                           uint32_t* label, uint8_t* valid, int32_t* n_valid, float* ms_device);
+
+/* ---- FeatureTracker::trackDynamicKLT with its requiresSampling as ONE call (FeatureTracker.cc:500-862,1018-1149): the dynamic
+ * tracker of the shipped configuration (tracker_params.prefer_provided_optical_flow: false).  Nothing returns to the host between
+ * the stages.
+ *   images: prev_gray == cur_gray == NULL uses the resident pair of dynofront_next_frame; otherwise both are uploaded and the
+ *     resident pyramids are invalidated (as dynofront_klt_track).  The motion mask, the boundary mask (the initial
+ *     detection_mask_impl, 255 without one) and the mono image are the current frame's;
+ *   LK: forward cv::calcOpticalFlowPyrLK(prev, cur, prev_kp, ..., (win, win), max_level, (EPS|COUNT, max_count, epsilon), flags 0,
+ *     min_eig_threshold) with dynofront_klt_track's semantics.  The reference runs cv::cuda::SparsePyrLKOpticalFlow; the contract
+ *     here is CPU OpenCV with the criteria of the reference's own commented-out CPU call (:625-639: 21x21, 3 levels, 30, 0.03);
+ *   previous features (the usable dynamic features of the previous frame, in container order): prev_kp[n][2] as toOpenCV gives it
+ *     (float), label, age, tracklet id.  measured_flow[n][2] (may be NULL) = the previous feature's updated measuredFlow,
+ *     (double)kp_current - (double)prev_kp (:578), 0 where the feature is not tracked; the reference subtracts its double key-point,
+ *     which equals prev_kp for every key-point this tracker made (LK outputs and whole pixels);
+ *   per previous feature: lk_pts[n][2] / lk_status[n] (may be NULL) the LK result, state[n] (may be NULL) one of DYNOFRONT_DKLT_*:
+ *     TRACKED    accepted: label at the truncated pixel != 0 and == the previous label, contained, inside the shrunken image,
+ *                age + 1 <= max_dynamic_feature_age; it draws a filled circle of radius min_distance at the truncated (x, y) into
+ *                the detection mask (0) and the tracking mask (the label, last writer wins);
+ *     MASKED     the detection mask is 0 at the truncated pixel when the feature is visited (:704-710): the boundary mask or the
+ *                disc of an EARLIER accepted feature.  Not counted anywhere;
+ *     REJECTED   visited and counted under its predicted label (num_previous_track, the background / different-label counters,
+ *                num_outside_shrunken_image) but not accepted -- including age + 1 > max_dynamic_feature_age, which drops the
+ *                feature (no circle, no num_track; trackDynamic hands out a new id instead);
+ *     OUTSIDE    status good, but the truncated pixel lies outside the image (cv::Mat::at out of range in the reference): dropped,
+ *                counted in *n_outside_image only;
+ *     LOST       LK status 0;
+ *   objects[n_objects] (ids > 0, distinct, at most 64) and inner_bb[n_objects][4] (x, y, w, h) as ObjectBoundaryMaskResult holds
+ *     objects_detected and inner_boarder_object_bounding_boxes;
+ *   requiresSampling, object by object in the given order: an object without a status row is new (sampled, object_new and
+ *     object_resampled set); an object with a row (made by any counted feature whose predicted label it is) but no tracked feature
+ *     is skipped (:1080-1085); otherwise it is sampled when geriatric / num_track > 0.8 (age > max_dynamic_feature_age - max(3,
+ *     age_buffer)), num_track < min_tracks or calculateIoU(inner_bb, cv::boundingRect(tracked float key-points)) < min_iou
+ *     (cv::Rect intersection, int areas; OpenCVUtils.cc:87-102);
+ *   re-sampling of each sampled object: goodFeaturesToTrack(mono, max_features, quality_level, min_distance, (motion_mask == id) &
+ *     detection_mask_impl) on the raw mono image (block size 3, no Harris, no CLAHE); the range-tree ANMS with K = max(max_features
+ *     - num_track, 0) and tolerance 0.01 under the conventions of dynofront_anms_range_tree (K = 0: nothing, K = 1: the first point
+ *     in visiting order; every key has response 1 after KeyPoint::convert, so the visiting order is P_n); num_sampled = the ANMS
+ *     output size; then the shrunken-image test, before a tracklet id is taken (:538-542);
+ *   output features: first the tracked ones grouped by ascending object id (tracks_per_object is an ordered map), each group in
+ *     input order, then the new ones object by object in objects order, each object's in ANMS order (the reference keeps them in a
+ *     tbb::concurrent_unordered_map, so its order, and that of their ids, is unspecified).  Per feature: keypoint[2] (double), age
+ *     (previous + 1, or 0), tracklet id (the previous one, or counting up from *next_tracklet_id, which is updated), label and
+ *     source (index of the previous feature, -1 for a new one).  *n_features = how many; the first min(n_features, capacity) rows
+ *     are written;
+ *   status[n_objects + 1]: row 0 is label 0, row 1 + o is objects[o] (the PerObjectStatus counters the call touches);
+ *   detection_mask_out / tracking_mask_out (u8[H][W], may be NULL): detection_mask_impl after the circles and the tracking mask.
+ *     The detection mask also stays on the device, as after dynofront_track_dynamic.
+ * Refused with -1: an image whose side plus the widest ANMS width exceeds 65535 or that has more than 2^26 pixels,
+ * max_dynamic_feature_age - max(3, age_buffer) <= 0 (a CHECK in the reference), min_distance outside [0, 15]. */
+enum { DYNOFRONT_DKLT_TRACKED = 1, DYNOFRONT_DKLT_MASKED = 2, DYNOFRONT_DKLT_REJECTED = 3, DYNOFRONT_DKLT_OUTSIDE = 4, DYNOFRONT_DKLT_LOST = 5 };
+typedef struct {
+  int32_t win, max_level, max_count; double epsilon; double min_eig_threshold;   /* LK: 21, 3, 30, 0.03, 1e-4 */
+  dynofront_track_params track;     /* max_dynamic_feature_age 20, min_distance_btw_tracked_and_detected_dynamic_features 2, shrink 0 */
+  int32_t max_features;             /* max_dynamic_features_per_frame 200: GFTT maxCorners and the base of the ANMS K */
+  double quality_level;             /* GFTT quality 0.01 (FeatureTracker.cc:783) */
+  int32_t age_buffer, min_tracks;   /* dynamic_feature_age_buffer 3, min_dynamic_tracks 20 */
+  double min_iou;                   /* min_dynamic_mask_iou 0.1 */
+} dynofront_klt_dynamic_params;
+typedef struct {
+  int32_t object_id;                /* 0 for row 0 */
+  int32_t exists;                   /* FeatureTrackerInfo holds a PerObjectStatus for it after the call */
+  int32_t num_previous_track, num_track, num_outside_shrunken_image, num_tracked_with_different_label, num_tracked_with_background_label;
+  int32_t object_new, object_resampled;
+  int32_t sampled;                  /* re-sampled at this frame (in objects_to_sample) */
+  int32_t num_sampled;
+} dynofront_object_status;
+void dynofront_klt_dynamic_default_params(dynofront_klt_dynamic_params* p);
+int dynofront_track_dynamic_klt(dynofront_handle h, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n, const float* prev_kp,
+                                const int32_t* prev_label, const int32_t* prev_age, const int64_t* prev_tracklet, int32_t n_objects,
+                                const int32_t* objects, const int32_t* inner_bb, const dynofront_klt_dynamic_params* prm, int64_t* next_tracklet_id,
+                                float* lk_pts, uint8_t* lk_status, uint8_t* state, double* measured_flow, int32_t capacity, double* keypoint,
+                                int32_t* age, int64_t* tracklet, int32_t* label, int32_t* source, int32_t* n_features,
+                                dynofront_object_status* status, int32_t* n_outside_image, uint8_t* detection_mask_out, uint8_t* tracking_mask_out,
+                                float* ms_device);
 
 /* parity hooks: pyramid level / Scharr derivative of the last prev image (level l): sizes via w,h out */
 int dynofront_get_pyramid_level(dynofront_handle h, int32_t which /*0 prev,1 cur*/, int32_t level, int32_t* w, int32_t* hgt,
