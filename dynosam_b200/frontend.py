@@ -17,7 +17,8 @@ EXPORTS = ["dynofront_create", "dynofront_destroy", "dynofront_last_error", "dyn
            "dynofront_detect_static", "dynofront_detect_last_stages", "dynofront_set_depth", "dynofront_update_depths",
            "dynofront_back_project", "dynofront_dense_cloud", "dynofront_homography_default_params", "dynofront_find_homography_batch",
            "dynofront_homography_last_trace", "dynofront_homography_record_counts", "dynofront_klt_track_points",
-           "dynofront_klt_dynamic_default_params", "dynofront_track_dynamic_klt"]
+           "dynofront_klt_dynamic_default_params", "dynofront_track_dynamic_klt", "dynofront_fundamental_default_params",
+           "dynofront_find_fundamental_batch", "dynofront_fundamental_last_trace", "dynofront_fundamental_record"]
 
 
 class TrackParamsC(C.Structure):
@@ -91,6 +92,24 @@ class HomographyParams:
 
 
 HOM_OK, HOM_TOO_FEW, HOM_FOUR_POINT, HOM_RANSAC_FAILED = 0, 1, 2, 3     # dynofront_find_homography_batch status
+
+
+class FundamentalParamsC(C.Structure):
+    _fields_ = [("threshold_px", C.c_double), ("confidence", C.c_double), ("max_iters", C.c_int32)]
+
+
+@dataclass
+class FundamentalParams:
+    """cv::findFundamentalMat(p1, p2, FM_RANSAC, threshold_px, confidence, max_iters) as stereoTrack calls it"""
+    threshold_px: float = 1.0
+    confidence: float = 0.99
+    max_iters: int = 1000
+
+    def c(self):
+        return FundamentalParamsC(float(self.threshold_px), float(self.confidence), int(self.max_iters))
+
+
+FUND_OK, FUND_LMEDS, FUND_SEVEN_POINT, FUND_TOO_FEW, FUND_FAILED = 0, 1, 2, 3, 4     # dynofront_find_fundamental_batch status
 
 
 class KltDynamicParamsC(C.Structure):
@@ -182,6 +201,12 @@ def load():
                                                      [C.c_void_p]*5 + [C.POINTER(C.c_float)]
         L.dynofront_homography_last_trace.argtypes = [C.c_void_p] + [C.c_void_p]*4 + [C.c_int32, C.c_void_p, C.POINTER(C.c_int32)]
         L.dynofront_homography_record_counts.argtypes = [C.c_void_p, C.c_int32]
+        L.dynofront_fundamental_default_params.argtypes = [C.POINTER(FundamentalParamsC)]
+        L.dynofront_fundamental_default_params.restype = None
+        L.dynofront_find_fundamental_batch.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(FundamentalParamsC)] + \
+                                                      [C.c_void_p]*6 + [C.POINTER(C.c_float)]
+        L.dynofront_fundamental_last_trace.argtypes = [C.c_void_p] + [C.c_void_p]*5 + [C.c_int32, C.c_void_p, C.POINTER(C.c_int32)]
+        L.dynofront_fundamental_record.argtypes = [C.c_void_p, C.c_int32]
         L.dynofront_klt_track_points.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.POINTER(KltFbParamsC), C.POINTER(HomographyParamsC)] + [C.c_void_p]*4 + \
                                                 [C.POINTER(C.c_int32)]*4 + [C.POINTER(C.c_float)]
@@ -508,6 +533,45 @@ class FeatureTrackerGPU:
         self._ck(self.lib.dynofront_homography_last_trace(self.h, _p(st), _p(g), _p(rj), _p(b), int(counts_cap), _p(cnt) if counts_cap else None,
                                                           C.byref(npb)))
         return dict(status=st[:P], groups=g[:P], rejected=rj[:P], best=b[:P], counts=cnt[:P, :counts_cap])
+
+    def find_fundamental_batch(self, problems, prm: FundamentalParams | None = None):
+        """cv::findFundamentalMat(p1, p2, FM_RANSAC, ...) on every problem in one launch.  problems: sequence of (p1 [n][2],
+        p2 [n][2]).  Returns a dict: F [P][3][3][3] (up to 3 models, 0 past n_models), n_models, masks (one u8 array per problem),
+        n_inliers, status (FUND_*), iterations."""
+        p1s = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1, 2) for a, _ in problems]
+        p2s = [np.ascontiguousarray(b, dtype=np.float32).reshape(-1, 2) for _, b in problems]
+        if any(a.shape != b.shape for a, b in zip(p1s, p2s)):
+            raise ValueError("find_fundamental_batch: p1 and p2 of a problem must have the same length")
+        P = len(p1s)
+        off = np.zeros(P + 1, np.int32); off[1:] = np.cumsum([len(a) for a in p1s])
+        p1 = np.ascontiguousarray(np.concatenate(p1s) if P else np.zeros((0, 2), np.float32))
+        p2 = np.ascontiguousarray(np.concatenate(p2s) if P else np.zeros((0, 2), np.float32))
+        m = max(P, 1)
+        F = np.zeros((m, 27)); mask = np.zeros(max(int(off[-1]), 1), np.uint8)
+        nm = np.zeros(m, np.int32); ninl = np.zeros(m, np.int32); st = np.zeros(m, np.int32); it = np.zeros(m, np.int32); ms = C.c_float()
+        pc = (prm or FundamentalParams()).c()
+        self._ck(self.lib.dynofront_find_fundamental_batch(self.h, P, _p(off), _p(p1), _p(p2), C.byref(pc), _p(F), _p(nm), _p(mask), _p(ninl),
+                                                           _p(st), _p(it), C.byref(ms)))
+        self.last_ms = ms.value
+        return dict(F=F[:P].reshape(P, 3, 3, 3), n_models=nm[:P], masks=[mask[off[p]:off[p + 1]].copy() for p in range(P)],
+                    n_inliers=ninl[:P], status=st[:P], iterations=it[:P])
+
+    def fundamental_record(self, iters_cap):
+        """record (models, scores) of each of the first iters_cap iterations in the following calls (0: none, the default)"""
+        self._ck(self.lib.dynofront_fundamental_record(self.h, int(iters_cap)))
+
+    def fundamental_trace(self, iters_cap=0):
+        """the draw trace of the last find_fundamental_batch: groups, rejected, best (iteration), best_root, success per problem,
+        and record [P][iters_cap][4] = (models of the draw, score of root 0, 1, 2) as recorded after fundamental_record (NaN
+        where nothing was recorded; the score is the inlier count under RANSAC, the median error under LMedS)"""
+        npb = C.c_int32()
+        self._ck(self.lib.dynofront_fundamental_last_trace(self.h, None, None, None, None, None, 0, None, C.byref(npb)))
+        P = npb.value; m = max(P, 1)
+        a = [np.zeros(m, np.int32) for _ in range(5)]
+        rec = np.zeros((m, max(iters_cap, 1), 4), np.float32)
+        self._ck(self.lib.dynofront_fundamental_last_trace(self.h, *[_p(x) for x in a], int(iters_cap), _p(rec) if iters_cap else None,
+                                                           C.byref(npb)))
+        return dict(groups=a[0][:P], rejected=a[1][:P], best=a[2][:P], best_root=a[3][:P], success=a[4][:P], record=rec[:P, :iters_cap])
 
     def stereo_track(self, left_gray, right_gray, left_pts, fx, baseline):
         """FeatureTracker::stereoTrack without its RANSAC: (right_pts, status, depth, valid)"""

@@ -80,6 +80,9 @@ struct dynofront_ctx {
   // homography RANSAC: inputs, point / inlier lists, outputs, per-problem statistics (6 arrays of hm_np) and per-iteration counts
   DevBuf<int> hm_off, hm_cidx, hm_lidx, hm_stat, hm_counts; DevBuf<float> hm_src, hm_dst; DevBuf<float4> hm_inl; DevBuf<double> hm_H; DevBuf<uint8_t> hm_mask;
   int hm_np = 0, hm_cap = 0, hm_record = 0;       // problems and recorded iterations of the last call; iterations to record
+  // fundamental-matrix RANSAC: inputs, outputs, per-problem statistics (9 arrays of fm_np) and the per-iteration record
+  DevBuf<int> fm_off, fm_stat; DevBuf<float> fm_src, fm_dst, fm_rec; DevBuf<double> fm_F; DevBuf<uint8_t> fm_mask;
+  int fm_np = 0, fm_cap = 0, fm_record = 0;
   // trackDynamicKLT (also uses the trackDynamic, KLT, detection and ANMS scratch): status rows, counters, per-object lists (tk_int:
   // bb[4][64], K, cand, off, corners, selected), tracked sort keys, eigen image, GFTT corners, output features
   DevBuf<unsigned char> tk_rows, tk_cnt; DevBuf<int> tk_int, tk_corners; DevBuf<unsigned long long> tk_keys; DevBuf<float> tk_eig;
@@ -1287,11 +1290,13 @@ __device__ bool hom_kernel4(const float* Ms, const float* ms, double* H) {
   hom_from_ltl(L, c, s, H);
   return true;
 }
-__device__ bool hom_collinear(const float* p) {       // haveCollinearPoints(ms, 4): float differences, double products
-  for (int j = 0; j < 3; j++) {
-    const double dx1 = p[2*j] - p[6], dy1 = p[2*j + 1] - p[7];
+// haveCollinearPoints(ms, K): triples (j, k, K-1), k < j, float differences, double products
+template <int K> __device__ bool hom_collinear(const float* p) {
+  const int i = K - 1;
+  for (int j = 0; j < i; j++) {
+    const double dx1 = p[2*j] - p[2*i], dy1 = p[2*j + 1] - p[2*i + 1];
     for (int k = 0; k < j; k++) {
-      const double dx2 = p[2*k] - p[6], dy2 = p[2*k + 1] - p[7];
+      const double dx2 = p[2*k] - p[2*i], dy2 = p[2*k + 1] - p[2*i + 1];
       if (fabs(dx2*dy1 - dy2*dx1) <= FLT_EPSILON*(fabs(dx1) + fabs(dy1) + fabs(dx2) + fabs(dy2))) return true;
     }
   }
@@ -1302,7 +1307,7 @@ __device__ __forceinline__ double hom_det3(const float* p, int a, int b, int c) 
   return a00*(a11*1.0 - a21*1.0) - a01*(a10*1.0 - a20*1.0) + 1.0*(a10*a21 - a20*a11);
 }
 __device__ bool hom_check_subset(const float* S, const float* D) {
-  if (hom_collinear(S) || hom_collinear(D)) return false;
+  if (hom_collinear<4>(S) || hom_collinear<4>(D)) return false;
   const int tt[4][3] = {{0, 1, 2}, {1, 2, 3}, {0, 2, 3}, {0, 1, 3}};
   int neg = 0;
   for (int i = 0; i < 4; i++) neg += hom_det3(S, tt[i][0], tt[i][1], tt[i][2])*hom_det3(D, tt[i][0], tt[i][1], tt[i][2]) < 0;
@@ -1313,10 +1318,10 @@ __device__ __forceinline__ float hom_err(const float* Hf, float x, float y, floa
   const float dx = (Hf[0]*x + Hf[1]*y + Hf[2])*ww - u, dy = (Hf[3]*x + Hf[4]*y + Hf[5])*ww - v;
   return dx*dx + dy*dy;
 }
-// RANSACUpdateNumIters(p, ep, 4, niters)
-__device__ int hom_update_iters(double p, double ep, int max_iters) {
+// RANSACUpdateNumIters(p, ep, model_points, niters)
+__device__ int hom_update_iters(double p, double ep, int model_points, int max_iters) {
   p = fmin(fmax(p, 0.), 1.); ep = fmin(fmax(ep, 0.), 1.);
-  double num = fmax(1. - p, DBL_MIN), denom = 1. - pow(1. - ep, 4.0);
+  double num = fmax(1. - p, DBL_MIN), denom = 1. - pow(1. - ep, (double)model_points);
   if (denom < DBL_MIN) return 0;
   num = log(num); denom = log(denom);
   return denom >= 0 || -num >= max_iters*(-denom) ? max_iters : __double2int_rn(num/denom);
@@ -1364,6 +1369,18 @@ template <class F, class G> __device__ int hom_compact(int n, F flag, G value, i
   }
   return base;
 }
+// the next `count` groups of K distinct indices in [0, n) from cv::RNG state st (getSubset: a duplicate is re-drawn at once) into
+// grp[count][K]; returns the new state
+template <int K> __device__ unsigned long long hom_draw_groups(unsigned long long st, int n, int count, int* grp) {
+  for (int g = 0; g < count; g++)
+    for (int i = 0; i < K;) {
+      st = (unsigned long long)(unsigned)st*4164903690ull + (st >> 32);
+      const int k = (int)((unsigned)st % (unsigned)n);
+      bool dup = false; for (int j = 0; j < i; j++) dup |= grp[K*g + j] == k;
+      if (!dup) grp[K*g + i++] = k;
+    }
+  return st;
+}
 
 __global__ void __launch_bounds__(HOM_THREADS) hom_ransac_kernel(HomBatch B) {
   __shared__ int sh_grp[HOM_CHUNK][4];
@@ -1409,17 +1426,7 @@ __global__ void __launch_bounds__(HOM_THREADS) hom_ransac_kernel(HomBatch B) {
   int* counts = B.counts ? B.counts + (size_t)pb*B.counts_cap : nullptr;
   for (int c = 0; !sh_done; c++) {
     const int nch = min(HOM_CHUNK, 32 << min(c, 3));
-    if (t == 0) {                                // the draw stream, cut into groups of 4 distinct indices
-      unsigned long long st = sh_rng;
-      for (int g = 0; g < nch; g++)
-        for (int i = 0; i < 4;) {
-          st = (unsigned long long)(unsigned)st*4164903690ull + (st >> 32);
-          const int k = (int)((unsigned)st % (unsigned)n);
-          bool dup = false; for (int j = 0; j < i; j++) dup |= sh_grp[g][j] == k;
-          if (!dup) sh_grp[g][i++] = k;
-        }
-      sh_rng = st;
-    }
+    if (t == 0) sh_rng = hom_draw_groups<4>(sh_rng, n, nch, &sh_grp[0][0]);     // the draw stream, cut into groups of 4
     __syncthreads();
     if (t < nch) {                               // subset test and 4-point model, one thread per group
       float Ms[8], ms[8];
@@ -1463,7 +1470,7 @@ __global__ void __launch_bounds__(HOM_THREADS) hom_ransac_kernel(HomBatch B) {
         if (cnt > max(best, 3)) {
           best = cnt; sh_best_it = it;
           for (int e = 0; e < 9; e++) sh_best[e] = sh_H[m][e];
-          niters = hom_update_iters(B.conf, (double)(n - cnt)/n, niters);
+          niters = hom_update_iters(B.conf, (double)(n - cnt)/n, 4, niters);
         }
         if (++it >= niters) { done = true; break; }
       }
@@ -1603,6 +1610,359 @@ __global__ void __launch_bounds__(HOM_THREADS) hom_ransac_kernel(HomBatch B) {
   if (t < 9) Hout[t] = sh_best[t];
   if (t == 0) { B.status[pb] = HOM_OK; B.n_inl[pb] = sh_ninl; B.iters[pb] = sh_it; B.groups[pb] = sh_groups; B.rejected[pb] = sh_rej; B.best[pb] = sh_best_it; }
 }
+// ---------------------------------------------------------------------------------------------------- fundamental-matrix RANSAC
+// cv::findFundamentalMat(p1, p2, FM_RANSAC, thr, conf, max_iters) as FeatureTracker::stereoTrack calls it (FeatureTracker.cc:279-281),
+// one persistent CTA per problem.  tests/fundamental_oracle.py restates the orders, tests/test_fundamental.py pins them against cv2:
+//  * draws: the homography's cv::RNG stream and duplicate rule, groups of 7; subset test = haveCollinearPoints on either set; 10 000
+//    (RANSAC) or 1000 (LMedS) rejections in a row end the loop (fail it in iteration 0);
+//  * model: run7Point, one thread per draw: Hartley normalisation, OpenCV's one-sided Jacobi SVD of the 7x9 system with the null
+//    space rows completed from cv::RNG(0x12345678), the determinant cubic, cv::solveCubic, per root lambda / mu scaling,
+//    de-normalisation and F / F22;
+//  * n >= 15: RANSAC.  Warps count the inliers of every (draw, root) model over points staged through shared memory; thread 0
+//    replays the loop in (draw, root) order (best when count > max(best, 6), then RANSACUpdateNumIters(conf, ., 7, niters)), so
+//    nothing depends on the chunk size;
+//  * 8 <= n < 15: LMedS.  One thread per model takes the (n/2)-th smallest float error (n is at most 14); a strictly smaller median
+//    wins; the mask is err <= sigma^2 with OpenCV's sigma;
+//  * n == 7: run7Point alone (up to 3 models, mask all ones); n < 7: no model.
+// A draw whose cubic counts as all zero (solveCubic returns -1, which cv2 4.13 does not guard and raises on) has no model.
+#define FUND_THREADS 128
+#define FUND_WARPS (FUND_THREADS/32)
+#define FUND_CHUNK 128
+enum { FUND_OK = 0, FUND_LMEDS = 1, FUND_SEVEN_POINT = 2, FUND_TOO_FEW = 3, FUND_FAILED = 4 };
+
+struct FundBatch {
+  const int* off; const float* src; const float* dst;
+  float thr2; double conf; int max_iters;
+  double* F; uint8_t* mask;                      // F[P][27]: up to 3 models, row-major
+  int* stat;                                     // 9 arrays of P: n_models, n_inliers, status, iterations, groups, rejected, best, best_root, success
+  float* rec; int rec_cap;                       // parity hook: per iteration (models, score of root 0, 1, 2), the first rec_cap iterations
+};
+
+// cv::solveCubic (OpenCV 4.13) of (a0, a1, a2, a3): the number of roots (-1: every coefficient counts as 0), roots in x.
+// Every coefficient is 0 when max|a_i| < DBL_EPSILON; a leading coefficient with |a_i * (1 / max|a_j|)| < DBL_EPSILON counts as
+// 0, cascading down; the quadratic / linear branches use the unscaled coefficients, the cubic branch the scaled ones.
+__device__ int cv_solve_cubic(double a0, double a1, double a2, double a3, double* x) {
+  x[0] = x[1] = x[2] = 0;
+  const double m = fmax(fmax(fabs(a0), fabs(a1)), fmax(fabs(a2), fabs(a3)));
+  if (!(m >= DBL_EPSILON)) return -1;
+  const double inv = 1./m;
+  auto small = [inv](double v) { return fabs(v*inv) < DBL_EPSILON; };
+  if (!small(a0)) { a0 *= inv; a1 *= inv; a2 *= inv; a3 *= inv; }
+  else { a0 = 0; if (small(a1)) { a1 = 0; if (small(a2)) { a2 = 0; if (small(a3)) a3 = 0; } } }
+  if (a0 == 0) {
+    if (a1 == 0) {
+      if (a2 == 0) return a3 == 0 ? -1 : 0;
+      x[0] = -a3/a2; return 1;
+    }
+    double d = a2*a2 - 4*a1*a3;
+    if (d < 0) return 0;
+    d = sqrt(d);
+    const double q1 = (-a2 + d)*0.5, q2 = (a2 + d)*-0.5;
+    if (fabs(q1) > fabs(q2)) { x[0] = q1/a1; x[1] = a3/q1; } else { x[0] = q2/a1; x[1] = a3/q2; }
+    return d > 0 ? 2 : 1;
+  }
+  a0 = 1./a0; a1 *= a0; a2 *= a0; a3 *= a0;
+  const double Q = (a1*a1 - 3*a2)*(1./9);
+  const double R = (a1*(2*a1*a1 - 9*a2) + 27*a3)*(1./54);
+  const double Qcubed = Q*Q*Q;
+  double d = (a1*a1*(a2*a2 - 4*a1*a3) + 2*a2*(9*a1*a3 - 2*a2*a2) - 27*a3*a3)*(1./108);
+  if (d > 0) {
+    const double theta = acos(R/sqrt(Qcubed)), t0 = -2*sqrt(Q), t1 = theta*(1./3), t2 = a1*(1./3);
+    x[0] = t0*cos(t1) - t2; x[1] = t0*cos(t1 + (2.*CUDART_PI/3)) - t2; x[2] = t0*cos(t1 + (4.*CUDART_PI/3)) - t2;
+    return 3;
+  }
+  if (d == 0) {
+    if (R >= 0) { x[0] = -2*pow(R, 1./3) - a1/3; x[1] = pow(R, 1./3) - a1/3; }
+    else { x[0] = 2*pow(-R, 1./3) - a1/3; x[1] = -pow(-R, 1./3) - a1/3; }
+    const bool one = x[0] == x[1];
+    if (one) x[1] = 0;
+    return one ? 1 : 2;
+  }
+  d = sqrt(-d);
+  double e = pow(d + fabs(R), 1./3);
+  if (R > 0) e = -e;
+  x[0] = (e + Q/e) - a1*(1./3);
+  return 1;
+}
+// JacobiSVDImpl_'s completion of row i of U[9][9] from the generator state st (the rows before it are orthonormal)
+__device__ void cv_svd_complete(double* U, int i, unsigned long long& st) {
+  const double eps = DBL_EPSILON*10;
+  double sd = 0;
+  for (int ii = 0; ii < 100 && sd <= DBL_MIN; ii++) {
+    for (int k = 0; k < 9; k++) {
+      st = (unsigned long long)(unsigned)st*4164903690ull + (st >> 32);
+      U[9*i + k] = ((unsigned)st & 256) != 0 ? 1./9 : -(1./9);
+    }
+    for (int it = 0; it < 2; it++)
+      for (int j = 0; j < i; j++) {
+        sd = 0; for (int k = 0; k < 9; k++) sd += U[9*i + k]*U[9*j + k];
+        double asum = 0;
+        for (int k = 0; k < 9; k++) { const double t = U[9*i + k] - sd*U[9*j + k]; U[9*i + k] = t; asum += fabs(t); }
+        asum = asum > eps*100 ? 1/asum : 0;
+        for (int k = 0; k < 9; k++) U[9*i + k] *= asum;
+      }
+    sd = 0; for (int k = 0; k < 9; k++) sd += U[9*i + k]*U[9*i + k];
+    sd = sqrt(sd);
+  }
+  const double s = sd > DBL_MIN ? 1/sd : 0.;
+  for (int k = 0; k < 9; k++) U[9*i + k] *= s;
+}
+// SVDecomp(A, W, U, Vt, MODIFY_A | FULL_UV) of the 7x9 A held in U's first 7 rows: U becomes Vt (9x9).  OpenCV transposes the
+// problem, so the one-sided Jacobi rotates the 7 rows; rows past the rank come from cv::RNG(0x12345678).
+__device__ void cv_svd7x9(double* U) {
+  const double eps = DBL_EPSILON*10;
+  double W[7];
+  for (int i = 0; i < 7; i++) { double s = 0; for (int k = 0; k < 9; k++) s += U[9*i + k]*U[9*i + k]; W[i] = s; }
+  for (int iter = 0; iter < 30; iter++) {
+    bool changed = false;
+    for (int i = 0; i < 6; i++)
+      for (int j = i + 1; j < 7; j++) {
+        double* Ai = U + 9*i; double* Aj = U + 9*j;
+        const double a = W[i], b = W[j];
+        double p = 0; for (int k = 0; k < 9; k++) p += Ai[k]*Aj[k];
+        if (fabs(p) <= eps*sqrt(a*b)) continue;
+        p *= 2;
+        const double beta = a - b, gamma = cv_hypot(p, beta);
+        double c, s;
+        if (beta < 0) { const double delta = (gamma - beta)*0.5; s = sqrt(delta/gamma); c = p/(gamma*s*2); }
+        else { c = sqrt((gamma + beta)/(gamma*2)); s = p/(gamma*c*2); }
+        double na = 0, nb = 0;
+        for (int k = 0; k < 9; k++) {
+          const double t0 = c*Ai[k] + s*Aj[k], t1 = -s*Ai[k] + c*Aj[k];
+          Ai[k] = t0; Aj[k] = t1; na += t0*t0; nb += t1*t1;
+        }
+        W[i] = na; W[j] = nb;
+        changed = true;
+      }
+    if (!changed) break;
+  }
+  for (int i = 0; i < 7; i++) { double s = 0; for (int k = 0; k < 9; k++) s += U[9*i + k]*U[9*i + k]; W[i] = sqrt(s); }
+  for (int i = 0; i < 6; i++) {
+    int j = i; for (int k = i + 1; k < 7; k++) if (W[j] < W[k]) j = k;
+    if (i != j) { const double w = W[i]; W[i] = W[j]; W[j] = w; for (int k = 0; k < 9; k++) { const double q = U[9*i + k]; U[9*i + k] = U[9*j + k]; U[9*j + k] = q; } }
+  }
+  unsigned long long st = 0x12345678ull;
+  for (int i = 0; i < 9; i++) {
+    const double sd = i < 7 ? W[i] : 0;
+    if (sd <= DBL_MIN) cv_svd_complete(U, i, st);
+    else { const double s = 1/sd; for (int k = 0; k < 9; k++) U[9*i + k] *= s; }
+  }
+}
+// run7Point on 7 correspondences P1 -> P2 ([7][2] float): the number of models written to F[3][9] (-1: all-zero cubic, 0: none)
+__device__ int fund_run7(const float* P1, const float* P2, double* F) {
+  double c1x = 0, c1y = 0, c2x = 0, c2y = 0;
+  for (int i = 0; i < 7; i++) { c1x += P1[2*i]; c1y += P1[2*i + 1]; c2x += P2[2*i]; c2y += P2[2*i + 1]; }
+  const double t = 1./7;
+  c1x *= t; c1y *= t; c2x *= t; c2y *= t;
+  double s1 = 0, s2 = 0;
+  for (int i = 0; i < 7; i++) {
+    const double dx1 = P1[2*i] - c1x, dy1 = P1[2*i + 1] - c1y, dx2 = P2[2*i] - c2x, dy2 = P2[2*i + 1] - c2y;
+    s1 += sqrt(dx1*dx1 + dy1*dy1); s2 += sqrt(dx2*dx2 + dy2*dy2);
+  }
+  s1 *= t; s2 *= t;
+  if (s1 < FLT_EPSILON || s2 < FLT_EPSILON) return 0;
+  s1 = sqrt(2.)/s1; s2 = sqrt(2.)/s2;
+  double U[81];
+  for (int i = 0; i < 7; i++) {
+    const double x0 = (P1[2*i] - c1x)*s1, y0 = (P1[2*i + 1] - c1y)*s1, x1 = (P2[2*i] - c2x)*s2, y1 = (P2[2*i + 1] - c2y)*s2;
+    double* a = U + 9*i;
+    a[0] = x1*x0; a[1] = x1*y0; a[2] = x1; a[3] = y1*x0; a[4] = y1*y0; a[5] = y1; a[6] = x0; a[7] = y0; a[8] = 1;
+  }
+  cv_svd7x9(U);
+  double f1[9], f2[9];
+  for (int i = 0; i < 9; i++) { f2[i] = U[72 + i]; f1[i] = U[63 + i] - f2[i]; }
+  double t0 = f2[4]*f2[8] - f2[5]*f2[7], t1 = f2[3]*f2[8] - f2[5]*f2[6], t2 = f2[3]*f2[7] - f2[4]*f2[6];
+  const double c3 = f2[0]*t0 - f2[1]*t1 + f2[2]*t2;
+  const double c2 = f1[0]*t0 - f1[1]*t1 + f1[2]*t2 - f1[3]*(f2[1]*f2[8] - f2[2]*f2[7]) + f1[4]*(f2[0]*f2[8] - f2[2]*f2[6])
+                  - f1[5]*(f2[0]*f2[7] - f2[1]*f2[6]) + f1[6]*(f2[1]*f2[5] - f2[2]*f2[4]) - f1[7]*(f2[0]*f2[5] - f2[2]*f2[3])
+                  + f1[8]*(f2[0]*f2[4] - f2[1]*f2[3]);
+  t0 = f1[4]*f1[8] - f1[5]*f1[7]; t1 = f1[3]*f1[8] - f1[5]*f1[6]; t2 = f1[3]*f1[7] - f1[4]*f1[6];
+  const double c1 = f2[0]*t0 - f2[1]*t1 + f2[2]*t2 - f2[3]*(f1[1]*f1[8] - f1[2]*f1[7]) + f2[4]*(f1[0]*f1[8] - f1[2]*f1[6])
+                  - f2[5]*(f1[0]*f1[7] - f1[1]*f1[6]) + f2[6]*(f1[1]*f1[5] - f1[2]*f1[4]) - f2[7]*(f1[0]*f1[5] - f1[2]*f1[3])
+                  + f2[8]*(f1[0]*f1[4] - f1[1]*f1[3]);
+  const double c0 = f1[0]*t0 - f1[1]*t1 + f1[2]*t2;
+  double r[3];
+  const int n = cv_solve_cubic(c0, c1, c2, c3, r);
+  if (n < 1 || n > 3) return n;
+  const double T1[9] = {s1, 0, -s1*c1x, 0, s1, -s1*c1y, 0, 0, 1};
+  const double T2t[9] = {s2, 0, 0, 0, s2, 0, -s2*c2x, -s2*c2y, 1};
+  for (int k = 0; k < n; k++) {
+    double lambda = r[k], mu = 1., fm[9];
+    const double s = f1[8]*r[k] + f2[8];
+    if (fabs(s) > DBL_EPSILON) { mu = 1./s; lambda *= mu; fm[8] = 1.; } else fm[8] = 0.;
+    for (int i = 0; i < 8; i++) fm[i] = f1[i]*lambda + f2[i]*mu;
+    double T[9], R[9];                           // (T2^T F) T1, Matx products (sums from 0, left to right)
+    for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) { double a = 0; for (int q = 0; q < 3; q++) a += T2t[3*i + q]*fm[3*q + j]; T[3*i + j] = a; }
+    for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) { double a = 0; for (int q = 0; q < 3; q++) a += T[3*i + q]*T1[3*q + j]; R[3*i + j] = a; }
+    if (fabs(R[8]) > FLT_EPSILON) { const double inv = 1./R[8]; for (int e = 0; e < 9; e++) R[e] *= inv; }
+    for (int e = 0; e < 9; e++) F[9*k + e] = R[e];
+  }
+  return n;
+}
+// computeError: the larger squared distance to the two epipolar lines, in double, stored as float
+__device__ __forceinline__ float fund_err(const double* F, float x1f, float y1f, float x2f, float y2f) {
+  const double x1 = x1f, y1 = y1f, x2 = x2f, y2 = y2f;
+  double a = F[0]*x1 + F[1]*y1 + F[2], b = F[3]*x1 + F[4]*y1 + F[5], c = F[6]*x1 + F[7]*y1 + F[8];
+  const double s2 = 1./(a*a + b*b), d2 = x2*a + y2*b + c;
+  a = F[0]*x2 + F[3]*y2 + F[6]; b = F[1]*x2 + F[4]*y2 + F[7]; c = F[2]*x2 + F[5]*y2 + F[8];
+  const double s1 = 1./(a*a + b*b), d1 = x1*a + y1*b + c;
+  const double e1 = d1*d1*s1, e2 = d2*d2*s2;
+  return (float)(e1 < e2 ? e2 : e1);             // std::max(e1, e2)
+}
+
+__global__ void __launch_bounds__(FUND_THREADS) fund_ransac_kernel(FundBatch B) {
+  __shared__ int sh_grp[FUND_CHUNK][7];
+  __shared__ int sh_nm[FUND_CHUNK];              // -2: rejected by the subset test, else run7Point's root count
+  __shared__ double sh_F[FUND_CHUNK][27];
+  __shared__ float sh_score[FUND_CHUNK][3];      // inlier count (RANSAC) or median (LMedS) per model
+  __shared__ float4 sh_tile[FUND_THREADS];
+  __shared__ double sh_best[9];
+  __shared__ float sh_best_med;
+  __shared__ unsigned long long sh_rng;
+  __shared__ int sh_it, sh_niters, sh_best_cnt, sh_best_it, sh_best_root, sh_groups, sh_rej, sh_run, sh_done, sh_fail, sh_ninl;
+  const int pb = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int r0 = B.off[pb], n = B.off[pb + 1] - r0;
+  const float2* src = reinterpret_cast<const float2*>(B.src) + r0; const float2* dst = reinterpret_cast<const float2*>(B.dst) + r0;
+  uint8_t* mask = B.mask + r0;
+  double* Fout = B.F + 27*(size_t)pb;
+  const size_t P = gridDim.x;
+  int* n_models = B.stat; int* n_inl = B.stat + P; int* status = B.stat + 2*P; int* iters = B.stat + 3*P; int* groups = B.stat + 4*P;
+  int* rejected = B.stat + 5*P; int* best = B.stat + 6*P; int* best_root = B.stat + 7*P; int* success = B.stat + 8*P;
+  for (int i = t; i < n; i += FUND_THREADS) mask[i] = 0;
+  for (int e = t; e < 27; e += FUND_THREADS) Fout[e] = 0;
+  __syncthreads();                               // the zeros above land before any thread writes the outputs below
+  if (n <= 7) {                                  // fewer than 7: no model; exactly 7: run7Point alone
+    if (t == 0) {
+      int nm = 0;
+      if (n == 7) {
+        float P1[14], P2[14];
+        for (int i = 0; i < 7; i++) { P1[2*i] = src[i].x; P1[2*i + 1] = src[i].y; P2[2*i] = dst[i].x; P2[2*i + 1] = dst[i].y; }
+        double F[27]; nm = fund_run7(P1, P2, F);
+        if (nm > 0) for (int e = 0; e < 9*nm; e++) Fout[e] = F[e];
+        if (B.rec && B.rec_cap > 0) { float* rc = B.rec + (size_t)pb*4*B.rec_cap; rc[0] = (float)nm; }
+      }
+      const int m = nm > 0 ? nm : 0;
+      for (int i = 0; i < n; i++) mask[i] = m > 0;
+      n_models[pb] = m; n_inl[pb] = m > 0 ? n : 0; status[pb] = n == 7 ? FUND_SEVEN_POINT : FUND_TOO_FEW; iters[pb] = 0; groups[pb] = 0;
+      rejected[pb] = 0; best[pb] = -1; best_root[pb] = -1; success[pb] = m > 0;
+    }
+    return;
+  }
+  const bool lmeds = n < 15;
+  const int attempts = lmeds ? 1000 : 10000;
+  if (t == 0) {
+    sh_rng = ~0ull; sh_it = 0; sh_best_cnt = 0; sh_best_it = -1; sh_best_root = -1; sh_groups = 0; sh_rej = 0; sh_run = 0;
+    sh_done = 0; sh_fail = 0; sh_best_med = CUDART_INF_F;
+    sh_niters = lmeds ? max(hom_update_iters(B.conf, 0.45, 7, B.max_iters), 3) : max(B.max_iters, 1);
+  }
+  __syncthreads();
+  float* rec = B.rec ? B.rec + (size_t)pb*4*B.rec_cap : nullptr;
+  for (int c = 0; !sh_done; c++) {
+    const int nch = min(FUND_CHUNK, 32 << min(c, 2));
+    if (t == 0) sh_rng = hom_draw_groups<7>(sh_rng, n, nch, &sh_grp[0][0]);
+    __syncthreads();
+    if (t < nch) {                               // subset test and run7Point, one thread per draw
+      float P1[14], P2[14];
+      for (int i = 0; i < 7; i++) { const int r = sh_grp[t][i]; P1[2*i] = src[r].x; P1[2*i + 1] = src[r].y; P2[2*i] = dst[r].x; P2[2*i + 1] = dst[r].y; }
+      int nm = -2;
+      if (!hom_collinear<7>(P1) && !hom_collinear<7>(P2)) nm = fund_run7(P1, P2, sh_F[t]);
+      sh_nm[t] = nm;
+      for (int r = 0; r < 3; r++) sh_score[t][r] = 0;
+      if (lmeds) {                               // the (n/2)-th smallest error of each model (n <= 14), ordered by bit pattern
+        for (int r = 0; r < nm; r++) {
+          int e[14];
+          for (int i = 0; i < n; i++) {
+            const int v = __float_as_int(fund_err(sh_F[t] + 9*r, src[i].x, src[i].y, dst[i].x, dst[i].y));
+            int j = i; while (j > 0 && e[j - 1] > v) { e[j] = e[j - 1]; j--; }
+            e[j] = v;
+          }
+          sh_score[t][r] = __int_as_float(e[n/2]);
+        }
+      }
+    }
+    if (!lmeds) {
+      for (int tile0 = 0; tile0 < n; tile0 += FUND_THREADS) {   // inlier counts, points staged through shared memory
+        const int tn = min(FUND_THREADS, n - tile0);
+        __syncthreads();
+        if (t < tn) { const float2 a = src[tile0 + t], b = dst[tile0 + t]; sh_tile[t] = make_float4(a.x, a.y, b.x, b.y); }
+        __syncthreads();
+        for (int q = warp; q < 3*nch; q += FUND_WARPS) {
+          const int m = q/3, r = q - 3*m;
+          if (r >= sh_nm[m]) continue;
+          const double* F = sh_F[m] + 9*r;
+          int cnt = 0;
+          for (int j0 = 0; j0 < tn; j0 += 32) {
+            const int j = j0 + lane;
+            bool in = false;
+            if (j < tn) { const float4 p = sh_tile[j]; in = fund_err(F, p.x, p.y, p.z, p.w) <= B.thr2; }
+            cnt += __popc(__ballot_sync(0xffffffffu, in));
+          }
+          if (lane == 0) sh_score[m][r] += (float)cnt;
+        }
+      }
+    }
+    __syncthreads();
+    if (t == 0) {                                // the sequential loop over this chunk in (draw, root) order
+      int it = sh_it, niters = sh_niters, bcnt = sh_best_cnt, run = sh_run, grp = sh_groups, rej = sh_rej;
+      float bmed = sh_best_med;
+      bool done = false;
+      for (int m = 0; m < nch; m++) {
+        grp++;
+        if (sh_nm[m] == -2) {
+          rej++;
+          if (++run >= attempts) { done = true; if (it == 0) sh_fail = 1; break; }
+          continue;
+        }
+        run = 0;
+        const int nm = sh_nm[m];
+        if (rec && it < B.rec_cap) { float* rc = rec + 4*(size_t)it; rc[0] = (float)nm; for (int r = 0; r < nm; r++) rc[1 + r] = sh_score[m][r]; }
+        for (int r = 0; r < nm; r++) {
+          const float sc = sh_score[m][r];
+          bool take;
+          if (lmeds) { take = sc < bmed; if (take) bmed = sc; }
+          else {
+            const int cnt = (int)sc;
+            take = cnt > max(bcnt, 6);
+            if (take) { bcnt = cnt; niters = hom_update_iters(B.conf, (double)(n - cnt)/n, 7, niters); }
+          }
+          if (take) { sh_best_it = it; sh_best_root = r; for (int e = 0; e < 9; e++) sh_best[e] = sh_F[m][9*r + e]; }
+        }
+        if (++it >= niters) { done = true; break; }
+      }
+      sh_it = it; sh_niters = niters; sh_best_cnt = bcnt; sh_best_med = bmed; sh_run = run; sh_groups = grp; sh_rej = rej; sh_done = done;
+    }
+    __syncthreads();
+  }
+  if (sh_fail || sh_best_it < 0) {               // no model: F = 0, mask all zeros
+    if (t == 0) {
+      n_models[pb] = 0; n_inl[pb] = 0; status[pb] = FUND_FAILED; iters[pb] = sh_fail ? 0 : sh_it; groups[pb] = sh_groups;
+      rejected[pb] = sh_rej; best[pb] = -1; best_root[pb] = -1; success[pb] = 0;
+    }
+    return;
+  }
+  float thr2 = B.thr2;
+  if (lmeds) {
+    double sigma = 2.5*1.4826*(1 + 5./(n - 7))*sqrt((double)sh_best_med);
+    sigma = fmax(sigma, 0.001);
+    thr2 = (float)(sigma*sigma);
+  }
+  if (t == 0) sh_ninl = 0;
+  __syncthreads();
+  int cnt = 0;
+  for (int i = t; i < n; i += FUND_THREADS) {
+    const bool in = fund_err(sh_best, src[i].x, src[i].y, dst[i].x, dst[i].y) <= thr2;
+    mask[i] = in; cnt += in;
+  }
+  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if (lane == 0) atomicAdd(&sh_ninl, cnt);
+  __syncthreads();
+  if (t < 9) Fout[t] = sh_best[t];
+  if (t == 0) {
+    n_models[pb] = 1; n_inl[pb] = sh_ninl; status[pb] = lmeds ? FUND_LMEDS : FUND_OK; iters[pb] = sh_it; groups[pb] = sh_groups;
+    rejected[pb] = sh_rej; best[pb] = sh_best_it; best_root[pb] = sh_best_root; success[pb] = lmeds ? sh_ninl >= 7 : 1;
+  }
+}
+
 // klt_track_points: verified = the homography mask (0 on rows the forward-backward test dropped), keep = keep && verified
 __global__ void ktp_post_kernel(int n, const uint8_t* __restrict__ verified, uint8_t* __restrict__ keep, int check, int* __restrict__ count) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x;
@@ -2488,6 +2848,78 @@ int dynofront_homography_last_trace(dynofront_handle h, int32_t* status, int32_t
     const int w = std::min(counts_cap, h->hm_cap);
     if (w > 0)
     FCK(cudaMemcpy2D(counts, 4*(size_t)counts_cap, h->hm_counts, 4*(size_t)h->hm_cap, 4*(size_t)w, np, cudaMemcpyDeviceToHost));
+  }
+  return 0;
+}
+// ---- fundamental-matrix RANSAC
+void dynofront_fundamental_default_params(dynofront_fundamental_params* p) {
+  if (!p) return;
+  p->threshold_px = 1.0; p->confidence = 0.99; p->max_iters = 1000;      // FeatureTracker.cc:280-281, the 6-argument overload
+}
+int dynofront_fundamental_record(dynofront_handle h, int32_t iters_cap) {
+  if (!h || iters_cap < 0) return -1;
+  h->fm_record = iters_cap; return 0;
+}
+int dynofront_find_fundamental_batch(dynofront_handle h, int32_t n_problems, const int32_t* offsets, const float* p1, const float* p2,
+                                     const dynofront_fundamental_params* prm, double* F, int32_t* n_models, uint8_t* mask, int32_t* n_inliers,
+                                     int32_t* status, int32_t* iterations, float* ms_device) {
+  if (!h || n_problems < 0 || !offsets || !F || !n_models || !n_inliers || !status) return -1;
+  dynofront_fundamental_params P; if (prm) P = *prm; else dynofront_fundamental_default_params(&P);
+  if (!(P.threshold_px > 0) || !std::isfinite(P.threshold_px) || !(P.confidence > 0 && P.confidence < 1) || P.max_iters > (1 << 20)) {
+    h->err = "fundamental params: threshold_px > 0, 0 < confidence < 1, max_iters <= 2^20"; return -1;
+  }
+  if (offsets[0] != 0) { h->err = "offsets[0] must be 0"; return -1; }
+  for (int p = 0; p < n_problems; p++) if (offsets[p + 1] < offsets[p]) { h->err = "offsets must not decrease"; return -1; }
+  const size_t rows = (size_t)offsets[n_problems];
+  if (rows > 0 && (!p1 || !p2 || !mask)) return -1;
+  for (size_t i = 0; i < 2*rows; i++) if (!std::isfinite(p1[i]) || !std::isfinite(p2[i])) { h->err = "non-finite point"; return -1; }
+  cudaSetDevice(h->dev);
+  const size_t nr = std::max(rows, (size_t)1), np = (size_t)n_problems;
+  const int cap = h->fm_record;
+  if (grow(h, h->fm_off, np + 1, h->fm_src, 2*nr, h->fm_dst, 2*nr, h->fm_mask, nr, h->fm_F, 27*std::max(np, (size_t)1),
+           h->fm_stat, 9*std::max(np, (size_t)1))) return -3;
+  if (cap && grow(h, h->fm_rec, 4*np*cap + 1)) return -3;
+  FCK(cudaEventRecord(h->e0, h->s));
+  FCK(cudaMemcpyAsync(h->fm_off, offsets, 4*(np + 1), cudaMemcpyHostToDevice, h->s));
+  if (rows) {
+    FCK(cudaMemcpyAsync(h->fm_src, p1, 8*rows, cudaMemcpyHostToDevice, h->s));
+    FCK(cudaMemcpyAsync(h->fm_dst, p2, 8*rows, cudaMemcpyHostToDevice, h->s));
+  }
+  if (cap) FCK(cudaMemsetAsync(h->fm_rec, 0xff, 16*np*cap, h->s));        // NaN: not recorded
+  FundBatch B{};
+  B.off = h->fm_off; B.src = h->fm_src; B.dst = h->fm_dst; B.thr2 = (float)(P.threshold_px*P.threshold_px); B.conf = P.confidence;
+  B.max_iters = P.max_iters; B.F = h->fm_F; B.mask = h->fm_mask; B.stat = h->fm_stat; B.rec = cap ? (float*)h->fm_rec : nullptr; B.rec_cap = cap;
+  if (np) fund_ransac_kernel<<<(unsigned)np, FUND_THREADS, 0, h->s>>>(B);
+  FCK(cudaGetLastError());
+  h->fm_np = n_problems; h->fm_cap = cap;
+  if (np) {
+    FCK(cudaMemcpyAsync(F, h->fm_F, 216*np, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(n_models, h->fm_stat, 4*np, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(n_inliers, h->fm_stat + np, 4*np, cudaMemcpyDeviceToHost, h->s));
+    FCK(cudaMemcpyAsync(status, h->fm_stat + 2*np, 4*np, cudaMemcpyDeviceToHost, h->s));
+    if (iterations) FCK(cudaMemcpyAsync(iterations, h->fm_stat + 3*np, 4*np, cudaMemcpyDeviceToHost, h->s));
+  }
+  if (rows) FCK(cudaMemcpyAsync(mask, h->fm_mask, rows, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  FCK(cudaGetLastError());
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+int dynofront_fundamental_last_trace(dynofront_handle h, int32_t* groups, int32_t* rejected, int32_t* best, int32_t* best_root,
+                                     int32_t* success, int32_t iters_cap, float* record, int32_t* n_problems) {
+  if (!h || !n_problems) return -1;
+  cudaSetDevice(h->dev);
+  const size_t np = (size_t)h->fm_np;
+  *n_problems = h->fm_np;
+  if (np == 0) return 0;
+  int32_t* outs[5] = {groups, rejected, best, best_root, success};
+  for (int k = 0; k < 5; k++) if (outs[k]) FCK(cudaMemcpy(outs[k], h->fm_stat + (4 + k)*np, 4*np, cudaMemcpyDeviceToHost));
+  if (record && iters_cap > 0) {
+    std::fill(record, record + 4*(size_t)iters_cap*np, std::nanf(""));
+    const int w = std::min(iters_cap, h->fm_cap);
+    if (w > 0)
+      FCK(cudaMemcpy2D(record, 16*(size_t)iters_cap, h->fm_rec, 16*(size_t)h->fm_cap, 16*(size_t)w, np, cudaMemcpyDeviceToHost));
   }
   return 0;
 }

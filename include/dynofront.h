@@ -12,6 +12,7 @@
  *   dynofront_klt_track_fb      KltFeatureTracker::trackPoints: forward + backward LK, round-trip test, label / border / age checks (:486-592)
  *   dynofront_klt_track_points  KltFeatureTracker::trackPoints steps 1-4: klt_track_fb + geometricVerification's cv::findHomography (:486-639)
  *   dynofront_find_homography_batch  cv::findHomography(RANSAC) on many point sets in one launch
+ *   dynofront_find_fundamental_batch cv::findFundamentalMat(FM_RANSAC) (with its LMedS and 7-point paths) on many point sets in one launch
  *   dynofront_detect_static     KltFeatureTracker::detectFeatures: mask, CLAHE, GFTT, range-tree ANMS, cornerSubPix  StaticFeatureTracker.cc:330-418
  *   dynofront_stereo_track      FeatureTracker::stereoTrack: left -> right LK + disparity / depth test  FeatureTracker.cc:194-337
  *   dynofront_update_depths     Frame::updateDepths                 dynosam/src/frontend/vision/Frame.cc:241-251,430-467
@@ -169,6 +170,41 @@ int dynofront_find_homography_batch(dynofront_handle h, int32_t n_problems, cons
 int dynofront_homography_record_counts(dynofront_handle h, int32_t counts_cap);
 int dynofront_homography_last_trace(dynofront_handle h, int32_t* status, int32_t* groups, int32_t* rejected, int32_t* best, int32_t counts_cap,
                                     int32_t* counts, int32_t* n_problems);
+/* ---- fundamental-matrix RANSAC: cv::findFundamentalMat(p1, p2, cv::FM_RANSAC, threshold_px, confidence, max_iters, mask) as
+ * FeatureTracker::stereoTrack calls it (FeatureTracker.cc:279-281), with OpenCV's draw sequence (cv::RNG seeded with (uint64)-1 on
+ * every call), collinearity subset test, run7Point (Hartley normalisation, OpenCV's Jacobi SVD with its seeded completion of the
+ * null space, cv::solveCubic, up to 3 models per draw), epipolar error in float and stopping rule.  Per problem status:
+ *   DYNOFRONT_FUND_OK          n >= 15: RANSAC; F (row-major, F22 = 1 where |F22| > FLT_EPSILON) and its inlier mask;
+ *   DYNOFRONT_FUND_LMEDS       8 <= n < 15: OpenCV's LMedS fallback (threshold_px is ignored); the mask is err <= sigma^2.
+ *                              cv::findFundamentalMat returns an empty F when fewer than 7 points are inliers (success = 0 in
+ *                              the trace) but the mask is written, and so it is here;
+ *   DYNOFRONT_FUND_SEVEN_POINT n == 7: run7Point alone, n_models (0-3) models, mask all ones (zeros without a model);
+ *   DYNOFRONT_FUND_TOO_FEW     n < 7: no model, mask all zeros;
+ *   DYNOFRONT_FUND_FAILED      no subset passed the test, or no model was found: F = 0, mask all zeros (cv2 leaves it unwritten).
+ * A draw whose determinant cubic counts as all zero under solveCubic's thresholds (every coefficient below DBL_EPSILON) has no
+ * model here; OpenCV 4.13 raises there (-215, rowRange), e.g. on collinear points under a pure shift. */
+enum { DYNOFRONT_FUND_OK = 0, DYNOFRONT_FUND_LMEDS = 1, DYNOFRONT_FUND_SEVEN_POINT = 2, DYNOFRONT_FUND_TOO_FEW = 3, DYNOFRONT_FUND_FAILED = 4 };
+typedef struct {
+  double threshold_px;   /* 1.0 (FeatureTracker.cc:281); refused <= 0 */
+  double confidence;     /* 0.99; refused outside (0, 1) */
+  int32_t max_iters;     /* 1000; values below 1 count as 1, as in OpenCV */
+} dynofront_fundamental_params;
+void dynofront_fundamental_default_params(dynofront_fundamental_params* p);
+/* n_problems problems in one launch: problem p is p1 / p2 rows [offsets[p], offsets[p+1]) ([row][2] float, (x, y)).
+ * F[n_problems][3][9] (up to 3 models, 0 past n_models), n_models / n_inliers / status / iterations (may be NULL) [n_problems],
+ * mask[offsets[n_problems]]. */
+int dynofront_find_fundamental_batch(dynofront_handle h, int32_t n_problems, const int32_t* offsets, const float* p1, const float* p2,
+                                     const dynofront_fundamental_params* prm, double* F, int32_t* n_models, uint8_t* mask, int32_t* n_inliers,
+                                     int32_t* status, int32_t* iterations, float* ms_device);
+/* parity hooks.  dynofront_fundamental_record(h, cap): the following calls record, for each of the first cap iterations per problem,
+ * (models of the draw, score of root 0, 1, 2) where the score is the inlier count (RANSAC) or the median error (LMedS); the models of
+ * a draw are run7Point's root count (-1: all-zero cubic, 0: none).  Default 0: nothing is recorded and no memory is set aside.
+ * dynofront_fundamental_last_trace, after dynofront_find_fundamental_batch: per problem the groups of 7 drawn, those the subset test
+ * rejected, the (iteration, root) of the best model (-1: none), success (LMedS: at least 7 inliers) and record[p][cap][4] (NaN where
+ * nothing was recorded).  Any output may be NULL. */
+int dynofront_fundamental_record(dynofront_handle h, int32_t iters_cap);
+int dynofront_fundamental_last_trace(dynofront_handle h, int32_t* groups, int32_t* rejected, int32_t* best, int32_t* best_root,
+                                     int32_t* success, int32_t iters_cap, float* record, int32_t* n_problems);
 /* KltFeatureTracker::trackPoints steps 1-4 as ONE call (StaticFeatureTracker.cc:486-625): the stages of dynofront_klt_track_fb,
  * then the homography above over the points whose status is set, in order (good_previous -> good_current), then
  * verified[i] = status[i] && mask[rank of i] (so !verified is what determineOutlierIds reports) and, with fb->check_static,
