@@ -632,7 +632,7 @@ static inline void band_add(double* AB, int ld, int i, int j, double v) {
   *p += v;
 }
 
-#define MAXGP 96   /* max distinct pose variables touching one landmark group */
+#define MAXGP 256  /* max distinct pose variables touching one landmark group (a 128-frame hybrid track) */
 #define MAXGL 96   /* max scalar landmark dims of one group */
 
 /* Per-group quantities.  mode 0: accumulate reduced system into AB/gS.
