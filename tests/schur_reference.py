@@ -122,7 +122,14 @@ class Reference:
         return self.Hll_inv @ (self.g_l - self.Hpl.T @ dp)
 
     def pose_step(self):
-        return np.linalg.solve(self.S, self.gS)
+        d = np.sqrt(np.diag(self.S))          # equilibrated: rows of a 1e-6-sigma prior keep their digits
+        return np.linalg.solve(self.S/d[:, None]/d[None, :], self.gS/d)/d
+
+    def kappa_s(self):
+        """condition number of D^-1/2 S D^-1/2, D = diag S: what the pose step's forward error scales with"""
+        d = np.sqrt(np.diag(self.S))
+        ev = np.linalg.eigvalsh(self.S/d[:, None]/d[None, :])
+        return float(ev.max()/ev.min())
 
     # comparator (module docstring)
     def s_err(self, S):

@@ -7,6 +7,7 @@ checked entry by entry against a dense fp64 elimination of the device's own Jaco
 import numpy as np
 import pytest
 
+import band_reference as BR
 import schur_reference as SR
 from dynosam_b200 import synth
 from dynosam_b200.problem import (BETWEEN6, FLOWPROJ2, HYBRID3, HYBRID_STEREO3, MOTIONPOSE3, POSE2POINT3, PRIOR6,
@@ -15,6 +16,9 @@ from dynosam_b200.problem import (BETWEEN6, FLOWPROJ2, HYBRID3, HYBRID_STEREO3, 
 pytestmark = pytest.mark.gpu
 
 REL_CHI2 = 1e-6
+# pose step of the cell scheme, forward error in units of diag S (band_reference.forward_error): measured at most
+# 6.5e-8 against the oracle and 4.7e-8 against the plain band on an H100 80GB HBM3 (700 W)
+CELL_FWD = 1e-6
 
 
 def _solver(p):
@@ -263,18 +267,26 @@ def test_cell_partition_matches_plain_band():
     lam = 1e-4
     rc, do = o.schur_solve(lam)
     assert rc == 0
+    npz = 6*p.n_pose
     steps = {}
     for cells in (-1, 1, 2, 4, 8):
         s = _solver(p); s.set_partition(cells)
         info = s.info()
         wb = (info["bandwidth"] + 31)//32
         assert info["reduced_dim"]//32 >= (4*8 - 1)*max(wb, 2), "graph too short for 8 cells"
+        if cells == -1:
+            dS = np.diag(s.reduced_system(lam)[0]).copy()      # the units of the pose-step comparator (band_reference)
         d = s.solve(lam)
-        assert np.linalg.norm(d - do) <= 1e-6*np.linalg.norm(do), cells
+        fwd = BR.forward_error(dS, d[:npz], do[:npz])
+        print(f"cells {cells}: pose step forward error against the oracle {fwd:.2e}")
+        assert fwd <= CELL_FWD and np.linalg.norm(d[npz:] - do[npz:]) <= 1e-6*np.linalg.norm(do[npz:]), (cells, fwd)
         steps[cells] = d
         s.close()
     for cells in (1, 2, 4, 8):
-        assert np.linalg.norm(steps[cells] - steps[-1]) <= 1e-7*np.linalg.norm(steps[-1]), cells
+        fwd = BR.forward_error(dS, steps[cells][:npz], steps[-1][:npz])
+        print(f"cells {cells}: pose step forward error against the plain band {fwd:.2e}")
+        assert fwd <= CELL_FWD, (cells, fwd)
+        assert np.linalg.norm(steps[cells][npz:] - steps[-1][npz:]) <= 1e-7*np.linalg.norm(steps[-1][npz:]), cells
     so = o.optimize(max_iterations=5)
     for cells in (2, 8):
         s = _solver(p); s.set_partition(cells)

@@ -12,16 +12,23 @@ lambdas and every cell layout:
     general_wcme    1.9e-15  1.0e-15  1.8e-15
     general_wcpe    2.1e-15  1.4e-15  2.8e-16
     all_types       1.7e-15  3.9e-15  1.4e-14
+
+The pose step's forward error (band_reference.forward_error, units of diag S) is bounded by FWD_PER_KAPPA kappa_s u, with
+kappa_s the condition number of the equilibrated S and u = 2^-52; measured at most 0.67 kappa_s u (simple, lambda 1e-4)
+on an H100 80GB HBM3 (700 W).  kappa_s ranges from 5e4 (all_types) to 1e11 (general_wcpe, lambda 1e-4): there the bound
+is about 1e-3 and says little, and the pose backward error at TOL is what guards the step.
 """
 import numpy as np
 import pytest
 
+import band_reference as BR
 import schur_reference as SR
 from dynosam_b200.binding import Solver
 
 pytestmark = pytest.mark.gpu
 
 TOL = 1e-11
+FWD_PER_KAPPA = 50.0     # pose step: forward error <= FWD_PER_KAPPA kappa_s u
 LAMBDAS = (1e-4, 1e-1)
 GRAPHS = sorted(SR.ROUTE_GRAPHS)
 _cache = {}
@@ -39,11 +46,9 @@ def _reference(s, p, lam):
 
 
 def _max_cells(s):
-    """the most cells the band layout can cut this reduced system into (kernels_band.cu band_plan_layout)"""
+    """the most cells the band layout can cut this reduced system into"""
     info = s.info()
-    NT = (info["reduced_dim"] + 31)//32
-    WB = min(max((info["bandwidth"] + 31)//32, 1), NT - 1)
-    return (NT + WB)//(2*WB + 2*max(WB, 2))
+    return BR.layout(info["reduced_dim"], info["bandwidth"]).cmax
 
 
 def _check_solve(s, p, R, lam):
@@ -54,8 +59,7 @@ def _check_solve(s, p, R, lam):
     # the pose step solves the reference system: backward error in the comparator's units, and the dense solve
     sc = np.sqrt(R.Hdiag[:npz])
     back = float((np.abs(R.S @ dp - R.gS)/(sc*(R.r + np.abs(sc*dp).max()))).max())
-    ref = R.pose_step()
-    fwd = np.linalg.norm(dp - ref)/np.linalg.norm(ref)
+    fwd = BR.forward_error(np.diag(R.S), dp, R.pose_step())/(R.kappa_s()*np.finfo(float).eps)
     return el, back, fwd
 
 
@@ -87,8 +91,8 @@ def test_damped_solve_matches_reference(name):
         for lam in LAMBDAS:
             R = _reference(s, p, lam)
             el, back, fwd = _check_solve(s, p, R, lam)
-            print(f"{name} cells {cells} lambda {lam:g}: dl {el:.2e} pose backward {back:.2e} forward {fwd:.2e}")
-            assert el <= TOL and back <= TOL and fwd <= 1e-6, (cells, lam, el, back, fwd)
+            print(f"{name} cells {cells} lambda {lam:g}: dl {el:.2e} pose backward {back:.2e} forward {fwd:.2f} kappa_s u")
+            assert el <= TOL and back <= TOL and fwd <= FWD_PER_KAPPA, (cells, lam, el, back, fwd)
         s.close()
 
 
@@ -102,7 +106,7 @@ def test_shuffled_factors_match_reference(name):
     S, g = s.reduced_system(lam)
     assert R.s_err(S) <= TOL and R.g_err(g) <= TOL, (R.s_err(S), R.g_err(g))
     el, back, fwd = _check_solve(s, q, R, lam)
-    assert el <= TOL and back <= TOL and fwd <= 1e-6, (el, back, fwd)
+    assert el <= TOL and back <= TOL and fwd <= FWD_PER_KAPPA, (el, back, fwd)
     s.close()
 
 
