@@ -18,7 +18,8 @@ EXPORTS = ["dynofront_create", "dynofront_destroy", "dynofront_last_error", "dyn
            "dynofront_back_project", "dynofront_dense_cloud", "dynofront_homography_default_params", "dynofront_find_homography_batch",
            "dynofront_homography_last_trace", "dynofront_homography_record_counts", "dynofront_klt_track_points",
            "dynofront_klt_dynamic_default_params", "dynofront_track_dynamic_klt", "dynofront_fundamental_default_params",
-           "dynofront_find_fundamental_batch", "dynofront_fundamental_last_trace", "dynofront_fundamental_record"]
+           "dynofront_find_fundamental_batch", "dynofront_fundamental_last_trace", "dynofront_fundamental_record", "dynofront_set_right",
+           "dynofront_stereo_match"]
 
 
 class TrackParamsC(C.Structure):
@@ -110,6 +111,7 @@ class FundamentalParams:
 
 
 FUND_OK, FUND_LMEDS, FUND_SEVEN_POINT, FUND_TOO_FEW, FUND_FAILED = 0, 1, 2, 3, 4     # dynofront_find_fundamental_batch status
+STEREO_UNTOUCHED, STEREO_MATCHED, STEREO_LOST, STEREO_EPIPOLAR, STEREO_DISPARITY = 0, 1, 2, 3, 4   # dynofront_stereo_match per-feature state
 
 
 class KltDynamicParamsC(C.Structure):
@@ -176,6 +178,10 @@ def load():
                                              C.POINTER(KltFbParamsC), C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float)]
         L.dynofront_stereo_track.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_double,
                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_float)]
+        L.dynofront_set_right.argtypes = [C.c_void_p, C.c_void_p]
+        L.dynofront_stereo_match.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_double,
+                                             C.POINTER(FundamentalParamsC), C.POINTER(C.c_int32)] + [C.c_void_p]*6 + [C.POINTER(C.c_int32)]*4 + \
+                                            [C.POINTER(C.c_float)]
         L.dynofront_klt_last_min_eig.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
         L.dynofront_track_static_flow.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
                                                   C.POINTER(C.c_int64)] + [C.c_void_p]*8 + [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
@@ -581,6 +587,33 @@ class FeatureTrackerGPU:
         self._ck(self.lib.dynofront_stereo_track(self.h, _p(lg), _p(rg), n, _p(p0), _p(rp), _p(st), float(fx), float(baseline), _p(depth), _p(valid), C.byref(ms)))
         self.last_ms = ms.value
         return rp, st, depth, valid
+
+    def set_right(self, right):
+        """upload the current frame's right image (uint8 [H][W]) and build its pyramid; call after next_frame, which marks it
+        stale.  A C-contiguous uint8 array is passed as is (pin it for an asynchronous copy and keep it untouched until the next call)."""
+        r = np.ascontiguousarray(right, dtype=np.uint8)
+        assert r.shape == (self.H, self.W)
+        self._keep_right = r                                     # the copy may still be in flight when this returns
+        self._ck(self.lib.dynofront_set_right(self.h, _p(r)))
+
+    def stereo_match(self, left_pts, fx, baseline, prm: FundamentalParams | None = None, left=None, right=None):
+        """FeatureTracker::stereoTrack in one call (dynofront_stereo_match): LK left -> right, cv::findFundamentalMat(FM_RANSAC)
+        over the LK-good points, the disparity test.  left = right = None: the resident current frame of next_frame and the
+        right image of set_right.  left_pts [n][2]: the usable static features in container order.  Returns a dict: matched (the
+        reference's return value), per point state (STEREO_*), depth and right_u (NaN unless MATCHED), right_pts / lk_status (the
+        LK result), F [3][3], fund_status (FUND_*, -1 when the RANSAC did not run), n_tracked, n_inliers, n_stereo."""
+        lg = None if left is None else np.ascontiguousarray(left, dtype=np.uint8)
+        rg = None if right is None else np.ascontiguousarray(right, dtype=np.uint8)
+        p0 = np.ascontiguousarray(left_pts, dtype=np.float32).reshape(-1, 2); n = p0.shape[0]
+        state = np.zeros(n, np.uint8); depth = np.zeros(n); ru = np.zeros(n); rp = np.zeros((n, 2), np.float32); st = np.zeros(n, np.uint8)
+        F = np.zeros(9); mt = C.c_int32(); fs = C.c_int32(); nt = C.c_int32(); ni = C.c_int32(); ns = C.c_int32(); ms = C.c_float()
+        pc = (prm or FundamentalParams()).c()
+        self._ck(self.lib.dynofront_stereo_match(self.h, _p(lg), _p(rg), n, _p(p0), float(fx), float(baseline), C.byref(pc), C.byref(mt), _p(state),
+                                                 _p(depth), _p(ru), _p(rp), _p(st), _p(F), C.byref(fs), C.byref(nt), C.byref(ni), C.byref(ns),
+                                                 C.byref(ms)))
+        self.last_ms = ms.value
+        return dict(matched=bool(mt.value), state=state, depth=depth, right_u=ru, right_pts=rp, lk_status=st, F=F.reshape(3, 3),
+                    fund_status=fs.value, n_tracked=nt.value, n_inliers=ni.value, n_stereo=ns.value)
 
     # ---- depth and back-projection
     def set_depth(self, depth):

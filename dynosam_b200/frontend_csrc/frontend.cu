@@ -63,6 +63,11 @@ struct dynofront_ctx {
   std::vector<DevBuf<uint8_t>> pyr[2]; std::vector<DevBuf<short>> der, der2; std::vector<int> lw, lh;
   DevBuf<float> k_prev, k_next, k_err, k_back, k_eig; DevBuf<uint8_t> k_st, k_st2, k_keep; DevBuf<int32_t> k_age; DevBuf<int> k_count;
   DevBuf<double> st_depth;                        // stereoTrack
+  // stereo matching: pyramids of its own (0: a given left image, with st_der; 1: a given right image; 2: dynofront_set_right's),
+  // never the temporal pair above; LK points, compaction (input row per rank, rank per row, compacted rows), offsets, counts
+  std::vector<DevBuf<uint8_t>> st_pyr[3]; std::vector<DevBuf<short>> st_der; bool has_right = false;
+  DevBuf<float> sm_left, sm_right, sm_cl, sm_cr; DevBuf<uint8_t> sm_st, sm_state; DevBuf<int> sm_idx, sm_rank, sm_off, sm_cnt;
+  DevBuf<double> sm_depth, sm_ru;
   // external-flow static tracker scratch
   DevBuf<double> sf_kp, sf_flow, sf_pred; DevBuf<int32_t> sf_age, sf_det, sf_oage; DevBuf<uint8_t> sf_use, sf_pass, sf_acc;
   DevBuf<int> sf_cell, sf_win, sf_win2, sf_cnt; DevBuf<long long> sf_otid;
@@ -2235,7 +2240,7 @@ int dynofront_set_frame(dynofront_handle h, const float* flow, const int32_t* mo
   if (detection_mask) { FCK(cudaMemcpyAsync(h->det, detection_mask, npx, cudaMemcpyHostToDevice, h->s)); h->has_det = true; }
   else h->has_det = false;
   h->det_work_valid = false;
-  h->has_depth = false; h->has_frame = h->has_frame || motion_mask;
+  h->has_depth = false; h->has_right = false; h->has_frame = h->has_frame || motion_mask;
   FCK(cudaStreamSynchronize(h->s));
   return 0;
 }
@@ -2620,29 +2625,50 @@ int dynofront_unpin_host(dynofront_handle h, void* ptr) {
   FCK(cudaHostUnregister(ptr));
   return 0;
 }
-static int build_pyramid(dynofront_ctx* h, int which, const uint8_t* host_img, int max_level, int win, bool with_deriv) {
-  const int W = h->W, H = h->H;
-  if (h->lw.empty()) {
-    for (int l = 0, w = W, hh = H; l < 8; l++) {
-      h->lw.push_back(w); h->lh.push_back(hh);
-      w = (w + 1)/2; hh = (hh + 1)/2;
-      if (w < 2 || hh < 2) break;
-    }
-    const size_t L = h->lw.size();
-    h->pyr[0].resize(L); h->pyr[1].resize(L); h->der.resize(L); h->der2.resize(L);
+// the level sizes of every pyramid of the handle (levels down to 2 px)
+static void pyramid_sizes(dynofront_ctx* h) {
+  if (!h->lw.empty()) return;
+  for (int l = 0, w = h->W, hh = h->H; l < 8; l++) {
+    h->lw.push_back(w); h->lh.push_back(hh);
+    w = (w + 1)/2; hh = (hh + 1)/2;
+    if (w < 2 || hh < 2) break;
   }
+  const size_t L = h->lw.size();
+  h->pyr[0].resize(L); h->pyr[1].resize(L); h->der.resize(L); h->der2.resize(L);
+}
+// uploads host_img into level 0 of pyr and builds levels 1..max_level (and the Scharr derivatives of levels 0..max_level into der
+// when it is given); the arrays must be allocated
+static int build_levels(dynofront_ctx* h, std::vector<DevBuf<uint8_t>>& pyr, std::vector<DevBuf<short>>* der, const uint8_t* host_img, int max_level) {
+  FCK(cudaMemcpyAsync(pyr[0], host_img, (size_t)h->W*h->H, cudaMemcpyHostToDevice, h->s));
+  const dim3 blk(32, 8);
+  for (int l = 0; l <= max_level && l < (int)h->lw.size(); l++) {
+    const int w = h->lw[l], hh = h->lh[l];
+    if (l > 0) pyr_down_kernel<<<dim3((w + 31)/32, (hh + 7)/8), blk, 0, h->s>>>(pyr[l-1], h->lw[l-1], h->lh[l-1], pyr[l], w, hh);
+    if (der) scharr_kernel<<<dim3((w + 31)/32, (hh + 7)/8), blk, 0, h->s>>>(pyr[l], w, hh, (*der)[l]);
+  }
+  return 0;
+}
+static int build_pyramid(dynofront_ctx* h, int which, const uint8_t* host_img, int max_level, int win, bool with_deriv) {
+  pyramid_sizes(h);
   for (size_t l = 0; l < h->lw.size(); l++) {
     const size_t n = (size_t)h->lw[l]*h->lh[l];
     if (grow(h, h->pyr[0][l], n, h->pyr[1][l], n, h->der[l], 2*n, h->der2[l], 2*n)) return -3;
   }
-  FCK(cudaMemcpyAsync(h->pyr[which][0], host_img, (size_t)W*H, cudaMemcpyHostToDevice, h->s));
-  const dim3 blk(32, 8);
-  for (int l = 0; l <= max_level && l < (int)h->lw.size(); l++) {
-    const int w = h->lw[l], hh = h->lh[l];
-    if (l > 0) pyr_down_kernel<<<dim3((w + 31)/32, (hh + 7)/8), blk, 0, h->s>>>(h->pyr[which][l-1], h->lw[l-1], h->lh[l-1], h->pyr[which][l], w, hh);
-    if (with_deriv) scharr_kernel<<<dim3((w + 31)/32, (hh + 7)/8), blk, 0, h->s>>>(h->pyr[which][l], w, hh, which == 0 ? h->der[l] : h->der2[l]);
+  if (which == 1) h->has_right = false;                         // a new current image: the right image no longer belongs to it
+  return build_levels(h, h->pyr[which], with_deriv ? (which == 0 ? &h->der : &h->der2) : nullptr, host_img, max_level);
+}
+// a stereo slot of its own (st_pyr[slot], with st_der when with_deriv), never the temporal pair
+static int build_stereo_pyramid(dynofront_ctx* h, int slot, const uint8_t* host_img, int max_level, bool with_deriv) {
+  pyramid_sizes(h);
+  std::vector<DevBuf<uint8_t>>& pyr = h->st_pyr[slot];
+  pyr.resize(h->lw.size());
+  if (with_deriv) h->st_der.resize(h->lw.size());
+  for (size_t l = 0; l < h->lw.size(); l++) {
+    const size_t n = (size_t)h->lw[l]*h->lh[l];
+    if (grow(h, pyr[l], n)) return -3;
+    if (with_deriv && grow(h, h->st_der[l], 2*n)) return -3;
   }
-  return 0;
+  return build_levels(h, pyr, with_deriv ? &h->st_der : nullptr, host_img, max_level);
 }
 
 // buildOpticalFlowPyramid's top level: stop when a level is not larger than the window (lkpyramid.cpp)
@@ -2860,14 +2886,35 @@ int dynofront_fundamental_record(dynofront_handle h, int32_t iters_cap) {
   if (!h || iters_cap < 0) return -1;
   h->fm_record = iters_cap; return 0;
 }
+static int fund_check_params(dynofront_ctx* h, const dynofront_fundamental_params& P) {
+  if (!(P.threshold_px > 0) || !std::isfinite(P.threshold_px) || !(P.confidence > 0 && P.confidence < 1) || P.max_iters > (1 << 20)) {
+    h->err = "fundamental params: threshold_px > 0, 0 < confidence < 1, max_iters <= 2^20"; return -1;
+  }
+  return 0;
+}
+// one CTA per problem over rows [off[p], off[p+1]) of src / dst (device; the offsets are read on the device, so a count computed
+// there never visits the host); outputs in fm_F / fm_mask / fm_stat, the per-iteration record in fm_rec after dynofront_fundamental_record
+static int fund_launch(dynofront_ctx* h, int np, const int* d_off, const float* src, const float* dst, size_t rows,
+                       const dynofront_fundamental_params& P) {
+  const size_t nr = std::max(rows, (size_t)1), npp = std::max((size_t)np, (size_t)1);
+  const int cap = h->fm_record;
+  if (grow(h, h->fm_mask, nr, h->fm_F, 27*npp, h->fm_stat, 9*npp)) return -3;
+  if (cap && grow(h, h->fm_rec, 4*(size_t)np*cap + 1)) return -3;
+  if (cap) FCK(cudaMemsetAsync(h->fm_rec, 0xff, 16*(size_t)np*cap, h->s));        // NaN: not recorded
+  FundBatch B{};
+  B.off = d_off; B.src = src; B.dst = dst; B.thr2 = (float)(P.threshold_px*P.threshold_px); B.conf = P.confidence;
+  B.max_iters = P.max_iters; B.F = h->fm_F; B.mask = h->fm_mask; B.stat = h->fm_stat; B.rec = cap ? (float*)h->fm_rec : nullptr; B.rec_cap = cap;
+  if (np) fund_ransac_kernel<<<(unsigned)np, FUND_THREADS, 0, h->s>>>(B);
+  FCK(cudaGetLastError());
+  h->fm_np = np; h->fm_cap = cap;
+  return 0;
+}
 int dynofront_find_fundamental_batch(dynofront_handle h, int32_t n_problems, const int32_t* offsets, const float* p1, const float* p2,
                                      const dynofront_fundamental_params* prm, double* F, int32_t* n_models, uint8_t* mask, int32_t* n_inliers,
                                      int32_t* status, int32_t* iterations, float* ms_device) {
   if (!h || n_problems < 0 || !offsets || !F || !n_models || !n_inliers || !status) return -1;
   dynofront_fundamental_params P; if (prm) P = *prm; else dynofront_fundamental_default_params(&P);
-  if (!(P.threshold_px > 0) || !std::isfinite(P.threshold_px) || !(P.confidence > 0 && P.confidence < 1) || P.max_iters > (1 << 20)) {
-    h->err = "fundamental params: threshold_px > 0, 0 < confidence < 1, max_iters <= 2^20"; return -1;
-  }
+  if (fund_check_params(h, P)) return -1;
   if (offsets[0] != 0) { h->err = "offsets[0] must be 0"; return -1; }
   for (int p = 0; p < n_problems; p++) if (offsets[p + 1] < offsets[p]) { h->err = "offsets must not decrease"; return -1; }
   const size_t rows = (size_t)offsets[n_problems];
@@ -2875,23 +2922,14 @@ int dynofront_find_fundamental_batch(dynofront_handle h, int32_t n_problems, con
   for (size_t i = 0; i < 2*rows; i++) if (!std::isfinite(p1[i]) || !std::isfinite(p2[i])) { h->err = "non-finite point"; return -1; }
   cudaSetDevice(h->dev);
   const size_t nr = std::max(rows, (size_t)1), np = (size_t)n_problems;
-  const int cap = h->fm_record;
-  if (grow(h, h->fm_off, np + 1, h->fm_src, 2*nr, h->fm_dst, 2*nr, h->fm_mask, nr, h->fm_F, 27*std::max(np, (size_t)1),
-           h->fm_stat, 9*std::max(np, (size_t)1))) return -3;
-  if (cap && grow(h, h->fm_rec, 4*np*cap + 1)) return -3;
+  if (grow(h, h->fm_off, np + 1, h->fm_src, 2*nr, h->fm_dst, 2*nr)) return -3;
   FCK(cudaEventRecord(h->e0, h->s));
   FCK(cudaMemcpyAsync(h->fm_off, offsets, 4*(np + 1), cudaMemcpyHostToDevice, h->s));
   if (rows) {
     FCK(cudaMemcpyAsync(h->fm_src, p1, 8*rows, cudaMemcpyHostToDevice, h->s));
     FCK(cudaMemcpyAsync(h->fm_dst, p2, 8*rows, cudaMemcpyHostToDevice, h->s));
   }
-  if (cap) FCK(cudaMemsetAsync(h->fm_rec, 0xff, 16*np*cap, h->s));        // NaN: not recorded
-  FundBatch B{};
-  B.off = h->fm_off; B.src = h->fm_src; B.dst = h->fm_dst; B.thr2 = (float)(P.threshold_px*P.threshold_px); B.conf = P.confidence;
-  B.max_iters = P.max_iters; B.F = h->fm_F; B.mask = h->fm_mask; B.stat = h->fm_stat; B.rec = cap ? (float*)h->fm_rec : nullptr; B.rec_cap = cap;
-  if (np) fund_ransac_kernel<<<(unsigned)np, FUND_THREADS, 0, h->s>>>(B);
-  FCK(cudaGetLastError());
-  h->fm_np = n_problems; h->fm_cap = cap;
+  if (int rc = fund_launch(h, n_problems, h->fm_off, h->fm_src, h->fm_dst, rows, P)) return rc;
   if (np) {
     FCK(cudaMemcpyAsync(F, h->fm_F, 216*np, cudaMemcpyDeviceToHost, h->s));
     FCK(cudaMemcpyAsync(n_models, h->fm_stat, 4*np, cudaMemcpyDeviceToHost, h->s));
@@ -2963,16 +3001,61 @@ int dynofront_klt_track_points(dynofront_handle h, const uint8_t* prev_gray, con
 // FeatureTracker::stereoTrack (FeatureTracker.cc:194-337): left -> right LK (21x21, 5 levels, OpenCV default criteria), then per
 // matched point disparity = uL - uR, rejected when <= 1 px or uR < 0, depth = fx * baseline / disparity.  (The reference also
 // runs the right -> left pass but its round-trip filter is commented out, :240-253, and a fundamental-matrix RANSAC sits between
-// the LK status and the disparity test: host code outside section 8 -- final = status & ransac_mask & valid.)
+// the LK status and the disparity test: dynofront_stereo_match below runs the whole chain in one call.)
+// the per-point rule of FeatureTracker.cc:307-321: false when disparity = uL - uR (in double) <= 1 or uR < 0, else
+// depth = fx * baseline / disparity
+__device__ __forceinline__ bool stereo_disparity(float uLf, float uRf, double fx, double baseline, double* depth) {
+  const double uL = (double)uLf, uR = (double)uRf;
+  const double disparity = uL - uR;
+  if (disparity <= 1.0 || uR < 0.0f) return false;
+  *depth = fx*baseline/disparity;
+  return true;
+}
 __global__ void stereo_post_kernel(int n, const float* __restrict__ left, const float* __restrict__ right, const uint8_t* __restrict__ st, double fx,
                                    double baseline, double* __restrict__ depth, uint8_t* __restrict__ valid) {
   const int i = blockIdx.x*blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const double uL = (double)left[2*i], uR = (double)right[2*i];
-  const double disparity = uL - uR;
-  const bool ok = st[i] && !(disparity <= 1.0 || right[2*i] < 0.0f);
+  double d = 0.0;
+  const bool ok = st[i] && stereo_disparity(left[2*i], right[2*i], fx, baseline, &d);
   valid[i] = ok ? 1 : 0;
-  depth[i] = ok ? fx*baseline/disparity : 0.0;
+  depth[i] = ok ? d : 0.0;
+}
+// dynofront_stereo_match, between the LK and the RANSAC (one CTA): the LK-good rows in input order -- stereoTrack's
+// pts_left_tracked / pts_right_tracked -- as idx[rank] = row, rank[row] = rank, cl / cr = the rows' float points; off = {0, m}, or
+// {0, 0} when m < 8 (the reference returns before its RANSAC), cnt = {m, 0, 0}
+__global__ void __launch_bounds__(HOM_THREADS) stereo_compact_kernel(int n, const float* __restrict__ left, const float* __restrict__ right,
+                                                                     const uint8_t* __restrict__ st, int* __restrict__ idx, int* __restrict__ rank,
+                                                                     float* __restrict__ cl, float* __restrict__ cr, int* __restrict__ off,
+                                                                     int* __restrict__ cnt) {
+  __shared__ int sh_wcnt[HOM_WARPS];
+  const int m = hom_compact(n, [&](int i) { return st[i] != 0; }, [](int i) { return i; }, idx, sh_wcnt);
+  for (int k = threadIdx.x; k < m; k += HOM_THREADS) {
+    const int i = idx[k];
+    rank[i] = k;
+    cl[2*k] = left[2*i]; cl[2*k + 1] = left[2*i + 1]; cr[2*k] = right[2*i]; cr[2*k + 1] = right[2*i + 1];
+  }
+  if (threadIdx.x == 0) { off[0] = 0; off[1] = m >= 8 ? m : 0; cnt[0] = m; cnt[1] = 0; cnt[2] = 0; }
+}
+// the per-feature loop of stereoTrack (FeatureTracker.cc:273-335) after the RANSAC: state, depth and uR per input row; cnt[1] / cnt[2]
+// count the mask ones and the stereo features
+__global__ void stereo_match_post_kernel(int n, const float* __restrict__ left, const float* __restrict__ right, const uint8_t* __restrict__ st,
+                                         const int* __restrict__ rank, const uint8_t* __restrict__ mask, double fx, double baseline,
+                                         uint8_t* __restrict__ state, double* __restrict__ depth, double* __restrict__ right_u, int* __restrict__ cnt) {
+  const int i = blockIdx.x*blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint8_t s = DYNOFRONT_STEREO_UNTOUCHED;
+  double d = CUDART_NAN, u = CUDART_NAN;
+  if (cnt[0] >= 8) {                                         // fewer than 8 tracked: the reference returns false, nothing marked
+    if (!st[i]) s = DYNOFRONT_STEREO_LOST;
+    else if (!mask[rank[i]]) s = DYNOFRONT_STEREO_EPIPOLAR;
+    else {
+      atomicAdd(cnt + 1, 1);
+      double dd;
+      if (stereo_disparity(left[2*i], right[2*i], fx, baseline, &dd)) { s = DYNOFRONT_STEREO_MATCHED; d = dd; u = (double)right[2*i]; atomicAdd(cnt + 2, 1); }
+      else s = DYNOFRONT_STEREO_DISPARITY;
+    }
+  }
+  state[i] = s; depth[i] = d; right_u[i] = u;
 }
 int dynofront_stereo_track(dynofront_handle h, const uint8_t* left_gray, const uint8_t* right_gray, int32_t n, const float* left_pts, float* right_pts,
                            uint8_t* status, double fx, double baseline, double* depth, uint8_t* valid, float* ms_device) {
@@ -2996,6 +3079,81 @@ int dynofront_stereo_track(dynofront_handle h, const uint8_t* left_gray, const u
   FCK(cudaEventRecord(h->e1, h->s));
   FCK(cudaStreamSynchronize(h->s));
   FCK(cudaGetLastError());
+  if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
+  return 0;
+}
+
+// The right image's pyramid has no Scharr derivatives: LK reads derivatives of the image it tracks FROM only, and the reference's
+// right -> left pass (FeatureTracker.cc:230-232) is computed but never used (its round-trip filter, :240-253, is commented out),
+// so that pass does not run here.
+int dynofront_set_right(dynofront_handle h, const uint8_t* right_gray) {
+  if (!h || !right_gray) return -1;
+  cudaSetDevice(h->dev);
+  if (build_stereo_pyramid(h, 2, right_gray, klt_top_level(h, 5, 21), false)) return -3;
+  h->has_right = true;
+  return 0;                                                     // no synchronisation, as dynofront_next_frame
+}
+int dynofront_stereo_match(dynofront_handle h, const uint8_t* left_gray, const uint8_t* right_gray, int32_t n, const float* left_pts,
+                           double fx, double baseline, const dynofront_fundamental_params* fund, int32_t* matched, uint8_t* state,
+                           double* depth, double* right_u, float* right_pts, uint8_t* lk_status, double* F, int32_t* fund_status,
+                           int32_t* n_tracked, int32_t* n_inliers, int32_t* n_stereo, float* ms_device) {
+  if (!h || n < 0 || (n > 0 && !left_pts) || !matched || !state || !depth || !right_u) return -1;
+  const bool resident = !left_gray && !right_gray;
+  if (!resident && (!left_gray || !right_gray)) { h->err = "pass both images, or none for the resident frame and right image"; return -1; }
+  dynofront_fundamental_params P; if (fund) P = *fund; else dynofront_fundamental_default_params(&P);
+  if (fund_check_params(h, P)) return -1;
+  for (size_t i = 0; i < 2*(size_t)n; i++) if (!std::isfinite(left_pts[i])) { h->err = "non-finite point"; return -1; }
+  if (resident && !h->have_pyr_cur) { h->err = "no current frame on the device: call dynofront_next_frame first"; return -2; }
+  if (resident && !h->has_right) { h->err = "no right image for the current frame: call dynofront_set_right after dynofront_next_frame"; return -2; }
+  cudaSetDevice(h->dev);
+  *matched = 0;
+  if (n < 8) {                                                  // FeatureTracker.cc:205: nothing runs, nothing is marked
+    for (int i = 0; i < n; i++) { state[i] = DYNOFRONT_STEREO_UNTOUCHED; depth[i] = right_u[i] = std::nan(""); }
+    if (right_pts) std::copy(left_pts, left_pts + 2*(size_t)n, right_pts);
+    if (lk_status) std::fill(lk_status, lk_status + n, 0);
+    if (F) std::fill(F, F + 9, 0.0);
+    if (fund_status) *fund_status = -1;
+    if (n_tracked) *n_tracked = 0; if (n_inliers) *n_inliers = 0; if (n_stereo) *n_stereo = 0;
+    h->fm_np = 0;                                               // the trace holds no problem
+    if (ms_device) *ms_device = 0.f;
+    return 0;
+  }
+  const int win = 21, levels = klt_top_level(h, 5, win);
+  const size_t cap = feature_cap(n);
+  if (grow(h, h->sm_left, 2*cap, h->sm_right, 2*cap, h->sm_cl, 2*cap, h->sm_cr, 2*cap, h->sm_st, cap, h->sm_state, cap, h->sm_idx, cap,
+           h->sm_rank, cap, h->sm_off, 2, h->sm_cnt, 3, h->sm_depth, cap, h->sm_ru, cap, h->k_err, cap)) return -3;   // (klt_launch writes k_err)
+  FCK(cudaEventRecord(h->e0, h->s));
+  KltLevels L; L.nlev = levels + 1;
+  if (!resident) {
+    if (build_stereo_pyramid(h, 0, left_gray, levels, true)) return -3;
+    if (build_stereo_pyramid(h, 1, right_gray, levels, false)) return -3;
+  }
+  for (int l = 0; l <= levels; l++) {                           // left: the current frame (pyramid 1, der2) or stereo slot 0
+    L.I[l] = resident ? h->pyr[1][l] : h->st_pyr[0][l]; L.D[l] = resident ? h->der2[l] : h->st_der[l];
+    L.J[l] = h->st_pyr[resident ? 2 : 1][l]; L.w[l] = h->lw[l]; L.h[l] = h->lh[l];
+  }
+  FCK(cudaMemcpyAsync(h->sm_left, left_pts, 8*(size_t)n, cudaMemcpyHostToDevice, h->s));
+  FCK(cudaMemcpyAsync(h->sm_right, h->sm_left, 8*(size_t)n, cudaMemcpyDeviceToDevice, h->s));   // right_feature_points = left_feature_points
+  klt_launch(h, L, n, h->sm_left, h->sm_right, h->sm_st, win, 30, 0.01, 0, 1e-4f, nullptr);
+  stereo_compact_kernel<<<1, HOM_THREADS, 0, h->s>>>(n, h->sm_left, h->sm_right, h->sm_st, h->sm_idx, h->sm_rank, h->sm_cl, h->sm_cr, h->sm_off, h->sm_cnt);
+  if (int rc = fund_launch(h, 1, h->sm_off, h->sm_cl, h->sm_cr, (size_t)n, P)) return rc;
+  stereo_match_post_kernel<<<(n + 255)/256, 256, 0, h->s>>>(n, h->sm_left, h->sm_right, h->sm_st, h->sm_rank, h->fm_mask, fx, baseline, h->sm_state,
+                                                            h->sm_depth, h->sm_ru, h->sm_cnt);
+  int cnt[3] = {0, 0, 0}, fst = -1;
+  FCK(cudaMemcpyAsync(state, h->sm_state, n, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(depth, h->sm_depth, 8*(size_t)n, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(right_u, h->sm_ru, 8*(size_t)n, cudaMemcpyDeviceToHost, h->s));
+  if (right_pts) FCK(cudaMemcpyAsync(right_pts, h->sm_right, 8*(size_t)n, cudaMemcpyDeviceToHost, h->s));
+  if (lk_status) FCK(cudaMemcpyAsync(lk_status, h->sm_st, n, cudaMemcpyDeviceToHost, h->s));
+  if (F) FCK(cudaMemcpyAsync(F, h->fm_F, 72, cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaMemcpyAsync(&fst, h->fm_stat + 2, 4, cudaMemcpyDeviceToHost, h->s));       // status of problem 0 (9 arrays of 1)
+  FCK(cudaMemcpyAsync(cnt, h->sm_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaEventRecord(h->e1, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  FCK(cudaGetLastError());
+  *matched = cnt[0] >= 8;
+  if (fund_status) *fund_status = cnt[0] >= 8 ? fst : -1;
+  if (n_tracked) *n_tracked = cnt[0]; if (n_inliers) *n_inliers = cnt[1]; if (n_stereo) *n_stereo = cnt[2];
   if (ms_device) FCK(cudaEventElapsedTime(ms_device, h->e0, h->e1));
   return 0;
 }

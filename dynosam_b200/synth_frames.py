@@ -77,3 +77,34 @@ class SyntheticStream:
         for j, (ys, xs) in self.depth_edge_pixels().items():
             d[ys, xs] = self.DEPTH_EDGE_VALUES[j]
         return d
+
+    def right(self, k, fx=721.5377, baseline=0.5372):
+        """the right view (gray uint8 [H,W]) of a rectified stereo pair whose left view is frame(k), rendered from frame(k) and
+        depth(k): the left pixel (x, y) lands at x - fx * baseline / depth(x, y) on the same row (zero disparity where the depth is
+        not finite or not positive).  Each row is resampled linearly between neighbouring left pixels of one surface (disparities
+        within 1 px); where several surfaces cover a right pixel the nearer one (larger disparity) wins, and pixels no surface
+        covers take seeded noise.  frame(k) and depth(k) are unchanged."""
+        gray, _, _ = self.frame(k)
+        d = self.depth(k)
+        disp = np.where(np.isfinite(d) & (d > 0), fx*baseline/np.where(np.isfinite(d) & (d > 0), d, 1.0), 0.0)
+        g = gray.astype(np.float64)
+        H_, W_ = gray.shape
+        xr = np.arange(W_)[None, :] - disp                             # right position of every left pixel
+        a, b = xr[:, :-1], xr[:, 1:]                                   # one segment per pair of horizontal neighbours
+        seg = np.abs(disp[:, 1:] - disp[:, :-1]) <= 1.0
+        lo = np.ceil(np.minimum(a, b)).clip(0, W_); hi = np.floor(np.maximum(a, b)).clip(-1, W_ - 1)
+        cnt = np.where(seg, np.maximum(hi - lo + 1, 0), 0).astype(np.int64).ravel()
+        rows, cols = np.divmod(np.repeat(np.arange(cnt.size), cnt), W_ - 1)
+        first = np.repeat(np.cumsum(cnt) - cnt, cnt)
+        xp = lo.ravel()[rows*(W_ - 1) + cols] + (np.arange(cnt.sum()) - first)      # the covered right pixels of each segment
+        x0, x1 = xr[rows, cols], xr[rows, cols + 1]
+        t = np.where(x1 != x0, (xp - x0)/np.where(x1 != x0, x1 - x0, 1.0), 0.0)
+        val = (1 - t)*g[rows, cols] + t*g[rows, cols + 1]
+        dv = (1 - t)*disp[rows, cols] + t*disp[rows, cols + 1]
+        pix = rows*W_ + xp.astype(np.int64)
+        order = np.lexsort((dv, pix))                                  # by pixel, then disparity: the last of each pixel is the nearest
+        pix, val = pix[order], val[order]
+        last = np.r_[pix[1:] != pix[:-1], True]
+        out = np.random.default_rng([self.seed, 0x7269676874, k]).uniform(0, 255, H_*W_)
+        out[pix[last]] = val[last]
+        return np.clip(np.rint(out), 0, 255).astype(np.uint8).reshape(H_, W_)

@@ -15,6 +15,7 @@
  *   dynofront_find_fundamental_batch cv::findFundamentalMat(FM_RANSAC) (with its LMedS and 7-point paths) on many point sets in one launch
  *   dynofront_detect_static     KltFeatureTracker::detectFeatures: mask, CLAHE, GFTT, range-tree ANMS, cornerSubPix  StaticFeatureTracker.cc:330-418
  *   dynofront_stereo_track      FeatureTracker::stereoTrack: left -> right LK + disparity / depth test  FeatureTracker.cc:194-337
+ *   dynofront_stereo_match      FeatureTracker::stereoTrack in one call: LK, compaction, findFundamentalMat(FM_RANSAC), per-feature loop
  *   dynofront_update_depths     Frame::updateDepths                 dynosam/src/frontend/vision/Frame.cc:241-251,430-467
  *   dynofront_back_project      RGBDInstanceFrontendModule::fillOutputPacketWithTracks, per feature  RGBDInstanceFrontendModule.cc:391-486
  *   dynofront_dense_cloud       Frame::projectToDenseCloud          Frame.cc:172-238
@@ -217,10 +218,42 @@ int dynofront_klt_track_points(dynofront_handle h, const uint8_t* prev_gray, con
                                int32_t* n_verified, int32_t* n_keep, float* ms_device);
 /* FeatureTracker::stereoTrack (FeatureTracker.cc:194-337): LK from the left to the right image (21x21, 5 levels, OpenCV default
  * criteria) and the per-point disparity test: valid[i] = status[i] && !(uL - uR <= 1 || uR < 0), depth[i] = fx * baseline /
- * (uL - uR) (0 where invalid).  The fundamental-matrix RANSAC the reference runs between the two is host code:
- * final = status & ransac_mask & valid. */
+ * (uL - uR) (0 where invalid).  The fundamental-matrix RANSAC the reference runs between the two is not part of this call
+ * (final = status & ransac_mask & valid); dynofront_stereo_match runs the whole chain. */
 int dynofront_stereo_track(dynofront_handle h, const uint8_t* left_gray, const uint8_t* right_gray, int32_t n, const float* left_pts,
                            float* right_pts, uint8_t* status, double fx, double baseline, double* depth, uint8_t* valid, float* ms_device);
+/* The right image of the current frame: uploaded (asynchronously from a dynofront_pin_host buffer, which must then stay untouched
+ * until the next dynofront call returns) and its pyramid built in a slot of its own, without Scharr derivatives (nothing tracks
+ * from the right image).  dynofront_set_frame, dynofront_next_frame and every call that rebuilds the current pyramid from a host
+ * image mark it stale, as set_frame / next_frame do the depth.  Returns without synchronising. */
+int dynofront_set_right(dynofront_handle h, const uint8_t* right_gray);
+/* FeatureTracker::stereoTrack (FeatureTracker.cc:194-337) as ONE call, nothing returning to the host between the stages:
+ * LK from the left to the right image (21x21, maxLevel 5, criteria (30, 0.01), flags 0, minEigThreshold 1e-4), the LK-good
+ * points compacted in input order, cv::findFundamentalMat(FM_RANSAC) over them exactly as dynofront_find_fundamental_batch
+ * (fund == NULL: 1.0 px, 0.99, 1000 iterations), then the per-feature loop.  left_pts[n][2] are the usable static features in
+ * container order as floats (toOpenCV(&ids, true), Feature.cc:389-401).
+ * Images: both NULL -- the left image is the resident current frame of dynofront_next_frame and the right one that of
+ * dynofront_set_right (-2 without either); both given -- they are uploaded into stereo slots of their own.  Neither mode
+ * touches the resident previous / current frame pair that dynofront_klt_track_points and dynofront_track_dynamic_klt read.
+ * *matched = the reference's return value: 0 when n < 8 (nothing runs) or fewer than 8 points were tracked.  state[n]:
+ *   UNTOUCHED  the call returned false: nothing is marked;
+ *   LOST       LK status 0 (determineOutlierIds marks it an outlier);
+ *   EPIPOLAR   the RANSAC mask is 0 (an outlier too).  A failed RANSAC (DYNOFRONT_FUND_FAILED) leaves the reference's
+ *              std::vector mask at its m zeros, so every tracked point is EPIPOLAR; under LMedS the mask is used even when
+ *              findFundamentalMat returns an empty F (fewer than 7 inliers), as the reference does;
+ *   DISPARITY  disparity = uL - uR <= 1 or uR < 0 (markOutlier);
+ *   MATCHED    a stereo feature: depth[i] = fx * baseline / disparity, right_u[i] = uR (the right_u of dynofront_back_project).
+ * depth and right_u are NaN for every other state.  For parity (any may be NULL): right_pts[n][2] / lk_status[n] (the LK
+ * result; right_pts = left_pts and status 0 when n < 8), F[9] (0 without a model), fund_status (DYNOFRONT_FUND_*, -1 when the
+ * RANSAC did not run), n_tracked (LK-good points), n_inliers (mask ones), n_stereo (MATCHED points).  Afterwards
+ * dynofront_fundamental_last_trace describes the call's RANSAC as one problem (of 0 points when fewer than 8 were tracked; no
+ * problem when n < 8).  Refused with -1: non-finite points, fundamental parameters as in dynofront_find_fundamental_batch. */
+enum { DYNOFRONT_STEREO_UNTOUCHED = 0, DYNOFRONT_STEREO_MATCHED = 1, DYNOFRONT_STEREO_LOST = 2, DYNOFRONT_STEREO_EPIPOLAR = 3,
+       DYNOFRONT_STEREO_DISPARITY = 4 };
+int dynofront_stereo_match(dynofront_handle h, const uint8_t* left_gray, const uint8_t* right_gray, int32_t n, const float* left_pts,
+                           double fx, double baseline, const dynofront_fundamental_params* fund, int32_t* matched, uint8_t* state,
+                           double* depth, double* right_u, float* right_pts, uint8_t* lk_status, double* F, int32_t* fund_status,
+                           int32_t* n_tracked, int32_t* n_inliers, int32_t* n_stereo, float* ms_device);
 /* parity hook: (min eigenvalue, trace/(2 win^2)) of the level-0 spatial gradient matrix of the last forward pass, [n][2] */
 int dynofront_klt_last_min_eig(dynofront_handle h, int32_t n, float* out);
 
@@ -299,7 +332,7 @@ int dynofront_update_depths(dynofront_handle h, int32_t n, const double* kp, con
                             float* ms_device);
 /* The per-feature half of RGBDInstanceFrontendModule::fillOutputPacketWithTracks (:391-486), on the usable features in input
  * order: kp[n][2], depth[n] (NaN = no depth), usable[n]; right_u[n] (may be NULL; NaN = none) carries the right key-points of
- * dynofront_stereo_track (FeatureTracker.cc:314-324).
+ * stereoTrack (FeatureTracker.cc:314-324): dynofront_stereo_match's depth[n] and right_u[n] go here as they are.
  *   with depth: point = X_world * BackprojectFromCamera(Cal3_S2::calibrate(kp), depth) (Camera::backProject, Camera.cc:95-99;
  *     calibrate in GTSAM 4.2's operation order, transformFrom as ((R_i0 x + R_i1 y) + R_i2 z) + t_i; X_world NULL: the camera
  *     frame, the identity transform not applied);
