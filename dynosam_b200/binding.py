@@ -12,7 +12,7 @@ from .problem import ARITY, DIM, JCOLS, MEAS_DIM, Problem
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdynoba.so")
 
-POSE6, POINT3, FLOW2 = 0, 1, 2
+POSE6, POINT3, FLOW2, VEL3, BIAS6 = 0, 1, 2, 3, 4
 OK, ERR_BAD_ARG, ERR_STATE, ERR_CUDA, ERR_INDETERMINATE, ERR_UNSUPPORTED, ERR_COMM = 0, -1, -2, -3, -4, -5, -6
 
 c_dp = C.POINTER(C.c_double)
@@ -24,7 +24,7 @@ REDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.
 EXPORTS = [
     "dynoba_version", "dynoba_status_string", "dynoba_last_error", "dynoba_create", "dynoba_destroy",
     "dynoba_lm_default_params", "dynoba_set_variables", "dynoba_set_aux_poses", "dynoba_set_calibration",
-    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_marginal", "dynoba_finalize", "dynoba_error",
+    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_marginal", "dynoba_finalize", "dynoba_error",
     "dynoba_optimize", "dynoba_get_variables", "dynoba_get_keys", "dynoba_num_variables", "dynoba_problem_info",
     "dynoba_linearize", "dynoba_linearize_block", "dynoba_get_linearization", "dynoba_get_factor_errors", "dynoba_solve",
     "dynoba_get_reduced_system", "dynoba_retract", "dynoba_flow_pose_default_params", "dynoba_flow_pose_batch",
@@ -95,6 +95,7 @@ def load():
         L.dynoba_set_calibration.argtypes = [C.c_void_p, c_dp]
         L.dynoba_add_factors.argtypes = [C.c_void_p, C.c_int, C.c_int64, c_ip, c_dp, c_dp, C.c_int, C.c_int64, C.c_double, c_ip]
         L.dynoba_set_pose_order.argtypes = [C.c_void_p, C.c_int64, c_ip]
+        L.dynoba_set_variable_order.argtypes = [C.c_void_p, C.c_int, C.c_int64, c_ip]
         L.dynoba_set_shard.argtypes = [C.c_void_p, C.c_int, C.c_int, ALLREDUCE_FN, C.c_void_p, C.c_int]
         L.dynoba_set_reduce.argtypes = [C.c_void_p, REDUCE_FN, C.c_void_p]
         L.dynoba_set_partition.argtypes = [C.c_void_p, C.c_int]
@@ -202,6 +203,11 @@ class Solver:
             self.add_factors(b)
         if p.pose_order is not None:
             self._ck(L.dynoba_set_pose_order(self.h, p.n_pose, _ip(p.pose_order)))
+        for kind, arr, order in ((VEL3, p.vel, p.vel_order), (BIAS6, p.bias, p.bias_order)):
+            if arr.shape[0]:
+                self._ck(L.dynoba_set_variables(self.h, kind, arr.shape[0], C.cast(None, c_u64p), _dp(arr)))
+            if order is not None:
+                self._ck(L.dynoba_set_variable_order(self.h, kind, arr.shape[0], _ip(order)))
         for pr in getattr(p, "linear_priors", []):
             self.add_linear_prior(pr["idx"], pr["lin"], pr["G"], pr["g"], pr.get("f", 0.0))
 
@@ -268,6 +274,19 @@ class Solver:
             self._ck(self.lib.dynoba_set_variables(self.h, POINT3, p.n_point, C.cast(None, c_u64p), _dp(p.point)))
         if p.n_flow:
             self._ck(self.lib.dynoba_set_variables(self.h, FLOW2, p.n_flow, C.cast(None, c_u64p), _dp(p.flow)))
+        for kind, arr in ((VEL3, p.vel), (BIAS6, p.bias)):
+            if arr.shape[0]:
+                self._ck(self.lib.dynoba_set_variables(self.h, kind, arr.shape[0], C.cast(None, c_u64p), _dp(arr)))
+
+    def set_variables(self, kind, data, keys=None):
+        data = np.ascontiguousarray(data, dtype=np.float64)
+        n = data.shape[0] if data.ndim > 1 else 0
+        k = np.ascontiguousarray(keys, dtype=np.uint64).ctypes.data_as(c_u64p) if keys is not None else C.cast(None, c_u64p)
+        self._ck(self.lib.dynoba_set_variables(self.h, kind, n, k, _dp(data)))
+
+    def set_variable_order(self, kind, rank):
+        rank = np.ascontiguousarray(rank, dtype=np.int32)
+        self._ck(self.lib.dynoba_set_variable_order(self.h, kind, rank.size, _ip(rank)))
 
     def finalize(self):
         self._ck(self.lib.dynoba_finalize(self.h))
@@ -308,12 +327,13 @@ class Solver:
 
     def solve(self, lam):
         p = self.problem
-        d = np.zeros(6*p.n_pose + 3*p.n_point + 2*p.n_flow)
+        d = np.zeros(6*p.n_pose + 3*p.n_point + 2*p.n_flow + 3*p.n_vel + 6*p.n_bias)
         self._ck(self.lib.dynoba_solve(self.h, float(lam), _dp(d)))
         return d
 
     def reduced_system(self, lam):
-        n = 6*self.problem.n_pose
+        p = self.problem
+        n = 6*p.n_pose + 3*p.n_vel + 6*p.n_bias
         S = np.zeros((n, n)); g = np.zeros(n)
         self._ck(self.lib.dynoba_get_reduced_system(self.h, float(lam), _dp(S), _dp(g)))
         return S, g
@@ -336,6 +356,16 @@ class Solver:
         if p.n_flow:
             self._ck(self.lib.dynoba_get_variables(self.h, FLOW2, p.n_flow, _dp(flow)))
         return pose, point, flow
+
+    def nav_values(self):
+        """(velocities [n_vel, 3], biases [n_bias, 6]) at the current values"""
+        p = self.problem
+        vel = np.zeros((p.n_vel, 3)); bias = np.zeros((p.n_bias, 6))
+        if p.n_vel:
+            self._ck(self.lib.dynoba_get_variables(self.h, VEL3, p.n_vel, _dp(vel)))
+        if p.n_bias:
+            self._ck(self.lib.dynoba_get_variables(self.h, BIAS6, p.n_bias, _dp(bias)))
+        return vel, bias
 
 
 def _cat(problems, key, width):

@@ -60,6 +60,9 @@ struct dynoba_solver {
   std::vector<double> pose, point, flow, aux; std::vector<uint64_t> kpose, kpoint, kflow;
   double calib[6] = { 721.5377, 721.5377, 0.0, 609.5593, 172.854, 0.5372 };
   std::vector<int32_t> hint;
+  // navigation variables (DYNOBA_VEL3 / DYNOBA_BIAS6): pose-like, solver positions pos[np + i] / pos[np + nv + i]
+  std::vector<double> vel, bias; std::vector<uint64_t> kvel, kbias; std::vector<int32_t> vhint, bhint;
+  int2* d_nav = nullptr; int n_nav = 0;   // device (position, dimension) of every velocity and bias
   std::vector<HostBlock> blocks;
   std::vector<HostPrior> priors;
   bool finalized = false, linearized = false, supported = true;
@@ -222,15 +225,47 @@ int dynoba_destroy(dynoba_handle h) {
   return DYNOBA_OK;
 }
 
+static std::vector<double>* var_store(dynoba_solver* h, int kind) {
+  switch (kind) {
+    case DYNOBA_POSE6: return &h->pose; case DYNOBA_POINT3: return &h->point; case DYNOBA_FLOW2: return &h->flow;
+    case DYNOBA_VEL3: return &h->vel; case DYNOBA_BIAS6: return &h->bias; default: return nullptr;
+  }
+}
+static std::vector<uint64_t>* key_store(dynoba_solver* h, int kind) {
+  switch (kind) {
+    case DYNOBA_POSE6: return &h->kpose; case DYNOBA_POINT3: return &h->kpoint; case DYNOBA_FLOW2: return &h->kflow;
+    case DYNOBA_VEL3: return &h->kvel; case DYNOBA_BIAS6: return &h->kbias; default: return nullptr;
+  }
+}
+static int kind_width(int kind) { return kind == DYNOBA_POSE6 ? 12 : (kind == DYNOBA_POINT3 || kind == DYNOBA_VEL3 ? 3 : (kind == DYNOBA_BIAS6 ? 6 : 2)); }
+static bool has_nav(const dynoba_solver* h) { return !h->vel.empty() || !h->bias.empty(); }
+
 int dynoba_set_variables(dynoba_handle h, int kind, int64_t n, const uint64_t* keys, const double* data) {
   ARG(h, "null handle"); ARG(n >= 0 && (n == 0 || data), "null data");
-  const int w = kind == DYNOBA_POSE6 ? 12 : (kind == DYNOBA_POINT3 ? 3 : 2);
-  std::vector<double>* dst = kind == DYNOBA_POSE6 ? &h->pose : (kind == DYNOBA_POINT3 ? &h->point : (kind == DYNOBA_FLOW2 ? &h->flow : nullptr));
-  std::vector<uint64_t>* kd = kind == DYNOBA_POSE6 ? &h->kpose : (kind == DYNOBA_POINT3 ? &h->kpoint : &h->kflow);
+  const int w = kind_width(kind);
+  std::vector<double>* dst = var_store(h, kind);
+  std::vector<uint64_t>* kd = key_store(h, kind);
   ARG(dst, "bad variable kind");
   const bool same_shape = dst->size() == (size_t)n*w;
   dst->assign(data, data + (size_t)n*w);
   if (keys) kd->assign(keys, keys + n); else if (!same_shape) kd->clear();   // a value refresh keeps the keys
+  if (h->finalized && same_shape && (has_nav(h) || kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6)) {
+    // pose-like values of a visual-inertial graph: the pose SoA holds poses, velocities and biases, so only the rows of
+    // the refreshed kind are replaced in the current device image
+    const int64_t np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3;
+    const int64_t base = kind == DYNOBA_POSE6 ? 0 : (kind == DYNOBA_VEL3 ? np : np + nv);
+    const int st = h->cur.np_stride;
+    if (kind == DYNOBA_POSE6 || kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6) {
+      if (n == 0) return DYNOBA_OK;
+      cudaSetDevice(h->device);
+      std::vector<double> soa((size_t)12*st);
+      CK(cudaMemcpy(soa.data(), h->cur.pose, soa.size()*8, cudaMemcpyDeviceToHost));
+      for (int64_t i = 0; i < n; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*st + h->pos[base + i]] = k < w ? data[i*w + k] : 0.0;
+      CK(cudaMemcpy(h->cur.pose, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
+      h->linearized = false;
+      return DYNOBA_OK;
+    }
+  }
   if (h->finalized && same_shape) {
     // refresh device values only (layout unchanged)
     cudaSetDevice(h->device);
@@ -275,14 +310,27 @@ int dynoba_add_factors(dynoba_handle h, int type, int64_t n, const int32_t* idx,
   ARG(h, "null handle"); ARG(type >= 0 && type < F_NUM_TYPES, "bad factor type");
   const TypeInfo ti = type_info(type);
   ARG(n >= 0 && (n == 0 || idx), "null idx"); ARG(ti.meas == 0 || n == 0 || meas, "factor type needs measurements");
-  ARG(sigma && (sigma_dim == 1 || sigma_dim == ti.dim), "sigma_dim must be 1 or the residual dimension");
+  const bool imu = type == F_COMBINED_IMU15;
+  // the reference never robustifies the visual-inertial factors (VisionImuBackendModule.hpp:114-243)
+  if (is_nav_type(type) && robust_k > 0) { h->err = "the IMU factor and the velocity / bias priors take no robust kernel (robust_k must be <= 0)"; return DYNOBA_ERR_UNSUPPORTED; }
+  if (imu) {
+    ARG(sigma && sigma_dim == IMU_SQRT_INFO, "COMBINED_IMU15 takes its 15x15 square-root information: sigma_dim must be 225");
+  } else {
+    ARG(sigma && (sigma_dim == 1 || sigma_dim == ti.dim), "sigma_dim must be 1 or the residual dimension");
+  }
   ARG(sigma_count == 1 || sigma_count == n, "sigma_count must be 1 or n"); ARG(!ti.needs_aux || n == 0 || aux_idx, "factor type needs aux_idx");
   HostBlock b; b.type = type; b.n = n;
   par_assign(b.idx, idx, (size_t)n*ti.arity);
   if (ti.meas) par_assign(b.meas, meas, (size_t)n*ti.meas);
   b.sigma_dim = sigma_dim; b.bcast = sigma_count == 1 && n != 1;
   b.sigma.assign(sigma, sigma + (size_t)sigma_count*sigma_dim);
-  for (double s : b.sigma) ARG(s > 0, "sigma must be positive");
+  if (imu) {
+    // noiseModel::Gaussian's R: finite, upper triangular Cholesky factor with a positive diagonal
+    for (double s : b.sigma) ARG(std::isfinite(s), "square-root information must be finite");
+    for (size_t o = 0; o < b.sigma.size(); o += IMU_SQRT_INFO) for (int k = 0; k < 15; k++) ARG(b.sigma[o + 16*k] > 0, "square-root information must have a positive diagonal");
+  }
+  else for (double s : b.sigma) ARG(s > 0, "sigma must be positive");
+  if (imu) for (size_t i = 0; i < b.meas.size(); i++) ARG(std::isfinite(b.meas[i]), "IMU measurement must be finite");
   b.robust_k = robust_k;
   if (aux_idx) { par_assign(b.aux, aux_idx, (size_t)n); b.has_aux = true; }
   h->blocks.push_back(std::move(b));
@@ -292,6 +340,7 @@ int dynoba_add_factors(dynoba_handle h, int type, int64_t n, const int32_t* idx,
 
 int dynoba_add_linear_prior(dynoba_handle h, int32_t n, const int32_t* pose_idx, const double* lin_poses, const double* G, const double* g, double f) {
   ARG(h, "null handle"); ARG(n > 0 && n <= 512 && pose_idx && lin_poses && G && g, "bad prior");
+  if (has_nav(h)) { h->err = "dynoba_add_linear_prior is not available with velocity / bias variables"; return DYNOBA_ERR_UNSUPPORTED; }
   HostPrior P; P.idx.assign(pose_idx, pose_idx + n); P.lin.assign(lin_poses, lin_poses + (size_t)12*n);
   P.G.assign(G, G + (size_t)36*n*n); P.g.assign(g, g + (size_t)6*n); P.f = f;
   { std::vector<int32_t> srt = P.idx; std::sort(srt.begin(), srt.end()); ARG(std::adjacent_find(srt.begin(), srt.end()) == srt.end(), "a prior lists a variable twice"); }
@@ -309,8 +358,17 @@ int dynoba_set_pose_order(dynoba_handle h, int64_t n, const int32_t* rank) {
   return DYNOBA_OK;
 }
 
+int dynoba_set_variable_order(dynoba_handle h, int kind, int64_t n, const int32_t* rank) {
+  ARG(h, "null handle"); ARG(kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6, "variable order hints are for DYNOBA_VEL3 / DYNOBA_BIAS6 (poses: dynoba_set_pose_order)");
+  ARG(n >= 0 && (n == 0 || rank), "null rank");
+  (kind == DYNOBA_VEL3 ? h->vhint : h->bhint).assign(rank, rank + n);
+  if (h->finalized) free_device(h);
+  return DYNOBA_OK;
+}
+
 int dynoba_set_reduce(dynoba_handle h, dynoba_reduce_fn fn, void* ctx) {
   ARG(h, "null handle");
+  if (fn && has_nav(h)) { h->err = "dynoba_set_reduce is not available with velocity / bias variables"; return DYNOBA_ERR_UNSUPPORTED; }
   h->reduce = fn; h->red_ctx = ctx;
   return DYNOBA_OK;
 }
@@ -339,6 +397,7 @@ int dynoba_set_partition(dynoba_handle h, int ncells) {
 
 int dynoba_set_shard(dynoba_handle h, int rank, int world, dynoba_allreduce_fn fn, void* ctx, int min_bandwidth) {
   ARG(h, "null handle"); ARG(world >= 1 && rank >= 0 && rank < world, "bad rank/world"); ARG(world == 1 || fn, "world > 1 needs an all-reduce");
+  if (world > 1 && has_nav(h)) { h->err = "dynoba_set_shard is not available with velocity / bias variables"; return DYNOBA_ERR_UNSUPPORTED; }
   h->rank = rank; h->world = world; h->allreduce = fn; h->ar_ctx = ctx; h->min_bw = min_bandwidth;
   if (h->finalized) free_device(h);
   return DYNOBA_OK;
@@ -359,7 +418,16 @@ static int finalize_impl(dynoba_solver* h) {
   auto lap = [&](const char* what) { if (!timing) return; auto t = std::chrono::steady_clock::now();
     std::fprintf(stderr, "[dynoba finalize] %-28s %8.1f ms\n", what, std::chrono::duration<double, std::milli>(t - t_last).count()); t_last = t; };
   const int64_t np = (int64_t)h->pose.size()/12, npt = (int64_t)h->point.size()/3, nfl = (int64_t)h->flow.size()/2, naux = (int64_t)h->aux.size()/12;
+  const int64_t nv = (int64_t)h->vel.size()/3, nb = (int64_t)h->bias.size()/6, NP = np + nv + nb;   // NP: pose-like variables
   ARG(h->hint.empty() || (int64_t)h->hint.size() == np, "pose order hint length != number of poses");
+  ARG(h->vhint.empty() || (int64_t)h->vhint.size() == nv, "velocity order hint length != number of velocities");
+  ARG(h->bhint.empty() || (int64_t)h->bhint.size() == nb, "bias order hint length != number of biases");
+  if (NP > np && (!h->priors.empty() || h->world > 1 || h->reduce)) {
+    h->err = "velocity / bias variables cannot be combined with dynoba_add_linear_prior, dynoba_set_shard or dynoba_set_reduce";
+    return DYNOBA_ERR_UNSUPPORTED;
+  }
+  // pose-like index of a key slot: poses [0, np), velocities [np, np + nv), biases [np + nv, NP)
+  auto plx = [&](int cls, int32_t ix) -> int64_t { return cls == VC_POSE ? ix : (cls == VC_VEL ? np + ix : np + nv + ix); };
   // ---- validate indices
   for (auto& b : h->blocks) {
     const TypeInfo ti = type_info(b.type);
@@ -368,7 +436,8 @@ static int finalize_impl(dynoba_solver* h) {
     for (int64_t i = 0; i < b.n; i++) {
       for (int k = 0; k < ti.arity; k++) {
         const int32_t ix = b.idx[i*ti.arity + k];
-        const int64_t lim = ti.cls[k] == VC_POSE ? np : (ti.cls[k] == VC_POINT ? npt : nfl);
+        const int c = ti.cls[k];
+        const int64_t lim = c == VC_POSE ? np : (c == VC_POINT ? npt : (c == VC_FLOW ? nfl : (c == VC_VEL ? nv : nb)));
         if (!(ix >= 0 && ix < lim)) bad |= 1;
       }
       if (b.has_aux && !(b.aux[i] >= 0 && b.aux[i] < naux)) bad |= 2;
@@ -377,11 +446,21 @@ static int finalize_impl(dynoba_solver* h) {
   }
   lap("validate");
   // ---- pose ordering
-  h->pos.resize(np);
-  {
+  h->pos.resize(NP);
+  if (NP == np) {
     std::vector<int32_t> ord(np); std::iota(ord.begin(), ord.end(), 0);
     if (!h->hint.empty()) std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return h->hint[a] < h->hint[b]; });
     for (int64_t i = 0; i < np; i++) h->pos[ord[i]] = (int32_t)i;
+  } else {
+    // visual-inertial graph: ordered by (rank, kind: pose < velocity < bias, index); a kind without a hint ranks by index,
+    // so X_k, V_k, b_k with the frame as rank sit next to each other and the system stays banded
+    std::vector<int32_t> ord(NP), rk(NP);
+    std::iota(ord.begin(), ord.end(), 0);
+    for (int64_t i = 0; i < np; i++) rk[i] = h->hint.empty() ? (int32_t)i : h->hint[i];
+    for (int64_t i = 0; i < nv; i++) rk[np + i] = h->vhint.empty() ? (int32_t)i : h->vhint[i];
+    for (int64_t i = 0; i < nb; i++) rk[np + nv + i] = h->bhint.empty() ? (int32_t)i : h->bhint[i];
+    std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return rk[a] < rk[b]; });
+    for (int64_t i = 0; i < NP; i++) h->pos[ord[i]] = (int32_t)i;
   }
   // ---- landmark groups (union-find across factors that touch two landmarks)
   const int64_t nl = npt + nfl;
@@ -407,12 +486,12 @@ static int finalize_impl(dynoba_solver* h) {
   for (size_t bi = 0; bi < h->blocks.size(); bi++) {
     auto& b = h->blocks[bi]; const TypeInfo ti = type_info(b.type);
     b.pose_only = ti.nlmk == 0;
-    int lslot = -1; for (int k = 0; k < ti.arity; k++) if (ti.cls[k] != VC_POSE) { lslot = k; break; }
+    int lslot = -1; for (int k = 0; k < ti.arity; k++) if (!is_poselike(ti.cls[k])) { lslot = k; break; }
     int bspread = 0, blo = INT32_MAX, bhi = -1;
 #pragma omp parallel for schedule(static) reduction(max:bspread) reduction(min:blo) reduction(max:bhi)
     for (int64_t i = 0; i < b.n; i++) {
       int lo = INT32_MAX, hi = -1;
-      for (int k = 0; k < ti.arity; k++) if (ti.cls[k] == VC_POSE) { const int p = h->pos[b.idx[i*ti.arity + k]]; lo = std::min(lo, p); hi = std::max(hi, p); }
+      for (int k = 0; k < ti.arity; k++) if (is_poselike(ti.cls[k])) { const int p = h->pos[plx(ti.cls[k], b.idx[i*ti.arity + k])]; lo = std::min(lo, p); hi = std::max(hi, p); }
       blo = std::min(blo, lo); bhi = std::max(bhi, hi);
       if (lslot < 0) { bspread = std::max(bspread, hi - lo); continue; }
       const int g = root[lmk_id(ti.cls[lslot], b.idx[i*ti.arity + lslot])];
@@ -479,7 +558,7 @@ static int finalize_impl(dynoba_solver* h) {
   // ---- band structure: cell decomposition of the reduced system (kernels_band.cu)
   {
     int bw = 6*spread + 5; if (bw < h->min_bw) bw = h->min_bw;
-    if (band_plan_layout(h->plan, (int)(6*np), bw, h->ncell_request, h->rank, h->world)) { h->err = "band layout failed"; return DYNOBA_ERR_BAD_ARG; }
+    if (band_plan_layout(h->plan, (int)(6*NP), bw, h->ncell_request, h->rank, h->world)) { h->err = "band layout failed"; return DYNOBA_ERR_BAD_ARG; }
     double* dbuf; int* ibuf; char* desc; double* dp = nullptr; int rc;
     if ((rc = dalloc(h, &dbuf, h->plan.n_doubles, false))) return rc;     // accumulated part: band_clear; work buffers: written before read
     if ((rc = dalloc(h, &ibuf, h->plan.n_ints, false))) return rc;        // flags: cleared before every factorisation launch
@@ -517,7 +596,7 @@ static int finalize_impl(dynoba_solver* h) {
   DevBand& B = h->band;
   // ---- variables
   DevVars& V = h->cur;
-  V.np = (int)np; V.np_stride = pad32(np); V.nl = (int)npt; V.nl_stride = pad32(npt); V.nf = (int)nfl; V.nf_stride = pad32(nfl);
+  V.np = (int)NP; V.np_stride = pad32(NP); V.nl = (int)npt; V.nl_stride = pad32(npt); V.nf = (int)nfl; V.nf_stride = pad32(nfl);
   V.naux = (int)naux; V.naux_stride = pad32(naux);
   for (int i = 0; i < 6; i++) V.K[i] = h->calib[i];
   h->cand = V;
@@ -525,6 +604,8 @@ static int finalize_impl(dynoba_solver* h) {
     std::vector<double> soa((size_t)12*V.np_stride, 0.0);
     for (int p = 0; p < V.np_stride; p++) soa[(size_t)0*V.np_stride + p] = soa[(size_t)4*V.np_stride + p] = soa[(size_t)8*V.np_stride + p] = 1.0;
     for (int64_t i = 0; i < np; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.np_stride + h->pos[i]] = h->pose[i*12 + k];
+    for (int64_t i = 0; i < nv; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.np_stride + h->pos[np + i]] = k < 3 ? h->vel[i*3 + k] : 0.0;
+    for (int64_t i = 0; i < nb; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.np_stride + h->pos[np + nv + i]] = k < 6 ? h->bias[i*6 + k] : 0.0;
     int rc = dalloc(h, &h->cur.pose, soa.size()); if (rc) return rc; rc = dalloc(h, &h->cand.pose, soa.size()); if (rc) return rc;
     CK(cudaMemcpy(h->cur.pose, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(h->cand.pose, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
@@ -548,7 +629,7 @@ static int finalize_impl(dynoba_solver* h) {
   }
   lap("band + variables upload");
   // ---- factor blocks
-  h->supported = true; h->jac_bytes = 96*(np + naux) + 24*npt + 16*nfl;
+  h->supported = true; h->jac_bytes = 96*(np + naux) + 24*npt + 16*nfl + 24*nv + 48*nb;
   int part = 0, bs = 0;
   struct GenRef { int32_t rank, blk, idx; };
   std::vector<GenRef> gen_refs;
@@ -563,7 +644,7 @@ static int finalize_impl(dynoba_solver* h) {
     auto& b = h->blocks[bi]; const TypeInfo ti = type_info(b.type);
     const int64_t n = b.n; const int stride = pad32(n);
     int lslot = -1, pslot = -1;
-    for (int k = 0; k < ti.arity; k++) { if (ti.cls[k] != VC_POSE && lslot < 0) lslot = k; if (ti.cls[k] == VC_POSE && pslot < 0) pslot = k; }
+    for (int k = 0; k < ti.arity; k++) { if (!is_poselike(ti.cls[k]) && lslot < 0) lslot = k; if (ti.cls[k] == VC_POSE && pslot < 0) pslot = k; }
     // (serial value-initialisation of 10^7-element vectors costs tens of milliseconds each: first-touch them in parallel)
     b.perm.resize(n);
 #pragma omp parallel for schedule(static)
@@ -658,10 +739,13 @@ static int finalize_impl(dynoba_solver* h) {
       const int64_t o = b.perm[s];
       for (int k = 0; k < ti.arity; k++) {
         const int32_t ix = b.idx[o*ti.arity + k];
-        hidx[(size_t)k*stride + s] = ti.cls[k] == VC_POSE ? h->pos[ix] : (ti.cls[k] == VC_POINT ? h->pt_new[ix] : h->fl_new[ix]);
+        hidx[(size_t)k*stride + s] = is_poselike(ti.cls[k]) ? h->pos[plx(ti.cls[k], ix)] : (ti.cls[k] == VC_POINT ? h->pt_new[ix] : h->fl_new[ix]);
       }
       for (int k = 0; k < ti.meas; k++) hmeas[(size_t)k*stride + s] = b.meas[o*ti.meas + k];
-      for (int k = 0; k < b.sigma_dim; k++) hsig[(size_t)k*stride + s] = 1.0/(b.bcast ? b.sigma[k] : b.sigma[o*b.sigma_dim + k]);
+      if (b.type == F_COMBINED_IMU15)   // square-root information, used as given
+        for (int k = 0; k < b.sigma_dim; k++) hsig[(size_t)k*stride + s] = b.bcast ? b.sigma[k] : b.sigma[o*b.sigma_dim + k];
+      else
+        for (int k = 0; k < b.sigma_dim; k++) hsig[(size_t)k*stride + s] = 1.0/(b.bcast ? b.sigma[k] : b.sigma[o*b.sigma_dim + k]);
       if (b.has_aux) haux[s] = b.aux[o];
     }
     lap("  blk soa fill");
@@ -723,7 +807,7 @@ static int finalize_impl(dynoba_solver* h) {
 #pragma omp parallel for schedule(static, 1)
         for (int t = 0; t < nseg; t++) {
           const int ga = (int)((int64_t)ng*t/nseg), gb_ = (int)((int64_t)ng*(t + 1)/nseg);
-          std::vector<int32_t> stamp(np, -1), gstamp(np, -1), inchunk(np, -1), cur;
+          std::vector<int32_t> stamp(NP, -1), gstamp(NP, -1), inchunk(NP, -1), cur;   // indexed by solver position
           int cur_g0 = ga, chunk_id = 0; SegOut& out = seg[t];
           auto close_chunk = [&](int g_end) {
             std::vector<int32_t> sorted = cur; std::sort(sorted.begin(), sorted.end());
@@ -796,7 +880,7 @@ static int finalize_impl(dynoba_solver* h) {
       }
     }
     lap("  blk groups+windows");
-    b.part_off = part; part += linearize_grid((int)n);
+    b.part_off = part; part += is_nav_type(b.type) ? nav_grid(b.type, (int)n) : linearize_grid((int)n);
     b.bs_off = bs; bs += b.pose_only ? (int)((n + 127)/128) : backsub_grid(d.n_groups);
     const int64_t rd = 4*ti.arity + 8*ti.meas + 8*b.sigma_dim + (b.has_aux ? 4 : 0), wr = 8*(ti.dim*ti.jcols + ti.dim);
     h->jac_bytes += n*(rd + wr);
@@ -845,6 +929,15 @@ static int finalize_impl(dynoba_solver* h) {
     if ((rc = dalloc(h, &dd, (size_t)6*n))) return rc; if ((rc = dalloc(h, &dgc, (size_t)6*n))) return rc;
     P.dev = DevPrior{ n, dpos, dlin, dG, dg, P.f, dd, dgc };
     P.part_off = part; part += 1; P.bs_off = bs; bs += 1;
+  }
+  h->n_nav = 0; h->d_nav = nullptr;
+  if (NP > np) {
+    std::vector<int2> nav(nv + nb);
+    for (int64_t i = 0; i < nv; i++) nav[i] = make_int2(h->pos[np + i], 3);
+    for (int64_t i = 0; i < nb; i++) nav[nv + i] = make_int2(h->pos[np + nv + i], 6);
+    int rc; if ((rc = dalloc(h, &h->d_nav, nav.size(), false))) return rc;
+    CK(cudaMemcpy(h->d_nav, nav.data(), nav.size()*sizeof(int2), cudaMemcpyHostToDevice));
+    h->n_nav = (int)nav.size();
   }
   h->gen_bs_off = bs; bs += general_grid(h->gen.n_groups);
   h->n_lin_partials = part; h->n_bs_partials = bs + pose_norm_grid(B.n);
@@ -937,6 +1030,7 @@ static int do_linearize(dynoba_solver* h) {
 static int build_reduced(dynoba_solver* h, double lambda, bool full_sum = false) {
   CK(cudaMemsetAsync(h->fail, 0, 4, h->stream));
   h->launches += launch_band_clear(h->band, lambda, h->rank, (h->world > 1 && h->reduce && h->band.ncell > 0 && !full_sum) ? h->world : 1, h->stream);
+  h->launches += launch_nav_inert(h->band, h->d_nav, h->n_nav, h->stream);
   for (auto& b : h->blocks) {
     if (b.pose_only) h->launches += launch_pose_factors(b.dev, h->band, h->stream);
     else {
@@ -1023,12 +1117,16 @@ int dynoba_finalize(dynoba_handle h) { if (!h) return DYNOBA_ERR_BAD_ARG; return
 
 int dynoba_num_variables(dynoba_handle h, int kind, int64_t* out) {
   ARG(h && out, "null");
-  *out = kind == DYNOBA_POSE6 ? (int64_t)h->pose.size()/12 : (kind == DYNOBA_POINT3 ? (int64_t)h->point.size()/3 : (int64_t)h->flow.size()/2);
+  const std::vector<double>* v = var_store(h, kind);
+  ARG(v, "bad variable kind");
+  *out = (int64_t)v->size()/kind_width(kind);
   return DYNOBA_OK;
 }
 int dynoba_get_keys(dynoba_handle h, int kind, int64_t n, uint64_t* out) {
   ARG(h && out, "null");
-  auto& k = kind == DYNOBA_POSE6 ? h->kpose : (kind == DYNOBA_POINT3 ? h->kpoint : h->kflow);
+  const std::vector<uint64_t>* kp = key_store(h, kind);
+  ARG(kp, "bad variable kind");
+  const auto& k = *kp;
   ARG((int64_t)k.size() == n, "no keys stored / size mismatch");
   std::copy(k.begin(), k.end(), out);
   return DYNOBA_OK;
@@ -1121,22 +1219,29 @@ int dynoba_get_reduced_system(dynoba_handle h, double lambda, double* S, double*
     if (p.ff) p.ff = hacc.data() + (p.ff - B.acc); if (p.gf) p.gf = hacc.data() + (p.gf - B.acc);
   }
   DevBand HB = B; HB.chains = hch.data(); HB.cells = h->plan.cells.data();
-  const int n = B.n; const int64_t np = n/6;
-  std::vector<int32_t> inv(np); for (int64_t i = 0; i < np; i++) inv[h->pos[i]] = (int32_t)i;
-  auto user = [&](int s) { return 6*inv[s/6] + s%6; };
+  // caller layout [poses 6 | velocities 3 | biases 6]; the inert scalars of the velocity blocks are left out
+  const int nb_ = B.n; const int64_t NP = nb_/6, np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3;
+  std::vector<int32_t> usr(nb_, -1);
+  for (int64_t i = 0; i < NP; i++) {
+    const int64_t off = i < np ? 6*i : (i < np + nv ? 6*np + 3*(i - np) : 6*np + 3*nv + 6*(i - np - nv));
+    const int d = i >= np && i < np + nv ? 3 : 6;
+    for (int c = 0; c < d; c++) usr[6*(size_t)h->pos[i] + c] = (int32_t)(off + c);
+  }
+  const int n = (int)(nb_ - 3*nv);
   if (S) {
     std::fill(S, S + (size_t)n*n, 0.0);
-    for (int j = 0; j < n; j++) for (int i = j; i < n && i <= j + B.bw; i++) {
+    for (int j = 0; j < nb_; j++) for (int i = j; i < nb_ && i <= j + B.bw; i++) {
+      if (usr[i] < 0 || usr[j] < 0) continue;
       const double v = *band_at(HB, i, j);
-      S[(size_t)user(i)*n + user(j)] = v; S[(size_t)user(j)*n + user(i)] = v;
+      S[(size_t)usr[i]*n + usr[j]] = v; S[(size_t)usr[j]*n + usr[i]] = v;
     }
   }
-  if (g) for (int i = 0; i < n; i++) g[user(i)] = *rhs_at(HB, i);
+  if (g) for (int i = 0; i < nb_; i++) if (usr[i] >= 0) g[usr[i]] = *rhs_at(HB, i);
   return DYNOBA_OK;
 }
 
 static int download_delta(dynoba_solver* h, double* delta) {
-  const DevBand& B = h->band; const int64_t np = B.n/6, npt = h->cur.nl, nfl = h->cur.nf;
+  const DevBand& B = h->band; const int64_t np = (int64_t)h->pose.size()/12, npt = h->cur.nl, nfl = h->cur.nf;
   std::vector<double> hr(B.n_pad), hp((size_t)3*h->cur.nl_stride), hf((size_t)2*h->cur.nf_stride);
   CK(cudaMemcpyAsync(hr.data(), B.dp, hr.size()*8, cudaMemcpyDeviceToHost, h->stream));
   if (npt) CK(cudaMemcpyAsync(hp.data(), h->dl_point, hp.size()*8, cudaMemcpyDeviceToHost, h->stream));
@@ -1147,6 +1252,11 @@ static int download_delta(dynoba_solver* h, double* delta) {
   for (int64_t i = 0; i < npt; i++) for (int c = 0; c < 3; c++) dp[3*i + c] = hp[(size_t)c*h->cur.nl_stride + h->pt_new[i]];
   double* df = dp + 3*npt;
   for (int64_t i = 0; i < nfl; i++) for (int c = 0; c < 2; c++) df[2*i + c] = hf[(size_t)c*h->cur.nf_stride + h->fl_new[i]];
+  double* dn = df + 2*nfl;          // velocities (3), then biases (6)
+  for (int64_t i = np; i < (int64_t)h->pos.size(); i++) {
+    const int d = i < np + (int64_t)h->vel.size()/3 ? 3 : 6;
+    for (int c = 0; c < d; c++) *dn++ = hr[6*(size_t)h->pos[i] + c];
+  }
   return DYNOBA_OK;
 }
 
@@ -1165,17 +1275,23 @@ int dynoba_solve(dynoba_handle h, double lambda, double* delta) {
 int dynoba_retract(dynoba_handle h, const double* delta) {
   int rc = check_ready(h, false); if (rc) return rc;
   ARG(delta, "null delta");
-  const DevBand& B = h->band; const int64_t np = B.n/6, npt = h->cur.nl, nfl = h->cur.nf;
+  const DevBand& B = h->band; const int64_t np = (int64_t)h->pose.size()/12, npt = h->cur.nl, nfl = h->cur.nf;
   std::vector<double> hr(B.n_pad, 0.0), hp((size_t)3*h->cur.nl_stride, 0.0), hf((size_t)2*h->cur.nf_stride, 0.0);
   for (int64_t i = 0; i < np; i++) for (int c = 0; c < 6; c++) hr[6*(size_t)h->pos[i] + c] = delta[6*i + c];
   const double* dp = delta + 6*np;
   for (int64_t i = 0; i < npt; i++) for (int c = 0; c < 3; c++) hp[(size_t)c*h->cur.nl_stride + h->pt_new[i]] = dp[3*i + c];
   const double* df = dp + 3*npt;
   for (int64_t i = 0; i < nfl; i++) for (int c = 0; c < 2; c++) hf[(size_t)c*h->cur.nf_stride + h->fl_new[i]] = df[2*i + c];
+  const double* dn = df + 2*nfl;    // velocities (3), then biases (6)
+  for (int64_t i = np; i < (int64_t)h->pos.size(); i++) {
+    const int d = i < np + (int64_t)h->vel.size()/3 ? 3 : 6;
+    for (int c = 0; c < d; c++) hr[6*(size_t)h->pos[i] + c] = *dn++;
+  }
   CK(cudaMemcpyAsync(B.dp, hr.data(), hr.size()*8, cudaMemcpyHostToDevice, h->stream));
   if (npt) CK(cudaMemcpyAsync(h->dl_point, hp.data(), hp.size()*8, cudaMemcpyHostToDevice, h->stream));
   if (nfl) CK(cudaMemcpyAsync(h->dl_flow, hf.data(), hf.size()*8, cudaMemcpyHostToDevice, h->stream));
   h->launches += launch_retract(h->cur, h->cand, h->band, h->dl_point, h->dl_flow, h->stream);
+  h->launches += launch_nav_retract(h->cur, h->cand, h->band, h->d_nav, h->n_nav, h->stream);
   CK(cudaStreamSynchronize(h->stream));
   std::swap(h->cur, h->cand);
   h->linearized = false;
@@ -1189,6 +1305,7 @@ int dynoba_retract(dynoba_handle h, const double* delta) {
 int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_idx, double* G, double* g) {
   int rc = check_ready(h, true); if (rc) return rc;
   ARG(n_keep > 0 && keep_pose_idx && G && g, "bad arguments");
+  if (has_nav(h)) { h->err = "dynoba_marginal is not available with velocity / bias variables"; return DYNOBA_ERR_UNSUPPORTED; }
   const int64_t np = h->cur.np;
   ARG(n_keep <= np, "more variables than there are");
   if (h->world > 1) { h->err = "dynoba_marginal is a single-GPU entry point"; return DYNOBA_ERR_UNSUPPORTED; }
@@ -1264,11 +1381,13 @@ int dynoba_get_variables(dynoba_handle h, int kind, int64_t n, double* out) {
   int rc = check_ready(h, false); if (rc) return rc;
   ARG(out, "null out");
   const DevVars& V = h->cur;
-  if (kind == DYNOBA_POSE6) {
-    ARG(n == V.np, "size mismatch");
+  if (kind == DYNOBA_POSE6 || kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6) {
+    const int64_t np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3, w = kind_width(kind);
+    ARG(n == (int64_t)var_store(h, kind)->size()/w, "size mismatch");
+    const int64_t base = kind == DYNOBA_POSE6 ? 0 : (kind == DYNOBA_VEL3 ? np : np + nv);
     std::vector<double> soa((size_t)12*V.np_stride);
     CK(cudaMemcpy(soa.data(), V.pose, soa.size()*8, cudaMemcpyDeviceToHost));
-    for (int64_t i = 0; i < n; i++) for (int k = 0; k < 12; k++) out[i*12 + k] = soa[(size_t)k*V.np_stride + h->pos[i]];
+    for (int64_t i = 0; i < n; i++) for (int k = 0; k < w; k++) out[i*w + k] = soa[(size_t)k*V.np_stride + h->pos[base + i]];
   } else if (kind == DYNOBA_POINT3) {
     ARG(n == V.nl, "size mismatch");
     std::vector<double> soa((size_t)3*V.nl_stride);
@@ -1311,6 +1430,7 @@ int dynoba_optimize(dynoba_handle h, const dynoba_lm_params* prm, dynoba_lm_stat
         tick(3); rc = solve_step(h, lambda); if (rc) return rc;
         tick(4);
         h->launches += launch_retract(h->cur, h->cand, h->band, h->dl_point, h->dl_flow, h->stream);
+        h->launches += launch_nav_retract(h->cur, h->cand, h->band, h->d_nav, h->n_nav, h->stream);
         eval_error(h, h->cand, 2);
         tick(5);
         rc = read_scalars(h, sc, true); if (rc) return rc;

@@ -10,15 +10,22 @@ namespace dynoba {
 enum : int {
   F_PRIOR6 = 0, F_BETWEEN6 = 1, F_POSE2POINT3 = 2, F_STEREO3 = 3, F_TERNARY3 = 4, F_HYBRID3 = 5,
   F_HYBRID_STEREO3 = 6, F_MOTIONPOSE3 = 7, F_SMOOTH_HYBRID6 = 8, F_SMOOTH_POSE6 = 9, F_FLOWPROJ2 = 10,
-  F_NUM_TYPES = 11
+  F_PRIOR_VEL3 = 11, F_PRIOR_BIAS6 = 12, F_COMBINED_IMU15 = 13,
+  F_NUM_TYPES = 14
 };
-enum : int { VC_POSE = 0, VC_POINT = 1, VC_FLOW = 2 };
+// VC_VEL / VC_BIAS: the navigation variables of the visual-inertial graphs.  Like poses they live in the reduced system,
+// each in a 6-wide block (a velocity's last three scalars are inert), and are stored in the pose SoA at their position.
+enum : int { VC_POSE = 0, VC_POINT = 1, VC_FLOW = 2, VC_VEL = 3, VC_BIAS = 4 };
+__host__ __device__ constexpr bool is_poselike(int c) { return c == VC_POSE || c == VC_VEL || c == VC_BIAS; }
+__host__ __device__ constexpr bool is_nav_type(int t) { return t == F_PRIOR_VEL3 || t == F_PRIOR_BIAS6 || t == F_COMBINED_IMU15; }
+constexpr int IMU_MEAS = 70;       // meas record of COMBINED_IMU15 (include/dynoba.h)
+constexpr int IMU_SQRT_INFO = 225; // its 15 x 15 square-root information, row-major
 
 // static type tables (host + device constexpr)
 struct TypeInfo {
   int arity, dim, meas, jcols, npose, nlmk, ldim;
-  int cls[4];      // variable class per key slot
-  int coloff[4];   // first Jacobian column of the slot
+  int cls[6];      // variable class per key slot
+  int coloff[6];   // first Jacobian column of the slot
   bool needs_aux;
 };
 __host__ __device__ constexpr TypeInfo type_info(int t) {
@@ -34,10 +41,13 @@ __host__ __device__ constexpr TypeInfo type_info(int t) {
     case F_SMOOTH_HYBRID6: return { 3, 6, 0, 18, 3, 0, 0, { VC_POSE, VC_POSE, VC_POSE, -1 }, { 0, 6, 12, 0 }, true };
     case F_SMOOTH_POSE6:   return { 3, 6, 0, 18, 3, 0, 0, { VC_POSE, VC_POSE, VC_POSE, -1 }, { 0, 6, 12, 0 }, false };
     case F_FLOWPROJ2:      return { 2, 2, 15, 8, 1, 1, 2, { VC_FLOW, VC_POSE, -1, -1 }, { 0, 2, 0, 0 }, false };
+    case F_PRIOR_VEL3:     return { 1, 3, 3, 3, 0, 0, 0, { VC_VEL, -1, -1, -1, -1, -1 }, { 0, 0, 0, 0, 0, 0 }, false };
+    case F_PRIOR_BIAS6:    return { 1, 6, 6, 6, 0, 0, 0, { VC_BIAS, -1, -1, -1, -1, -1 }, { 0, 0, 0, 0, 0, 0 }, false };
+    case F_COMBINED_IMU15: return { 6, 15, IMU_MEAS, 30, 2, 0, 0, { VC_POSE, VC_VEL, VC_POSE, VC_VEL, VC_BIAS, VC_BIAS }, { 0, 6, 9, 15, 18, 24 }, false };
     default:               return { 0, 0, 0, 0, 0, 0, 0, { -1, -1, -1, -1 }, { 0, 0, 0, 0 }, false };
   }
 }
-__host__ __device__ constexpr int class_dim(int c) { return c == VC_POSE ? 6 : (c == VC_POINT ? 3 : 2); }
+__host__ __device__ constexpr int class_dim(int c) { return c == VC_POSE || c == VC_BIAS ? 6 : (c == VC_POINT || c == VC_VEL ? 3 : 2); }
 
 // Variables of one factor, gathered into registers.  Pose slots fill pose[] in key order, point/flow
 // slots fill pt[] in key order (a flow uses pt[.][0..1]).

@@ -283,6 +283,15 @@ int launch_pose_delta_norm(const DevBand& B, double lambda, double* partials, cu
 int pose_norm_grid(int n);
 int launch_retract(const DevVars& cur, const DevVars& cand, const DevBand& B, const double* dl_point,
                    const double* dl_flow, cudaStream_t s);
+// ---- navigation variables and visual-inertial factors (kernels_imu.cu).  nav[i] = (solver position, dimension) of every
+// velocity (3) and bias (6).
+int nav_grid(int type, int n);      // partial sums a linearize / error launch of a navigation factor block writes
+int launch_nav_linearize(const DevBlock& blk, const DevVars& v, double* partials, cudaStream_t s);
+int launch_nav_error(const DevBlock& blk, const DevVars& v, double* partials, double* per_factor, cudaStream_t s);
+int launch_nav_factors(const DevBlock& blk, const DevBand& B, cudaStream_t s);
+int launch_nav_model(const DevBlock& blk, const DevBand& B, double* partials, cudaStream_t s);
+int launch_nav_retract(const DevVars& cur, const DevVars& cand, const DevBand& B, const int2* nav, int n, cudaStream_t s);
+int launch_nav_inert(const DevBand& B, const int2* nav, int n, cudaStream_t s);
 
 // ---- per-frame batch entry points (kernels_star.cu, kernels_ransac.cu).  Per-device state kept between calls (these entry
 // points run every frame): one stream and one grow-only workspace, so a call costs copies + one launch -- no cudaMalloc /

@@ -305,6 +305,7 @@ __global__ void pose_factors_kernel(DevBlock blk, DevBand B, int arity) {
 }
 int launch_pose_factors(const DevBlock& blk, const DevBand& B, cudaStream_t s) {
   if (blk.n == 0) return 0;
+  if (is_nav_type(blk.type)) return launch_nav_factors(blk, B, s);
   pose_factors_kernel<<<(blk.n + 127)/128, 128, 0, s>>>(blk, B, type_info(blk.type).arity);
   return 1;
 }
@@ -430,6 +431,7 @@ __global__ void pose_model_kernel(DevBlock blk, DevBand B, int arity, double* __
 }
 int launch_pose_model(const DevBlock& blk, const DevBand& B, double* partials, cudaStream_t s) {
   if (blk.n == 0) return 0;
+  if (is_nav_type(blk.type)) return launch_nav_model(blk, B, partials, s);
   pose_model_kernel<<<(blk.n + 127)/128, 128, 0, s>>>(blk, B, type_info(blk.type).arity, partials);
   return 1;
 }

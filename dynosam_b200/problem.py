@@ -15,19 +15,21 @@ import numpy as np
 
 # factor type ids == include/dynoba.h enum dynoba_factor_type
 PRIOR6, BETWEEN6, POSE2POINT3, STEREO3, TERNARY3, HYBRID3, HYBRID_STEREO3, MOTIONPOSE3, \
-    SMOOTH_HYBRID6, SMOOTH_POSE6, FLOWPROJ2 = range(11)
+    SMOOTH_HYBRID6, SMOOTH_POSE6, FLOWPROJ2, PRIOR_VEL3, PRIOR_BIAS6, COMBINED_IMU15 = range(14)
 TYPE_NAMES = ["PRIOR6", "BETWEEN6", "POSE2POINT3", "STEREO3", "TERNARY3", "HYBRID3", "HYBRID_STEREO3",
-              "MOTIONPOSE3", "SMOOTH_HYBRID6", "SMOOTH_POSE6", "FLOWPROJ2"]
-ARITY = [1, 2, 2, 2, 3, 3, 3, 4, 3, 3, 2]
-DIM = [6, 6, 3, 3, 3, 3, 3, 3, 6, 6, 2]
-MEAS_DIM = [12, 12, 3, 3, 0, 3, 3, 0, 0, 0, 15]
-# variable class per key slot: 0 pose(6), 1 point(3), 2 flow(2)
+              "MOTIONPOSE3", "SMOOTH_HYBRID6", "SMOOTH_POSE6", "FLOWPROJ2", "PRIOR_VEL3", "PRIOR_BIAS6", "COMBINED_IMU15"]
+ARITY = [1, 2, 2, 2, 3, 3, 3, 4, 3, 3, 2, 1, 1, 6]
+DIM = [6, 6, 3, 3, 3, 3, 3, 3, 6, 6, 2, 3, 6, 15]
+MEAS_DIM = [12, 12, 3, 3, 0, 3, 3, 0, 0, 0, 15, 3, 6, 70]
+# variable class per key slot: 0 pose(6), 1 point(3), 2 flow(2), 3 velocity(3), 4 IMU bias(6)
 SLOT_CLASS = [
     [0], [0, 0], [0, 1], [0, 1], [1, 1, 0], [0, 0, 1], [0, 0, 1], [1, 1, 0, 0], [0, 0, 0], [0, 0, 0], [2, 0],
+    [3], [4], [0, 3, 0, 3, 4, 4],
 ]
-CLASS_DIM = [6, 3, 2]
+CLASS_DIM = [6, 3, 2, 3, 6]
 JCOLS = [sum(CLASS_DIM[c] for c in s) for s in SLOT_CLASS]
-NEEDS_AUX = [False, False, False, False, False, True, True, False, True, False, False]
+NEEDS_AUX = [False, False, False, False, False, True, True, False, True, False, False, False, False, False]
+IMU_SQRT_INFO_DIM = 225   # COMBINED_IMU15's sigma: the 15x15 square-root information R, row-major
 
 
 @dataclass
@@ -82,6 +84,12 @@ class Problem:
     # gtsam::LinearContainerFactor(HessianFactor) priors over pose-like variables (sliding-window marginals): dicts with
     # idx int32[n], lin [n,12], G [6n,6n], g [6n], f
     linear_priors: list = field(default_factory=list)
+    # navigation variables of visual-inertial graphs: nav-frame velocities [n_vel, 3], IMU biases [n_bias, 6] (acc | gyro),
+    # and their ordering hints (frame id), as pose_order is for the poses
+    vel: np.ndarray = field(default_factory=lambda: np.zeros((0, 3)))
+    bias: np.ndarray = field(default_factory=lambda: np.zeros((0, 6)))
+    vel_order: Optional[np.ndarray] = None
+    bias_order: Optional[np.ndarray] = None
 
     def __post_init__(self):
         self.pose = np.ascontiguousarray(self.pose, dtype=np.float64).reshape(-1, 12)
@@ -91,6 +99,11 @@ class Problem:
         self.calib = np.ascontiguousarray(self.calib, dtype=np.float64).reshape(6)
         if self.pose_order is not None:
             self.pose_order = np.ascontiguousarray(self.pose_order, dtype=np.int32)
+        self.vel = np.ascontiguousarray(self.vel, dtype=np.float64).reshape(-1, 3)
+        self.bias = np.ascontiguousarray(self.bias, dtype=np.float64).reshape(-1, 6)
+        for k in ("vel_order", "bias_order"):
+            if getattr(self, k) is not None:
+                setattr(self, k, np.ascontiguousarray(getattr(self, k), dtype=np.int32))
 
     @property
     def n_pose(self): return self.pose.shape[0]
@@ -99,11 +112,16 @@ class Problem:
     @property
     def n_flow(self): return self.flow.shape[0]
     @property
+    def n_vel(self): return self.vel.shape[0]
+    @property
+    def n_bias(self): return self.bias.shape[0]
+    @property
     def n_factors(self): return sum(b.n for b in self.blocks)
 
     def copy(self) -> "Problem":
         return Problem(self.pose.copy(), self.point.copy(), self.flow.copy(), self.aux_pose, self.calib, self.blocks,
-                       self.pose_order, self.pose_keys, self.point_keys, dict(self.meta))
+                       self.pose_order, self.pose_keys, self.point_keys, dict(self.meta), vel=self.vel.copy(),
+                       bias=self.bias.copy(), vel_order=self.vel_order, bias_order=self.bias_order)
 
     def jacobian_bytes(self) -> int:
         """Algorithmic bytes of one materialising linearize() (SURVEY.md 8d): every factor record read once,
@@ -113,7 +131,7 @@ class Problem:
             rd = 4*ARITY[b.type] + 8*MEAS_DIM[b.type] + 8*b.sigma_dim + (4 if b.aux_idx is not None else 0)
             wr = 8*(DIM[b.type]*JCOLS[b.type] + DIM[b.type])
             total += b.n*(rd + wr)
-        total += 96*(self.n_pose + self.aux_pose.shape[0]) + 24*self.n_point + 16*self.n_flow
+        total += 96*(self.n_pose + self.aux_pose.shape[0]) + 24*self.n_point + 16*self.n_flow + 24*self.n_vel + 48*self.n_bias
         return total
 
 
@@ -140,6 +158,8 @@ def cantor_depair(z):
 
 
 def camera_pose_key(frame): return symbol_key('X', frame)
+def velocity_key(frame): return symbol_key('V', frame)
+def imu_bias_key(frame): return symbol_key('b', frame)
 def static_landmark_key(tracklet): return symbol_key('l', tracklet)
 def dynamic_landmark_key(frame, tracklet): return symbol_key('m', cantor_pair(tracklet, frame))
 def object_motion_key(obj, frame): return labeled_symbol_key('H', np.asarray(obj, dtype=np.uint64) + np.uint64(ord('0')), frame)

@@ -59,7 +59,9 @@ def _expand(life):
 def make_problem(n_frames=20, n_objects=1, n_static=700, n_dynamic=300, formulation="hybrid", seed=42,
                  sigma_point=0.2, sigma_ternary=0.01, huber_k=1e-4, robust=True, meas_noise=None,
                  init_noise_rot=0.01, init_noise_trans=0.05, object_span=None, max_static_age=15,
-                 max_dynamic_age=20, with_odometry=True) -> Problem:
+                 max_dynamic_age=20, with_odometry=True, imu=False) -> Problem:
+    """imu=True: the camera chain is visual-inertial (synth_imu.add_imu_chain): velocities, biases, their priors and one
+    COMBINED_IMU15 per frame pair replace the odometry factors."""
     assert formulation in ("hybrid", "wcme", "wcpe")
     rng = np.random.default_rng(seed)
     N = int(n_frames)
@@ -192,7 +194,13 @@ def make_problem(n_frames=20, n_objects=1, n_static=700, n_dynamic=300, formulat
 
     # ---------------- camera chain
     blocks.append(FactorBlock(PRIOR6, np.array([[0]]), X_gt[:1], np.full(6, 1e-6)))
-    if with_odometry and N > 1:
+    nav = None
+    if imu:
+        from .synth_imu import add_imu_chain
+        vel0, bias0, imu_blocks, imu_meta = add_imu_chain(X_gt, xi_cam, seed + 7919)
+        blocks.extend(imu_blocks)
+        nav = dict(vel=vel0, bias=bias0, vel_order=np.arange(N, dtype=np.int32), bias_order=np.arange(N, dtype=np.int32))
+    elif with_odometry and N > 1:
         rel = lie.between(X_gt[:-1], X_gt[1:])
         rel = lie.retract(rel, np.concatenate([rng.normal(0, 0.02, (N - 1, 3)), rng.normal(0, 0.01, (N - 1, 3))], 1))
         blocks.append(FactorBlock(BETWEEN6, np.stack([np.arange(N - 1), np.arange(1, N)], 1), rel,
@@ -200,9 +208,11 @@ def make_problem(n_frames=20, n_objects=1, n_static=700, n_dynamic=300, formulat
 
     prob = Problem(np.concatenate(pose_list), np.concatenate(pts_init), aux_pose=aux, calib=KITTI_K, blocks=blocks,
                    pose_order=np.concatenate(order_hint).astype(np.int32),
-                   pose_keys=np.concatenate(pose_keys), point_keys=np.concatenate(pt_keys))
+                   pose_keys=np.concatenate(pose_keys), point_keys=np.concatenate(pt_keys), **(nav or {}))
     prob.meta = dict(n_frames=N, n_objects=J, n_static=ns, n_dynamic=nd, formulation=formulation, seed=seed,
                      gt_camera=X_gt, gt_motion=gt_motion, dyn_obs=dyn_obs)
+    if imu:
+        prob.meta.update(imu_meta)
     return prob
 
 

@@ -37,8 +37,12 @@ typedef enum {
 } dynoba_status;
 
 /* Variable kinds (reference value types: gtsam::Pose3, gtsam::Point3, gtsam::Point2 optical-flow variable
- * of Pose3FlowProjectionFactor, dynosam/include/dynosam/factors/Pose3FlowProjectionFactor.h:45-71). */
-typedef enum { DYNOBA_POSE6 = 0, DYNOBA_POINT3 = 1, DYNOBA_FLOW2 = 2 } dynoba_var_kind;
+ * of Pose3FlowProjectionFactor, dynosam/include/dynosam/factors/Pose3FlowProjectionFactor.h:45-71; the navigation
+ * variables of the visual-inertial graph, VisionImuBackendModule.hpp:114-243: VEL3 = nav-frame velocity V_k
+ * (gtsam::Vector3), BIAS6 = gtsam::imuBias::ConstantBias b_k, vector order accelerometer then gyroscope).  VEL3 and
+ * BIAS6 retract by vector addition.  Like poses they are pose-like variables of the reduced system: each takes a 6-wide
+ * block (a velocity's last three scalars are inert), so a visual-inertial graph's reduced_dim counts 6 per velocity. */
+typedef enum { DYNOBA_POSE6 = 0, DYNOBA_POINT3 = 1, DYNOBA_FLOW2 = 2, DYNOBA_VEL3 = 3, DYNOBA_BIAS6 = 4 } dynoba_var_kind;
 
 /* Factor types.  idx columns are the factor's keys in the reference's constructor order.
  *  type               reference factor (file:line)                                           keys (idx columns)            meas            */
@@ -54,8 +58,22 @@ typedef enum {
   DYNOBA_SMOOTH_HYBRID6 = 8,/* HybridSmoothingFactor       (HybridFormulationFactors.cc:274-322)       H_k-2, H_k-1, H_k    aux L_e           */
   DYNOBA_SMOOTH_POSE6 = 9,  /* LandmarkPoseSmoothingFactor (src/factors/LandmarkPoseSmoothingFactor.cc:37-95) L_k-2, L_k-1, L_k   -            */
   DYNOBA_FLOWPROJ2 = 10,    /* Pose3FlowProjectionFactor   (factors/Pose3FlowProjectionFactor.h:73-133) flow, pose          kp(2),depth,X_prev(12) */
-  DYNOBA_NUM_FACTOR_TYPES = 11
+  DYNOBA_PRIOR_VEL3 = 11,   /* gtsam::PriorFactor<Vector3> (VisionImuBackendModule.hpp:114-166)      vel                  prior (3)         */
+  DYNOBA_PRIOR_BIAS6 = 12,  /* gtsam::PriorFactor<imuBias::ConstantBias> (same)                      bias                 prior (6)         */
+  DYNOBA_COMBINED_IMU15 = 13,/* gtsam::CombinedImuFactor   (VisionImuBackendModule.hpp:168-243)      pose_i, vel_i, pose_j, vel_j, bias_i, bias_j   pim (70) */
+  DYNOBA_NUM_FACTOR_TYPES = 14
 } dynoba_factor_type;
+/* PRIOR_VEL3 / PRIOR_BIAS6: e = x - prior, H = I.
+ * COMBINED_IMU15: CombinedImuFactor::evaluateError of GTSAM 4.2.0 with ManifoldPreintegration and no Coriolis term,
+ * r = [PreintegrationBase::computeErrorAndJacobians (9: rotation, position, velocity), b_i - b_j (6)], 15 rows.
+ * meas[70] = what ManifoldPreintegration holds: deltaRij (9, row-major) | deltaPij (3) | deltaVij (3) | deltaTij (1) |
+ * biasHat (6: acc, gyro) | delRdelBiasOmega (9) | delPdelBiasAcc (9) | delPdelBiasOmega (9) | delVdelBiasAcc (9) |
+ * delVdelBiasOmega (9) (3x3 blocks row-major) | n_gravity (3).  Its noise is the full square-root information of
+ * noiseModel::Gaussian: sigma_dim = 225, sigma = the 15x15 R row-major (noiseModel()->R()), whitening r_w = R r.
+ * sigma_dim = 225 is accepted for this type only; R must be finite with a positive diagonal (else DYNOBA_ERR_BAD_ARG).
+ * robust_k > 0 is refused (DYNOBA_ERR_UNSUPPORTED) for COMBINED_IMU15, PRIOR_VEL3 and PRIOR_BIAS6: the reference never
+ * robustifies them.
+ * Jacobian columns (dynoba_get_linearization): pose_i (6) | vel_i (3) | pose_j (6) | vel_j (3) | bias_i (6) | bias_j (6). */
 
 /* gtsam::LevenbergMarquardtParams (defaults = GTSAM 4.2.0, see dynoba_lm_default_params) */
 typedef struct {
@@ -91,7 +109,8 @@ int dynoba_destroy(dynoba_handle h);
 void dynoba_lm_default_params(dynoba_lm_params* p);
 
 /* ---- problem ingest (gtsam::Values / NonlinearFactorGraph equivalents) */
-/* kind POSE6: data[n][12] = R row-major (9) | t (3);  POINT3: data[n][3];  FLOW2: data[n][2].
+/* kind POSE6: data[n][12] = R row-major (9) | t (3);  POINT3: data[n][3];  FLOW2: data[n][2];  VEL3: data[n][3];
+ * BIAS6: data[n][6].
  * keys (optional, may be NULL): opaque gtsam::Key values, round-tripped by dynoba_get_keys. */
 int dynoba_set_variables(dynoba_handle h, int kind, int64_t n, const uint64_t* keys, const double* data);
 /* Fixed poses referenced through aux_idx (HybridMotionFactor's L_e): data[n][12]. */
@@ -126,6 +145,12 @@ int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_id
 /* Optional elimination-order hint for pose-like variables (e.g. the frame id encoded in the key):
  * variables are ordered by (rank, index).  Without it the given order is used. */
 int dynoba_set_pose_order(dynoba_handle h, int64_t n, const int32_t* rank);
+/* The same hint for the velocities / biases (kind DYNOBA_VEL3 or DYNOBA_BIAS6).  The pose-like variables are ordered by
+ * (rank, kind: pose < velocity < bias, index); a kind without a hint ranks by index.  Passing the frame id as the rank of
+ * X_k, V_k and b_k puts them next to each other, which keeps the reduced system banded.
+ * Velocity / bias variables cannot be combined with dynoba_add_linear_prior, dynoba_marginal, dynoba_set_shard (world > 1)
+ * or dynoba_set_reduce: those return DYNOBA_ERR_UNSUPPORTED. */
+int dynoba_set_variable_order(dynoba_handle h, int kind, int64_t n, const int32_t* rank);
 /* Multi-GPU: rank/world of the landmark shard held by this handle and the all-reduce used for the reduced
  * system and the scalar sums.  min_bandwidth forces a common band layout on all ranks (0 = local). */
 int dynoba_set_shard(dynoba_handle h, int rank, int world, dynoba_allreduce_fn fn, void* ctx, int min_bandwidth);
@@ -178,9 +203,10 @@ int dynoba_get_linearization(dynoba_handle h, int block_index, double* A, double
 /* Per-factor nonlinear error of one block (0.5|r_w|^2 or Huber rho). */
 int dynoba_get_factor_errors(dynoba_handle h, int block_index, double* err);
 /* One damped solve (J^T J + lambda I) delta = J^T b through Schur + band Cholesky at the current
- * linearization; delta laid out [poses(6) in caller order | points(3) | flows(2)]. */
+ * linearization; delta laid out [poses(6) in caller order | points(3) | flows(2) | velocities(3) | biases(6)]. */
 int dynoba_solve(dynoba_handle h, double lambda, double* delta);
-/* Dense copy of the reduced camera/motion system S (dim x dim, row-major, caller pose order) and g_S. */
+/* Dense copy of the reduced camera/motion system S (dim x dim, row-major) and g_S over [poses (6) | velocities (3) |
+ * biases (6)] in caller order: dim = 6 n_pose + 3 n_vel + 6 n_bias. */
 int dynoba_get_reduced_system(dynoba_handle h, double lambda, double* S, double* g);
 /* values.retract(delta), same layout as dynoba_solve */
 int dynoba_retract(dynoba_handle h, const double* delta);

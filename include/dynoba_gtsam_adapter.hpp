@@ -21,6 +21,8 @@
 #include <gtsam/inference/LabeledSymbol.h>
 #include <gtsam/inference/Symbol.h>
 #include <gtsam/linear/NoiseModel.h>
+#include <gtsam/navigation/CombinedImuFactor.h>
+#include <gtsam/navigation/ImuBias.h>
 #include <gtsam/linear/linearExceptions.h>
 #include <gtsam/nonlinear/LevenbergMarquardtOptimizer.h>
 #include <gtsam/nonlinear/NonlinearFactorGraph.h>
@@ -105,12 +107,24 @@ class LevenbergMarquardtOptimizer {
     if (c == 'H' || c == 'L') return static_cast<int32_t>(gtsam::LabeledSymbol(k).index());
     return static_cast<int32_t>(gtsam::Symbol(k).index());
   }
+  // VisionImuBackendModule.hpp:114-243: velocities are gtsam::Vector3 under the Symbol character 'V', biases
+  // imuBias::ConstantBias under 'b'.  In GTSAM 4.2 Vector3 and Point3 are the same type, so the key character -- not the
+  // value type -- tells a velocity from a landmark.
+  static bool isVelocityKey(gtsam::Key k) { return gtsam::Symbol(k).chr() == 'V'; }
   void ingestValues(const gtsam::Values& v) {
-    std::vector<double> poses, points, flows; std::vector<uint64_t> pk, qk, fk; std::vector<int32_t> order;
+    std::vector<double> poses, points, flows, vels, biases; std::vector<uint64_t> pk, qk, fk, vk, bk;
+    std::vector<int32_t> order, vorder, border;
     for (const auto kv : v) {   // Values iterates in key order: X.., H(label, frame).., l.., m..
       if (auto* p = dynamic_cast<const gtsam::GenericValue<gtsam::Pose3>*>(&kv.value)) {
         pose_index_[kv.key] = static_cast<int32_t>(pk.size()); pk.push_back(kv.key); packPose(p->value(), poses);
         order.push_back(frameOfKey(kv.key));
+      } else if (auto* b = dynamic_cast<const gtsam::GenericValue<gtsam::imuBias::ConstantBias>*>(&kv.value)) {
+        bias_index_[kv.key] = static_cast<int32_t>(bk.size()); bk.push_back(kv.key); border.push_back(frameOfKey(kv.key));
+        for (int i = 0; i < 3; i++) biases.push_back(b->value().accelerometer()(i));
+        for (int i = 0; i < 3; i++) biases.push_back(b->value().gyroscope()(i));
+      } else if (auto* q = dynamic_cast<const gtsam::GenericValue<gtsam::Point3>*>(&kv.value); q && isVelocityKey(kv.key)) {
+        vel_index_[kv.key] = static_cast<int32_t>(vk.size()); vk.push_back(kv.key); vorder.push_back(frameOfKey(kv.key));
+        for (int i = 0; i < 3; i++) vels.push_back(q->value()(i));
       } else if (auto* q = dynamic_cast<const gtsam::GenericValue<gtsam::Point3>*>(&kv.value)) {
         point_index_[kv.key] = static_cast<int32_t>(qk.size()); qk.push_back(kv.key);
         for (int i = 0; i < 3; i++) points.push_back(q->value()(i));
@@ -121,11 +135,30 @@ class LevenbergMarquardtOptimizer {
         throw std::runtime_error("libdynoba adapter: unsupported value type");
       }
     }
-    pose_keys_ = pk; point_keys_ = qk; flow_keys_ = fk;
+    pose_keys_ = pk; point_keys_ = qk; flow_keys_ = fk; vel_keys_ = vk; bias_keys_ = bk;
     check(dynoba_set_variables(h_.h, DYNOBA_POSE6, pk.size(), pk.data(), poses.data()));
     check(dynoba_set_variables(h_.h, DYNOBA_POINT3, qk.size(), qk.data(), points.data()));
     if (!fk.empty()) check(dynoba_set_variables(h_.h, DYNOBA_FLOW2, fk.size(), fk.data(), flows.data()));
     check(dynoba_set_pose_order(h_.h, order.size(), order.data()));
+    if (!vk.empty()) { check(dynoba_set_variables(h_.h, DYNOBA_VEL3, vk.size(), vk.data(), vels.data()));
+                       check(dynoba_set_variable_order(h_.h, DYNOBA_VEL3, vorder.size(), vorder.data())); }
+    if (!bk.empty()) { check(dynoba_set_variables(h_.h, DYNOBA_BIAS6, bk.size(), bk.data(), biases.data()));
+                       check(dynoba_set_variable_order(h_.h, DYNOBA_BIAS6, border.size(), border.data())); }
+  }
+  // PreintegratedCombinedMeasurements -> the 70-double record of DYNOBA_COMBINED_IMU15 (include/dynoba.h)
+  static void packPim(const gtsam::PreintegratedCombinedMeasurements& m, std::vector<double>& out) {
+    if (m.p().omegaCoriolis) throw std::runtime_error("libdynoba adapter: CombinedImuFactor with a Coriolis rate is not on the accelerated path");
+    const gtsam::Matrix3 R = m.deltaRij().matrix();
+    for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) out.push_back(R(i, j));
+    const gtsam::Vector3 dp = m.deltaPij(), dv = m.deltaVij();
+    for (int i = 0; i < 3; i++) out.push_back(dp(i));
+    for (int i = 0; i < 3; i++) out.push_back(dv(i));
+    out.push_back(m.deltaTij());
+    for (int i = 0; i < 3; i++) out.push_back(m.biasHat().accelerometer()(i));
+    for (int i = 0; i < 3; i++) out.push_back(m.biasHat().gyroscope()(i));
+    for (const gtsam::Matrix3* M : { &m.delRdelBiasOmega(), &m.delPdelBiasAcc(), &m.delPdelBiasOmega(), &m.delVdelBiasAcc(), &m.delVdelBiasOmega() })
+      for (int i = 0; i < 3; i++) for (int j = 0; j < 3; j++) out.push_back((*M)(i, j));
+    for (int i = 0; i < 3; i++) out.push_back(m.p().n_gravity(i));
   }
   struct Block { std::vector<int32_t> idx, aux; std::vector<double> meas, sigma; int sigma_dim = 0; double k = 0; };
   // noise: Isotropic / Diagonal, optionally wrapped in Robust(Huber) (BackendDefinitions.cc:124-196)
@@ -147,6 +180,8 @@ class LevenbergMarquardtOptimizer {
     auto Q = [&](gtsam::Key k) { return point_index_.at(k); };
     auto blk = [&](int type, double k) -> Block& { long long bits; std::memcpy(&bits, &k, 8); return blocks[{type, bits}]; };
     auto F = [&](gtsam::Key k) { return flow_index_.at(k); };
+    auto V = [&](gtsam::Key k) { return vel_index_.at(k); };
+    auto B = [&](gtsam::Key k) { return bias_index_.at(k); };
     // one calibration per solver (Cal3_S2Stereo: fx, fy, skew, u0, v0, baseline): every factor must carry the same one
     bool have_calib = false; double calib[6] = {0, 0, 0, 0, 0, 0};
     auto useCalib = [&](double fx, double fy, double s, double u0, double v0, double b) {
@@ -161,7 +196,29 @@ class LevenbergMarquardtOptimizer {
       auto nm = boost::dynamic_pointer_cast<gtsam::NoiseModelFactor>(f);
       if (!nm) throw std::runtime_error("libdynoba adapter: factor without a noise model");
       std::vector<double> sig; double hk;
-      if (auto x = boost::dynamic_pointer_cast<gtsam::PoseToPointFactor<gtsam::Pose3, gtsam::Point3>>(f)) {
+      if (auto x = boost::dynamic_pointer_cast<gtsam::CombinedImuFactor>(f)) {
+        // full square-root information of noiseModel::Gaussian (never robustified by the reference)
+        auto gn = boost::dynamic_pointer_cast<gtsam::noiseModel::Gaussian>(nm->noiseModel());
+        if (!gn) throw std::runtime_error("libdynoba adapter: CombinedImuFactor needs a Gaussian noise model");
+        const gtsam::Matrix R = gn->R();
+        if (R.rows() != 15 || R.cols() != 15) throw std::runtime_error("libdynoba adapter: CombinedImuFactor noise is not 15x15");
+        Block& b = blk(DYNOBA_COMBINED_IMU15, 0.0);
+        b.idx.insert(b.idx.end(), { P(x->key1()), V(x->key2()), P(x->key3()), V(x->key4()), B(x->key5()), B(x->key6()) });
+        packPim(x->preintegratedMeasurements(), b.meas);
+        for (int i = 0; i < 15; i++) for (int j = 0; j < 15; j++) b.sigma.push_back(R(i, j));
+        b.sigma_dim = 225;
+      } else if (auto x = boost::dynamic_pointer_cast<gtsam::PriorFactor<gtsam::imuBias::ConstantBias>>(f)) {
+        noiseOf(nm->noiseModel(), 6, sig, hk); Block& b = blk(DYNOBA_PRIOR_BIAS6, hk);
+        b.idx.push_back(B(x->key()));
+        for (int i = 0; i < 3; i++) b.meas.push_back(x->prior().accelerometer()(i));
+        for (int i = 0; i < 3; i++) b.meas.push_back(x->prior().gyroscope()(i));
+        b.sigma.insert(b.sigma.end(), sig.begin(), sig.end()); b.sigma_dim = 6; b.k = hk;
+      } else if (auto x = boost::dynamic_pointer_cast<gtsam::PriorFactor<gtsam::Vector3>>(f); x && isVelocityKey(x->key())) {
+        noiseOf(nm->noiseModel(), 3, sig, hk); Block& b = blk(DYNOBA_PRIOR_VEL3, hk);
+        b.idx.push_back(V(x->key()));
+        for (int i = 0; i < 3; i++) b.meas.push_back(x->prior()(i));
+        b.sigma.insert(b.sigma.end(), sig.begin(), sig.end()); b.sigma_dim = 3; b.k = hk;
+      } else if (auto x = boost::dynamic_pointer_cast<gtsam::PoseToPointFactor<gtsam::Pose3, gtsam::Point3>>(f)) {
         noiseOf(nm->noiseModel(), 3, sig, hk); Block& b = blk(DYNOBA_POSE2POINT3, hk);
         b.idx.insert(b.idx.end(), { P(x->key1()), Q(x->key2()) });
         for (int i = 0; i < 3; i++) b.meas.push_back(x->measured()(i));
@@ -230,7 +287,7 @@ class LevenbergMarquardtOptimizer {
     if (!aux_poses.empty()) check(dynoba_set_aux_poses(h_.h, aux_poses.size()/12, aux_poses.data()));
     for (auto& kv : blocks) {
       Block& b = kv.second; const int type = kv.first.first;
-      const int arity = type == DYNOBA_PRIOR6 ? 1 : (type == DYNOBA_BETWEEN6 || type == DYNOBA_POSE2POINT3 || type == DYNOBA_STEREO3 || type == DYNOBA_FLOWPROJ2 ? 2 : (type == DYNOBA_MOTIONPOSE3 ? 4 : 3));
+      const int arity = type == DYNOBA_COMBINED_IMU15 ? 6 : (type == DYNOBA_PRIOR6 || type == DYNOBA_PRIOR_VEL3 || type == DYNOBA_PRIOR_BIAS6) ? 1 : (type == DYNOBA_BETWEEN6 || type == DYNOBA_POSE2POINT3 || type == DYNOBA_STEREO3 || type == DYNOBA_FLOWPROJ2 ? 2 : (type == DYNOBA_MOTIONPOSE3 ? 4 : 3));
       const int64_t n = static_cast<int64_t>(b.idx.size()/arity);
       check(dynoba_add_factors(h_.h, type, n, b.idx.data(), b.meas.empty() ? nullptr : b.meas.data(), b.sigma.data(),
                                b.sigma_dim, n, b.k, b.aux.empty() ? nullptr : b.aux.data()));
@@ -251,6 +308,17 @@ class LevenbergMarquardtOptimizer {
       check(dynoba_get_variables(h_.h, DYNOBA_FLOW2, flow_keys_.size(), flows.data()));
       for (size_t i = 0; i < flow_keys_.size(); i++) values_.update(flow_keys_[i], gtsam::Point2(flows[i*2], flows[i*2 + 1]));
     }
+    if (!vel_keys_.empty()) {
+      std::vector<double> vels(vel_keys_.size()*3);
+      check(dynoba_get_variables(h_.h, DYNOBA_VEL3, vel_keys_.size(), vels.data()));
+      for (size_t i = 0; i < vel_keys_.size(); i++) values_.update(vel_keys_[i], gtsam::Vector3(vels[i*3], vels[i*3 + 1], vels[i*3 + 2]));
+    }
+    if (!bias_keys_.empty()) {
+      std::vector<double> bs(bias_keys_.size()*6);
+      check(dynoba_get_variables(h_.h, DYNOBA_BIAS6, bias_keys_.size(), bs.data()));
+      for (size_t i = 0; i < bias_keys_.size(); i++)
+        values_.update(bias_keys_[i], gtsam::imuBias::ConstantBias(gtsam::Vector3(bs[i*6], bs[i*6 + 1], bs[i*6 + 2]), gtsam::Vector3(bs[i*6 + 3], bs[i*6 + 4], bs[i*6 + 5])));
+    }
   }
 
   const gtsam::NonlinearFactorGraph& graph_;
@@ -260,8 +328,8 @@ class LevenbergMarquardtOptimizer {
   dynoba_lm_params p_{};
   dynoba_lm_stats stats_{};
   double error_ = 0.0;
-  std::unordered_map<gtsam::Key, int32_t> pose_index_, point_index_, flow_index_;
-  std::vector<uint64_t> pose_keys_, point_keys_, flow_keys_;
+  std::unordered_map<gtsam::Key, int32_t> pose_index_, point_index_, flow_index_, vel_index_, bias_index_;
+  std::vector<uint64_t> pose_keys_, point_keys_, flow_keys_, vel_keys_, bias_keys_;
 };
 
 }  // namespace gpu
