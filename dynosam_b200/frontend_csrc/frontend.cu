@@ -2680,6 +2680,13 @@ static int klt_top_level(const dynofront_ctx* h, int max_level, int win) {
   }
   return levels;
 }
+// klt_kernel reaches level-0 window pixels from -win to W + win - 1 (and H likewise) through one reflect101, which stays inside
+// the image only when both sides are at least win + 1; cv2 would loop its borderInterpolate there, no dataset frame is that
+// small, so such a frame is refused
+static int klt_check_frame(dynofront_ctx* h, int win) {
+  if (h->W < win + 1 || h->H < win + 1) { h->err = "frame smaller than the LK window: width and height must be at least win + 1"; return -1; }
+  return 0;
+}
 // levels 0..top of one direction: I = pyramid `from` with its derivatives (der for pyramid 0, der2 for pyramid 1), J = the other
 static KltLevels klt_levels(const dynofront_ctx* h, int top, int from) {
   KltLevels L; L.nlev = top + 1;
@@ -2703,6 +2710,7 @@ int dynofront_klt_track(dynofront_handle h, const uint8_t* prev_gray, const uint
                         double min_eig, float* ms_device) {
   if (!h || !prev_gray || !cur_gray || n < 0 || !prev_pts || !next_pts || !status) return -1;
   if (win < 3 || win > KLT_MAXWIN || max_level < 0) { h->err = "win must be in [3,31]"; return -1; }
+  if (klt_check_frame(h, win)) return -1;
   cudaSetDevice(h->dev);
   const int levels = klt_top_level(h, max_level, win);
   const size_t cap = feature_cap(n);
@@ -2735,6 +2743,7 @@ int dynofront_klt_track_fb(dynofront_handle h, const uint8_t* prev_gray, const u
   if (resident && !(h->have_pyr && h->have_pyr_cur)) { h->err = "two frames are needed on the device"; return -2; }
   if (P->win < 3 || P->win > KLT_MAXWIN || P->win_back < 3 || P->win_back > KLT_MAXWIN || P->max_level < 0 || P->max_level_back < 0) { h->err = "win must be in [3,31]"; return -1; }
   if (P->check_static && (!prev_age || !keep)) { h->err = "check_static needs prev_age and keep"; return -1; }
+  if (klt_check_frame(h, std::max(P->win, P->win_back))) return -1;
   if (int rc = klt_fb_stages(h, resident, prev_gray, cur_gray, n, prev_pts, next_pts, P, prev_age)) return rc;
   int counts[2] = {0, 0};
   FCK(cudaMemcpyAsync(next_pts, h->k_next, 2*(size_t)n*4, cudaMemcpyDeviceToHost, h->s));
@@ -2971,6 +2980,7 @@ int dynofront_klt_track_points(dynofront_handle h, const uint8_t* prev_gray, con
   if (resident && !(h->have_pyr && h->have_pyr_cur)) { h->err = "two frames are needed on the device"; return -2; }
   if (fb->win < 3 || fb->win > KLT_MAXWIN || fb->win_back < 3 || fb->win_back > KLT_MAXWIN || fb->max_level < 0 || fb->max_level_back < 0) { h->err = "win must be in [3,31]"; return -1; }
   if (fb->check_static && (!prev_age || !keep)) { h->err = "check_static needs prev_age and keep"; return -1; }
+  if (klt_check_frame(h, std::max(fb->win, fb->win_back))) return -1;
   dynofront_homography_params P; if (hom) P = *hom; else dynofront_homography_default_params(&P);
   if (hom_check_params(h, P)) return -1;
   if (int rc = klt_fb_stages(h, resident, prev_gray, cur_gray, n, prev_pts, next_pts, fb, prev_age)) return rc;
@@ -3060,6 +3070,7 @@ __global__ void stereo_match_post_kernel(int n, const float* __restrict__ left, 
 int dynofront_stereo_track(dynofront_handle h, const uint8_t* left_gray, const uint8_t* right_gray, int32_t n, const float* left_pts, float* right_pts,
                            uint8_t* status, double fx, double baseline, double* depth, uint8_t* valid, float* ms_device) {
   if (!h || !left_gray || !right_gray || n < 0 || !left_pts || !right_pts || !status || !depth || !valid) return -1;
+  if (klt_check_frame(h, 21)) return -1;
   cudaSetDevice(h->dev);
   const int win = 21, levels = klt_top_level(h, 5, win);
   const size_t cap = feature_cap(n);
@@ -3102,6 +3113,7 @@ int dynofront_stereo_match(dynofront_handle h, const uint8_t* left_gray, const u
   if (!resident && (!left_gray || !right_gray)) { h->err = "pass both images, or none for the resident frame and right image"; return -1; }
   dynofront_fundamental_params P; if (fund) P = *fund; else dynofront_fundamental_default_params(&P);
   if (fund_check_params(h, P)) return -1;
+  if (klt_check_frame(h, 21)) return -1;
   for (size_t i = 0; i < 2*(size_t)n; i++) if (!std::isfinite(left_pts[i])) { h->err = "non-finite point"; return -1; }
   if (resident && !h->have_pyr_cur) { h->err = "no current frame on the device: call dynofront_next_frame first"; return -2; }
   if (resident && !h->has_right) { h->err = "no right image for the current frame: call dynofront_set_right after dynofront_next_frame"; return -2; }
@@ -3362,6 +3374,7 @@ int dynofront_track_dynamic_klt(dynofront_handle h, const uint8_t* prev_gray, co
   const dynofront_track_params& T = prm->track;
   if (T.min_distance < 0 || T.min_distance > 15) { h->err = "min_distance must be in [0,15]"; return -1; }
   if (prm->win < 3 || prm->win > KLT_MAXWIN || prm->max_level < 0) { h->err = "win must be in [3,31]"; return -1; }
+  if (klt_check_frame(h, prm->win)) return -1;
   const int expiry = T.max_dynamic_feature_age - std::max(3, prm->age_buffer);
   if (expiry <= 0) { h->err = "max_dynamic_feature_age - max(3, age_buffer) must be > 0"; return -1; }
   if (prm->min_tracks < 0 || prm->max_features < 0) { h->err = "min_tracks and max_features must be >= 0"; return -1; }

@@ -117,7 +117,10 @@ int dynofront_propagate_mask(dynofront_handle h, int32_t n, const double* prev_p
                              int32_t min_votes, int32_t* current_mask);
 
 /* Pyramidal Lucas-Kanade, OpenCV semantics (fixed-point bilinear weights, int16 Scharr derivatives).
- * next_pts is in/out when use_initial_flow != 0.  err may be NULL. */
+ * next_pts is in/out when use_initial_flow != 0.  err may be NULL.
+ * Every LK entry point (this one, _klt_track_fb, _klt_track_points, _track_dynamic_klt, _stereo_track, _stereo_match) refuses
+ * with -1, before anything runs, a handle whose width or height is below win + 1 (21 + 1 for the stereo calls): the window is
+ * reflected into the image once, where OpenCV would loop its border interpolation. */
 int dynofront_klt_track(dynofront_handle h, const uint8_t* prev_gray, const uint8_t* cur_gray, int32_t n,
                         const float* prev_pts, float* next_pts, uint8_t* status, float* err, int32_t win,
                         int32_t max_level, int32_t max_count, double epsilon, int32_t use_initial_flow,

@@ -59,6 +59,77 @@ def opencv_float_orders_apply():
                 and "AVX2" in [t.lstrip("*") for t in cv2.getCPUFeaturesLine().split()])
 
 
+def sobel_simd_end(W):
+    """the first column of the Sobel y-derivative row pass that takes OpenCV's scalar tail: (W / 32) * 32"""
+    return (W//32)*32
+
+
+def min_eigen_image(img, simd_end=sobel_simd_end):
+    """cv2.cornerMinEigenVal(img, 3, 3) in the float order DESIGN section 4 and the head of frontend.cu's detection section state,
+    with numpy's correctly rounded float32 / float64 operations (fma(a, b, c) as one rounding of the exact a * b + c, which float64
+    holds exactly for these operands).  simd_end(W) is the column where the y derivative's row pass leaves the FMA chain."""
+    img = np.asarray(img, np.uint8)
+    H, W = img.shape
+    f32, f64 = np.float32, np.float64
+    s = 1.0/(4*3*255.0)
+    f1, f0 = f32(s), f32(2*s)
+
+    def r101(i, n):
+        i = np.abs(i)
+        return np.where(i >= n, 2*n - 2 - i, i)
+
+    def fma(a, b, c):
+        return (f64(a)*f64(b) + f64(c)).astype(f32)
+
+    I = img.astype(f32)
+    x = np.arange(W); xm, xp = r101(x - 1, W), r101(x + 1, W)
+    y = np.arange(H); ym, yp = r101(y - 1, H), r101(y + 1, H)
+    rd = I[:, xp] - I[:, xm]                                    # exact row differences
+    dx = fma(rd[ym] + rd[yp], f1, rd*f0)
+    L, M, R = I[:, xm], I, I[:, xp]
+    simd = (x < simd_end(W))[None, :]
+    rs = np.where(simd, fma(R, f1, fma(M, f0, L*f1)), (f1*L + f0*M) + f1*R)
+    dy = rs[yp] - rs[ym]
+    box = []
+    for U, V in ((dx, dx), (dx, dy), (dy, dy)):
+        P = (U*V).astype(f64)
+        rows = (P[:, xm] + P) + P[:, xp]                        # (c[-1] + c[0]) + c[+1] in double
+        rowat = lambda k: rows[r101(np.array(k), H)]
+        out = np.empty((H, W), f32)
+        rm, r0, rp = rowat(-1), rowat(0), rowat(1)
+        S = (0.0 + rm) + r0
+        for k in range(H):                                      # the running column sum: add the entering row, drop the leaving one
+            s0 = S + rp
+            out[k] = s0.astype(f32); S = s0 - rm
+            rm, r0 = r0, rp
+            rp = rowat(k + 2) if k + 2 <= H else np.zeros(W)
+        box.append(out)
+    a, b, c = box[0]*f32(0.5), box[1], box[2]*f32(0.5)
+    return (a + c) - np.sqrt((a - c)*(a - c) + b*b)
+
+
+def processed(gray, use_clahe=True):
+    """the image detection works on: CLAHE(2.0, 8x8) or the plain frame"""
+    import cv2
+    return cv2.createCLAHE(2.0, (8, 8)).apply(gray) if use_clahe else gray
+
+
+def assert_keypoints(got, ref, proc, starts):
+    """Bit-exact, except for points whose cornerSubPix sampling window left the image during the iterations: there cv2's
+    getRectSubPix takes its clamped-rectangle path, whose float sums the device reproduces up to the last bit of some patch
+    entries, and a position may differ by at most 1e-4 px.  For every such point the iteration is replayed from its start
+    corner with cv2's own patches (subpix_window_clamped), which must show that a window really was clamped.  Returns the
+    number of such points."""
+    assert got.shape == ref.shape, (got.shape, ref.shape)
+    diff = np.flatnonzero(np.any(got != ref, axis=1))
+    for i in diff:
+        assert np.abs(got[i] - ref[i]).max() <= 1e-4, (i, got[i], ref[i])
+        clamped, end = subpix_window_clamped(proc, starts[i])
+        assert clamped, (i, starts[i], ref[i])
+        assert np.abs(np.array(end) - ref[i]).max() <= 1e-3, (i, end, ref[i])       # the replay follows cv2.cornerSubPix
+    return len(diff)
+
+
 def subpix_window_clamped(img, start, win=5, max_iter=40, eps=0.001, margin=1e-3):
     """Replays cv2.cornerSubPix from `start` with cv2.getRectSubPix patches and tells whether any visited (win+1)*2+1
     sampling window left the image, i.e. took getRectSubPix's clamped-rectangle path (within `margin` px of doing so counts,

@@ -12,53 +12,9 @@ import numpy as np
 import pytest
 
 import detection_oracle as DO
-from dynosam_b200.synth_frames import SyntheticStream
+from frame_cases import c4, cur_features, dev_params, texture
 
 W, H = 1242, 375
-
-
-def _c4(k, seed=42):
-    g, m, f = SyntheticStream(n_objects=10, seed=seed).frame(k)
-    return np.ascontiguousarray(g.astype(np.uint8)), np.ascontiguousarray(m.astype(np.int32)), np.ascontiguousarray(f.astype(np.float32))
-
-
-def _texture(h, w, seed):
-    import cv2
-    rng = np.random.default_rng(seed)
-    return np.ascontiguousarray(cv2.GaussianBlur(rng.integers(0, 256, (h, w)).astype(np.uint8), (0, 0), 1.2))
-
-
-def _cur_features(rng, m, n):
-    ys, xs = np.nonzero(m == 0)
-    s = rng.choice(len(ys), n, replace=False)
-    return np.stack([xs[s] + rng.uniform(0, 1, n), ys[s] + rng.uniform(0, 1, n)], 1)
-
-
-def _dev_params(p: DO.Params):
-    from dynosam_b200.frontend import DetectParams
-    return DetectParams(use_clahe=p.use_clahe, use_anms=p.use_anms, use_subpix=p.use_subpix, max_corners=p.max_corners,
-                        quality_level=p.quality_level, min_distance=p.min_distance, max_features=p.max_features,
-                        shrink_row=p.shrink_row, shrink_col=p.shrink_col)
-
-
-def _proc(g, use_clahe=True):
-    import cv2
-    return cv2.createCLAHE(2.0, (8, 8)).apply(g) if use_clahe else g
-
-
-def _assert_keypoints(got, ref, proc, starts):
-    """Bit-exact, except for points whose cornerSubPix sampling window left the image during the iterations: there cv2's
-    getRectSubPix takes its clamped-rectangle path, whose float sums the device reproduces up to the last bit of some patch
-    entries, and a position may differ by at most 1e-4 px.  For every such point the iteration is replayed from its start
-    corner with cv2's own patches (DO.subpix_window_clamped), which must show that a window really was clamped."""
-    assert got.shape == ref.shape, (got.shape, ref.shape)
-    diff = np.flatnonzero(np.any(got != ref, axis=1))
-    for i in diff:
-        assert np.abs(got[i] - ref[i]).max() <= 1e-4, (i, got[i], ref[i])
-        clamped, end = DO.subpix_window_clamped(proc, starts[i])
-        assert clamped, (i, starts[i], ref[i])
-        assert np.abs(np.array(end) - ref[i]).max() <= 1e-3, (i, end, ref[i])       # the replay follows cv2.cornerSubPix
-    return len(diff)
 
 
 needs_opencv_orders = pytest.mark.skipif(not DO.opencv_float_orders_apply(),
@@ -72,16 +28,16 @@ def test_stages_bit_exact(which):
     import cv2
     from dynosam_b200.frontend import FeatureTrackerGPU
     if which == "c4":
-        g, m, f = _c4(3)
+        g, m, f = c4(3)
     else:
-        g = _texture(251, 333, 1); m = np.zeros(g.shape, np.int32); m[50:90, 100:160] = 2; f = np.zeros(g.shape + (2,), np.float32)
+        g = texture(251, 333, 1); m = np.zeros(g.shape, np.int32); m[50:90, 100:160] = 2; f = np.zeros(g.shape + (2,), np.float32)
     rows, cols = g.shape
     rng = np.random.default_rng(1)
-    kp = _cur_features(rng, m, 150)
+    kp = cur_features(rng, m, 150)
     t = FeatureTrackerGPU(cols, rows)
     t.set_frame(f, m, None)
     for p in (DO.Params(), DO.Params(min_distance=8, max_corners=3000)):
-        t.detect_static(g, kp, _dev_params(p), 0)
+        t.detect_static(g, kp, dev_params(p), 0)
         cl, eig, corners = t.detect_stages()
         mask = DO.detection_mask(m, None, kp, p.min_distance)
         ref_cl, ref_eig, ref_pts, _ = DO.stages(g, mask, p)
@@ -95,10 +51,10 @@ def test_stages_bit_exact(which):
 @pytest.mark.parametrize("case", ["first", "n300", "n800", "boundary_shrink", "no_clahe", "no_anms", "no_subpix", "r8"])
 def test_detect_static_bit_exact(case):
     from dynosam_b200.frontend import FeatureTrackerGPU
-    g, m, f = _c4(4)
+    g, m, f = c4(4)
     rng = np.random.default_rng(7)
     n = {"first": 0, "n800": 820}.get(case, 300)
-    kp = _cur_features(rng, m, n)
+    kp = cur_features(rng, m, n)
     p = DO.Params()
     boundary = None
     if case == "boundary_shrink":
@@ -110,10 +66,10 @@ def test_detect_static_bit_exact(case):
     if case == "r8": p.min_distance = 8
     t = FeatureTrackerGPU(W, H)
     t.set_frame(f, m, boundary)
-    got, gid, gnext, gnc = t.detect_static(g, kp, _dev_params(p), 5000)
+    got, gid, gnext, gnc = t.detect_static(g, kp, dev_params(p), 5000)
     ref, rid, rnext, rnc, starts = DO.detect(g, m, boundary, kp, p, 5000)
     assert gnc == rnc
-    off = _assert_keypoints(got, ref, _proc(g, p.use_clahe), starts) if p.use_subpix else _assert_keypoints(got, ref, None, None)
+    off = DO.assert_keypoints(got, ref, DO.processed(g, p.use_clahe), starts) if p.use_subpix else DO.assert_keypoints(got, ref, None, None)
     assert np.array_equal(gid, rid) and gnext == rnext
     if case == "n800":
         assert len(got) == 0 and gnc > 0                           # K = 0: no new features
@@ -130,14 +86,14 @@ def test_detect_streaming_equals_call_by_call():
     track_dynamic has drawn into its working copy."""
     from dynosam_b200.frontend import DetectParams, FeatureTrackerGPU, TrackParams
     rng = np.random.default_rng(11)
-    frames = [_c4(k, seed=9) for k in range(3)]
+    frames = [c4(k, seed=9) for k in range(3)]
     boundary = np.full((H, W), 255, np.uint8); boundary[:40, :] = 0
     a = FeatureTrackerGPU(W, H); b = FeatureTrackerGPU(W, H)
     prm = DetectParams()
     a.next_frame(frames[0][0], frames[0][2], frames[0][1], boundary)
     for k in (1, 2):
         g, m, f = frames[k]
-        kp = _cur_features(rng, m, 250)
+        kp = cur_features(rng, m, 250)
         a.next_frame(g, f, m, boundary)
         ys, xs = np.nonzero(m > 0); s = rng.choice(len(ys), 300, replace=False)
         dyn = np.stack([xs[s] + 0.5, ys[s] + 0.5], 1)
@@ -147,7 +103,7 @@ def test_detect_streaming_equals_call_by_call():
         rb = b.detect_static(g, kp, prm, 100)
         assert np.array_equal(ra[0], rb[0]) and np.array_equal(ra[1], rb[1]) and ra[2:] == rb[2:]
         ref = DO.detect(g, m, boundary, kp, DO.Params(), 100)
-        _assert_keypoints(ra[0], ref[0], _proc(g), ref[4])
+        DO.assert_keypoints(ra[0], ref[0], DO.processed(g), ref[4])
         assert np.array_equal(ra[1], ref[1]) and ra[2] == ref[2]
 
 
@@ -173,21 +129,21 @@ def test_detect_corners_at_image_corners(use_anms):
     g = _corner_image(h, w, 3); m = np.zeros((h, w), np.int32); f = np.zeros((h, w, 2), np.float32)
     p = DO.Params(use_anms=use_anms, min_distance=5, max_corners=3000, max_features=800)
     t = FeatureTrackerGPU(w, h); t.set_frame(f, m, None)
-    got, gid, gnext, gnc = t.detect_static(g, np.zeros((0, 2)), _dev_params(p), 0)
+    got, gid, gnext, gnc = t.detect_static(g, np.zeros((0, 2)), dev_params(p), 0)
     ref, rid, rnext, rnc, starts = DO.detect(g, m, None, np.zeros((0, 2)), p, 0)
     assert gnc == rnc and np.array_equal(gid, rid) and gnext == rnext
     near = lambda q, dx, dy: ((np.abs(q[:, 0] - dx) <= 6) & (np.abs(q[:, 1] - dy) <= 6)).any()
     if not use_anms:                                             # every image corner has a refined point next to it
         for cx, cy in ((0, 0), (w - 1, 0), (0, h - 1), (w - 1, h - 1)):
             assert near(starts, cx, cy), (cx, cy)
-    off = _assert_keypoints(got, ref, _proc(g), starts)
+    off = DO.assert_keypoints(got, ref, DO.processed(g), starts)
     print("corners", use_anms, len(got), "features,", off, "within 1e-4 px with a clamped window")
 
 
 @pytest.mark.gpu
 def test_detect_capacity():
     from dynosam_b200.frontend import DetectParams, FeatureTrackerGPU, _p
-    g, m, f = _c4(5)
+    g, m, f = c4(5)
     t = FeatureTrackerGPU(W, H); t.set_frame(f, m, None)
     prm = DetectParams()
     full = t.detect_static(g, np.zeros((0, 2)), prm, 10)
@@ -206,7 +162,7 @@ def test_detect_capacity():
 @pytest.mark.gpu
 def test_detect_refusals():
     from dynosam_b200.frontend import DetectParams, FeatureTrackerGPU, FrontendError
-    g, m, f = _c4(2)
+    g, m, f = c4(2)
     t = FeatureTrackerGPU(W, H); t.set_frame(f, m, None)
     for bad in (DetectParams(use_harris=True), DetectParams(block_size=5), DetectParams(min_distance=16)):
         with pytest.raises(FrontendError):
