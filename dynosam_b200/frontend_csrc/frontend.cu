@@ -58,7 +58,7 @@ struct dynofront_ctx {
   // sampling scratch
   DevBuf<int> tile_cnt, obj_tot, d_objs, d_zero, d_idx;
   // propagate scratch
-  DevBuf<int32_t> pmask, cmask; DevBuf<float> pflow; DevBuf<int> pflag;
+  DevBuf<int32_t> pmask, cmask; DevBuf<float> pflow; DevBuf<int> pflag, pm_votes;
   // KLT; der2: Scharr derivatives of the CURRENT image (backward pass)
   std::vector<DevBuf<uint8_t>> pyr[2]; std::vector<DevBuf<short>> der, der2; std::vector<int> lw, lh;
   DevBuf<float> k_prev, k_next, k_err, k_back, k_eig; DevBuf<uint8_t> k_st, k_st2, k_keep; DevBuf<int32_t> k_age; DevBuf<int> k_count;
@@ -219,13 +219,23 @@ __global__ void td_trk_final_kernel(size_t npx, const int* trk_idx, const int32_
   if (p >= npx) return;
   const int t = trk_idx[p];
   const int l = t ? olab[t - 1] : 0;
-  trk[p] = (uint8_t)(l > 255 ? 255 : l);
+  trk[p] = (uint8_t)(l < 0 ? 0 : l > 255 ? 255 : l);       // cv::Scalar(label) drawn into CV_8U saturates
 }
 __global__ void fill_u8_kernel(uint8_t* p, size_t n, uint8_t v) { const size_t i = (size_t)blockIdx.x*blockDim.x + threadIdx.x; if (i < n) p[i] = v; }
 __global__ void fill_i32_kernel(int* p, size_t n, int v) { const size_t i = (size_t)blockIdx.x*blockDim.x + threadIdx.x; if (i < n) p[i] = v; }
 
 // ---------------------------------------------------------------------------------------------------- sampleDynamic scan
 constexpr int ST_TILE = 1024, ST_MAXOBJ = 64;
+// the object list of a per-object entry point: at most ST_MAXOBJ ids, each > 0 and none twice (the reference's callers pass a
+// std::set<ObjectId> of detected objects); checked before anything is launched
+static int check_objects(dynofront_ctx* h, int n, const int32_t* objects) {
+  if (n > ST_MAXOBJ) { h->err = "at most 64 objects"; return -1; }
+  for (int o = 0; o < n; o++) {
+    if (objects[o] <= 0) { h->err = "object ids must be > 0 (0 is the background)"; return -1; }
+    for (int q = 0; q < o; q++) if (objects[q] == objects[o]) { h->err = "object ids must be distinct"; return -1; }
+  }
+  return 0;
+}
 __device__ __forceinline__ int sample_slot(size_t p, int W, int H, const uint8_t* det, const int32_t* mask, const float* flow, const int* objs, int nobj,
                                            dynofront_track_params prm, bool* zero) {
   *zero = false;
@@ -477,26 +487,126 @@ __global__ void sd_construct_kernel(const int* __restrict__ off, const int* __re
 }
 
 // ---------------------------------------------------------------------------------------------------- propogateMask
-__global__ void __launch_bounds__(256) pm_vote_kernel(int n, const double* kp, const int32_t* lab, int label, const int32_t* cur, int W, int H,
-                                                     int min_votes, int* flag) {
-  __shared__ int hist[256]; __shared__ int total;
-  hist[threadIdx.x] = 0; if (threadIdx.x == 0) total = 0;
+// The vote of one object is sorted[0] of std::sort(pairs, a.second > b.second) over the (label, count) pairs of a
+// std::map<int, int>, i.e. in ascending label order.  pm_introsort_loop restates libstdc++'s __introsort_loop (<bits/stl_algo.h>:
+// threshold 16, depth limit 2 floor(log2 n), median of three moved to the front, unguarded partition, heap sort at the depth
+// limit).  The final insertion sort that follows it is stable, so sorted[0] is the first pair of largest count after the loop.
+struct PmPair { int l, c; };
+__device__ void pm_adjust_heap(PmPair* a, int hole, int len, PmPair v) {       // __adjust_heap + __push_heap
+  const int top = hole;
+  int child = hole;
+  while (child < (len - 1)/2) {
+    child = 2*(child + 1);
+    if (a[child].c > a[child - 1].c) child--;
+    a[hole] = a[child]; hole = child;
+  }
+  if ((len & 1) == 0 && child == (len - 2)/2) { child = 2*(child + 1); a[hole] = a[child - 1]; hole = child - 1; }
+  int parent = (hole - 1)/2;
+  while (hole > top && a[parent].c > v.c) { a[hole] = a[parent]; hole = parent; parent = (hole - 1)/2; }
+  a[hole] = v;
+}
+__device__ void pm_heap_sort(PmPair* a, int len) {                            // __partial_sort(first, last, last): make_heap, sort_heap
+  for (int parent = (len - 2)/2; len >= 2; parent--) { pm_adjust_heap(a, parent, len, a[parent]); if (parent == 0) break; }
+  for (int last = len - 1; last > 0; last--) { const PmPair v = a[last]; a[last] = a[0]; pm_adjust_heap(a, 0, last, v); }
+}
+__device__ int pm_partition_pivot(PmPair* a, int first, int last) {           // __unguarded_partition_pivot
+  const int x = first + 1, y = first + (last - first)/2, z = last - 1;
+  int m;
+  if (a[x].c > a[y].c) m = a[y].c > a[z].c ? y : a[x].c > a[z].c ? z : x;
+  else m = a[x].c > a[z].c ? x : a[y].c > a[z].c ? z : y;
+  PmPair t = a[first]; a[first] = a[m]; a[m] = t;
+  const int pc = a[first].c;
+  int i = first + 1, j = last;
+  for (;;) {
+    while (a[i].c > pc) i++;
+    j--;
+    while (pc > a[j].c) j--;
+    if (!(i < j)) return i;
+    t = a[i]; a[i] = a[j]; a[j] = t;
+    i++;
+  }
+}
+__device__ void pm_introsort_loop(PmPair* a, int n) {
+  // ranges still to sort; the depths on the stack fall strictly from bottom to top, so it holds at most 2*31 + 1 entries
+  struct Range { int first, last, depth; } st[64];
+  int top = 0;
+  if (n > 1) st[top++] = Range{0, n, 2*(31 - __clz(n))};
+  while (top) {
+    Range r = st[--top];
+    while (r.last - r.first > 16) {
+      if (r.depth == 0) { pm_heap_sort(a + r.first, r.last - r.first); break; }
+      r.depth--;
+      const int cut = pm_partition_pivot(a, r.first, r.last);
+      st[top++] = Range{cut, r.last, r.depth};
+      r.last = cut;
+    }
+  }
+}
+// one CTA: the votes (current-mask labels under the object's predicted key-points, any int32) are counted into (label, count)
+// pairs in ascending label order, labels in [0, 256) in a shared histogram, the others gathered into votes (n ints) and sorted;
+// *flag = 1 when there are >= min_votes votes and sorted[0] is label 0.  pairs holds n pairs.
+constexpr int PM_THREADS = 256, PM_SMEM = 2048;
+__global__ void __launch_bounds__(PM_THREADS) pm_vote_kernel(int n, const double* kp, const int32_t* lab, int label, const int32_t* cur, int W, int H,
+                                                             int min_votes, int* votes, PmPair* pairs, int* flag) {
+  static_assert(PM_THREADS == 256, "one histogram bin per thread");
+  __shared__ int hist[256]; __shared__ int s_v[PM_SMEM]; __shared__ int s_total, s_out, s_max, s_best;
+  hist[threadIdx.x] = 0;
+  if (threadIdx.x == 0) { s_total = 0; s_out = 0; s_max = 0; s_best = 256; }
   __syncthreads();
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+  for (int i = threadIdx.x; i < n; i += PM_THREADS) {
     if (lab[i] != label) continue;
     const int u = (int)kp[2*i], v = (int)kp[2*i + 1];
     if (u < W && u > 0 && v < H && v > 0) {
       const int l = cur[(size_t)v*W + u];
-      atomicAdd(&total, 1);
-      if (l >= 0 && l < 256) atomicAdd(&hist[l], 1);
+      atomicAdd(&s_total, 1);
+      if (l >= 0 && l < 256) atomicAdd(&hist[l], 1); else votes[atomicAdd(&s_out, 1)] = l;
     }
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    int best = -1, bc = -1;
-    for (int l = 0; l < 256; l++) if (hist[l] > 0 && hist[l] > bc) { bc = hist[l]; best = l; }   // first maximum in ascending label order
-    *flag = (total >= min_votes && best == 0) ? 1 : 0;
+  const int c = hist[threadIdx.x], m = s_out, total = s_total;
+  const int np_hist = __syncthreads_count(c > 0);
+  if (total == 0 || total < min_votes) { if (threadIdx.x == 0) *flag = 0; return; }
+  if (m == 0 && np_hist <= 16) {                   // std::sort of <= 16 pairs is an insertion sort: the first maximum in label order
+    if (c > 0) atomicMax(&s_max, c);
+    __syncthreads();
+    if (c > 0 && c == s_max) atomicMin(&s_best, (int)threadIdx.x);
+    __syncthreads();
+    if (threadIdx.x == 0) *flag = s_best == 0 ? 1 : 0;
+    return;
   }
+  int* v = votes;
+  if (m <= PM_SMEM) {
+    for (int i = threadIdx.x; i < m; i += PM_THREADS) s_v[i] = votes[i];
+    v = s_v;
+    __syncthreads();
+  }
+  unsigned N = 1;
+  while (N < (unsigned)m) N <<= 1;
+  for (unsigned k = 2; k <= N; k <<= 1) {          // bitonic sort, every compare-exchange ascending: the padding up to N is +inf
+    for (unsigned j = k >> 1; j > 0; j >>= 1) {
+      for (unsigned i = threadIdx.x; i < N; i += PM_THREADS) {
+        const unsigned l = j == k >> 1 ? i ^ (k - 1) : i ^ j;
+        if (l > i && l < (unsigned)m) { const int a = v[i], b = v[l]; if (a > b) { v[i] = b; v[l] = a; } }
+      }
+      __syncthreads();
+    }
+  }
+  if (threadIdx.x != 0) return;
+  int np = 0, i = 0;
+  auto runs = [&](bool negative) {                 // the sorted votes outside [0, 256): the negative ones, then those >= 256
+    int run = 0;
+    for (; i < m && (v[i] < 0) == negative; i++) {
+      run++;
+      if (i == m - 1 || v[i + 1] != v[i]) { pairs[np++] = PmPair{v[i], run}; run = 0; }
+    }
+  };
+  runs(true);
+  for (int l = 0; l < 256; l++) if (hist[l]) pairs[np++] = PmPair{l, hist[l]};
+  runs(false);
+  pm_introsort_loop(pairs, np);
+  int best = 0;
+  for (int q = 1; q < np; q++) if (pairs[q].c > pairs[best].c) best = q;
+  *flag = pairs[best].l == 0 ? 1 : 0;
 }
 __global__ void pm_warp_kernel(size_t npx, int W, int H, const int32_t* pmask, const float* pflow, int label, dynofront_track_params prm,
                                const int* flag, int32_t* cur) {
@@ -2321,7 +2431,8 @@ int dynofront_track_dynamic(dynofront_handle h, int32_t n, const double* kp, con
 
 int dynofront_sample_candidates(dynofront_handle h, int32_t nobj, const int32_t* objects, const dynofront_track_params* prm, int32_t* counts,
                                 int32_t* offsets, int32_t* zero_flow, int32_t* indices, int64_t capacity) {
-  if (!h || !prm || nobj < 0 || nobj > ST_MAXOBJ || !counts || !offsets) return -1;
+  if (!h || !prm || nobj < 0 || !counts || !offsets || (nobj && !objects)) return -1;
+  if (check_objects(h, nobj, objects)) return -1;
   cudaSetDevice(h->dev);
   const size_t npx = (size_t)h->W*h->H; const int ntiles = (int)((npx + ST_TILE - 1)/ST_TILE);
   if (!h->det_work_valid) prepare_det_work(h);
@@ -2401,8 +2512,9 @@ int dynofront_sample_dynamic(dynofront_handle h, int32_t nobj, const int32_t* ob
                              const dynofront_track_params* prm, int64_t* next_tracklet_id, int32_t* counts, int32_t* num_sampled, int32_t* zero_flow,
                              int32_t capacity, double* keypoint, double* flow_out, double* predicted, int64_t* tracklet, int32_t* label,
                              int32_t* n_features, float* ms_device) {
-  if (!h || !prm || nobj < 0 || nobj > ST_MAXOBJ || capacity < 0 || !next_tracklet_id || !num_sampled || !n_features) return -1;
+  if (!h || !prm || nobj < 0 || capacity < 0 || !next_tracklet_id || !num_sampled || !n_features) return -1;
   if (nobj && (!objects || !num_track)) return -1;
+  if (check_objects(h, nobj, objects)) return -1;
   if (capacity && (!keypoint || !flow_out || !predicted || !tracklet)) { h->err = "null feature array"; return -1; }
   const long long cmax = std::max(h->W, h->H) - 1;       // no width of the search, for any K the objects can need, may wrap
   bool wraps = cmax > 65535;
@@ -2585,7 +2697,9 @@ int dynofront_propagate_mask(dynofront_handle h, int32_t n, const double* kp, co
   if (!resident && (!prev_mask || !prev_flow || !current_mask)) { h->err = "pass all three images, or none for the resident frames"; return -1; }
   if (resident && !h->have_prev) { h->err = "no previous frame on the device"; return -2; }
   cudaSetDevice(h->dev);
-  if (grow(h, h->f_kp, 2*feature_cap(n), h->f_lab, feature_cap(n))) return -3;
+  const size_t cap = feature_cap(n);
+  if (grow(h, h->f_kp, 2*cap, h->f_lab, cap, h->pm_votes, 3*cap)) return -3;
+  PmPair* const pairs = reinterpret_cast<PmPair*>(h->pm_votes.p + cap);
   const size_t npx = (size_t)h->W*h->H;
   FCK(cudaMemcpyAsync(h->f_kp, kp, 2*(size_t)n*8, cudaMemcpyHostToDevice, h->s));
   FCK(cudaMemcpyAsync(h->f_lab, lab, (size_t)n*4, cudaMemcpyHostToDevice, h->s));
@@ -2599,7 +2713,7 @@ int dynofront_propagate_mask(dynofront_handle h, int32_t n, const double* kp, co
   std::vector<int32_t> labels(lab, lab + n);
   std::sort(labels.begin(), labels.end()); labels.erase(std::unique(labels.begin(), labels.end()), labels.end());
   for (int32_t l : labels) {      // objects in ascending label order, sequentially (FeatureTracker.cc:1262)
-    pm_vote_kernel<<<1, 256, 0, h->s>>>(n, h->f_kp, h->f_lab, l, cmask, h->W, h->H, min_votes, h->pflag);
+    pm_vote_kernel<<<1, PM_THREADS, 0, h->s>>>(n, h->f_kp, h->f_lab, l, cmask, h->W, h->H, min_votes, h->pm_votes, pairs, h->pflag);
     pm_warp_kernel<<<(unsigned)((npx + 255)/256), 256, 0, h->s>>>(npx, h->W, h->H, pmask, pflow, l, *prm, h->pflag, cmask);
   }
   if (!resident) FCK(cudaMemcpyAsync(current_mask, h->cmask, npx*4, cudaMemcpyDeviceToHost, h->s));
@@ -3365,10 +3479,8 @@ int dynofront_track_dynamic_klt(dynofront_handle h, const uint8_t* prev_gray, co
   if (n && (!prev_kp || !prev_label || !prev_age || !prev_tracklet)) { h->err = "null previous-feature array"; return -1; }
   if (n_objects && (!objects || !inner_bb)) { h->err = "null object array"; return -1; }
   if (capacity && (!keypoint || !age || !tracklet || !label || !source)) { h->err = "null feature array"; return -1; }
-  if (n_objects > ST_MAXOBJ) { h->err = "at most 64 objects"; return -1; }
+  if (check_objects(h, n_objects, objects)) return -1;
   for (int o = 0; o < n_objects; o++) {
-    if (objects[o] <= 0) { h->err = "object ids must be > 0 (0 is the background)"; return -1; }
-    for (int q = 0; q < o; q++) if (objects[q] == objects[o]) { h->err = "object ids must be distinct"; return -1; }
     if (inner_bb[4*o + 2] < 0 || inner_bb[4*o + 3] < 0) { h->err = "bounding boxes must have width, height >= 0"; return -1; }
   }
   const dynofront_track_params& T = prm->track;

@@ -71,7 +71,8 @@ int dynofront_track_dynamic(dynofront_handle h, int32_t n, const double* prev_pr
                             uint8_t* tracking_mask_out);
 
 /* sampleDynamic candidate scan over the whole image, using the detection mask left on the device by
- * dynofront_track_dynamic (or the uploaded one).  For each of the n_objects labels: counts[o] candidates whose
+ * dynofront_track_dynamic (or the uploaded one).  objects: at most 64 distinct ids > 0 (also for
+ * dynofront_sample_dynamic; -1 with a message otherwise).  For each of the n_objects labels: counts[o] candidates whose
  * linear pixel indices (row*W + col, ascending) are written to indices + offsets[o]; zero_flow[o] = pixels of the
  * object skipped because a flow component is exactly 0.  capacity = size of indices. */
 int dynofront_sample_candidates(dynofront_handle h, int32_t n_objects, const int32_t* objects, const dynofront_track_params* prm,

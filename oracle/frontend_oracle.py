@@ -29,6 +29,82 @@ class TrackParams:
     shrink_col: int = 0
 
 
+def saturate_u8(label) -> int:
+    """cv::Scalar(label) drawn into a CV_8U image: saturate_cast<uchar>"""
+    return min(max(int(label), 0), 255)
+
+
+def libstdcxx_sort(seq, comp, heap_ranges=None):
+    """std::sort(first, last, comp) of libstdc++ (<bits/stl_algo.h>), element moves and all: __introsort_loop (threshold 16,
+    depth limit 2 floor(log2 n), __move_median_to_first of (first + 1, mid, last - 1), __unguarded_partition, __partial_sort
+    = make_heap + sort_heap at the depth limit), then __final_insertion_sort.  Not stable: where comp ties, the result
+    depends on all of these steps.  Returns a sorted copy; heap_ranges (a list), when given, receives the (first, last) of
+    every range heap-sorted at the depth limit."""
+    a = list(seq)
+    n = len(a)
+
+    def adjust_heap(f, hole, ln, v):
+        top = hole; child = hole
+        while child < (ln - 1)//2:
+            child = 2*(child + 1)
+            if comp(a[f + child], a[f + child - 1]):
+                child -= 1
+            a[f + hole] = a[f + child]; hole = child
+        if ln % 2 == 0 and child == (ln - 2)//2:
+            child = 2*(child + 1); a[f + hole] = a[f + child - 1]; hole = child - 1
+        parent = (hole - 1)//2
+        while hole > top and comp(a[f + parent], v):
+            a[f + hole] = a[f + parent]; hole = parent; parent = (hole - 1)//2
+        a[f + hole] = v
+
+    def heap_sort(f, ln):
+        if ln >= 2:
+            for parent in range((ln - 2)//2, -1, -1):
+                adjust_heap(f, parent, ln, a[f + parent])
+        for last in range(ln - 1, 0, -1):
+            v = a[f + last]; a[f + last] = a[f]; adjust_heap(f, 0, last, v)
+
+    def partition_pivot(first, last):
+        x, y, z = first + 1, first + (last - first)//2, last - 1
+        if comp(a[x], a[y]):
+            m = y if comp(a[y], a[z]) else (z if comp(a[x], a[z]) else x)
+        else:
+            m = x if comp(a[x], a[z]) else (z if comp(a[y], a[z]) else y)
+        a[first], a[m] = a[m], a[first]
+        i, j = first + 1, last
+        while True:
+            while comp(a[i], a[first]):
+                i += 1
+            j -= 1
+            while comp(a[first], a[j]):
+                j -= 1
+            if not i < j:
+                return i
+            a[i], a[j] = a[j], a[i]
+            i += 1
+
+    def introsort_loop(first, last, depth):
+        while last - first > 16:
+            if depth == 0:
+                if heap_ranges is not None:
+                    heap_ranges.append((first, last))
+                heap_sort(first, last - first)
+                return
+            depth -= 1
+            cut = partition_pivot(first, last)
+            introsort_loop(cut, last, depth)
+            last = cut
+
+    if n > 1:
+        introsort_loop(0, n, 2*(n.bit_length() - 1))
+        for i in range(1, n):                            # the guarded and unguarded insertion sorts move alike
+            v = a[i]
+            while i > 0 and comp(v, a[i - 1]):
+                a[i] = a[i - 1]; i -= 1
+            a[i] = v
+    return a
+
+
 def within_shrunken(kp, rows, cols, prm: TrackParams) -> bool:
     pc = int(kp[0]); pr = int(kp[1])          # C++ static_cast<int>: truncation toward zero
     return pr > prm.shrink_row and pr < rows - prm.shrink_row and pc > prm.shrink_col and pc < cols - prm.shrink_col
@@ -70,7 +146,7 @@ def track_dynamic(prev_pred_kp, prev_label, prev_age, prev_tracklet, flow, motio
                 new_age = 0
             acc[i] = 1; pk[i] = predicted; fl[i] = (fx, fy); age[i] = new_age; tid[i] = t; lab[i] = predicted_label
             cv2.circle(det, (x, y), prm.min_distance, 0, cv2.FILLED)
-            cv2.circle(trk, (x, y), prm.min_distance, int(predicted_label) & 0xFF, cv2.FILLED)
+            cv2.circle(trk, (x, y), prm.min_distance, saturate_u8(predicted_label), cv2.FILLED)
     return acc, pk, fl, age, tid, lab, next_tracklet_id, det, trk
 
 
@@ -109,15 +185,13 @@ def propagate_mask(prev_pred_kp, prev_label, prev_mask, prev_flow, current_mask,
             u = int(prev_pred_kp[i][0]); v = int(prev_pred_kp[i][1])
             if u < cols and u > 0 and v < rows and v > 0:
                 temp.append(int(cur[v, u]))
-        if len(temp) < min_votes:
+        if not temp or len(temp) < min_votes:          # no vote: nothing to sort (the device's flag stays 0)
             continue
         counts = {}
         for k in temp:
             counts[k] = counts.get(k, -1) + 1      # first occurrence counts 0 (reference quirk)
-        best = None
-        for k in sorted(counts):                   # std::map order, stable insertion sort for <= 16 entries
-            if best is None or counts[k] > counts[best]:
-                best = k
+        pairs = [(k, counts[k]) for k in sorted(counts)]                  # std::map order
+        best = libstdcxx_sort(pairs, lambda a, b: a[1] > b[1])[0][0]
         if best != 0:
             continue
         for j in range(rows):
