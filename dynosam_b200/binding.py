@@ -25,7 +25,7 @@ EXPORTS = [
     "dynoba_version", "dynoba_status_string", "dynoba_last_error", "dynoba_create", "dynoba_destroy",
     "dynoba_lm_default_params", "dynoba_set_variables", "dynoba_set_aux_poses", "dynoba_set_calibration",
     "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_marginal", "dynoba_finalize", "dynoba_error",
-    "dynoba_optimize", "dynoba_get_variables", "dynoba_get_keys", "dynoba_num_variables", "dynoba_problem_info",
+    "dynoba_optimize", "dynoba_get_variables", "dynoba_get_keys", "dynoba_num_variables", "dynoba_problem_info", "dynoba_window_census",
     "dynoba_linearize", "dynoba_linearize_block", "dynoba_get_linearization", "dynoba_get_factor_errors", "dynoba_solve",
     "dynoba_get_reduced_system", "dynoba_retract", "dynoba_flow_pose_default_params", "dynoba_flow_pose_batch",
     "dynoba_motion_refine_default_params", "dynoba_motion_refine_batch", "dynoba_batch_release",
@@ -111,6 +111,7 @@ def load():
         L.dynoba_get_keys.argtypes = [C.c_void_p, C.c_int, C.c_int64, c_u64p]
         L.dynoba_num_variables.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int64)]
         L.dynoba_problem_info.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
+        L.dynoba_window_census.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         L.dynoba_linearize.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
         L.dynoba_linearize_block.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_int64)]
         L.dynoba_get_linearization.argtypes = [C.c_void_p, C.c_int, c_dp, c_dp]
@@ -345,7 +346,12 @@ class Solver:
     def info(self):
         n = C.c_int32(); bw = C.c_int32(); jb = C.c_int64()
         self._ck(self.lib.dynoba_problem_info(self.h, C.byref(n), C.byref(bw), C.byref(jb)))
-        return dict(reduced_dim=n.value, bandwidth=bw.value, jacobian_bytes=jb.value)
+        ctas = (C.c_int64*2)(); flushed = (C.c_int64*2)()
+        self._ck(self.lib.dynoba_window_census(self.h, ctas, flushed))
+        # window path per damped solve, [static (NP = 1), dynamic (NP = 2)] factor blocks: accumulate-kernel CTAs and
+        # 6x6 blocks of S it adds into memory
+        return dict(reduced_dim=n.value, bandwidth=bw.value, jacobian_bytes=jb.value,
+                    window_accum_ctas=list(ctas), window_blocks_flushed=list(flushed))
 
     def values(self):
         p = self.problem

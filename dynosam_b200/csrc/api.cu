@@ -46,6 +46,7 @@ struct HostBlock {
   bool simple = false, pose_only = false;
   int part_off = 0, bs_off = 0;
   DevWindows win{}; bool use_window = false; bool all_window = false;   // all_window: no group left for the per-landmark atomics kernel
+  int64_t win_ctas = 0, win_flushed = 0;   // accumulate-kernel CTAs and 6x6 blocks it flushes, per damped solve
 };
 
 struct HostPrior {      // gtsam::LinearContainerFactor(HessianFactor) over pose-like variables
@@ -791,33 +792,49 @@ static int finalize_impl(dynoba_solver* h) {
       b.simple = true;
       // ---- window decomposition (kernels_window.cu) for the 3-dof landmark types
       const bool win_type = b.type == F_POSE2POINT3 || b.type == F_STEREO3 || b.type == F_HYBRID3 || b.type == F_HYBRID_STEREO3;
-      b.use_window = false; b.all_window = false; b.win = DevWindows{};
+      b.use_window = false; b.all_window = false; b.win = DevWindows{}; b.win_ctas = 0; b.win_flushed = 0;
       if (win_type && !gl.empty()) {
         const int ng = (int)gl.size(), NPs = ti.npose;
         std::vector<unsigned char> gwin(ng, 0);
         std::vector<unsigned char, NoInitAlloc<unsigned char>> lvar((size_t)NPs*stride);   // only read for window-path factors
-        std::vector<int32_t> chunk_nloc, cvars; std::vector<int4> jobs, batches;
+        std::vector<int32_t> chunk_batch, cvars; std::vector<int4> jobs, batches;
         int pose_slot[2] = {0, 0}; { int c = 0; for (int k = 0; k < ti.arity; k++) if (ti.cls[k] == VC_POSE && c < 2) pose_slot[c++] = k; }
         // window size: one 512-thread CTA holds 16 tiles of 8x4 blocks; NLOC 24 -> 12 tiles (one stripe), NLOC 40 -> 30 (two)
         int cap = NPs == 1 ? 24 : 40;
+        // NP = 2: a variable keeps its window slot over the consecutive chunks that contain it, and the accumulate kernel
+        // walks runs of chunks.  NP = 1 chunks (~1000 landmarks each) are runs of their own, slots in position order.
+        const bool slide = NPs == 2;
         // greedy chunking, independently inside parallel segments of the group list (a chunk never crosses a segment)
         const int nseg = std::max(1, std::min<int>(omp_get_max_threads(), ng/4096 + 1));
-        struct SegOut { std::vector<int32_t> g0, nloc, cv, b0; std::vector<int4> bat; };   // b0: first batch of each chunk (+ end)
+        // per chunk: first group, slots spanned (highest occupied slot + 1), slot -> position row, first batch (+ end)
+        struct SegOut { std::vector<int32_t> g0, nslot, cv, b0; std::vector<int4> bat; int64_t flushed = 0; };
         std::vector<SegOut> seg(nseg);
 #pragma omp parallel for schedule(static, 1)
         for (int t = 0; t < nseg; t++) {
           const int ga = (int)((int64_t)ng*t/nseg), gb_ = (int)((int64_t)ng*(t + 1)/nseg);
           std::vector<int32_t> stamp(NP, -1), gstamp(NP, -1), inchunk(NP, -1), cur;   // indexed by solver position
+          std::vector<int32_t> wslot(NP, -1), occ(WIN_NLOC_MAX, -1);                 // window slot of a position, occupant of a slot
           int cur_g0 = ga, chunk_id = 0; SegOut& out = seg[t];
           auto close_chunk = [&](int g_end) {
             std::vector<int32_t> sorted = cur; std::sort(sorted.begin(), sorted.end());
-            for (size_t i = 0; i < sorted.size(); i++) stamp[sorted[i]] = (int32_t)i;       // position -> local index
+            std::vector<int32_t> row(WIN_NLOC_MAX, -1);
+            if (slide) {     // variables that stay keep their slot; entering ones take the lowest free slots
+              for (int32_t p_ : sorted) stamp[p_] = -2;
+              for (int s_ = 0; s_ < WIN_NLOC_MAX; s_++) if (occ[s_] >= 0 && stamp[occ[s_]] != -2) occ[s_] = -1;
+              for (int32_t p_ : sorted) if (wslot[p_] >= 0 && occ[wslot[p_]] == p_) stamp[p_] = wslot[p_];
+              int fs = 0;
+              for (int32_t p_ : sorted) if (stamp[p_] == -2) { while (occ[fs] >= 0) fs++; occ[fs] = p_; wslot[p_] = fs; stamp[p_] = fs; }
+              row = occ;
+            } else {
+              for (size_t i = 0; i < sorted.size(); i++) { stamp[sorted[i]] = (int32_t)i; row[i] = sorted[i]; }   // position -> local index
+            }
             for (int g = cur_g0; g < g_end; g++) if (gwin[g] == 1)
               for (int s_ = gp[g]; s_ < gp[g+1]; s_++) for (int k = 0; k < NPs; k++)
                 lvar[(size_t)k*stride + s_] = (unsigned char)stamp[hidx[(size_t)pose_slot[k]*stride + s_]];
             for (size_t i = 0; i < sorted.size(); i++) stamp[sorted[i]] = -1;
-            out.g0.push_back(cur_g0); out.nloc.push_back((int32_t)sorted.size());
-            sorted.resize(WIN_NLOC_MAX, 0); out.cv.insert(out.cv.end(), sorted.begin(), sorted.end());
+            int ext = 0; for (int s_ = 0; s_ < WIN_NLOC_MAX; s_++) if (row[s_] >= 0) ext = s_ + 1;
+            out.g0.push_back(cur_g0); out.nslot.push_back(ext);
+            out.cv.insert(out.cv.end(), row.begin(), row.end());
             // batches of the chunk: runs of window-path landmarks (other groups end a run), bounded in landmarks and slots
             out.b0.push_back((int32_t)out.bat.size());
             int rg0 = -1, rslots = 0;
@@ -854,27 +871,74 @@ static int finalize_impl(dynoba_solver* h) {
             gwin[g] = 1;
           }
           close_chunk(gb_);
+          out.b0.push_back((int32_t)out.bat.size());
         }
-        for (int t = 0; t < nseg; t++) for (size_t c = 0; c < seg[t].g0.size(); c++) {
-          const int chunk_id = (int)chunk_nloc.size();
-          chunk_nloc.push_back(seg[t].nloc[c]);
-          cvars.insert(cvars.end(), seg[t].cv.begin() + c*WIN_NLOC_MAX, seg[t].cv.begin() + (c + 1)*WIN_NLOC_MAX);
-          const int nl_ = seg[t].nloc[c]; const int ntile = win_ntiles(nl_);
-          const size_t sb0 = seg[t].b0[c], sb1 = c + 1 < seg[t].b0.size() ? seg[t].b0[c + 1] : seg[t].bat.size();
-          const int b0 = (int)batches.size();
-          batches.insert(batches.end(), seg[t].bat.begin() + sb0, seg[t].bat.begin() + sb1);
-          const int b1 = (int)batches.size();
-          if (b1 > b0) for (int st = 0; st*WIN_ACC_WARPS < ntile; st++) jobs.push_back(make_int4(chunk_id, st, b0, b1));
+        // runs: a segment's chunks that have batches, run_len at a time (never across a segment: the slots restart there)
+        auto has_batches = [&](const SegOut& o, size_t c) { return o.b0[c + 1] > o.b0[c]; };
+        size_t nch = 0; for (int t = 0; t < nseg; t++) for (size_t c = 0; c + 1 < seg[t].b0.size(); c++) nch += has_batches(seg[t], c);
+        const int run_len = slide ? std::max<int>(WIN_RUN_MIN_CHUNKS, (int)((nch + WIN_RUNS - 1)/WIN_RUNS)) : 1;
+        // census: the blocks the accumulate kernel flushes per solve, by its rule (a slot pair that a landmark's clique
+        // touched, when either slot changes variable and at the run's end)
+#pragma omp parallel for schedule(static, 1)
+        for (int t = 0; t < nseg; t++) {
+          SegOut& o = seg[t];
+          uint64_t tch[WIN_NLOC_MAX] = {};      // tch[a] bit b: slot pair (a, b) touched since its last flush
+          auto flush = [&](uint64_t E) {        // E: slots that change variable
+            for (int a_ = 0; a_ < WIN_NLOC_MAX; a_++) {
+              const uint64_t low = tch[a_] & ((2ull << a_) - 1);
+              o.flushed += __builtin_popcountll((E >> a_) & 1 ? low : low & E);
+            }
+            for (int a_ = 0; a_ < WIN_NLOC_MAX; a_++) tch[a_] = (E >> a_) & 1 ? 0 : tch[a_] & ~E;
+          };
+          int in_run = 0; int prev = -1;
+          for (size_t c = 0; c + 1 < o.b0.size(); c++) {
+            if (!has_batches(o, c)) continue;
+            uint64_t E = 0;
+            if (in_run == run_len) { E = ~0ull; in_run = 0; }
+            else if (prev >= 0) for (int s_ = 0; s_ < WIN_NLOC_MAX; s_++) if (o.cv[(size_t)prev*WIN_NLOC_MAX + s_] != o.cv[c*WIN_NLOC_MAX + s_]) E |= 1ull << s_;
+            flush(E);
+            in_run++; prev = (int)c;
+            const int ge = c + 1 < o.g0.size() ? o.g0[c + 1] : (int)((int64_t)ng*(t + 1)/nseg);
+            for (int g = o.g0[c]; g < ge; g++) if (gwin[g] == 1) {
+              uint64_t m = 0;
+              for (int s_ = gp[g]; s_ < gp[g+1]; s_++) for (int k = 0; k < NPs; k++) m |= 1ull << lvar[(size_t)k*stride + s_];
+              for (uint64_t r_ = m; r_; r_ &= r_ - 1) tch[__builtin_ctzll(r_)] |= m;
+            }
+          }
+          flush(~0ull);
         }
-        int4* djobs; int4* dbat; int* dnl; int* dcv; unsigned char* dlv; unsigned char* dgw; double* dslots;
+        b.win_ctas = 0; b.win_flushed = 0;
+        for (int t = 0; t < nseg; t++) {
+          const SegOut& o = seg[t];
+          b.win_flushed += o.flushed;
+          int r0 = -1, in_run = 0, ext = 0;
+          auto close_run = [&]() {
+            if (r0 < 0) return;
+            const int nst = (win_ntiles(ext) + WIN_ACC_WARPS - 1)/WIN_ACC_WARPS;
+            for (int st = 0; st < nst; st++) jobs.push_back(make_int4(r0, (int)chunk_batch.size(), st, ext));
+            b.win_ctas += nst; r0 = -1; in_run = 0; ext = 0;
+          };
+          for (size_t c = 0; c + 1 < o.b0.size(); c++) {
+            if (!has_batches(o, c)) continue;
+            if (in_run == run_len) close_run();
+            if (r0 < 0) r0 = (int)chunk_batch.size();
+            chunk_batch.push_back((int32_t)batches.size());
+            batches.insert(batches.end(), o.bat.begin() + o.b0[c], o.bat.begin() + o.b0[c + 1]);
+            cvars.insert(cvars.end(), o.cv.begin() + c*WIN_NLOC_MAX, o.cv.begin() + (c + 1)*WIN_NLOC_MAX);
+            ext = std::max(ext, o.nslot[c]); in_run++;
+          }
+          close_run();
+        }
+        chunk_batch.push_back((int32_t)batches.size());
+        int4* djobs; int4* dbat; int* dcb; int* dcv; unsigned char* dlv; unsigned char* dgw; double* dslots;
         if ((rc = dalloc(h, &djobs, jobs.size()))) return rc; if (!jobs.empty()) CK(cudaMemcpy(djobs, jobs.data(), jobs.size()*sizeof(int4), cudaMemcpyHostToDevice));
         if ((rc = dalloc(h, &dbat, batches.size()))) return rc; if (!batches.empty()) CK(cudaMemcpy(dbat, batches.data(), batches.size()*sizeof(int4), cudaMemcpyHostToDevice));
-        if ((rc = dalloc(h, &dnl, chunk_nloc.size()))) return rc; CK(cudaMemcpy(dnl, chunk_nloc.data(), chunk_nloc.size()*4, cudaMemcpyHostToDevice));
-        if ((rc = dalloc(h, &dcv, cvars.size()))) return rc; CK(cudaMemcpy(dcv, cvars.data(), cvars.size()*4, cudaMemcpyHostToDevice));
+        if ((rc = dalloc(h, &dcb, chunk_batch.size()))) return rc; CK(cudaMemcpy(dcb, chunk_batch.data(), chunk_batch.size()*4, cudaMemcpyHostToDevice));
+        if ((rc = dalloc(h, &dcv, cvars.size()))) return rc; if (!cvars.empty()) CK(cudaMemcpy(dcv, cvars.data(), cvars.size()*4, cudaMemcpyHostToDevice));
         if ((rc = dalloc(h, &dlv, lvar.size()))) return rc; CK(cudaMemcpy(dlv, lvar.data(), lvar.size(), cudaMemcpyHostToDevice));
         if ((rc = dalloc(h, &dgw, gwin.size()))) return rc; CK(cudaMemcpy(dgw, gwin.data(), gwin.size(), cudaMemcpyHostToDevice));
         if ((rc = dalloc(h, &dslots, (size_t)n*NPs*WIN_SLOT_DOUBLES, false))) return rc;
-        b.win.n_jobs = (int)jobs.size(); b.win.jobs = djobs; b.win.batches = dbat; b.win.chunk_nloc = dnl; b.win.cvars = dcv; b.win.lvar = dlv; b.win.grp_win = dgw; b.win.slots = dslots;
+        b.win.n_jobs = (int)jobs.size(); b.win.jobs = djobs; b.win.batches = dbat; b.win.chunk_batch = dcb; b.win.cvars = dcv; b.win.lvar = dlv; b.win.grp_win = dgw; b.win.slots = dslots;
         b.use_window = true;
         { size_t nw = 0; for (int g = 0; g < ng; g++) nw += gwin[g] == 1 || gl[g] < 0; b.all_window = nw == (size_t)ng; }
       }
@@ -1134,6 +1198,17 @@ int dynoba_get_keys(dynoba_handle h, int kind, int64_t n, uint64_t* out) {
 int dynoba_problem_info(dynoba_handle h, int32_t* reduced_dim, int32_t* bandwidth, int64_t* jacobian_bytes) {
   int rc = check_ready(h, false); if (rc) return rc;
   if (reduced_dim) *reduced_dim = h->band.n; if (bandwidth) *bandwidth = h->band.bw; if (jacobian_bytes) *jacobian_bytes = h->jac_bytes;
+  return DYNOBA_OK;
+}
+
+int dynoba_window_census(dynoba_handle h, int64_t* accum_ctas, int64_t* blocks_flushed) {
+  int rc = check_ready(h, false); if (rc) return rc;
+  for (int k = 0; k < 2; k++) { if (accum_ctas) accum_ctas[k] = 0; if (blocks_flushed) blocks_flushed[k] = 0; }
+  for (const HostBlock& b : h->blocks) if (b.use_window) {
+    const int k = (b.type == F_HYBRID3 || b.type == F_HYBRID_STEREO3) ? 1 : 0;
+    if (accum_ctas) accum_ctas[k] += b.win_ctas;
+    if (blocks_flushed) blocks_flushed[k] += b.win_flushed;
+  }
   return DYNOBA_OK;
 }
 

@@ -195,7 +195,7 @@ struct GeneralGroups {
 };
 
 // Window decomposition of a factor block for kernels_window.cu (built by the host in finalize)
-constexpr int WIN_NLOC_MAX = 48;          // largest window (local pose-like variables of a chunk)
+constexpr int WIN_NLOC_MAX = 48;          // largest window (local pose-like variables of a chunk; window slots)
 constexpr int WIN_TMAX = 24;              // factors per landmark on the window path (larger ones: kernels_schur.cu)
 constexpr int WIN_SLOT_DOUBLES = 42;      // one staged clique variable of one factor: Wt[3][6] | A[3][6] | rb[3] | meta | pad[2]
 constexpr int WIN_BATCH_SLOTS = 256;      // slots per shared-memory buffer of the accumulate kernel
@@ -208,14 +208,21 @@ __host__ __device__ __forceinline__ int win_ntiles(int nloc) {
   return n;
 }
 constexpr int WIN_ACC_WARPS = 16;         // tiles per CTA (stripe) of the accumulate kernel
+// NP = 2 chunks are accumulated in RUNS of consecutive chunks, one CTA per (run, stripe) walking the run's chunks in
+// order: a block stays in registers while both of its variables stay in the window.  A factor block's chunks are cut
+// into about WIN_RUNS runs (four per SM of an H100: load balance at one 172 KB CTA per SM), of at least WIN_RUN_MIN_CHUNKS.
+constexpr int WIN_RUNS = 528;
+constexpr int WIN_RUN_MIN_CHUNKS = 8;
 struct DevWindows {
   int n_jobs;
-  const int4* jobs;              // (chunk, stripe of the window's lower-triangular blocks, first batch, end batch)
+  const int4* jobs;              // (first chunk, end chunk, stripe of the window's lower-triangular blocks, window slots)
   const int4* batches;           // (first group, end group, first factor, end factor): runs of window-path landmarks,
                                  // at most WIN_BATCH_LMK landmarks / WIN_BATCH_SLOTS slots, never crossing a chunk
-  const int* chunk_nloc;         // [n_chunks]
-  const int* cvars;              // [n_chunks][WIN_NLOC_MAX] solver positions, ascending
-  const unsigned char* lvar;     // [npose_slots][stride] local variable of each factor's pose slot
+  const int* chunk_batch;        // [n_chunks + 1] first batch of each chunk (every chunk has at least one)
+  const int* cvars;              // [n_chunks][WIN_NLOC_MAX] solver position of the variable in each window slot, -1: empty.
+                                 // NP = 1: slots in ascending position.  NP = 2: a variable keeps its slot over the
+                                 // consecutive chunks that contain it; an entering variable takes the lowest free slot
+  const unsigned char* lvar;     // [npose_slots][stride] window slot of each factor's pose slot
   const unsigned char* grp_win;  // [n_groups] 0: general path, 1: window path, 2: per-landmark atomics path
   double* slots;                 // [n*npose_slots][WIN_SLOT_DOUBLES] staged slots in factor order (HBM scratch)
 };

@@ -6,14 +6,18 @@
 //                            written once to an HBM scratch array that is laid out in factor order, so the slots of a
 //                            run of landmarks are ONE contiguous byte range.
 //   K4b schur_accum_kernel   the landmarks of a factor block are cut (on the host, DevWindows) into chunks whose cliques
-//                            live in a window of at most NLOC pose-like variables.  A CTA of 512 threads owns (a stripe
-//                            of) the window's lower-triangular 6x6 blocks, ONE BLOCK PER THREAD (a warp = an 8x4 tile of blocks), in registers
-//                            (output-stationary), and streams the chunk's slots through shared memory with bulk
-//                            asynchronous copies (cp.async.bulk + mbarrier, double-buffered); every thread adds
+//                            live in a window of at most NLOC pose-like variables, and the chunks into RUNS of
+//                            consecutive chunks.  A CTA of 512 threads owns (a stripe of) the lower-triangular 6x6 blocks
+//                            of the window's slot pairs, ONE BLOCK PER THREAD (a warp = an 8x4 tile of blocks), in
+//                            registers (output-stationary), and streams the run's slots, chunk after chunk, through shared
+//                            memory with bulk asynchronous copies (cp.async.bulk + mbarrier, double-buffered); every thread adds
 //                                S_ab += [same factor] A_a^T A_b - What_a What_b^T
 //                            for the landmarks whose clique contains both of its variables (What_a What_b^T =
-//                            W_a V^-1 W_b^T).  g_S is accumulated by the diagonal threads in shared memory.  Each
-//                            block is flushed once per chunk into the tiled band storage.
+//                            W_a V^-1 W_b^T).  g_S is accumulated by the diagonal threads in shared memory.  A variable
+//                            keeps its window slot while consecutive chunks contain it (NP = 2: a dynamic landmark's
+//                            chunk is ~28 landmarks of one object born at one frame, the next chunk is the same object a
+//                            frame later), so a block is flushed into the tiled band storage only when one of its two
+//                            slots changes variable, and at the run's end.
 // Arithmetic is the same as kernels_schur.cu (GTSAM's landmark elimination, SURVEY.md 8a a11).
 #include "internal.cuh"
 
@@ -182,23 +186,21 @@ schur_accum_kernel(DevWindows Wn, DevBand B) {
   short* map = reinterpret_cast<short*>(gs + WIN_NLOC_MAX*6);                            // [2][WIN_BATCH_LMK][WIN_NLOC_MAX]
   unsigned long long* bar = reinterpret_cast<unsigned long long*>(map + 2*WIN_BATCH_LMK*WIN_NLOC_MAX);   // [2]
   const int tid = threadIdx.x;
-  const int4 job = Wn.jobs[blockIdx.x];                 // (chunk, stripe, first batch, end batch)
-  const int chunk = job.x, b0 = job.z, b1 = job.w;
-  const int nloc = Wn.chunk_nloc[chunk];
-  const int* cvars = Wn.cvars + (size_t)chunk*WIN_NLOC_MAX;
-  // my block (a >= b): warp <-> 8x4 tile of the window's lower triangle, the stripes of a chunk split the tiles evenly
-  const int ntile = win_ntiles(nloc);
+  const int4 job = Wn.jobs[blockIdx.x];                 // (first chunk, end chunk, stripe, window slots)
+  const int nslot = job.w;
+  // my block (slots a >= b): warp <-> 8x4 tile of the window's lower triangle, the stripes of a run split the tiles evenly
+  const int ntile = win_ntiles(nslot);
   const int nst = (ntile + WIN_ACC_WARPS - 1)/WIN_ACC_WARPS;
   const int per = (ntile + nst - 1)/nst;
   int a = 0, b = 0; bool active = false;
   {
     const int warp = tid >> 5, lane = tid & 31;
-    int t = job.y*per + warp;
+    int t = job.z*per + warp;
     if (warp < per && t < ntile) {
       int tr = 0;
-      for (;; tr++) { const int rmax = (8*tr + 7 < nloc - 1) ? 8*tr + 7 : nloc - 1; const int n = rmax/4 + 1; if (t < n) break; t -= n; }
+      for (;; tr++) { const int rmax = (8*tr + 7 < nslot - 1) ? 8*tr + 7 : nslot - 1; const int n = rmax/4 + 1; if (t < n) break; t -= n; }
       a = 8*tr + (lane >> 2); b = 4*t + (lane & 3);
-      active = a < nloc && b <= a;
+      active = a < nslot && b <= a;
     }
   }
   const bool diag = active && a == b;
@@ -213,6 +215,7 @@ schur_accum_kernel(DevWindows Wn, DevBand B) {
   }
   __syncthreads();
   const int4* batches = Wn.batches;       // (first group, end group, first factor, end factor)
+  const int b0 = Wn.chunk_batch[job.x], b1 = Wn.chunk_batch[job.y];   // the run's batches, chunk after chunk
   if (tid == 0) {
     const int4 bt = batches[b0];
     const unsigned bytes = (unsigned)((bt.w - bt.z)*NP*WSLOT*8);
@@ -220,7 +223,53 @@ schur_accum_kernel(DevWindows Wn, DevBand B) {
     bulk_g2s(buf, Wn.slots + (size_t)bt.z*NP*WSLOT, bytes, bar);
   }
   int4 bt = batches[b0];
-  for (int bi = b0; bi < b1; bi++) {
+  int chunk = job.x - 1, cend = b0;       // batches of `chunk` end at cend
+  int pa = -1, pb = -1;                   // solver positions of the variables in slots a, b during `chunk`
+  for (int bi = b0;; bi++) {
+    if (bi == cend) {
+      // chunk boundary (and the run's end): a block whose slot changes variable goes to S, and its slot pair starts over
+      int na = -1, nb = -1;
+      if (bi < b1) {
+        chunk++; cend = Wn.chunk_batch[chunk + 1];
+        if (active) { na = Wn.cvars[(size_t)chunk*WIN_NLOC_MAX + a]; nb = Wn.cvars[(size_t)chunk*WIN_NLOC_MAX + b]; }
+      }
+      if (touched && (na != pa || nb != pb)) {
+        // block (pa, pb) of S, lower triangle: slots are not in position order, so a block with pa < pb goes in transposed
+        const bool tr = pa < pb;
+        const int pi = tr ? pb : pa, pj = tr ? pa : pb;
+        const BandBlockRef cref = band_block_ref(B, pi*6, pj*6);   // the block's storage, resolved once for its 36 entries
+        if (cref.fast) {
+          // inside one band chain: tile coordinates of the block's corner, then 36 additions with compile-time offsets (a
+          // block spans at most two tile rows and two tile columns)
+          const int li0 = cref.rev ? cref.oi - (pj*6 + 5) : pi*6 - cref.oi, lj0 = cref.rev ? cref.oi - (pi*6 + 5) : pj*6 - cref.oj;
+#pragma unroll
+          for (int r = 0; r < 6; r++)
+#pragma unroll
+            for (int c = 0; c < 6; c++) {
+              if (a == b && c > r) continue;
+              // natural: (li, lj) = (li0 + r, lj0 + c); reversed chain: row and column swap and run backwards
+              const int li = cref.rev ? li0 + (5 - c) : li0 + r, lj = cref.rev ? lj0 + (5 - r) : lj0 + c;
+              red_add(cref.base + tile_elem(cref.tpc, lj >> 5, (li >> 5) - (lj >> 5), li & 31, lj & 31), tr ? acc[c*6 + r] : acc[r*6 + c]);
+            }
+        } else {
+#pragma unroll 1
+          for (int e = 0; e < 36; e++) {
+            const int r = e/6, c = e - 6*r;
+            if (a == b && c > r) continue;
+            red_add(band_at_slow(B, pi*6 + r, pj*6 + c), acc_at(acc, tr ? c*6 + r : e));
+          }
+        }
+        if (diag) {
+#pragma unroll
+          for (int c = 0; c < 6; c++) { red_add(rhs_at(B, pa*6 + c), gs[a*6 + c]); gs[a*6 + c] = 0.0; }
+        }
+#pragma unroll
+        for (int i = 0; i < 36; i++) acc[i] = 0.0;
+        touched = false;
+      }
+      pa = na; pb = nb;
+      if (bi == b1) break;
+    }
     const int cur = (bi - b0) & 1;
     const unsigned parity = (unsigned)(((bi - b0) >> 1) & 1);
     int4 btn = bt;
@@ -288,35 +337,6 @@ schur_accum_kernel(DevWindows Wn, DevBand B) {
       }
     }
     bt = btn;
-  }
-  if (active && touched) {
-    const int pa = cvars[a], pb = cvars[b];   // cvars ascending => pa >= pb
-    const BandBlockRef cref = band_block_ref(B, pa*6, pb*6);   // the block's storage, resolved once for its 36 entries
-    if (cref.fast) {
-      // inside one band chain: tile coordinates of the block's corner, then 36 additions with compile-time offsets (a block
-      // spans at most two tile rows and two tile columns)
-      const int li0 = cref.rev ? cref.oi - (pb*6 + 5) : pa*6 - cref.oi, lj0 = cref.rev ? cref.oi - (pa*6 + 5) : pb*6 - cref.oj;
-#pragma unroll
-      for (int r = 0; r < 6; r++)
-#pragma unroll
-        for (int c = 0; c < 6; c++) {
-          if (a == b && c > r) continue;
-          // natural: (li, lj) = (li0 + r, lj0 + c); reversed chain: row and column swap and run backwards
-          const int li = cref.rev ? li0 + (5 - c) : li0 + r, lj = cref.rev ? lj0 + (5 - r) : lj0 + c;
-          red_add(cref.base + tile_elem(cref.tpc, lj >> 5, (li >> 5) - (lj >> 5), li & 31, lj & 31), acc[r*6 + c]);
-        }
-    } else {
-#pragma unroll 1
-      for (int e = 0; e < 36; e++) {
-        const int r = e/6, c = e - 6*r;
-        if (a == b && c > r) continue;
-        red_add(band_at_slow(B, pa*6 + r, pb*6 + c), acc_at(acc, e));
-      }
-    }
-    if (a == b) {
-#pragma unroll
-      for (int c = 0; c < 6; c++) red_add(rhs_at(B, pa*6 + c), gs[a*6 + c]);
-    }
   }
 }
 

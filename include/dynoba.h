@@ -189,6 +189,10 @@ int dynoba_num_variables(dynoba_handle h, int kind, int64_t* out);
  * the reduced solve. */
 int dynoba_fp64_rate(dynoba_handle h, double* tflops);
 int dynoba_problem_info(dynoba_handle h, int32_t* reduced_dim, int32_t* bandwidth, int64_t* jacobian_bytes);
+/* Census of the landmark elimination's window path, per damped solve, [0] for the static (one pose per factor) and [1]
+ * for the dynamic (camera pose + object motion per factor) factor blocks: the CTAs the accumulate kernel runs and the 6x6
+ * blocks of the reduced system it adds into memory (either array may be NULL).  Counted from the plan on the host. */
+int dynoba_window_census(dynoba_handle h, int64_t* accum_ctas, int64_t* blocks_flushed);
 
 /* ---- stepwise / parity hooks (what gtsam exposes as graph.linearize(values)) */
 /* Materialising linearize of every factor at the current values (the roofline kernel).  Returns the
