@@ -24,7 +24,7 @@ REDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.
 EXPORTS = [
     "dynoba_version", "dynoba_status_string", "dynoba_last_error", "dynoba_create", "dynoba_destroy",
     "dynoba_lm_default_params", "dynoba_set_variables", "dynoba_set_aux_poses", "dynoba_set_calibration",
-    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_marginal", "dynoba_finalize", "dynoba_error",
+    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_marginal", "dynoba_marginal_covariance", "dynoba_finalize", "dynoba_error",
     "dynoba_optimize", "dynoba_get_variables", "dynoba_get_keys", "dynoba_num_variables", "dynoba_problem_info", "dynoba_window_census",
     "dynoba_linearize", "dynoba_linearize_block", "dynoba_get_linearization", "dynoba_get_factor_errors", "dynoba_solve",
     "dynoba_get_reduced_system", "dynoba_retract", "dynoba_flow_pose_default_params", "dynoba_flow_pose_batch",
@@ -104,6 +104,7 @@ def load():
         L.dynoba_fp64_rate.argtypes = [C.c_void_p, c_dp]
         L.dynoba_add_linear_prior.argtypes = [C.c_void_p, C.c_int32, c_ip, c_dp, c_dp, c_dp, C.c_double]
         L.dynoba_marginal.argtypes = [C.c_void_p, C.c_int32, c_ip, c_dp, c_dp]
+        L.dynoba_marginal_covariance.argtypes = [C.c_void_p, C.c_int, C.c_int64, c_ip, c_dp]
         L.dynoba_finalize.argtypes = [C.c_void_p]
         L.dynoba_error.argtypes = [C.c_void_p, c_dp]
         L.dynoba_optimize.argtypes = [C.c_void_p, C.POINTER(LmParams), C.POINTER(LmStats)]
@@ -230,6 +231,21 @@ class Solver:
         G = np.zeros((6*k, 6*k)); g = np.zeros(6*k)
         self._ck(self.lib.dynoba_marginal(self.h, k, _ip(keep), _dp(G), _dp(g)))
         return G, g
+
+    def marginal_covariance(self, kind, idx=None):
+        """(n, d, d) marginal covariances of variables idx (all of the kind when None) at the current values:
+        gtsam::Marginals(graph, values, CHOLESKY).marginalCovariance, d = 6 (POSE6, BIAS6), 3 (POINT3, VEL3), 2 (FLOW2)"""
+        d = {POSE6: 6, BIAS6: 6, POINT3: 3, VEL3: 3, FLOW2: 2}[kind]
+        if idx is None:
+            n = C.c_int64()
+            self._ck(self.lib.dynoba_num_variables(self.h, kind, C.byref(n)))
+            n, ip = n.value, C.cast(None, c_ip)
+        else:
+            idx = np.ascontiguousarray(idx, dtype=np.int32).reshape(-1)
+            n, ip = idx.size, _ip(idx)
+        cov = np.zeros((n, d, d))
+        self._ck(self.lib.dynoba_marginal_covariance(self.h, kind, n, ip, _dp(cov)))
+        return cov
 
     def set_shard(self, rank, world, allreduce, min_bandwidth=0):
         """allreduce(dev_ptr:int, n:int, stream:int) -> None sums n doubles in place across ranks."""

@@ -77,6 +77,10 @@ struct dynoba_solver {
   GeneralGroups gen{}; int gen_bs_off = 0;
   std::vector<std::pair<void*, size_t>> allocs;   // device allocations (pointer, bytes)
   cudaEvent_t ev[8]{};
+  // dynoba_marginal_covariance: Sigma = S^-1 on the band of a plain layout of its own, and the landmark tables, kept from
+  // the first call at a linearisation point until the values change
+  BandPlan cov_plan{}; double* cov_stage = nullptr; double* cov_lmk = nullptr;
+  bool cov_live = false, cov_ready = false, cov_lmk_ready = false;
 };
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return DYNOBA_ERR_CUDA; } } while (0)
@@ -157,6 +161,34 @@ static void free_device(dynoba_solver* h) {
   for (auto& a : h->allocs) g_devcache.give(h->device, a.first, a.second);
   h->allocs.clear();
   h->finalized = false; h->linearized = false;
+  h->cov_live = h->cov_ready = h->cov_lmk_ready = false; h->cov_stage = nullptr; h->cov_lmk = nullptr;
+}
+// hands one allocation of the handle back to the cache
+static void release(dynoba_solver* h, void* q) {
+  auto it = std::find_if(h->allocs.begin(), h->allocs.end(), [&](const std::pair<void*, size_t>& a) { return a.first == q; });
+  if (it != h->allocs.end()) { g_devcache.give(h->device, it->first, it->second); h->allocs.erase(it); }
+}
+// One plain band problem (no cells) over the reduced system in buffers of its own, whatever partition the handle's solve
+// uses: dynoba_marginal (factorisation stopped before column kend) and dynoba_marginal_covariance (kend < 0: every column)
+static int plain_plan_create(dynoba_solver* h, BandPlan& mp, int kend) {
+  mp = BandPlan{}; mp.outer_weight = 0;
+  if (band_plan_layout(mp, h->band.n, h->band.bw, -1, 0, 1)) { h->err = "band layout failed"; return DYNOBA_ERR_BAD_ARG; }
+  if (kend >= 0) mp.chains[0].Kend = kend;
+  double* dbuf; int* ibuf; char* desc; int rc;
+  if ((rc = dalloc(h, &dbuf, mp.n_doubles, false))) return rc;
+  if ((rc = dalloc(h, &ibuf, mp.n_ints, false))) { release(h, dbuf); return rc; }
+  if ((rc = dalloc(h, &desc, mp.n_desc_bytes))) { release(h, dbuf); release(h, ibuf); return rc; }
+  band_plan_bind(mp, dbuf, ibuf, desc, nullptr);
+  return DYNOBA_OK;
+}
+static void plain_plan_release(dynoba_solver* h, BandPlan& mp) {
+  for (void* q : { (void*)mp.band.acc, (void*)mp.flags_base, (void*)mp.d_chains }) release(h, q);   // (d_chains: start of the descriptors)
+}
+// the values changed: the covariances of the old linearisation point go
+static void cov_invalidate(dynoba_solver* h) {
+  if (h->cov_live) { cudaStreamSynchronize(h->stream); plain_plan_release(h, h->cov_plan); release(h, h->cov_stage); }
+  if (h->cov_lmk) release(h, h->cov_lmk);
+  h->cov_live = h->cov_ready = h->cov_lmk_ready = false; h->cov_stage = nullptr; h->cov_lmk = nullptr;
 }
 
 // copy of a caller's array into the handle: parallel, so that the first touch of the fresh pages (the expensive part of a
@@ -263,7 +295,7 @@ int dynoba_set_variables(dynoba_handle h, int kind, int64_t n, const uint64_t* k
       CK(cudaMemcpy(soa.data(), h->cur.pose, soa.size()*8, cudaMemcpyDeviceToHost));
       for (int64_t i = 0; i < n; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*st + h->pos[base + i]] = k < w ? data[i*w + k] : 0.0;
       CK(cudaMemcpy(h->cur.pose, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
-      h->linearized = false;
+      h->linearized = false; cov_invalidate(h);
       return DYNOBA_OK;
     }
   }
@@ -286,7 +318,7 @@ int dynoba_set_variables(dynoba_handle h, int kind, int64_t n, const uint64_t* k
       CK(cudaMemcpyAsync(h->cur.flow, soa.data(), soa.size()*8, cudaMemcpyHostToDevice, h->stream));
     }
     CK(cudaStreamSynchronize(h->stream));
-    h->linearized = false;
+    h->linearized = false; cov_invalidate(h);
   } else if (h->finalized) {
     free_device(h);
   }
@@ -302,7 +334,7 @@ int dynoba_set_aux_poses(dynoba_handle h, int64_t n, const double* data) {
 int dynoba_set_calibration(dynoba_handle h, const double calib[6]) {
   ARG(h, "null handle"); ARG(calib, "null calib");
   for (int i = 0; i < 6; i++) { h->calib[i] = calib[i]; h->cur.K[i] = calib[i]; h->cand.K[i] = calib[i]; }
-  h->linearized = false;
+  h->linearized = false; cov_invalidate(h);
   return DYNOBA_OK;
 }
 
@@ -1369,7 +1401,7 @@ int dynoba_retract(dynoba_handle h, const double* delta) {
   h->launches += launch_nav_retract(h->cur, h->cand, h->band, h->d_nav, h->n_nav, h->stream);
   CK(cudaStreamSynchronize(h->stream));
   std::swap(h->cur, h->cand);
-  h->linearized = false;
+  h->linearized = false; cov_invalidate(h);
   return DYNOBA_OK;
 }
 
@@ -1394,16 +1426,11 @@ int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_id
   { std::vector<int> srt = slot; std::sort(srt.begin(), srt.end()); ARG(std::adjacent_find(srt.begin(), srt.end()) == srt.end(), "a variable is listed twice"); }
   if (!h->linearized) do_linearize(h);
   // a second, plain layout whose factorisation stops before the kept block
-  BandPlan mp{}; mp.outer_weight = 0;
-  if (band_plan_layout(mp, h->band.n, h->band.bw, -1, 0, 1)) { h->err = "band layout failed"; return DYNOBA_ERR_BAD_ARG; }
-  const int p0 = 6*(int)(np - n_keep), K0 = p0/TILE, NT = mp.band.NT, WBm = mp.band.WB;
-  if (NT - K0 > WBm + 1) { h->err = "the kept block is wider than the band of the reduced system"; return DYNOBA_ERR_UNSUPPORTED; }
-  mp.chains[0].Kend = K0;
-  double* dbuf; int* ibuf; char* desc;
-  if ((rc = dalloc(h, &dbuf, mp.n_doubles, false))) return rc;
-  if ((rc = dalloc(h, &ibuf, mp.n_ints, false))) return rc;
-  if ((rc = dalloc(h, &desc, mp.n_desc_bytes))) return rc;
-  band_plan_bind(mp, dbuf, ibuf, desc, nullptr);
+  const int p0 = 6*(int)(np - n_keep), K0 = p0/TILE;
+  BandPlan mp;
+  if ((rc = plain_plan_create(h, mp, K0))) return rc;
+  const int NT = mp.band.NT, WBm = mp.band.WB;
+  if (NT - K0 > WBm + 1) { plain_plan_release(h, mp); h->err = "the kept block is wider than the band of the reduced system"; return DYNOBA_ERR_UNSUPPORTED; }
   std::swap(h->plan, mp);                               // (h->band refers to h->plan.band)
   rc = build_reduced(h, 0.0);
   if (!rc) h->launches += launch_band_factor(h->plan, h->fail, h->stream);
@@ -1418,10 +1445,7 @@ int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_id
     CK(cudaStreamSynchronize(h->stream));
   }
   std::swap(h->plan, mp);
-  for (void* q : { (void*)dbuf, (void*)ibuf, (void*)desc }) {
-    auto it = std::find_if(h->allocs.begin(), h->allocs.end(), [&](const std::pair<void*, size_t>& a) { return a.first == q; });
-    if (it != h->allocs.end()) { g_devcache.give(h->device, it->first, it->second); h->allocs.erase(it); }
-  }
+  plain_plan_release(h, mp);
   if (rc) return rc;
   if (failed) { h->err = "the eliminated block is not positive definite"; return DYNOBA_ERR_INDETERMINATE; }
   // dense symmetric copy of the trailing block: local scalar q <-> solver position K0*32 + q
@@ -1449,6 +1473,100 @@ int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_id
     g[6*a + r] = rhs[qi];
     for (int b = 0; b < n_keep; b++) for (int c = 0; c < 6; c++) G[(size_t)(6*a + r)*dim + 6*b + c] = M[(size_t)qi*m + e + 6*slot[b] + c];
   }
+  return DYNOBA_OK;
+}
+
+}  // extern "C"
+
+// Sigma = S^-1 on the band of the plain layout, S the undamped reduced system at the current values: build, factor,
+// selected inversion.  DYNOBA_TIMING=1 prints the CUDA-event times of the stages.
+static int cov_band(dynoba_solver* h) {
+  int rc;
+  if (!h->linearized) do_linearize(h);
+  if (!h->cov_live) {
+    if ((rc = plain_plan_create(h, h->cov_plan, -1))) return rc;
+    if ((rc = dalloc(h, &h->cov_stage, selinv_stage_count(h->cov_plan.band.WB), false))) { plain_plan_release(h, h->cov_plan); return rc; }
+    h->cov_live = true;
+  }
+  std::swap(h->plan, h->cov_plan);                      // (h->band refers to h->plan.band)
+  cudaEventRecord(h->ev[0], h->stream);
+  rc = build_reduced(h, 0.0);
+  cudaEventRecord(h->ev[1], h->stream);
+  if (!rc) h->launches += launch_band_factor(h->plan, h->fail, h->stream);
+  cudaEventRecord(h->ev[2], h->stream);
+  std::swap(h->plan, h->cov_plan);
+  if (rc) return rc;
+  int failed = 0;
+  CK(cudaMemcpyAsync(&failed, h->fail, 4, cudaMemcpyDeviceToHost, h->stream)); CK(cudaStreamSynchronize(h->stream));
+  if (failed) { h->err = "the reduced system is not positive definite"; return DYNOBA_ERR_INDETERMINATE; }
+  h->launches += launch_band_selinv(h->cov_plan.chains[0], h->cov_plan.band.WB, h->cov_stage, h->stream);
+  cudaEventRecord(h->ev[3], h->stream);
+  CK(cudaStreamSynchronize(h->stream)); CK(cudaGetLastError());
+  if (getenv("DYNOBA_TIMING")) {
+    float t[3]; for (int k = 0; k < 3; k++) cudaEventElapsedTime(&t[k], h->ev[k], h->ev[k + 1]);
+    std::fprintf(stderr, "[dynoba covariance] reduced system %.3f ms  factor %.3f ms  selected inversion %.3f ms  (n %d, WB %d)\n",
+                 t[0], t[1], t[2], h->cov_plan.band.n, h->cov_plan.band.WB);
+  }
+  h->cov_ready = true;
+  return DYNOBA_OK;
+}
+// covariances of every point ([npt][9]) and flow ([nfl][4]) in device order, from Sigma on the band.  A landmark that no
+// factor touches keeps NaN.
+static int cov_landmarks(dynoba_solver* h) {
+  int rc;
+  const int64_t npt = h->cur.nl, nfl = h->cur.nf;
+  if (!h->cov_lmk && (rc = dalloc(h, &h->cov_lmk, (size_t)9*npt + 4*nfl, false))) return rc;
+  CK(cudaMemsetAsync(h->cov_lmk, 0xff, ((size_t)9*npt + 4*nfl)*8, h->stream));    // all-ones bits: NaN
+  CK(cudaMemsetAsync(h->fail, 0, 4, h->stream));
+  const BandProb& ch = h->cov_plan.chains[0];
+  cudaEventRecord(h->ev[0], h->stream);
+  for (auto& b : h->blocks) if (!b.pose_only) h->launches += launch_cov_simple(b.dev, ch.tiles, ch.TPC, h->cov_lmk, h->cov_lmk + 9*npt, h->fail, h->stream);
+  h->launches += launch_cov_general(h->gen, ch.tiles, ch.TPC, h->cov_lmk, h->fail, h->stream);
+  cudaEventRecord(h->ev[1], h->stream);
+  int failed = 0;
+  CK(cudaMemcpyAsync(&failed, h->fail, 4, cudaMemcpyDeviceToHost, h->stream)); CK(cudaStreamSynchronize(h->stream)); CK(cudaGetLastError());
+  if (getenv("DYNOBA_TIMING")) { float t; cudaEventElapsedTime(&t, h->ev[0], h->ev[1]); std::fprintf(stderr, "[dynoba covariance] landmarks %.3f ms (%lld points, %lld flows)\n", t, (long long)npt, (long long)nfl); }
+  if (failed) { h->err = "a landmark's information block is not positive definite"; return DYNOBA_ERR_INDETERMINATE; }
+  h->cov_lmk_ready = true;
+  return DYNOBA_OK;
+}
+
+extern "C" {
+
+int dynoba_marginal_covariance(dynoba_handle h, int kind, int64_t n, const int32_t* idx, double* cov) {
+  int rc = check_ready(h, true); if (rc) return rc;
+  if (h->world > 1) { h->err = "dynoba_marginal_covariance is a single-GPU entry point"; return DYNOBA_ERR_UNSUPPORTED; }
+  const std::vector<double>* store = var_store(h, kind);
+  ARG(store, "bad variable kind");
+  const int64_t nk = (int64_t)store->size()/kind_width(kind);
+  ARG(idx ? n >= 0 : n == nk, "idx == NULL asks for every variable of the kind: n must be their number");
+  ARG(n == 0 || cov, "null cov");
+  for (int64_t i = 0; idx && i < n; i++) ARG(idx[i] >= 0 && idx[i] < nk, "variable out of range");
+  if (n == 0) return DYNOBA_OK;
+  if (!h->cov_ready && (rc = cov_band(h))) return rc;
+  const bool poselike = kind == DYNOBA_POSE6 || kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6;
+  if (!poselike && !h->cov_lmk_ready && (rc = cov_landmarks(h))) return rc;
+  const int d = kind == DYNOBA_POSE6 || kind == DYNOBA_BIAS6 ? 6 : (kind == DYNOBA_FLOW2 ? 2 : 3);
+  // caller order -> scalar position of the block (pose-like) / device landmark index
+  std::vector<int32_t> at(n);
+  const int64_t np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3;
+  const int64_t base = kind == DYNOBA_VEL3 ? np : (kind == DYNOBA_BIAS6 ? np + nv : 0);
+  for (int64_t i = 0; i < n; i++) {
+    const int64_t v = idx ? idx[i] : i;
+    at[i] = poselike ? 6*h->pos[base + v] : (kind == DYNOBA_POINT3 ? h->pt_new[v] : h->fl_new[v]);
+  }
+  int* dat; double* dout;
+  if ((rc = dalloc(h, &dat, (size_t)n, false))) return rc;
+  if ((rc = dalloc(h, &dout, (size_t)n*d*d, false))) { release(h, dat); return rc; }
+  CK(cudaMemcpyAsync(dat, at.data(), (size_t)n*4, cudaMemcpyHostToDevice, h->stream));
+  const BandProb& ch = h->cov_plan.chains[0];
+  if (poselike) h->launches += launch_cov_pose_gather(ch.tiles, ch.TPC, dat, (int)n, d, dout, h->stream);
+  else h->launches += launch_cov_rows_gather(h->cov_lmk + (kind == DYNOBA_FLOW2 ? 9*h->cur.nl : 0), dat, (int)n, d*d, dout, h->stream);
+  CK(cudaMemcpyAsync(cov, dout, (size_t)n*d*d*8, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  release(h, dat); release(h, dout);
+  for (int64_t e = 0; e < n*d*d; e++)
+    if (std::isnan(cov[e])) { h->err = "a requested landmark is not touched by any factor"; return DYNOBA_ERR_INDETERMINATE; }
   return DYNOBA_OK;
 }
 
@@ -1538,6 +1656,7 @@ int dynoba_optimize(dynoba_handle h, const dynoba_lm_params* prm, dynoba_lm_stat
   S.iterations = iterations; S.inner_iterations = inner; S.error_final = err; S.lambda_final = lambda;
   S.kernel_launches = h->launches - launches0;
   if (st) *st = S;
+  if (iterations) cov_invalidate(h);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return DYNOBA_ERR_CUDA; }
   return DYNOBA_OK;

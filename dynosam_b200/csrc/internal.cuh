@@ -290,6 +290,15 @@ int launch_pose_delta_norm(const DevBand& B, double lambda, double* partials, cu
 int pose_norm_grid(int n);
 int launch_retract(const DevVars& cur, const DevVars& cand, const DevBand& B, const double* dl_point,
                    const double* dl_flow, cudaStream_t s);
+// ---- marginal covariances (kernels_cov.cu; general groups: kernels_chain.cu).  P is the plain chain (ncell == 0) after
+// launch_band_factor; stage holds selinv_stage_count(WB) doubles.  Sigma is left in P's tiles; the landmark tables are
+// [landmarks][DL*DL] in device order
+size_t selinv_stage_count(int WB);
+int launch_band_selinv(const BandProb& P, int WB, double* stage, cudaStream_t s);
+int launch_cov_pose_gather(const double* tiles, int TPC, const int* spos, int n, int d, double* out, cudaStream_t s);
+int launch_cov_rows_gather(const double* src, const int* rows, int n, int w, double* out, cudaStream_t s);
+int launch_cov_simple(const DevBlock& blk, const double* sig, int TPC, double* out_point, double* out_flow, int* fail, cudaStream_t s);
+int launch_cov_general(const GeneralGroups& G, const double* sig, int TPC, double* out_point, int* fail, cudaStream_t s);
 // ---- navigation variables and visual-inertial factors (kernels_imu.cu).  nav[i] = (solver position, dimension) of every
 // velocity (3) and bias (6).
 int nav_grid(int type, int n);      // partial sums a linearize / error launch of a navigation factor block writes

@@ -5,7 +5,7 @@
 // (SURVEY.md section 7 "hard parts"); with at most 21 points per tracklet it is handled densely:
 // one warp per group builds V (<= 63x63) in shared memory, inverts it through its Cholesky factor and scatters
 //   S += A_f^T (delta_ff' I - B_f Vinv[lm(f), lm(f')] B_f'^T) A_f'   over the group's factor pairs.
-#include "internal.cuh"
+#include "landmark.cuh"
 
 namespace dynoba {
 
@@ -235,7 +235,75 @@ backsub_general_kernel(const DevBlock* __restrict__ blocks, const int* __restric
   if (threadIdx.x == 0) partials[blockIdx.x] = sh[0] + sh[1];
 }
 
+// Marginal covariances of a general group's points (dynoba_marginal_covariance; here because it shares
+// group_inverse): with V^-1 the group's dense undamped inverse and Y = W^T Sigma_cc W summed over the pairs of
+// (factor, pose slot) terms, Sigma_points = V^-1 + V^-1 Y V^-1, of which each point's 3x3 diagonal block is kept.
+__global__ void __launch_bounds__(64)
+cov_general_kernel(const DevBlock* __restrict__ blocks, const int* __restrict__ gptr, const FRef* __restrict__ refs,
+                   const int* __restrict__ gl0, const int* __restrict__ gnl, int n_groups, const double* __restrict__ sig,
+                   int TPC, double* __restrict__ out, int* __restrict__ fail) {
+  extern __shared__ double sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = blockIdx.x*2 + warp;
+  if (g >= n_groups) return;
+  double* V = sm + (size_t)warp*(2*GG_N*GG_LD + 2*GG_N);
+  double* W = V + GG_N*GG_LD; double* gl = W + GG_N*GG_LD;
+  const int f0 = gptr[g], nf = gptr[g+1] - f0, l0 = gl0[g], nl = gnl[g], n = 3*nl;
+  const FRef* rf = refs + f0;
+  if (!group_inverse(blocks, rf, nf, l0, n, 0.0, V, gl, W, lane)) { if (lane == 0) atomicOr(fail, 1); return; }
+  double* Y = W;
+  for (int i = lane; i < n*GG_LD; i += 32) Y[i] = 0.0;
+  __syncwarp();
+  for (int p = lane; p < nf*nf; p += 32) {
+    const FView a = make_view(blocks, rf[p/nf]), b = make_view(blocks, rf[p%nf]);
+    for (int s1 = 0; s1 < a.np; s1++) for (int s2 = 0; s2 < b.np; s2++) {
+      const int pa = 6*a.pose(s1), pb = 6*b.pose(s2);
+      double Sg[36];
+      for (int c = 0; c < 6; c++) for (int c2 = 0; c2 < 6; c2++) Sg[c*6 + c2] = band_sym(sig, TPC, pa + c, pb + c2);
+      for (int t1 = 0; t1 < a.nl; t1++) {
+        double G[18];                                   // (B_a,t1^T A_a,s1) Sigma(pa, pb)
+        for (int k = 0; k < 3; k++) {
+          double ca[6];
+          for (int c = 0; c < 6; c++) { double x = 0; for (int r = 0; r < 3; r++) x += a.J(r, a.lcol[t1] + k)*a.J(r, a.pcol[s1] + c); ca[c] = x; }
+          for (int c2 = 0; c2 < 6; c2++) { double x = 0; for (int c = 0; c < 6; c++) x += ca[c]*Sg[c*6 + c2]; G[k*6 + c2] = x; }
+        }
+        for (int t2 = 0; t2 < b.nl; t2++) {
+          for (int k2 = 0; k2 < 3; k2++) {
+            double cb[6];
+            for (int c = 0; c < 6; c++) { double x = 0; for (int r = 0; r < 3; r++) x += b.J(r, b.lcol[t2] + k2)*b.J(r, b.pcol[s2] + c); cb[c] = x; }
+            for (int k = 0; k < 3; k++) {
+              double x = 0; for (int c = 0; c < 6; c++) x += G[k*6 + c]*cb[c];
+              atomicAdd(Y + (3*(a.lmk(t1) - l0) + k)*GG_LD + 3*(b.lmk(t2) - l0) + k2, x);
+            }
+          }
+        }
+      }
+    }
+  }
+  __syncwarp();
+  for (int e = lane; e < 6*nl; e += 32) {               // lower entries (r >= c) of each point's block
+    const int l = e/6, q = e%6, r = q < 1 ? 0 : (q < 3 ? 1 : 2), c = q - r*(r + 1)/2;
+    const int ir = 3*l + r, ic = 3*l + c;
+    double s = V[ir*GG_LD + ic];
+    for (int i = 0; i < n; i++) {
+      double t = 0;
+      for (int k = 0; k < n; k++) t += Y[i*GG_LD + k]*V[k*GG_LD + ic];
+      s += V[ir*GG_LD + i]*t;
+    }
+    double* o = out + (size_t)(l0 + l)*9;
+    o[r*3 + c] = s; o[c*3 + r] = s;
+  }
+}
+
 static size_t gg_smem() { return (size_t)2*(2*GG_N*GG_LD + 2*GG_N)*sizeof(double); }
+
+int launch_cov_general(const GeneralGroups& G, const double* sig, int TPC, double* out_point, int* fail, cudaStream_t s) {
+  if (G.n_groups == 0) return 0;
+  static bool attr = false;
+  if (!attr) { cudaFuncSetAttribute(cov_general_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gg_smem()); attr = true; }
+  cov_general_kernel<<<general_grid(G.n_groups), 64, gg_smem(), s>>>(G.blocks, G.gptr, (const FRef*)G.refs, G.gl0, G.gnl, G.n_groups, sig, TPC, out_point, fail);
+  return 1;
+}
 
 int general_grid(int n_groups) { return (n_groups + 1)/2; }
 

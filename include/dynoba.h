@@ -142,6 +142,17 @@ int dynoba_add_linear_prior(dynoba_handle h, int32_t n, const int32_t* pose_idx,
  * than the band of the reduced system (else DYNOBA_ERR_UNSUPPORTED).  Difference from the reference: it retains recent
  * LANDMARKS as well; here every landmark is eliminated into the prior.  Single GPU. */
 int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_idx, double* G, double* g);
+/* gtsam::Marginals(graph, values, Marginals::CHOLESKY).marginalCovariance(key) for many variables of one kind:
+ * the graph linearised at the current values (robust re-weighting as linearize does, no damping), H = J^T J,
+ * cov[i] = the diagonal block of H^-1 of variable idx[i] (caller order; idx == NULL: all n variables of the kind).
+ * kind POSE6: 6x6 in the tangent order [omega; v] of the solver's retraction; VEL3 3x3; BIAS6 6x6 (acc, gyro);
+ * POINT3 3x3; FLOW2 2x2.  Row-major and exactly symmetric.
+ * The selected inverse of the reduced system is computed once per linearisation point and kept until the values change
+ * (dynoba_retract, dynoba_optimize, dynoba_set_variables, dynoba_set_calibration): asking for poses and then for points
+ * factorises once.  The LM state is untouched.
+ * DYNOBA_ERR_INDETERMINATE where H is not positive definite (GTSAM throws IndeterminantLinearSystemException), also for
+ * a requested landmark no factor touches; single GPU (world > 1: DYNOBA_ERR_UNSUPPORTED). */
+int dynoba_marginal_covariance(dynoba_handle h, int kind, int64_t n, const int32_t* idx, double* cov);
 /* Optional elimination-order hint for pose-like variables (e.g. the frame id encoded in the key):
  * variables are ordered by (rank, index).  Without it the given order is used. */
 int dynoba_set_pose_order(dynoba_handle h, int64_t n, const int32_t* rank);
