@@ -3,7 +3,8 @@
 // Replaces GTSAM's multifrontal Cholesky on the COLAMD ordering (SURVEY.md 8a row a11, [GTSAM-ext]) for the
 // reduced system that is left after the landmarks are eliminated.  With pose-like variables ordered by frame
 // the system is banded (half-width = the co-visibility window, <= max track age), stored as 32x32 tiles.
-// Hopper's wgmma has no fp64 shape: tile updates run on mma.sync.m8n8k4.f64 (DMMA), triangular work on fp64 FMAs.
+// Hopper's wgmma has no fp64 shape: tile updates run on mma.sync (DMMA; m16n8k16 in the worker pools, m8n8k4 in the
+// spine), triangular work on fp64 FMAs.
 //
 // A band Cholesky is one long dependency chain (potrf(K,K) -> trsm -> update -> potrf(K+1,K+1)), so the time axis is
 // cut into CELLS (nested dissection in time; internal.cuh, tools/cell_proto.py): every cell is two chains that are
@@ -31,7 +32,7 @@ namespace cg = cooperative_groups;
 
 namespace dynoba {
 
-constexpr int TS = 40, TSZ = TILE*TS;      // column stride of shared-memory tiles that feed MMA operand fragments: conflict-free loads
+constexpr int TS = 40, TSZ = TILE*TS;      // column stride of the spine's shared-memory tiles that feed m8n8k4 operand fragments
 constexpr int FF_CH = 16;                  // columns per FF accumulation task
 constexpr int MAX_PROBS = 2*MAX_CELLS;
 
@@ -76,22 +77,6 @@ __device__ __forceinline__ void tile_stage(double* s, const double (&r)[TILE], i
   __syncwarp();
 }
 
-// asynchronous copy of one 32x32 tile (column-major, 8 KB) into a shared-memory tile with column stride TS
-__device__ __forceinline__ void tile_prefetch(double* s, const double* t, int lane) {
-#pragma unroll
-  for (int i = 0; i < 16; i++) {
-    const int ch = lane + 32*i, c = ch >> 4, part = ch & 15;
-    const unsigned dst = (unsigned)__cvta_generic_to_shared(s + c*TS + 2*part);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(dst), "l"(t + c*TILE + 2*part) : "memory");
-  }
-}
-__device__ __forceinline__ void sfrag_load(const double* t, double (&f)[TILE], int lane) {
-  const double* p = t + (lane & 3)*TS + (lane >> 2);
-#pragma unroll
-  for (int b = 0; b < 4; b++)
-#pragma unroll
-    for (int kb = 0; kb < 8; kb++) f[b*8 + kb] = p[4*kb*TS + 8*b];
-}
 // both flags set?  (non-blocking, acquire)
 __device__ __forceinline__ bool flags_ready(const int* fa, const int* fb, int lane) {
   int ok = 0;
@@ -111,9 +96,9 @@ __device__ __forceinline__ int* flag_ydone(const BandProb& P) { return P.flags +
 __device__ __forceinline__ int* flag_ffcnt(const BandProb& P) { return P.flags + (size_t)2*P.NT*P.TPC + P.NT; }
 
 // acc -= sum_{J = Jlo..Jhi} A_J B_J^T  with A_J = tile (J, A0 - A1*J), B_J = tile (J, B0 - B1*J) of problem P (same: A == B);
-// waits for the operand tiles' done flags.  stage: per-warp [2][2][TSZ] shared-memory operand buffers -- while update J
-// runs on the tensor pipe, the operand tiles of J+1 (when their flags are already up) stream into the other stage with
-// cp.async, so the L2 latency leaves the critical path.
+// waits for the operand tiles' done flags.  stage: per-warp [2][2][TILE2] swizzled shared-memory operand stages (band_tile.cuh)
+// -- while update J runs on the tensor pipe, the operand tiles of J+1 (when their flags are already up) stream into the
+// other stage with cp.async, so the L2 latency leaves the critical path.  Updates are m16n8k16 (frag16_gemm_sub).
 __device__ __forceinline__ void accumulate_updates(const BandProb& P, double (&acc)[TILE], int Jlo, int Jhi, int A0, int A1, int B0, int B1,
                                                    bool same, double* stage, int lane) {
   const int* done = flag_done(P);
@@ -124,8 +109,8 @@ __device__ __forceinline__ void accumulate_updates(const BandProb& P, double (&a
     if (!have) {
       wait_flag(done + oB, lane);
       if (!same) wait_flag(done + oA, lane);
-      tile_prefetch(stage + (size_t)(st*2 + 1)*TSZ, P.tiles + oB*TILE2, lane);
-      if (!same) tile_prefetch(stage + (size_t)(st*2)*TSZ, P.tiles + oA*TILE2, lane);
+      stage16_prefetch<32>(stage + (size_t)(st*2 + 1)*TILE2, P.tiles + oB*TILE2, lane);
+      if (!same) stage16_prefetch<32>(stage + (size_t)(st*2)*TILE2, P.tiles + oA*TILE2, lane);
       asm volatile("cp.async.commit_group;" ::: "memory");
     }
     bool next = false;
@@ -133,21 +118,15 @@ __device__ __forceinline__ void accumulate_updates(const BandProb& P, double (&a
       const size_t nA = (size_t)(J + 1)*TPC + (A0 - A1*(J + 1)), nB = (size_t)(J + 1)*TPC + (B0 - B1*(J + 1));
       next = flags_ready(done + nB, done + (same ? nB : nA), lane);
       if (next) {
-        tile_prefetch(stage + (size_t)((st ^ 1)*2 + 1)*TSZ, P.tiles + nB*TILE2, lane);
-        if (!same) tile_prefetch(stage + (size_t)((st ^ 1)*2)*TSZ, P.tiles + nA*TILE2, lane);
+        stage16_prefetch<32>(stage + (size_t)((st ^ 1)*2 + 1)*TILE2, P.tiles + nB*TILE2, lane);
+        if (!same) stage16_prefetch<32>(stage + (size_t)((st ^ 1)*2)*TILE2, P.tiles + nA*TILE2, lane);
         asm volatile("cp.async.commit_group;" ::: "memory");
       }
     }
     if (next) asm volatile("cp.async.wait_group 1;" ::: "memory"); else asm volatile("cp.async.wait_group 0;" ::: "memory");
     __syncwarp();
-    double fb[TILE];
-    sfrag_load(stage + (size_t)(st*2 + 1)*TSZ, fb, lane);
-    if (same) frag_gemm_sub(acc, fb, fb);
-    else {
-      double fa[TILE];
-      sfrag_load(stage + (size_t)(st*2)*TSZ, fa, lane);
-      frag_gemm_sub(acc, fa, fb);
-    }
+    const double* sb = stage + (size_t)(st*2 + 1)*TILE2;
+    stage16_gemm_sub(acc, same ? sb : stage + (size_t)(st*2)*TILE2, sb, lane);
     __syncwarp();            // the stage is free for the prefetch after next
     st ^= 1; have = next;
   }
@@ -163,9 +142,9 @@ __device__ __forceinline__ void accumulate_updates(const BandProb& P, double (&a
 // near the diagonal need more lead than the short tasks far from it.  Every operand of a task has a strictly smaller s,
 // so in-order blocking cannot deadlock (all CTAs are co-resident: cooperative launch).
 __device__ __forceinline__ void tile_finish_trsm(const BandProb& P, double (&acc)[TILE], int K, double* tp, int* doneflag, double* sb, double* sinv, int lane) {
-  // accumulator fragments -> one row per lane, through the warp's shared-memory tile
+  // accumulator fragments (m16n8k16 C map) -> one row per lane, through the warp's shared-memory tile
   __syncwarp();
-  cfrag_store(sb, acc, lane);
+  cfrag16_store(sb, acc, lane);
   __syncwarp();
 #pragma unroll
   for (int cc = 0; cc < TILE; cc++) acc[cc] = sb[cc*TILE + lane];
@@ -235,13 +214,13 @@ __device__ __forceinline__ void band_worker(const CholJob& job, int wid, int nwo
     double acc[TILE];                       // accumulator fragments while the updates run, one row per lane afterwards
     const size_t o = (size_t)K*TPC + dd;
     double* tp = P.tiles + o*TILE2;
-    cfrag_load(tp, acc, lane);
+    cfrag16_load(tp, acc, lane);
     // the spine finishes the tiles of columns <= Kend itself: it owns the last two updates of a diagonal tile and the last
     // update of a first sub-diagonal tile
     const int Jhi = min(dd == 0 ? (K <= P.Kend ? K - 3 : K - 1) : (dd == 1 ? K - 2 : K - 1), P.Kend - 1);
     accumulate_updates(P, acc, max(0, I - WB), Jhi, I, 1, K, 1, dd == 0, stage, lane);
     if (dd <= 2 || K >= P.Kend) {
-      cfrag_store(tp, acc, lane);
+      cfrag16_store(tp, acc, lane);
       set_flag(pre + o, lane);
     } else tile_finish_trsm(P, acc, K, tp, done + o, sb, sinv, lane);
   }
@@ -259,16 +238,19 @@ __device__ __forceinline__ void band_worker(const CholJob& job, int wid, int nwo
 // done(Z_r(J)) implies the earlier tiles of row r, so the bulk of a task (all steps but the last) runs as soon as the
 // operands of the step before the last exist, and the row chain Z_r(K-1) -> Z_r(K) only carries one update + the TRSM.
 // Operands come from pool A / the spine (which never wait on pool B) or from earlier tasks of this order: no deadlock.
+// Steps are m16n8k16 updates (frag16_gemm_sub) out of a three-stage ring of swizzled stages (band_tile.cuh): the loads
+// of step J+2 go into the stage step J-1 read, so the one barrier per step that publishes step J's stage also frees it.
 constexpr int SPK_ROWS = 8;
+constexpr int SPK_STAGES = 3;
 __device__ __forceinline__ void spike_cta_worker(const CholJob& job, int cw, int ncw, double* smem) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int WB = job.WB, W1 = WB + 1;
   const int G = (WB + SPK_ROWS - 1)/SPK_ROWS;
   int NGF = 0; for (int r2 = 0; r2 < WB; r2++) NGF += (WB - r2 + SPK_ROWS - 1)/SPK_ROWS;
   const int R = G + NGF;
-  double* sB = smem;                                  // [2][TSZ] shared B operand (also L_KK for the TRSM)
-  double* sA = smem + 2*TSZ + (size_t)warp*2*TSZ;     // [2][TSZ] this warp's A operand (also its layout-conversion scratch)
-  double* sinv = smem + 2*TSZ + (size_t)SPK_ROWS*2*TSZ;   // [32]
+  double* sB = smem;                                                  // [3][TILE2] shared B operand (also L_KK for the TRSM)
+  double* sA = smem + (size_t)(1 + warp)*SPK_STAGES*TILE2;            // [3][TILE2] this warp's A operand (also its layout-conversion scratch)
+  double* sinv = smem + (size_t)(1 + SPK_ROWS)*SPK_STAGES*TILE2;      // [32]
   const long long per_col = (long long)job.np*R;
   const long long ntasks = (long long)job.ncols*per_col;
   for (long long t = cw; t < ntasks; t += ncw) {
@@ -297,7 +279,7 @@ __device__ __forceinline__ void spike_cta_worker(const CholJob& job, int cw, int
     double acc[TILE];
     if (mine) {
       if (ff) wait_flag_ge(flag_ffcnt(P) + r*WB + r2, chunk, lane);
-      cfrag_load(tp, acc, lane);
+      cfrag16_load(tp, acc, lane);
     }
     if (Jhi >= Jlo) {
       // ---- operand flags.  FF: everything exists once the chunk's last column does.  Spike: the flags form monotone
@@ -322,43 +304,31 @@ __device__ __forceinline__ void spike_cta_worker(const CholJob& job, int cw, int
         if (J > frontB) { wait_flag(done + (size_t)J*TPC + (K - J), lane); frontB = J; }
       };
       auto stage_loads = [&](int J, int st) {
-        const double* b = P.tiles + ((size_t)J*TPC + (Bslot0 - Bslot1*J))*TILE2;
-        double* dst = sB + (size_t)st*TSZ;
-#pragma unroll
-        for (int i = 0; i < 2; i++) {
-          const int ch = threadIdx.x + 256*i, c = ch >> 4, part = ch & 15;
-          const unsigned d = (unsigned)__cvta_generic_to_shared(dst + c*TS + 2*part);
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(d), "l"(b + c*TILE + 2*part) : "memory");
-        }
-        if (mine) tile_prefetch(sA + (size_t)st*TSZ, P.tiles + ((size_t)J*TPC + W1 + r)*TILE2, lane);
+        need(J);
+        stage16_prefetch<256>(sB + (size_t)st*TILE2, P.tiles + ((size_t)J*TPC + (Bslot0 - Bslot1*J))*TILE2, threadIdx.x);
+        if (mine) stage16_prefetch<32>(sA + (size_t)st*TILE2, P.tiles + ((size_t)J*TPC + W1 + r)*TILE2, lane);
         asm volatile("cp.async.commit_group;" ::: "memory");
       };
-      int st = 0;
-      need(Jlo);
       stage_loads(Jlo, 0);
-      for (int J = Jlo; J <= Jhi; J++) {
-        if (J + 1 <= Jhi) {
-          need(J + 1);
-          stage_loads(J + 1, st ^ 1);
-          asm volatile("cp.async.wait_group 1;" ::: "memory");
-        } else asm volatile("cp.async.wait_group 0;" ::: "memory");
-        __syncthreads();
+      if (Jlo + 1 <= Jhi) stage_loads(Jlo + 1, 1);
+      for (int J = Jlo, st = 0; J <= Jhi; J++, st = st == SPK_STAGES - 1 ? 0 : st + 1) {
+        if (J + 1 <= Jhi) asm volatile("cp.async.wait_group 1;" ::: "memory");
+        else asm volatile("cp.async.wait_group 0;" ::: "memory");
+        __syncthreads();                               // stage st is complete for every warp, and every warp is done with step J-1
+        if (J + 2 <= Jhi) stage_loads(J + 2, st == 0 ? SPK_STAGES - 1 : st - 1);   // ... so step J-1's stage takes step J+2
         if (mine) {
-          double fb[TILE], fa[TILE];
-          sfrag_load(sB + (size_t)st*TSZ, fb, lane);
-          if (ff && r == r2) frag_gemm_sub(acc, fb, fb);
-          else { sfrag_load(sA + (size_t)st*TSZ, fa, lane); frag_gemm_sub(acc, fa, fb); }
+          const double* sb = sB + (size_t)st*TILE2;
+          stage16_gemm_sub(acc, ff && r == r2 ? sb : sA + (size_t)st*TILE2, sb, lane);
         }
-        __syncthreads();                               // the stage is free for the loads of the step after next
-        st ^= 1;
       }
+      __syncthreads();                                 // the ring is free for the next task
     }
     if (ff) {
-      if (mine) { cfrag_store(tp, acc, lane); set_flag_value(flag_ffcnt(P) + r*WB + r2, chunk + 1, lane); }
+      if (mine) { cfrag16_store(tp, acc, lane); set_flag_value(flag_ffcnt(P) + r*WB + r2, chunk + 1, lane); }
       continue;
     }
     if (K >= P.Kend) {                                 // spike tile of a separator column: its Schur complement, final
-      if (mine) { cfrag_store(tp, acc, lane); set_flag(flag_done(P) + (size_t)K*TPC + W1 + r, lane); }
+      if (mine) { cfrag16_store(tp, acc, lane); set_flag(flag_done(P) + (size_t)K*TPC + W1 + r, lane); }
       continue;
     }
     // ---- TRSM against L_KK (staged once for the CTA, column-major with stride TILE in the B buffer)
@@ -370,7 +340,7 @@ __device__ __forceinline__ void spike_cta_worker(const CholJob& job, int cw, int
     __syncthreads();
     if (mine) {
       __syncwarp();
-      cfrag_store(sA, acc, lane);                      // accumulator fragments -> one row per lane
+      cfrag16_store(sA, acc, lane);                    // accumulator fragments -> one row per lane
       __syncwarp();
 #pragma unroll
       for (int cc = 0; cc < TILE; cc++) acc[cc] = sA[cc*TILE + lane];
@@ -529,10 +499,12 @@ __device__ __forceinline__ void spine_trsm(double (&x)[TILE], int lane, const do
     }
   }
 }
-// Rank-32 update of an accumulator tile held as MMA fragments (see frag_gemm_sub): c -= XA XB^T, XA / XB k-major tiles in
+// Rank-32 update of an accumulator tile held as MMA fragments (see frag8_gemm_sub): c -= XA XB^T, XA / XB k-major tiles in
 // shared memory with column stride TS, applied in four rank-8 steps (two k-steps of the m8n8k4 MMA each) as the panels
 // of XB appear (ev_base >= 0: wait for event ev_base + p first).  16 LDS.64 + 32 DMMA per step: next to nothing on the
 // shared-memory pipe, which the FMA formulation (one LDS.128 per two FMAs) saturates when several spine warps run it.
+// This stays on m8n8k4 while the worker pools use m16n8k16: a k = 16 step needs two TRSM panels of XB, so it would wait
+// for the second one, and the step after the last panel -- the one on the chain's critical path -- would be twice as long.
 __device__ __forceinline__ void spine_rank32(double (&c)[TILE], const double* xa, const double* xb, bool same,
                                              volatile int* ev, int ev_base, int cval, int lane) {
   const int off = (lane & 3)*TS + (lane >> 2);
@@ -550,13 +522,13 @@ __device__ __forceinline__ void spine_rank32(double (&c)[TILE], const double* xa
 #pragma unroll
       for (int rb = 0; rb < 4; rb++)
 #pragma unroll
-        for (int cb = 0; cb < 4; cb++) dmma(c[(rb*4 + cb)*2], c[(rb*4 + cb)*2 + 1], fa[rb], fb[cb]);
+        for (int cb = 0; cb < 4; cb++) dmma8(c[(rb*4 + cb)*2], c[(rb*4 + cb)*2 + 1], fa[rb], fb[cb]);
     }
   }
 }
-// accumulator fragments <-> shared-memory tile with column stride S
+// m8n8k4 accumulator fragments <-> shared-memory tile with column stride S
 template <int S>
-__device__ __forceinline__ void cfrag_load_s(const double* t, double (&c)[TILE], int lane) {
+__device__ __forceinline__ void cfrag8_load_s(const double* t, double (&c)[TILE], int lane) {
   const double* p = t + 2*(lane & 3)*S + (lane >> 2);
 #pragma unroll
   for (int rb = 0; rb < 4; rb++)
@@ -564,7 +536,7 @@ __device__ __forceinline__ void cfrag_load_s(const double* t, double (&c)[TILE],
     for (int cb = 0; cb < 4; cb++) { c[(rb*4 + cb)*2] = p[8*cb*S + 8*rb]; c[(rb*4 + cb)*2 + 1] = p[(8*cb + 1)*S + 8*rb]; }
 }
 template <int S>
-__device__ __forceinline__ void cfrag_store_s(double* t, const double (&c)[TILE], int lane) {
+__device__ __forceinline__ void cfrag8_store_s(double* t, const double (&c)[TILE], int lane) {
   double* p = t + 2*(lane & 3)*S + (lane >> 2);
 #pragma unroll
   for (int rb = 0; rb < 4; rb++)
@@ -574,7 +546,7 @@ __device__ __forceinline__ void cfrag_store_s(double* t, const double (&c)[TILE]
 // accumulator fragments -> one row per lane through a private shared-memory tile
 __device__ __forceinline__ void cfrag_to_rows(double (&r)[TILE], double* scr, int lane) {
   __syncwarp();
-  cfrag_store_s<TILE>(scr, r, lane);
+  cfrag8_store_s<TILE>(scr, r, lane);
   __syncwarp();
 #pragma unroll
   for (int col = 0; col < TILE; col++) r[col] = scr[col*TILE + lane];
@@ -593,9 +565,9 @@ band_cholesky_dataflow_kernel_v3(CholJob job, int* __restrict__ fail) {
       if (job.profile && threadIdx.x == 0) atomicMax(&g_prof[33], gtimer());
       return;
     }
-    if (warp >= 4) return;       // four band worker warps per CTA (one per scheduler): [warp][2 stages][2 tiles][TSZ] | [TILE2] | [TILE]
-    double* base = chol_smem + (size_t)warp*(4*TSZ + TILE2 + TILE);
-    band_worker(job, w*4 + warp, job.band_ctas*4, base + 4*TSZ, base + 4*TSZ + TILE2, base, lane);
+    if (warp >= 4) return;       // four band worker warps per CTA (one per scheduler): [warp][2 stages][2 tiles][TILE2] | [TILE2] | [TILE]
+    double* base = chol_smem + (size_t)warp*(5*TILE2 + TILE);
+    band_worker(job, w*4 + warp, job.band_ctas*4, base + 4*TILE2, base + 5*TILE2, base, lane);
     if (job.profile && lane == 0) atomicMax(&g_prof[32], gtimer());
     return;
   }
@@ -624,7 +596,7 @@ band_cholesky_dataflow_kernel_v3(CholJob job, int* __restrict__ fail) {
         if (!spine_potrf(r, lane, sPan + (c & 1)*4*PANSZ, sIv + (c & 1)*TILE, ev, c + 1) && lane == 0) atomicOr(fail, 2);
       } else if (((c + 1) & 1) == i && c + 1 < NT) {
         ev_wait(ev, EV_DIN, c + 2, lane);
-        cfrag_load_s<TS>(sDin + ((c + 1) & 1)*TSZ, r, lane);      // r: accumulator fragments until cfrag_to_rows
+        cfrag8_load_s<TS>(sDin + ((c + 1) & 1)*TSZ, r, lane);      // r: accumulator fragments until cfrag_to_rows
         ev_signal(ev, EV_TK_D, c + 2, lane);
         // term 0: X2(c-1) = L(c+1, c-1), staged two columns ago and still in its buffer; term 1: X1(c), panel by panel
 #pragma unroll 1
@@ -649,7 +621,7 @@ band_cholesky_dataflow_kernel_v3(CholJob job, int* __restrict__ fail) {
         }
       } else if (((c + 1) & 1) == i && c + 2 < NT) {
         ev_wait(ev, EV_XNIN, c + 2, lane);
-        cfrag_load_s<TS>(sXnin + ((c + 1) & 1)*TSZ, r, lane);
+        cfrag8_load_s<TS>(sXnin + ((c + 1) & 1)*TSZ, r, lane);
         ev_signal(ev, EV_TK_XN, c + 2, lane);
         if (x2 && c >= 0) {
           ev_wait(ev, EV_X2, c + 1, lane);
@@ -1085,7 +1057,7 @@ static void chol_init() {
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   // one CTA per SM: every spine CTA is alone on its SM
-  const size_t need = std::max((size_t)(2*4*PANSZ + 2*TILE + 8*TSZ + 4*TILE2 + 64), std::max((size_t)4*(4*TSZ + TILE2 + TILE), (size_t)(2 + 2*SPK_ROWS)*TSZ + TILE))*sizeof(double);   // spine | band workers with prefetch stages | spike CTA
+  const size_t need = std::max((size_t)(2*4*PANSZ + 2*TILE + 8*TSZ + 4*TILE2 + 64), std::max((size_t)4*(5*TILE2 + TILE), (size_t)(1 + SPK_ROWS)*SPK_STAGES*TILE2 + TILE))*sizeof(double);   // spine | band workers with prefetch stages | spike CTA
   g_chol_smem = std::max(need, (size_t)(220*1024) - 2048);
   cudaFuncSetAttribute(band_cholesky_dataflow_kernel_v3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g_chol_smem);
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, band_cholesky_dataflow_kernel_v3, SP_WARPS*32, g_chol_smem);
@@ -1110,9 +1082,16 @@ static int chol_launch(const BandProb* dprobs, const BandProb* hprobs, int np, i
   if (grid > want) grid = (int)want;
   if (grid < np + 1 + (job.any_spiked ? 1 : 0)) grid = np + 1 + (job.any_spiked ? 1 : 0);
   // worker CTAs: without spikes all of them work on band tiles; else the two pools share them in proportion to their work
-  // (relative work per column 330 : 730, band tiles : spike + FF updates, timed on B200 and not re-timed on H100), pool A
-  // never below what keeps a chain
-  // at the spine's pace (~22 CTAs per chain)
+  // (relative work per column 330 : 730, band tiles : spike + FF updates), pool A never below what keeps a chain at the
+  // spine's pace (~22 CTAs per chain).  Re-timed on H100 80GB HBM3 (700 W) with the m16n8k16 workers, C5 (WB 30, two
+  // cells: plain chains of 4568 columns, spiked ones of 1016; 128 worker CTAs), tools/band_bench.py sweeping
+  // band_ctas_per_chain -- pool A CTAs: plain spines done / pool B done / ms_factor per damped solve:
+  //    84: 43.3 / 32.1 / 58.3 ms    88: 41.5 / 34.4 / 56.3    91 (these weights): 38.2 / 39.1 / 53.9
+  //    92: 39.7 / 36.8 / 54.6      100: 36.9 / 46.5 / 61.3   104: 35.9 / 53.8 / 68.6    116: 34.2 / 99.0 / 114.0
+  // The weights put the split where the plain chains and pool B finish together, so they stand.  Below ~21 CTAs per chain
+  // the plain chains lose the spine's pace (64 CTAs: 19.9 us per column, 91: 8.4).  Splits whose pool-A warp count is a
+  // multiple of the tasks per wavefront step (np * ceil((WB + 2) / skew) = 64 here: 80 or 96 CTAs) are much slower
+  // (96: plain 61.2 ms): every warp then always draws the same task slot.
   const int workers = grid - np;
   if (!job.any_spiked) job.band_ctas = workers;
   else {

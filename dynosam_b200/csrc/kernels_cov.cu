@@ -27,23 +27,23 @@ namespace dynoba {
 constexpr int SEL_WARPS = 4;
 constexpr int COV_WARPS = 4;
 
-// operand fragments (band_tile.cuh maps) of a column-major tile's TRANSPOSE, from global memory; of a tile / of its
+// m8n8k4 operand fragments (band_tile.cuh, frag8 maps) of a column-major tile's TRANSPOSE, from global memory; of a tile / of its
 // transpose staged in shared memory
-__device__ __forceinline__ void frag_load_t(const double* t, double (&f)[TILE], int lane) {
+__device__ __forceinline__ void frag8_load_t(const double* t, double (&f)[TILE], int lane) {
   const double* p = t + (lane >> 2)*TILE + (lane & 3);
 #pragma unroll
   for (int b = 0; b < 4; b++)
 #pragma unroll
     for (int kb = 0; kb < 8; kb++) f[b*8 + kb] = __ldcg(p + 8*b*TILE + 4*kb);
 }
-__device__ __forceinline__ void frag_load_s(const double* t, double (&f)[TILE], int lane) {
+__device__ __forceinline__ void frag8_load_s(const double* t, double (&f)[TILE], int lane) {
   const double* p = t + (lane & 3)*TILE + (lane >> 2);
 #pragma unroll
   for (int b = 0; b < 4; b++)
 #pragma unroll
     for (int kb = 0; kb < 8; kb++) f[b*8 + kb] = p[4*kb*TILE + 8*b];
 }
-__device__ __forceinline__ void frag_load_ts(const double* t, double (&f)[TILE], int lane) {
+__device__ __forceinline__ void frag8_load_ts(const double* t, double (&f)[TILE], int lane) {
   const double* p = t + (lane >> 2)*TILE + (lane & 3);
 #pragma unroll
   for (int b = 0; b < 4; b++)
@@ -70,29 +70,29 @@ __device__ __forceinline__ void selinv_x(const SelJob& j, int K, int dd, double*
   for (int e = 0; e < TILE; e++) acc[e] = 0.0;
   for (int J = Jhi; J > K; J--) {        // acc -= Sigma(I, J) L(J, K)
     double a[TILE], b[TILE];
-    if (I >= J) { wait_flag(sel_done(j, J, I - J), lane); frag_load(sel_tile(j, J, I - J), a, lane); }
-    else { wait_flag(sel_done(j, I, J - I), lane); frag_load_t(sel_tile(j, I, J - I), a, lane); }
-    frag_load_t(sel_tile(j, K, J - K), b, lane);
-    frag_gemm_sub(acc, a, b);
+    if (I >= J) { wait_flag(sel_done(j, J, I - J), lane); frag8_load(sel_tile(j, J, I - J), a, lane); }
+    else { wait_flag(sel_done(j, I, J - I), lane); frag8_load_t(sel_tile(j, I, J - I), a, lane); }
+    frag8_load_t(sel_tile(j, K, J - K), b, lane);
+    frag8_gemm_sub(acc, a, b);
   }
   const double* linv = j.linv + (size_t)K*TILE2;
   double a[TILE], b[TILE], c[TILE];
-  __syncwarp(); cfrag_store(sm, acc, lane); __syncwarp();
-  frag_load_s(sm, a, lane); frag_load_t(linv, b, lane);
+  __syncwarp(); cfrag8_store(sm, acc, lane); __syncwarp();
+  frag8_load_s(sm, a, lane); frag8_load_t(linv, b, lane);
 #pragma unroll
   for (int e = 0; e < TILE; e++) c[e] = 0.0;
-  frag_gemm_sub(c, a, b);                 // c = -acc L_KK^-1 = -X
-  __syncwarp(); cfrag_store(sm, c, lane); __syncwarp();
-  frag_load_ts(sm, b, lane); frag_load_t(sel_tile(j, K, dd), a, lane);
+  frag8_gemm_sub(c, a, b);                 // c = -acc L_KK^-1 = -X
+  __syncwarp(); cfrag8_store(sm, c, lane); __syncwarp();
+  frag8_load_ts(sm, b, lane); frag8_load_t(sel_tile(j, K, dd), a, lane);
 #pragma unroll
   for (int e = 0; e < TILE; e++) acc[e] = 0.0;
-  frag_gemm_sub(acc, a, b);               // acc = L(I,K)^T X = P
+  frag8_gemm_sub(acc, a, b);               // acc = L(I,K)^T X = P
 #pragma unroll
   for (int e = 0; e < TILE; e++) c[e] = -c[e];
   // the ring slot's previous column (K + R) must have been copied out
   if (K + j.R < j.NT && dd <= min(j.WB, j.NT - 1 - (K + j.R))) wait_flag(sel_done(j, K + j.R, dd), lane);
-  cfrag_store(sel_stage(j, K, dd, 0), c, lane);
-  cfrag_store(sel_stage(j, K, dd, 1), acc, lane);
+  cfrag8_store(sel_stage(j, K, dd, 0), c, lane);
+  cfrag8_store(sel_stage(j, K, dd, 1), acc, lane);
   set_flag(sel_x(j, K, dd), lane);
 }
 
@@ -100,21 +100,21 @@ __device__ __forceinline__ void selinv_d(const SelJob& j, int K, double* sm, int
   const int m = min(j.WB, j.NT - 1 - K);
   const double* linv = j.linv + (size_t)K*TILE2;
   double acc[TILE];
-  cfrag_load(linv, acc, lane);
+  cfrag8_load(linv, acc, lane);
   for (int dd = 1; dd <= m; dd++) {      // M = L_KK^-1 - sum_dd P_dd
     wait_flag(sel_x(j, K, dd), lane);
     double p[TILE];
-    cfrag_load(sel_stage(j, K, dd, 1), p, lane);
+    cfrag8_load(sel_stage(j, K, dd, 1), p, lane);
 #pragma unroll
     for (int e = 0; e < TILE; e++) acc[e] -= p[e];
   }
   double a[TILE], b[TILE];
-  __syncwarp(); cfrag_store(sm, acc, lane); __syncwarp();
-  frag_load_ts(sm, b, lane); frag_load_t(linv, a, lane);
+  __syncwarp(); cfrag8_store(sm, acc, lane); __syncwarp();
+  frag8_load_ts(sm, b, lane); frag8_load_t(linv, a, lane);
 #pragma unroll
   for (int e = 0; e < TILE; e++) acc[e] = 0.0;
-  frag_gemm_sub(acc, a, b);               // acc = -L_KK^-T M = -Sigma(K,K)
-  __syncwarp(); cfrag_store(sm, acc, lane); __syncwarp();
+  frag8_gemm_sub(acc, a, b);               // acc = -L_KK^-T M = -Sigma(K,K)
+  __syncwarp(); cfrag8_store(sm, acc, lane); __syncwarp();
   double* t = sel_tile(j, K, 0);
 #pragma unroll
   for (int c = 0; c < TILE; c++) t[c*TILE + lane] = -(lane >= c ? sm[c*TILE + lane] : sm[lane*TILE + c]);   // the lower triangle, mirrored
