@@ -79,11 +79,11 @@ def _skew(v):
 
 
 def _jr(x):
-    """SO(3) right Jacobian"""
+    """SO(3) right Jacobian; 1 - cos(th) as 2 sin^2(th/2), which does not cancel"""
     th = np.linalg.norm(x); W = _skew(x)
     if th < 1e-5:
         return np.eye(3) - 0.5*W + W@W/6.0
-    return np.eye(3) - (1 - np.cos(th))/th**2*W + (th - np.sin(th))/th**3*W@W
+    return np.eye(3) - 2*np.sin(th/2)**2/th**2*W + (th - np.sin(th))/th**3*W@W
 
 
 def imu_jacobian(Xi, vi, Xj, vj, bi, bj, rec):
