@@ -1597,8 +1597,10 @@ int dynoba_get_variables(dynoba_handle h, int kind, int64_t n, double* out) {
 
 // LevenbergMarquardtOptimizer::optimize()  [GTSAM-ext nonlinear/{NonlinearOptimizer,LevenbergMarquardtOptimizer}.cpp]
 int dynoba_optimize(dynoba_handle h, const dynoba_lm_params* prm, dynoba_lm_stats* st) {
-  int rc = check_ready(h, true); if (rc) return rc;
+  if (!h) return DYNOBA_ERR_BAD_ARG;
   dynoba_lm_params P; if (prm) P = *prm; else dynoba_lm_default_params(&P);
+  if (!lm_params_usable(P)) { h->err = "LM parameters under which tryLambda cannot end (see dynoba_lm_params)"; return DYNOBA_ERR_BAD_ARG; }
+  int rc = check_ready(h, true); if (rc) return rc;
   dynoba_lm_stats S; std::memset(&S, 0, sizeof(S));
   const int64_t launches0 = h->launches;
   cudaEvent_t* ev = h->ev;

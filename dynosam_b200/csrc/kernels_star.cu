@@ -577,7 +577,7 @@ int dynoba_flow_pose_batch(int device, int32_t n_problems, const int32_t* offset
   if (n_problems == 0) return DYNOBA_OK;
   dynoba_flow_pose_params P; if (prm) P = *prm; else dynoba_flow_pose_default_params(&P);
   if (n_problems < 0 || !offsets || !pose_init || !pose_prev || !calib5 || !pose_out || !err_before || !err_after || !iterations || !inner_iterations ||
-      !(P.flow_sigma > 0) || !(P.flow_prior_sigma > 0) || P.outlier_rounds < 0) return DYNOBA_ERR_BAD_ARG;
+      !(P.flow_sigma > 0) || !(P.flow_prior_sigma > 0) || P.outlier_rounds < 0 || !lm_params_usable(P.lm)) return DYNOBA_ERR_BAD_ARG;
   const int total = offsets[n_problems];
   if (offsets[0] != 0 || total < 0 || (total > 0 && (!kp_prev || !depth || !flow || !flow_out))) return DYNOBA_ERR_BAD_ARG;
   for (int p = 0; p < n_problems; p++) if (offsets[p + 1] < offsets[p]) return DYNOBA_ERR_BAD_ARG;
@@ -638,7 +638,8 @@ int dynoba_motion_refine_batch(int device, int32_t n_problems, const int32_t* of
   if (n_problems == 0) return DYNOBA_OK;
   dynoba_motion_refine_params P; if (prm) P = *prm; else dynoba_motion_refine_default_params(&P);
   if (n_problems < 0 || !offsets || !pose_prev || !pose_cur || !motion_init || !calib5 || !motion_out || !err_before || !err_after || !iterations ||
-      !inner_iterations || !(P.landmark_motion_sigma > 0) || !(P.projection_sigma > 0) || !(P.pose_prior_sigma > 0)) return DYNOBA_ERR_BAD_ARG;
+      !inner_iterations || !(P.landmark_motion_sigma > 0) || !(P.projection_sigma > 0) || !(P.pose_prior_sigma > 0) || !lm_params_usable(P.lm))
+    return DYNOBA_ERR_BAD_ARG;
   const int total = offsets[n_problems];
   if (offsets[0] != 0 || total < 0 || (total > 0 && (!kp_prev || !kp_cur || !points_init))) return DYNOBA_ERR_BAD_ARG;
   for (int p = 0; p < n_problems; p++) if (offsets[p + 1] < offsets[p]) return DYNOBA_ERR_BAD_ARG;

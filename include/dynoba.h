@@ -75,7 +75,13 @@ typedef enum {
  * robustifies them.
  * Jacobian columns (dynoba_get_linearization): pose_i (6) | vel_i (3) | pose_j (6) | vel_j (3) | bias_i (6) | bias_j (6). */
 
-/* gtsam::LevenbergMarquardtParams (defaults = GTSAM 4.2.0, see dynoba_lm_default_params) */
+/* gtsam::LevenbergMarquardtParams (defaults = GTSAM 4.2.0, see dynoba_lm_default_params).
+ * dynoba_optimize, dynoba_flow_pose_batch and dynoba_motion_refine_batch return DYNOBA_ERR_BAD_ARG, before any device
+ * work, unless lambda_initial is finite and > 0, lambda_factor is finite and > 1 and lambda_upper_bound is not NaN: a run
+ * of rejected steps ends only once lambda reaches lambda_upper_bound, which it could otherwise never do.  They also refuse a
+ * lambda_factor under which that climb, from min(lambda_initial, lambda_lower_bound) to min(lambda_upper_bound, DBL_MAX),
+ * takes more than 10^4 rejected steps.  lambda_lower_bound is raised to DBL_MIN where it is lower, so that lambda cannot
+ * underflow to 0 after many accepted steps. */
 typedef struct {
   double lambda_initial, lambda_factor, lambda_upper_bound, lambda_lower_bound;
   double min_model_fidelity;

@@ -33,19 +33,57 @@ DEFAULTS = dict(lambda_initial=1e-5, lambda_factor=10.0, lambda_upper_bound=1e5,
 CHI2_99 = {2: 9.210340371976184, 3: 11.344866730144373}      # chi_squared_quantile(dim, 0.99)
 
 
+EPS = np.finfo(float).eps
+
+
+def _margin(x, scale):
+    return abs(x)/scale if scale > 0 else np.inf
+
+
+def _equilibrated_kappa(H, lam):
+    """kappa of D^-1 (H + lam I) D^-1, D the square root of its diagonal -- the condition that bounds a Cholesky solve's
+    error whatever the scaling of the unknowns; taken at the first lambda of a linearisation (a larger lambda only improves it)"""
+    Hd = H + lam*np.eye(H.shape[0])
+    if not H.size or not np.isfinite(Hd).all() or not (np.diag(Hd) > 0).all():
+        return np.inf
+    d = 1.0/np.sqrt(np.diag(Hd))
+    ev = np.linalg.eigvalsh(Hd*np.outer(d, d))
+    return ev[-1]/ev[0] if ev[0] > 0 else np.inf
+
+
+def near_decision(trace, factor=64.0):
+    """the first decision of an LM trace whose margin lies within `factor` times its step bound (eps kappa of the damped
+    system it was taken on), or None: an implementation whose steps differ from this one's by rounding may decide it the
+    other way, so a different (iterations, inner) is a last-digit decision only when such a decision exists"""
+    for i, t in enumerate(trace):
+        for k in ("fidelity", "stop", "relative", "absolute"):
+            if k in t and t[k] <= factor*t["bound"]:
+                return i, k, t[k], t["bound"]
+    return None
+
+
 def dense_lm(error, linear_system, get_state, set_state, step, **kw):
     """LevenbergMarquardtOptimizer::optimize on callbacks: error() at the current values, linear_system() -> whitened (A, b) at
-    the current values, step(delta) retracts the current values, get/set_state snapshot them."""
+    the current values, step(delta) retracts the current values, get/set_state snapshot them.
+
+    `trace` records every decision with its margin, relative to the magnitudes it compares: per inner iteration the model
+    fidelity against min_model_fidelity and |cost| against relative_error_tol * err, per outer iteration the relative and
+    absolute decrease against their tolerances; `bound` is eps * kappa of the equilibrated damped system, the relative size of
+    a difference rounding may make in the step and so in the compared errors.
+    `ended` names what ended the loop."""
     P = dict(DEFAULTS); P.update(kw)
     err = error(); err0 = err
     lam = P["lambda_initial"]; iterations = inner = 0
+    trace = []; ended = "error_tol" if err <= P["error_tol"] else ("max_iterations" if P["max_iterations"] <= 0 else None)
     if not (err <= P["error_tol"]) and P["max_iterations"] > 0:
         new_error = err
         while True:
             current_error = new_error
             A, b = linear_system()
             H = A.T @ A; g = A.T @ b
+            kappa = _equilibrated_kappa(H, lam)
             while True:      # tryLambda
+                rec = dict(lam=lam, bound=EPS*kappa)
                 solved = True
                 try:
                     L = np.linalg.cholesky(H + lam*np.eye(H.shape[0]))
@@ -59,12 +97,17 @@ def dense_lm(error, linear_system, get_state, set_state, step, **kw):
                         keep = get_state()
                         step(delta)
                         nerr = error(); cost = err - nerr
+                        scale = abs(err) + abs(nerr)
                         if lin > np.finfo(float).eps*old_lin:
                             success = cost/lin > P["min_model_fidelity"]
+                            rec["fidelity"] = _margin(cost - P["min_model_fidelity"]*lin, scale + abs(P["min_model_fidelity"]*lin))
                         if abs(cost) < P["relative_error_tol"]*err:
                             stop = True
+                        if P["relative_error_tol"] > 0:
+                            rec["stop"] = _margin(abs(cost) - P["relative_error_tol"]*err, scale)
                         if not success:
                             set_state(keep)
+                trace.append(rec)
                 if success:
                     lam = max(P["lambda_lower_bound"], lam/P["lambda_factor"]); err = nerr; iterations += 1; inner += 1
                     break
@@ -79,9 +122,19 @@ def dense_lm(error, linear_system, get_state, set_state, step, **kw):
                 rel = np.float64(current_error - new_error)/np.float64(current_error)
             done = (new_error <= P["error_tol"]) or (P["relative_error_tol"] != 0.0 and rel <= P["relative_error_tol"]) \
                 or ((current_error - new_error) <= P["absolute_error_tol"])
+            scale = abs(current_error) + abs(new_error)
+            rec = dict(bound=trace[-1]["bound"] if trace else EPS)
+            if P["relative_error_tol"] != 0.0 and np.isfinite(rel):
+                rec["relative"] = _margin((current_error - new_error) - P["relative_error_tol"]*current_error, scale)
+            rec["absolute"] = _margin((current_error - new_error) - P["absolute_error_tol"], scale + abs(P["absolute_error_tol"]))
+            trace.append(rec)
             if not (iterations < P["max_iterations"] and not done and np.isfinite(current_error)):
+                ended = ("error_tol" if new_error <= P["error_tol"] else
+                         "relative" if P["relative_error_tol"] != 0.0 and rel <= P["relative_error_tol"] else
+                         "absolute" if (current_error - new_error) <= P["absolute_error_tol"] else
+                         "nonfinite" if not np.isfinite(current_error) else "max_iterations")
                 break
-    return dict(error_initial=err0, error_final=err, iterations=iterations, inner_iterations=inner)
+    return dict(error_initial=err0, error_final=err, iterations=iterations, inner_iterations=inner, trace=trace, ended=ended)
 
 
 # ------------------------------------------------------------------------------------------------ (1) flow + pose
@@ -137,19 +190,22 @@ def flow_pose_refine(pose_init, pose_prev, calib5, kp_prev, depth, flow, flow_si
     X0 = q.o.pose[0].copy()
     r = dense_lm(q.error, q.linear_system, q.get_state, q.set_state, q.step, **kw)
     err_before = r["error_initial"]; its, inner, rounds = r["iterations"], r["inner_iterations"], 0
+    trace = list(r["trace"]); ended = "no_rounds"
     if outlier_rounds > 0:
         out = q.active & (q.gaussian_errors() > thr)
+        ended = "no_outliers"
         if out.any():
             for _ in range(outlier_rounds):
                 q.active &= ~out
                 q.o.pose[0] = X0                                  # optimised_values.update(pose_key, initial_pose)
                 r = dense_lm(q.error, q.linear_system, q.get_state, q.set_state, q.step, **kw)
-                its += r["iterations"]; inner += r["inner_iterations"]; rounds += 1
+                its += r["iterations"]; inner += r["inner_iterations"]; rounds += 1; trace += r["trace"]
                 out = q.active & (q.gaussian_errors() > thr)
                 if not out.any():
                     break
+            ended = "cap" if out.any() else "no_outliers"
     return dict(pose=q.o.pose[0].copy(), flow=q.o.flow.copy(), inlier=q.active.copy(), error_initial=err_before, error_final=r["error_final"],
-                iterations=its, inner_iterations=inner, rounds=rounds)
+                iterations=its, inner_iterations=inner, rounds=rounds, trace=trace, ended=ended, lm_ended=r["ended"])
 
 
 # ------------------------------------------------------------------------------------------------ (2) object motion

@@ -266,11 +266,27 @@ def test_flow_pose_outlier_rounds_match_oracle():
             assert with_rounds >= 5
 
 
+def _proven_path(r, o):
+    """None if the device took the oracle's LM path (iterations, inner iterations); otherwise the oracle's decision that proves
+    the difference a last-digit one (its margin within its step bound, star_oracle.near_decision), or raises"""
+    if (r["iterations"], r["inner_iterations"]) == (o["iterations"], o["inner_iterations"]):
+        return None
+    from oracle import star_oracle as SO
+    d = SO.near_decision(o["trace"])
+    assert d is not None, ("LM paths differ without a decision within its step bound", r["iterations"], r["inner_iterations"], o["iterations"], o["inner_iterations"])
+    return d
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("soft", [False, True])
 def test_motion_refine_batch_matches_oracle(soft):
-    """Object-motion refinement, one CTA per problem: same LM run as the dense CPU restatement (fp64; the camera priors put
-    1e10 next to 1e6 in the Hessian, hence 1e-7 relative on chi^2 and 1e-6 on the values)."""
+    """Object-motion refinement, one CTA per problem: the same LM run as the dense CPU restatement.  A differing LM path is
+    accepted only where the oracle recorded a decision whose margin lies within its step bound (_proven_path); every problem
+    on the same path is compared.  The values after five LM iterations are compared at 1e-3 relative on chi^2, 1e-4 on the
+    motion and 1e-3 on the points: they are not bounded by the single-step bound (eps kappa of the equilibrated system, 2e-9
+    with the 1e-5 camera priors), because a step's rounding moves the next linearisation point along the weakly determined
+    point depths; measured on an H100: chi^2 8e-6 .. 1e-5 relative, points 4e-4.  Each single step is pinned to a 50-digit
+    reference in tests/test_star_cases_gpu.py."""
     from oracle import star_oracle as SO
     probs = motion_set()
     kw = dict(landmark_motion_sigma=0.05, huber_k=1.0, max_iterations=8) if soft else {}
@@ -280,8 +296,8 @@ def test_motion_refine_batch_matches_oracle(soft):
         o = SO.motion_refine_lm(q["pose_prev"], q["pose_cur"], q["motion_init"], K5, q["kp_prev"], q["kp_cur"], q["points_init"], **kw)
         assert abs(r["error_initial"] - o["error_initial"]) <= 1e-10*o["error_initial"]
         assert r["error_final"] < r["error_initial"]
-        if (r["iterations"], r["inner_iterations"]) != (o["iterations"], o["inner_iterations"]):
-            continue                                                 # a fidelity test decided on the last digits; counted below
+        if _proven_path(r, o) is not None:
+            continue
         same += 1
         worst["chi2"] = max(worst["chi2"], abs(r["error_final"] - o["error_final"])/o["error_final"])
         worst["motion"] = max(worst["motion"], np.abs(r["motion"] - o["motion"]).max())
@@ -289,9 +305,6 @@ def test_motion_refine_batch_matches_oracle(soft):
         worst["factor"] = max(worst["factor"], np.abs(r["motion_factor_error"] - o["motion_factor_error"]).max()/max(o["motion_factor_error"].max(), 1.0))
         assert np.abs(r["poses"] - o["poses"]).max() < 1e-6
     print("motion_refine parity", "soft" if soft else "reference-params", "same LM path:", same, "of", len(probs), worst)
-    # the pose priors (1e10) sit next to Huber-weighted entries many orders below: cond ~ 1e11, so a dense Cholesky and the
-    # eliminate-then-factor order agree to ~cond * eps per step; measured: chi^2 1e-6 .. 1e-5 relative
-    assert same >= len(probs) - 3, same
     assert worst["chi2"] < 1e-3 and worst["motion"] < 1e-4 and worst["points"] < 1e-3 and worst["factor"] < 1e-3, worst
 
 
@@ -329,19 +342,23 @@ def _check_star_flow(g, results, offset=0):
     assert same >= len(results) - 2, same
 
 
-def _check_star_motion(g, results, offset=0):
-    same = 0
+def _check_star_motion(g, results, offset=0, problems=None):
+    """results[i] against stored run offset + i; where the LM path differs, the oracle is re-run on problems[offset + i] and must
+    hold a decision within its step bound (_proven_path); where it agrees, the values agree as in
+    test_motion_refine_batch_matches_oracle"""
+    from oracle import star_oracle as SO
     for i, r in enumerate(results):
         j = offset + i
         assert len(r["points"]) == int(g["n"][j])
         assert abs(r["error_initial"] - g["error_initial"][j]) <= 1e-10*g["error_initial"][j]
-        if (r["iterations"], r["inner_iterations"]) != (int(g["iterations"][j]), int(g["inner_iterations"][j])):
+        q = problems[j]
+        o = SO.motion_refine_lm(q["pose_prev"], q["pose_cur"], q["motion_init"], K5, q["kp_prev"], q["kp_cur"], q["points_init"])
+        assert (o["iterations"], o["inner_iterations"]) == (int(g["iterations"][j]), int(g["inner_iterations"][j]))
+        if _proven_path(r, o) is not None:
             continue
-        same += 1
         assert abs(r["error_final"] - g["error_final"][j]) <= 1e-3*g["error_final"][j]
         assert np.abs(r["motion"] - g["motion"][j]).max() < 1e-4 and np.abs(r["poses"] - g["poses"][j]).max() < 1e-6
         assert abs(r["motion_factor_error"].sum() - g["factor_error_sum"][j]) <= 1e-3*max(g["factor_error_sum"][j], 1.0)
-    assert same >= len(results) - 3, same
 
 
 def test_oracle_reproduces_golden_star():
@@ -355,7 +372,7 @@ def test_oracle_reproduces_golden_star():
         _check_star_flow(_load_golden(name), rs, offset=lo)
     probs = synth_star.motion_set()
     rs = [SO.motion_refine_lm(q["pose_prev"], q["pose_cur"], q["motion_init"], synth_star.K5, q["kp_prev"], q["kp_cur"], q["points_init"]) for q in probs[:5]]
-    _check_star_motion(_load_golden("star_motion_refine.npz"), rs)
+    _check_star_motion(_load_golden("star_motion_refine.npz"), rs, problems=probs)
 
 
 @pytest.mark.gpu
@@ -364,4 +381,5 @@ def test_cuda_reproduces_golden_star():
     from dynosam_b200 import binding, synth_star
     _check_star_flow(_load_golden("star_flow_pose_lm.npz"), binding.flow_pose_batch(synth_star.flow_parity_set(), outlier_rounds=0, **STAR_SIGMAS))
     _check_star_flow(_load_golden("star_flow_pose_rounds.npz"), binding.flow_pose_batch(synth_star.flow_rounds_set(), **STAR_SIGMAS))
-    _check_star_motion(_load_golden("star_motion_refine.npz"), binding.motion_refine_batch(synth_star.motion_set()))
+    probs = synth_star.motion_set()
+    _check_star_motion(_load_golden("star_motion_refine.npz"), binding.motion_refine_batch(probs), problems=probs)
