@@ -15,6 +15,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <numeric>
 #include <string>
@@ -23,18 +24,11 @@
 
 #include "../../include/dynoba.h"
 #include "internal.cuh"
+#include "window_plan.cuh"
 
 using namespace dynoba;
 
 namespace {
-
-// std::vector without the serial value-initialisation pass (the elements are written in parallel right after resize)
-template <class T> struct NoInitAlloc : std::allocator<T> {
-  template <class U> struct rebind { using other = NoInitAlloc<U>; };
-  template <class U, class... A> void construct(U* p, A&&... a) {
-    if constexpr (sizeof...(A) == 0) ::new ((void*)p) U; else ::new ((void*)p) U(std::forward<A>(a)...);
-  }
-};
 
 struct HostBlock {
   int type = 0; int64_t n = 0;
@@ -105,6 +99,12 @@ struct PinnedArena {
   void* take(size_t bytes) { const size_t a = (off + 255) & ~(size_t)255; if (!base || a + bytes > cap) return nullptr; off = a + bytes; return base + a; }
 };
 PinnedArena g_arena;
+// staging image of one SoA array: a slice of the arena, else plain new[] (no value-initialisation pass over ~1 GB)
+template <class T> struct Staging {
+  T* p; size_t n; std::unique_ptr<T[]> own;
+  explicit Staging(size_t cnt) : p((T*)g_arena.take(cnt*sizeof(T))), n(cnt) { if (!p) { own.reset(new T[cnt]); p = own.get(); } }
+  T* data() { return p; } size_t size() const { return n; } T& operator[](size_t i) { return p[i]; }
+};
 }  // namespace
 
 // Process-wide cache of device allocations: a closed solver's blocks are kept and handed to the next one that asks for
@@ -156,6 +156,13 @@ template <class T> static int dalloc(dynoba_solver* h, T** p, size_t count, bool
   h->allocs.emplace_back(q, got);
   return DYNOBA_OK;
 }
+// device copy of a host array: a clean dalloc (an empty array gets one zero element) and a synchronous copy
+template <class T> static int upload(dynoba_solver* h, T** p, const T* src, size_t count) {
+  if (int rc = dalloc(h, p, count)) return rc;
+  if (count) CK(cudaMemcpy(*p, src, count*sizeof(T), cudaMemcpyHostToDevice));
+  return DYNOBA_OK;
+}
+template <class V> static int upload(dynoba_solver* h, typename V::value_type** p, const V& v) { return upload(h, p, v.data(), v.size()); }
 static void free_device(dynoba_solver* h) {
   if (!h->allocs.empty()) cudaDeviceSynchronize();      // cudaFree used to imply this; cached blocks must be idle too
   for (auto& a : h->allocs) g_devcache.give(h->device, a.first, a.second);
@@ -440,6 +447,11 @@ int dynoba_set_shard(dynoba_handle h, int rank, int world, dynoba_allreduce_fn f
 
 // ------------------------------------------------------------------------------------------------ finalize
 static int uf_find(std::vector<int32_t>& p, int x) { while (p[x] != x) { p[x] = p[p[x]]; x = p[x]; } return x; }
+// x = v where better(v, x), atomically with relaxed ordering (a min / max the parallel loops over factors share)
+template <class Better> static void atomic_keep(int32_t& x, int32_t v, Better better) {
+  int32_t cur = __atomic_load_n(&x, __ATOMIC_RELAXED);
+  while (better(v, cur) && !__atomic_compare_exchange_n(&x, &cur, v, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
+}
 
 static int finalize_impl(dynoba_solver* h) {
   if (h->finalized) return DYNOBA_OK;
@@ -528,14 +540,10 @@ static int finalize_impl(dynoba_solver* h) {
       blo = std::min(blo, lo); bhi = std::max(bhi, hi);
       if (lslot < 0) { bspread = std::max(bspread, hi - lo); continue; }
       const int g = root[lmk_id(ti.cls[lslot], b.idx[i*ti.arity + lslot])];
-      int32_t cur = __atomic_load_n(&gmin[g], __ATOMIC_RELAXED);
-      while (lo < cur && !__atomic_compare_exchange_n(&gmin[g], &cur, lo, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
-      cur = __atomic_load_n(&gmax[g], __ATOMIC_RELAXED);
-      while (hi > cur && !__atomic_compare_exchange_n(&gmax[g], &cur, hi, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
+      atomic_keep(gmin[g], lo, std::less<int32_t>()); atomic_keep(gmax[g], hi, std::greater<int32_t>());
       if (ti.npose >= 2) {   // secondary ordering key: user index of the last pose slot (object-major for DynOSAM's H keys)
         int last = -1; for (int k = 0; k < ti.arity; k++) if (ti.cls[k] == VC_POSE) last = b.idx[i*ti.arity + k];
-        cur = __atomic_load_n(&gsec[g], __ATOMIC_RELAXED);
-        while (last < cur && !__atomic_compare_exchange_n(&gsec[g], &cur, last, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
+        atomic_keep(gsec[g], last, std::less<int32_t>());
       }
       int32_t gb = __atomic_load_n(&gblk[g], __ATOMIC_RELAXED);
       while (gb != (int)bi && gb != -2) {
@@ -639,25 +647,17 @@ static int finalize_impl(dynoba_solver* h) {
     for (int64_t i = 0; i < np; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.np_stride + h->pos[i]] = h->pose[i*12 + k];
     for (int64_t i = 0; i < nv; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.np_stride + h->pos[np + i]] = k < 3 ? h->vel[i*3 + k] : 0.0;
     for (int64_t i = 0; i < nb; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.np_stride + h->pos[np + nv + i]] = k < 6 ? h->bias[i*6 + k] : 0.0;
-    int rc = dalloc(h, &h->cur.pose, soa.size()); if (rc) return rc; rc = dalloc(h, &h->cand.pose, soa.size()); if (rc) return rc;
-    CK(cudaMemcpy(h->cur.pose, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(h->cand.pose, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
+    int rc;
+    if ((rc = upload(h, &h->cur.pose, soa)) || (rc = upload(h, &h->cand.pose, soa))) return rc;
     soa.assign((size_t)3*V.nl_stride, 0.0);
     for (int64_t i = 0; i < npt; i++) for (int k = 0; k < 3; k++) soa[(size_t)k*V.nl_stride + h->pt_new[i]] = h->point[i*3 + k];
-    rc = dalloc(h, &h->cur.point, soa.size()); if (rc) return rc; rc = dalloc(h, &h->cand.point, soa.size()); if (rc) return rc;
-    rc = dalloc(h, &h->dl_point, soa.size()); if (rc) return rc;
-    CK(cudaMemcpy(h->cur.point, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
-    CK(cudaMemset(h->dl_point, 0, std::max<size_t>(soa.size(), 1)*8));
+    if ((rc = upload(h, &h->cur.point, soa)) || (rc = dalloc(h, &h->cand.point, soa.size())) || (rc = dalloc(h, &h->dl_point, soa.size()))) return rc;
     soa.assign((size_t)2*V.nf_stride, 0.0);
     for (int64_t i = 0; i < nfl; i++) for (int k = 0; k < 2; k++) soa[(size_t)k*V.nf_stride + h->fl_new[i]] = h->flow[i*2 + k];
-    rc = dalloc(h, &h->cur.flow, soa.size()); if (rc) return rc; rc = dalloc(h, &h->cand.flow, soa.size()); if (rc) return rc;
-    rc = dalloc(h, &h->dl_flow, soa.size()); if (rc) return rc;
-    CK(cudaMemcpy(h->cur.flow, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
-    CK(cudaMemset(h->dl_flow, 0, std::max<size_t>(soa.size(), 1)*8));
+    if ((rc = upload(h, &h->cur.flow, soa)) || (rc = dalloc(h, &h->cand.flow, soa.size())) || (rc = dalloc(h, &h->dl_flow, soa.size()))) return rc;
     soa.assign((size_t)12*V.naux_stride, 0.0);
     for (int64_t i = 0; i < naux; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.naux_stride + i] = h->aux[i*12 + k];
-    double* da; rc = dalloc(h, &da, soa.size()); if (rc) return rc;
-    CK(cudaMemcpy(da, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
+    double* da; if ((rc = upload(h, &da, soa))) return rc;
     h->cur.aux = da; h->cand.aux = da;
   }
   lap("band + variables upload");
@@ -691,66 +691,14 @@ static int finalize_impl(dynoba_solver* h) {
         frank[i] = lrank[lmk_id(ti.cls[lslot], b.idx[i*ti.arity + lslot])];
         key[i] = ((int64_t)frank[i] << 32) | (uint32_t)h->pos[b.idx[i*ti.arity + pslot]];
       }
-      int unsorted = 0;
-#pragma omp parallel for schedule(static) reduction(|:unsorted)
-      for (int64_t i = 1; i < n; i++) unsorted |= key[i-1] > key[i];
-      if (unsorted) {
-        // Fast path: the caller lists each landmark's factors contiguously with ascending poses (how DynOSAM's
-        // formulations add them) and only the ORDER OF THE LANDMARKS differs from ours -- then sorting the runs (one per
-        // landmark) replaces sorting the factors.  Anything else falls back to the general stable sort.
-        std::vector<int64_t> run0;                                 // first factor of each run of equal group rank
-        {
-          const int nseg = std::max(1, std::min<int>(omp_get_max_threads(), (int)(n/65536) + 1));
-          std::vector<std::vector<int64_t>> seg(nseg);
-#pragma omp parallel for schedule(static, 1)
-          for (int t = 0; t < nseg; t++) {
-            const int64_t s0 = n*t/nseg, s1 = n*(t + 1)/nseg;
-            for (int64_t i = s0; i < s1; i++) if (i == 0 || frank[i] != frank[i-1]) seg[t].push_back(i);
-          }
-          for (auto& v : seg) run0.insert(run0.end(), v.begin(), v.end());
-        }
-        const int64_t nrun = (int64_t)run0.size();
-        int bad = 0;                                               // a rank in two runs, or poses not ascending inside a run
-        std::vector<int64_t> order(nrun);
-        if (nrun <= (int64_t)gorder.size()) {
-#pragma omp parallel for schedule(static) reduction(|:bad)
-          for (int64_t r = 0; r < nrun; r++) {
-            order[r] = r;
-            const int64_t e = r + 1 < nrun ? run0[r + 1] : n;
-            for (int64_t i = run0[r] + 1; i < e; i++) bad |= key[i-1] > key[i];
-          }
-          if (!bad) {
-            __gnu_parallel::sort(order.begin(), order.end(), [&](int64_t a, int64_t c) { return frank[run0[a]] < frank[run0[c]]; });
-#pragma omp parallel for schedule(static) reduction(|:bad)
-            for (int64_t r = 1; r < nrun; r++) bad |= frank[run0[order[r-1]]] == frank[run0[order[r]]];
-          }
-        } else bad = 1;
-        if (!bad) {
-          std::vector<int64_t> dst(nrun + 1, 0);
-          for (int64_t r = 0; r < nrun; r++) { const int64_t a = order[r]; dst[r + 1] = dst[r] + ((a + 1 < nrun ? run0[a + 1] : n) - run0[a]); }
-#pragma omp parallel for schedule(static)
-          for (int64_t r = 0; r < nrun; r++) {
-            const int64_t a = order[r], len = dst[r + 1] - dst[r];
-            for (int64_t k = 0; k < len; k++) b.perm[dst[r] + k] = (int32_t)(run0[a] + k);
-          }
-        } else {
-          __gnu_parallel::stable_sort(b.perm.begin(), b.perm.end(), [&](int a, int c) { return key[a] < key[c]; });
-        }
-      }
+      order_block_factors(b.perm.data(), frank, key, n, gorder.size());
     }
     lap("  blk sort");
-    // SoA host images
-    // staging images: plain new[] (no value-initialisation pass over ~1 GB), padding filled explicitly below
-    struct Buf32 { std::unique_ptr<int32_t[]> p; size_t n; int32_t* data() { return p.get(); } size_t size() const { return n; } int32_t& operator[](size_t i) { return p[i]; } };
-    struct Buf64 { std::unique_ptr<double[]> p; size_t n; double* data() { return p.get(); } size_t size() const { return n; } double& operator[](size_t i) { return p[i]; } };
-    struct View32 { int32_t* p; size_t n; std::unique_ptr<int32_t[]> own; int32_t* data() { return p; } size_t size() const { return n; } int32_t& operator[](size_t i) { return p[i]; } };
-    struct View64 { double* p; size_t n; std::unique_ptr<double[]> own; double* data() { return p; } size_t size() const { return n; } double& operator[](size_t i) { return p[i]; } };
-    auto mk32 = [&](size_t cnt) { View32 v; v.n = cnt; v.p = (int32_t*)g_arena.take(cnt*4); if (!v.p) { v.own.reset(new int32_t[cnt]); v.p = v.own.get(); } return v; };
-    auto mk64 = [&](size_t cnt) { View64 v; v.n = cnt; v.p = (double*)g_arena.take(cnt*8); if (!v.p) { v.own.reset(new double[cnt]); v.p = v.own.get(); } return v; };
-    View32 hidx = mk32((size_t)ti.arity*stride);
-    View64 hmeas = mk64((size_t)std::max(ti.meas, 1)*stride);
-    View64 hsig = mk64((size_t)b.sigma_dim*stride);
-    View32 haux = mk32((size_t)stride);
+    // SoA host images, padding filled explicitly below
+    Staging<int32_t> hidx((size_t)ti.arity*stride);
+    Staging<double> hmeas((size_t)std::max(ti.meas, 1)*stride);
+    Staging<double> hsig((size_t)b.sigma_dim*stride);
+    Staging<int32_t> haux((size_t)stride);
     const bool pinned = !hidx.own && !hmeas.own && !hsig.own && !haux.own;
     auto h2d = [&](void* dst, const void* src, size_t bytes) { return pinned ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream2) : cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice); };
     for (int64_t s = n; s < stride; s++) {
@@ -818,8 +766,7 @@ static int finalize_impl(dynoba_solver* h) {
       }
       gp.push_back((int32_t)n);
       int* dgp; int* dgl;
-      if ((rc = dalloc(h, &dgp, gp.size()))) return rc; CK(cudaMemcpy(dgp, gp.data(), gp.size()*4, cudaMemcpyHostToDevice));
-      if ((rc = dalloc(h, &dgl, gl.size()))) return rc; if (!gl.empty()) CK(cudaMemcpy(dgl, gl.data(), gl.size()*4, cudaMemcpyHostToDevice));
+      if ((rc = upload(h, &dgp, gp)) || (rc = upload(h, &dgl, gl))) return rc;
       d.n_groups = (int)gl.size(); d.grp_ptr = dgp; d.grp_lmk = dgl;
       b.simple = true;
       // ---- window decomposition (kernels_window.cu) for the 3-dof landmark types
@@ -827,152 +774,18 @@ static int finalize_impl(dynoba_solver* h) {
       b.use_window = false; b.all_window = false; b.win = DevWindows{}; b.win_ctas = 0; b.win_flushed = 0;
       if (win_type && !gl.empty()) {
         const int ng = (int)gl.size(), NPs = ti.npose;
-        std::vector<unsigned char> gwin(ng, 0);
-        std::vector<unsigned char, NoInitAlloc<unsigned char>> lvar((size_t)NPs*stride);   // only read for window-path factors
-        std::vector<int32_t> chunk_batch, cvars; std::vector<int4> jobs, batches;
-        int pose_slot[2] = {0, 0}; { int c = 0; for (int k = 0; k < ti.arity; k++) if (ti.cls[k] == VC_POSE && c < 2) pose_slot[c++] = k; }
+        const int32_t* prow[2] = {nullptr, nullptr};
+        { int c = 0; for (int k = 0; k < ti.arity; k++) if (ti.cls[k] == VC_POSE && c < 2) prow[c++] = hidx.data() + (size_t)k*stride; }
         // window size: one 512-thread CTA holds 16 tiles of 8x4 blocks; NLOC 24 -> 12 tiles (one stripe), NLOC 40 -> 30 (two)
         int cap = NPs == 1 ? 24 : 40;
-        // NP = 2: a variable keeps its window slot over the consecutive chunks that contain it, and the accumulate kernel
-        // walks runs of chunks.  NP = 1 chunks (~1000 landmarks each) are runs of their own, slots in position order.
-        const bool slide = NPs == 2;
-        // greedy chunking, independently inside parallel segments of the group list (a chunk never crosses a segment)
         const int nseg = std::max(1, std::min<int>(omp_get_max_threads(), ng/4096 + 1));
-        // per chunk: first group, slots spanned (highest occupied slot + 1), slot -> position row, first batch (+ end)
-        struct SegOut { std::vector<int32_t> g0, nslot, cv, b0; std::vector<int4> bat; int64_t flushed = 0; };
-        std::vector<SegOut> seg(nseg);
-#pragma omp parallel for schedule(static, 1)
-        for (int t = 0; t < nseg; t++) {
-          const int ga = (int)((int64_t)ng*t/nseg), gb_ = (int)((int64_t)ng*(t + 1)/nseg);
-          std::vector<int32_t> stamp(NP, -1), gstamp(NP, -1), inchunk(NP, -1), cur;   // indexed by solver position
-          std::vector<int32_t> wslot(NP, -1), occ(WIN_NLOC_MAX, -1);                 // window slot of a position, occupant of a slot
-          int cur_g0 = ga, chunk_id = 0; SegOut& out = seg[t];
-          auto close_chunk = [&](int g_end) {
-            std::vector<int32_t> sorted = cur; std::sort(sorted.begin(), sorted.end());
-            std::vector<int32_t> row(WIN_NLOC_MAX, -1);
-            if (slide) {     // variables that stay keep their slot; entering ones take the lowest free slots
-              for (int32_t p_ : sorted) stamp[p_] = -2;
-              for (int s_ = 0; s_ < WIN_NLOC_MAX; s_++) if (occ[s_] >= 0 && stamp[occ[s_]] != -2) occ[s_] = -1;
-              for (int32_t p_ : sorted) if (wslot[p_] >= 0 && occ[wslot[p_]] == p_) stamp[p_] = wslot[p_];
-              int fs = 0;
-              for (int32_t p_ : sorted) if (stamp[p_] == -2) { while (occ[fs] >= 0) fs++; occ[fs] = p_; wslot[p_] = fs; stamp[p_] = fs; }
-              row = occ;
-            } else {
-              for (size_t i = 0; i < sorted.size(); i++) { stamp[sorted[i]] = (int32_t)i; row[i] = sorted[i]; }   // position -> local index
-            }
-            for (int g = cur_g0; g < g_end; g++) if (gwin[g] == 1)
-              for (int s_ = gp[g]; s_ < gp[g+1]; s_++) for (int k = 0; k < NPs; k++)
-                lvar[(size_t)k*stride + s_] = (unsigned char)stamp[hidx[(size_t)pose_slot[k]*stride + s_]];
-            for (size_t i = 0; i < sorted.size(); i++) stamp[sorted[i]] = -1;
-            int ext = 0; for (int s_ = 0; s_ < WIN_NLOC_MAX; s_++) if (row[s_] >= 0) ext = s_ + 1;
-            out.g0.push_back(cur_g0); out.nslot.push_back(ext);
-            out.cv.insert(out.cv.end(), row.begin(), row.end());
-            // batches of the chunk: runs of window-path landmarks (other groups end a run), bounded in landmarks and slots
-            out.b0.push_back((int32_t)out.bat.size());
-            int rg0 = -1, rslots = 0;
-            auto close_batch = [&](int ge) { if (rg0 >= 0) out.bat.push_back(make_int4(rg0, ge, gp[rg0], gp[ge])); rg0 = -1; rslots = 0; };
-            for (int g = cur_g0; g < g_end; g++) {
-              if (gwin[g] != 1) { close_batch(g); continue; }
-              const int ns_ = (gp[g+1] - gp[g])*NPs;
-              if (rg0 >= 0 && (rslots + ns_ > WIN_BATCH_SLOTS || g - rg0 >= WIN_BATCH_LMK)) close_batch(g);
-              if (rg0 < 0) rg0 = g;
-              rslots += ns_;
-            }
-            close_batch(g_end);
-            chunk_id++; cur.clear(); cur_g0 = g_end;
-          };
-          for (int g = ga; g < gb_; g++) {
-            if (gl[g] < 0) continue;
-            const int T = gp[g+1] - gp[g];
-            bool dup = false; int fresh = 0;
-            if (T > WIN_TMAX) { gwin[g] = 2; continue; }
-            for (int s_ = gp[g]; s_ < gp[g+1] && !dup; s_++) for (int k = 0; k < NPs; k++) {
-              const int p_ = hidx[(size_t)pose_slot[k]*stride + s_];
-              if (gstamp[p_] == g) { dup = true; break; }
-              gstamp[p_] = g;
-              if (inchunk[p_] != chunk_id) fresh++;
-            }
-            if (dup) { gwin[g] = 2; continue; }
-            if (!cur.empty() && (int)cur.size() + fresh > cap) {      // a landmark wider than cap gets a chunk of its own
-              close_chunk(g);
-            }
-            for (int s_ = gp[g]; s_ < gp[g+1]; s_++) for (int k = 0; k < NPs; k++) {
-              const int p_ = hidx[(size_t)pose_slot[k]*stride + s_];
-              if (inchunk[p_] != chunk_id) { inchunk[p_] = chunk_id; cur.push_back(p_); }
-            }
-            gwin[g] = 1;
-          }
-          close_chunk(gb_);
-          out.b0.push_back((int32_t)out.bat.size());
-        }
-        // runs: a segment's chunks that have batches, run_len at a time (never across a segment: the slots restart there)
-        auto has_batches = [&](const SegOut& o, size_t c) { return o.b0[c + 1] > o.b0[c]; };
-        size_t nch = 0; for (int t = 0; t < nseg; t++) for (size_t c = 0; c + 1 < seg[t].b0.size(); c++) nch += has_batches(seg[t], c);
-        const int run_len = slide ? std::max<int>(WIN_RUN_MIN_CHUNKS, (int)((nch + WIN_RUNS - 1)/WIN_RUNS)) : 1;
-        // census: the blocks the accumulate kernel flushes per solve, by its rule (a slot pair that a landmark's clique
-        // touched, when either slot changes variable and at the run's end)
-#pragma omp parallel for schedule(static, 1)
-        for (int t = 0; t < nseg; t++) {
-          SegOut& o = seg[t];
-          uint64_t tch[WIN_NLOC_MAX] = {};      // tch[a] bit b: slot pair (a, b) touched since its last flush
-          auto flush = [&](uint64_t E) {        // E: slots that change variable
-            for (int a_ = 0; a_ < WIN_NLOC_MAX; a_++) {
-              const uint64_t low = tch[a_] & ((2ull << a_) - 1);
-              o.flushed += __builtin_popcountll((E >> a_) & 1 ? low : low & E);
-            }
-            for (int a_ = 0; a_ < WIN_NLOC_MAX; a_++) tch[a_] = (E >> a_) & 1 ? 0 : tch[a_] & ~E;
-          };
-          int in_run = 0; int prev = -1;
-          for (size_t c = 0; c + 1 < o.b0.size(); c++) {
-            if (!has_batches(o, c)) continue;
-            uint64_t E = 0;
-            if (in_run == run_len) { E = ~0ull; in_run = 0; }
-            else if (prev >= 0) for (int s_ = 0; s_ < WIN_NLOC_MAX; s_++) if (o.cv[(size_t)prev*WIN_NLOC_MAX + s_] != o.cv[c*WIN_NLOC_MAX + s_]) E |= 1ull << s_;
-            flush(E);
-            in_run++; prev = (int)c;
-            const int ge = c + 1 < o.g0.size() ? o.g0[c + 1] : (int)((int64_t)ng*(t + 1)/nseg);
-            for (int g = o.g0[c]; g < ge; g++) if (gwin[g] == 1) {
-              uint64_t m = 0;
-              for (int s_ = gp[g]; s_ < gp[g+1]; s_++) for (int k = 0; k < NPs; k++) m |= 1ull << lvar[(size_t)k*stride + s_];
-              for (uint64_t r_ = m; r_; r_ &= r_ - 1) tch[__builtin_ctzll(r_)] |= m;
-            }
-          }
-          flush(~0ull);
-        }
-        b.win_ctas = 0; b.win_flushed = 0;
-        for (int t = 0; t < nseg; t++) {
-          const SegOut& o = seg[t];
-          b.win_flushed += o.flushed;
-          int r0 = -1, in_run = 0, ext = 0;
-          auto close_run = [&]() {
-            if (r0 < 0) return;
-            const int nst = (win_ntiles(ext) + WIN_ACC_WARPS - 1)/WIN_ACC_WARPS;
-            for (int st = 0; st < nst; st++) jobs.push_back(make_int4(r0, (int)chunk_batch.size(), st, ext));
-            b.win_ctas += nst; r0 = -1; in_run = 0; ext = 0;
-          };
-          for (size_t c = 0; c + 1 < o.b0.size(); c++) {
-            if (!has_batches(o, c)) continue;
-            if (in_run == run_len) close_run();
-            if (r0 < 0) r0 = (int)chunk_batch.size();
-            chunk_batch.push_back((int32_t)batches.size());
-            batches.insert(batches.end(), o.bat.begin() + o.b0[c], o.bat.begin() + o.b0[c + 1]);
-            cvars.insert(cvars.end(), o.cv.begin() + c*WIN_NLOC_MAX, o.cv.begin() + (c + 1)*WIN_NLOC_MAX);
-            ext = std::max(ext, o.nslot[c]); in_run++;
-          }
-          close_run();
-        }
-        chunk_batch.push_back((int32_t)batches.size());
+        const WindowPlan w = plan_windows(NPs, stride, NP, prow, gp.data(), gl.data(), ng, cap, nseg);
         int4* djobs; int4* dbat; int* dcb; int* dcv; unsigned char* dlv; unsigned char* dgw; double* dslots;
-        if ((rc = dalloc(h, &djobs, jobs.size()))) return rc; if (!jobs.empty()) CK(cudaMemcpy(djobs, jobs.data(), jobs.size()*sizeof(int4), cudaMemcpyHostToDevice));
-        if ((rc = dalloc(h, &dbat, batches.size()))) return rc; if (!batches.empty()) CK(cudaMemcpy(dbat, batches.data(), batches.size()*sizeof(int4), cudaMemcpyHostToDevice));
-        if ((rc = dalloc(h, &dcb, chunk_batch.size()))) return rc; CK(cudaMemcpy(dcb, chunk_batch.data(), chunk_batch.size()*4, cudaMemcpyHostToDevice));
-        if ((rc = dalloc(h, &dcv, cvars.size()))) return rc; if (!cvars.empty()) CK(cudaMemcpy(dcv, cvars.data(), cvars.size()*4, cudaMemcpyHostToDevice));
-        if ((rc = dalloc(h, &dlv, lvar.size()))) return rc; CK(cudaMemcpy(dlv, lvar.data(), lvar.size(), cudaMemcpyHostToDevice));
-        if ((rc = dalloc(h, &dgw, gwin.size()))) return rc; CK(cudaMemcpy(dgw, gwin.data(), gwin.size(), cudaMemcpyHostToDevice));
+        if ((rc = upload(h, &djobs, w.jobs)) || (rc = upload(h, &dbat, w.batches)) || (rc = upload(h, &dcb, w.chunk_batch)) ||
+            (rc = upload(h, &dcv, w.cvars)) || (rc = upload(h, &dlv, w.lvar)) || (rc = upload(h, &dgw, w.gwin))) return rc;
         if ((rc = dalloc(h, &dslots, (size_t)n*NPs*WIN_SLOT_DOUBLES, false))) return rc;
-        b.win.n_jobs = (int)jobs.size(); b.win.jobs = djobs; b.win.batches = dbat; b.win.chunk_batch = dcb; b.win.cvars = dcv; b.win.lvar = dlv; b.win.grp_win = dgw; b.win.slots = dslots;
-        b.use_window = true;
-        { size_t nw = 0; for (int g = 0; g < ng; g++) nw += gwin[g] == 1 || gl[g] < 0; b.all_window = nw == (size_t)ng; }
+        b.win.n_jobs = (int)w.jobs.size(); b.win.jobs = djobs; b.win.batches = dbat; b.win.chunk_batch = dcb; b.win.cvars = dcv; b.win.lvar = dlv; b.win.grp_win = dgw; b.win.slots = dslots;
+        b.use_window = true; b.all_window = w.all_window; b.win_ctas = w.win_ctas; b.win_flushed = w.win_flushed;
       }
     }
     lap("  blk groups+windows");
@@ -1007,21 +820,15 @@ static int finalize_impl(dynoba_solver* h) {
     }
     std::vector<DevBlock> hb; for (auto& b : h->blocks) hb.push_back(b.dev);
     DevBlock* dblk; int* dgptr; int* drefs; int* dgl0; int* dgnl; int rc;
-    if ((rc = dalloc(h, &dblk, hb.size()))) return rc; CK(cudaMemcpy(dblk, hb.data(), hb.size()*sizeof(DevBlock), cudaMemcpyHostToDevice));
-    if ((rc = dalloc(h, &dgptr, gptr.size()))) return rc; CK(cudaMemcpy(dgptr, gptr.data(), gptr.size()*4, cudaMemcpyHostToDevice));
-    if ((rc = dalloc(h, &drefs, refs.size()))) return rc; CK(cudaMemcpy(drefs, refs.data(), refs.size()*4, cudaMemcpyHostToDevice));
-    if ((rc = dalloc(h, &dgl0, gl0.size()))) return rc; CK(cudaMemcpy(dgl0, gl0.data(), gl0.size()*4, cudaMemcpyHostToDevice));
-    if ((rc = dalloc(h, &dgnl, gnl.size()))) return rc; CK(cudaMemcpy(dgnl, gnl.data(), gnl.size()*4, cudaMemcpyHostToDevice));
+    if ((rc = upload(h, &dblk, hb)) || (rc = upload(h, &dgptr, gptr)) || (rc = upload(h, &drefs, refs)) || (rc = upload(h, &dgl0, gl0)) ||
+        (rc = upload(h, &dgnl, gnl))) return rc;
     h->gen.n_groups = (int)gl0.size(); h->gen.blocks = dblk; h->gen.gptr = dgptr; h->gen.refs = drefs; h->gen.gl0 = dgl0; h->gen.gnl = dgnl;
   }
   for (auto& P : h->priors) {
     const int n = (int)P.idx.size(); std::vector<int32_t> ppos(n);
     for (int i = 0; i < n; i++) ppos[i] = h->pos[P.idx[i]];
     int* dpos; double *dlin, *dG, *dg, *dd, *dgc; int rc;
-    if ((rc = dalloc(h, &dpos, (size_t)n, false))) return rc; CK(cudaMemcpy(dpos, ppos.data(), (size_t)n*4, cudaMemcpyHostToDevice));
-    if ((rc = dalloc(h, &dlin, (size_t)12*n, false))) return rc; CK(cudaMemcpy(dlin, P.lin.data(), (size_t)12*n*8, cudaMemcpyHostToDevice));
-    if ((rc = dalloc(h, &dG, (size_t)36*n*n, false))) return rc; CK(cudaMemcpy(dG, P.G.data(), (size_t)36*n*n*8, cudaMemcpyHostToDevice));
-    if ((rc = dalloc(h, &dg, (size_t)6*n, false))) return rc; CK(cudaMemcpy(dg, P.g.data(), (size_t)6*n*8, cudaMemcpyHostToDevice));
+    if ((rc = upload(h, &dpos, ppos)) || (rc = upload(h, &dlin, P.lin)) || (rc = upload(h, &dG, P.G)) || (rc = upload(h, &dg, P.g))) return rc;
     if ((rc = dalloc(h, &dd, (size_t)6*n))) return rc; if ((rc = dalloc(h, &dgc, (size_t)6*n))) return rc;
     P.dev = DevPrior{ n, dpos, dlin, dG, dg, P.f, dd, dgc };
     P.part_off = part; part += 1; P.bs_off = bs; bs += 1;
@@ -1031,8 +838,7 @@ static int finalize_impl(dynoba_solver* h) {
     std::vector<int2> nav(nv + nb);
     for (int64_t i = 0; i < nv; i++) nav[i] = make_int2(h->pos[np + i], 3);
     for (int64_t i = 0; i < nb; i++) nav[nv + i] = make_int2(h->pos[np + nv + i], 6);
-    int rc; if ((rc = dalloc(h, &h->d_nav, nav.size(), false))) return rc;
-    CK(cudaMemcpy(h->d_nav, nav.data(), nav.size()*sizeof(int2), cudaMemcpyHostToDevice));
+    if (int rc = upload(h, &h->d_nav, nav)) return rc;
     h->n_nav = (int)nav.size();
   }
   h->gen_bs_off = bs; bs += general_grid(h->gen.n_groups);

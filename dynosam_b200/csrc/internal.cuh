@@ -214,7 +214,7 @@ struct GeneralGroups {
   const int* gnl;           // [n_groups] number of points (<= 21)
 };
 
-// Window decomposition of a factor block for kernels_window.cu (built by the host in finalize)
+// Window decomposition of a factor block for kernels_window.cu (planned on the host by plan_windows, window_plan.cuh)
 constexpr int WIN_NLOC_MAX = 48;          // largest window (local pose-like variables of a chunk; window slots)
 constexpr int WIN_TMAX = 24;              // factors per landmark on the window path (larger ones: kernels_schur.cu)
 constexpr int WIN_SLOT_DOUBLES = 42;      // one staged clique variable of one factor: Wt[3][6] | A[3][6] | rb[3] | meta | pad[2]

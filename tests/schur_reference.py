@@ -21,8 +21,9 @@ prior (H_aa ~ 1e12) loosens only its own rows:
 By Cauchy-Schwarz every term summed into S_ab is at most sqrt(H_aa H_bb) (and into g_a at most sqrt(H_aa) r), so
 fp64 reassociation stays near 1e-16 times the number of terms in these units.
 
-Route mirror.  ``routes(p)`` restates the symbolic phase (``finalize`` in csrc/api.cu): union-find over factors that
-touch two landmarks, then per factor block and group
+Route mirror.  ``routes(p)`` restates the symbolic phase (``finalize`` in csrc/api.cu, which leaves the window / simple
+split to ``plan_windows`` in csrc/window_plan.cuh): union-find over factors that touch two landmarks, then per factor
+block and group
     window   3-dof landmark type, the group's only block, one landmark, T <= WIN_TMAX, no pose repeated in the group
     simple   one landmark in one block otherwise (T > WIN_TMAX, a repeated pose, the flow type)
     general  several landmarks (chains), or a landmark with factors in several blocks; refused above GG_MAXL points
@@ -192,8 +193,8 @@ class Group:
     root: int                  # union-find root: the landmark's own index for one-landmark groups (flows after points)
 
 
-def routes(p: Problem):
-    """every (block, landmark group) of p with the route the symbolic phase gives it"""
+def landmark_roots(p: Problem):
+    """union-find root of every landmark (points, then flows) over the factors that touch two landmarks"""
     npt, nfl = p.n_point, p.n_flow
     nl = npt + nfl
     uf = np.arange(nl)
@@ -217,7 +218,13 @@ def routes(p: Problem):
                 c = find(lmk(SLOT_CLASS[b.type][k], row[k]))
                 if a != c:
                     uf[c] = a
-    root = np.array([find(i) for i in range(nl)], dtype=np.int64)
+    return np.array([find(i) for i in range(nl)], dtype=np.int64)
+
+
+def routes(p: Problem):
+    """every (block, landmark group) of p with the route the symbolic phase gives it"""
+    npt, nl = p.n_point, p.n_point + p.n_flow
+    root = landmark_roots(p)
     gcount = np.bincount(root, minlength=nl)
     blocks_of = {}
     per_block = []

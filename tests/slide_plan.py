@@ -1,7 +1,8 @@
-"""Mirror of the window plan's sliding part (``finalize`` in csrc/api.cu) and graphs that reach its boundaries.
+"""Mirror of the window plan (``plan_windows`` in csrc/window_plan.cuh) and graphs that reach its boundaries.
 
-For one factor block whose window-path landmarks form one host segment (fewer than schur_reference.HOST_SEGMENT_GROUPS
-groups), ``plan(p, bi)`` restates what the host builds for the accumulate kernel:
+For one factor block, ``plan(p, bi)`` restates what the host builds for the accumulate kernel when the block's groups
+form one host segment (fewer than schur_reference.HOST_SEGMENT_GROUPS groups); ``plan(p, bi, nseg)`` cuts the group list
+into nseg segments as the host does with nseg threads (chunks, slots and runs restart in each):
     chunks   greedy, in the symbolic phase's landmark order, at most CHUNK_CAP variables (schur_reference.chunk_stats)
     slots    NP = 2: a variable keeps its window slot over consecutive chunks that contain it, an entering variable takes
              the lowest free slot; NP = 1: slots in ascending solver position, chunk by chunk
@@ -46,38 +47,64 @@ class Plan:
         return sum(1 for _, c, ch in self.transitions() for s in ch if self.slots[c - 1][s] >= 0 and self.slots[c][s] >= 0)
 
 
-def plan(p, bi) -> Plan:
+def positions(p):
+    """solver position of every pose (the stable order of the pose hint)"""
+    pos = np.empty(p.n_pose, np.int64)
+    pos[np.argsort(p.pose_order if p.pose_order is not None else np.arange(p.n_pose), kind="stable")] = np.arange(p.n_pose)
+    return pos
+
+
+def block_groups(p, bi):
+    """the landmark groups of block bi in the symbolic phase's order, [(route, root, factors)]: by the smallest
+    last-slot pose index (two pose slots) or first pose position (one), then by root, the general groups last; a
+    group's factors by the position of the first pose slot"""
     b = p.blocks[bi]
     sc = SLOT_CLASS[b.type]
     pcols = [k for k, c in enumerate(sc) if c == 0]
     lcol = [k for k, c in enumerate(sc) if c != 0][0]
+    pos = positions(p)
+    route = {g.root: g.route for g in SR.routes(p) if g.block == bi}
+    g = SR.landmark_roots(p)[b.idx[:, lcol] + (0 if sc[lcol] == 1 else p.n_point)]
+    order = np.lexsort((pos[b.idx[:, pcols[0]]], g))
+    starts = np.flatnonzero(np.r_[True, g[order][1:] != g[order][:-1]])
+    out = []
+    for f in np.split(order, starts[1:]):
+        r = int(g[f[0]]); pp = b.idx[f][:, pcols]
+        key = int(pp[:, -1].min()) if len(pcols) >= 2 else int(pos[pp[:, 0]].min())
+        out.append(((route[r] in ("general", "unsupported"), key, r), route[r], r, f))
+    return [x[1:] for x in sorted(out, key=lambda x: x[0])]
+
+
+def plan(p, bi, nseg=None) -> Plan:
+    b = p.blocks[bi]
+    pcols = [k for k, c in enumerate(SLOT_CLASS[b.type]) if c == 0]
     NP = len(pcols)
     cap = SR.CHUNK_CAP[0] if NP == 1 else SR.CHUNK_CAP[1]
-    pos = np.empty(p.n_pose, np.int64)
-    pos[np.argsort(p.pose_order if p.pose_order is not None else np.arange(p.n_pose), kind="stable")] = np.arange(p.n_pose)
-    rs = [g for g in SR.routes(p) if g.block == bi]
-    assert len(rs) < SR.HOST_SEGMENT_GROUPS, "the mirror covers one host segment"
-    win = {g.root for g in rs if g.route == "window"}
-    fac = {}
-    for i, l in enumerate(b.idx[:, lcol]):
-        fac.setdefault(int(l), []).append(i)
-    keys = []
-    for l in win:
-        pp = b.idx[fac[l]][:, pcols]
-        keys.append((int(pp[:, -1].min()) if NP >= 2 else int(pos[pp[:, 0]].min()), l))
-    chunks, cliques, cur, cl = [], [], set(), []
-    for _, l in sorted(keys):
-        vs = set(pos[b.idx[fac[l]][:, pcols].reshape(-1)].tolist())
-        if cur and len(cur) + len(vs - cur) > cap:
-            chunks.append(cur); cliques.append(cl); cur, cl = set(), []
-        cur |= vs; cl.append(sorted(vs))
-    if cur:
-        chunks.append(cur); cliques.append(cl)
-    slots, occ, where = [], [-1]*SR.WIN_NLOC_MAX, {}
-    for ch in chunks:
+    pos = positions(p)
+    groups = block_groups(p, bi)
+    if nseg is None:
+        assert len(groups) < SR.HOST_SEGMENT_GROUPS, "the mirror covers one host segment"
+        nseg = 1
+    ng = len(groups)
+    chunks, cliques, seg = [], [], []
+    for t in range(nseg):
+        cur, cl = set(), []
+        for route, _, f in groups[ng*t//nseg:ng*(t + 1)//nseg]:
+            if route != "window":
+                continue
+            vs = set(pos[b.idx[f][:, pcols].reshape(-1)].tolist())
+            if cur and len(cur) + len(vs - cur) > cap:
+                chunks.append(cur); cliques.append(cl); seg.append(t); cur, cl = set(), []
+            cur |= vs; cl.append(sorted(vs))
+        if cur:
+            chunks.append(cur); cliques.append(cl); seg.append(t)
+    slots = []
+    for c, ch in enumerate(chunks):
         if NP == 1:
             row = sorted(ch) + [-1]*(SR.WIN_NLOC_MAX - len(ch))
         else:
+            if c == 0 or seg[c] != seg[c - 1]:
+                occ, where = [-1]*SR.WIN_NLOC_MAX, {}
             occ = [v if v in ch else -1 for v in occ]
             for v in sorted(ch):
                 if where.get(v, -1) >= 0 and occ[where[v]] == v:
@@ -87,7 +114,10 @@ def plan(p, bi) -> Plan:
             row = list(occ)
         slots.append(row)
     L = max(WIN_RUN_MIN_CHUNKS, -(-len(chunks)//WIN_RUNS)) if NP == 2 else 1
-    runs = [(c, min(c + L, len(chunks))) for c in range(0, len(chunks), L)]
+    runs = []
+    for t in sorted(set(seg)):
+        c0, c1 = seg.index(t), len(seg) - seg[::-1].index(t)
+        runs += [(c, min(c + L, c1)) for c in range(c0, c1, L)]
     ctas = flushed = 0
     for c0, c1 in runs:
         ext = max(max([s + 1 for s in range(SR.WIN_NLOC_MAX) if slots[c][s] >= 0], default=0) for c in range(c0, c1))
