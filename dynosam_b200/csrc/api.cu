@@ -48,6 +48,8 @@ struct HostPrior {      // gtsam::LinearContainerFactor(HessianFactor) over pose
   DevPrior dev{}; int part_off = 0, bs_off = 0;
 };
 
+constexpr int LM_TRACE_COLS = 10;   // columns of a dynoba_get_lm_trace row
+
 }  // namespace
 
 struct dynoba_solver {
@@ -71,6 +73,10 @@ struct dynoba_solver {
   GeneralGroups gen{}; int gen_bs_off = 0;
   std::vector<std::pair<void*, size_t>> allocs;   // device allocations (pointer, bytes)
   cudaEvent_t ev[8]{};
+  // parity hooks: {oldLin, lin, fail} of the latest trial step, and one row per trial of the latest dynoba_optimize
+  // (LM_TRACE_COLS doubles: iterations, inner, lambda, oldLin, lin, err, nerr, solved, success, stop)
+  double last_model[3] = {0.0, 0.0, 0.0};
+  std::vector<double> lm_trace;
   // dynoba_marginal_covariance: Sigma = S^-1 on the band of a plain layout of its own, and the landmark tables, kept from
   // the first call at a linearisation point until the values change
   BandPlan cov_plan{}; double* cov_stage = nullptr; double* cov_lmk = nullptr;
@@ -1180,6 +1186,7 @@ int dynoba_solve(dynoba_handle h, double lambda, double* delta) {
   rc = build_reduced(h, lambda); if (rc) return rc;
   rc = solve_step(h, lambda); if (rc) return rc;
   double s[4]; rc = read_scalars(h, s, true); if (rc) return rc;
+  h->last_model[0] = s[0]; h->last_model[1] = s[1]; h->last_model[2] = s[3];
   CK(cudaGetLastError());
   if (s[3] != 0.0) { h->err = "reduced system not positive definite"; return DYNOBA_ERR_INDETERMINATE; }
   return download_delta(h, delta);
@@ -1405,7 +1412,8 @@ int dynoba_get_variables(dynoba_handle h, int kind, int64_t n, double* out) {
 int dynoba_optimize(dynoba_handle h, const dynoba_lm_params* prm, dynoba_lm_stats* st) {
   if (!h) return DYNOBA_ERR_BAD_ARG;
   dynoba_lm_params P; if (prm) P = *prm; else dynoba_lm_default_params(&P);
-  if (!lm_params_usable(P)) { h->err = "LM parameters under which tryLambda cannot end (see dynoba_lm_params)"; return DYNOBA_ERR_BAD_ARG; }
+  h->lm_trace.clear();
+  if (!lm_params_usable(P)) { h->err = "LM parameters under which the LM loop need not end (see dynoba_lm_params)"; return DYNOBA_ERR_BAD_ARG; }
   int rc = check_ready(h, true); if (rc) return rc;
   dynoba_lm_stats S; std::memset(&S, 0, sizeof(S));
   const int64_t launches0 = h->launches;
@@ -1421,7 +1429,7 @@ int dynoba_optimize(dynoba_handle h, const dynoba_lm_params* prm, dynoba_lm_stat
   double err = sc[2], lambda = P.lambda_initial;
   S.error_initial = err; S.reduced_dim = h->band.n; S.bandwidth = h->band.bw;
   int iterations = 0, inner = 0;
-  if (!(err <= P.error_tol) && P.max_iterations > 0) {
+  if (lm_starts(err, P)) {
     double newError = err, currentError;
     do {
       currentError = newError;
@@ -1436,29 +1444,22 @@ int dynoba_optimize(dynoba_handle h, const dynoba_lm_params* prm, dynoba_lm_stat
         tick(5);
         rc = read_scalars(h, sc, true); if (rc) return rc;
         if (iterations + inner >= 0) { tock(2, 3, S.ms_schur); tock(3, 4, S.ms_factor); tock(4, 5, S.ms_error); }
-        const bool solved = sc[3] == 0.0 && std::isfinite(sc[1]);
-        bool success = false, stop = false; double nerr = INFINITY;
-        if (solved) {
-          const double oldLin = sc[0], lin = sc[1];
-          if (lin >= 0) {
-            nerr = sc[2];
-            const double cost = err - nerr;
-            if (lin > DBL_EPSILON*oldLin) { const double fid = cost/lin; success = fid > P.min_model_fidelity; }
-            if (std::fabs(cost) < P.relative_error_tol*err) stop = true;
-          }
-          if (P.verbosity > 0) std::fprintf(stderr, "[dynoba-lm] it %d inner %d lambda %.3e err %.12e -> %.12e lin %.6e %s\n", iterations, inner, lambda, err, nerr, lin, success ? "ok" : "rej");
-        } else if (P.verbosity > 0) std::fprintf(stderr, "[dynoba-lm] it %d inner %d lambda %.3e solve failed (flag %.0f)\n", iterations, inner, lambda, sc[3]);
-        if (success) { std::swap(h->cur, h->cand); h->linearized = false; lambda = std::max(P.lambda_lower_bound, lambda/P.lambda_factor); err = nerr; iterations++; inner++; break; }
-        else if (!stop) { lambda *= P.lambda_factor; inner++; if (lambda >= P.lambda_upper_bound) break; }
-        else break;
+        const bool solved = sc[3] == 0.0;
+        const double oldLin = sc[0], lin = sc[1], nerr = sc[2];
+        const LmDecision d = lm_decide(solved, oldLin, lin, err, nerr, P);
+        h->last_model[0] = oldLin; h->last_model[1] = lin; h->last_model[2] = sc[3];
+        const double row[LM_TRACE_COLS] = {(double)iterations, (double)inner, lambda, oldLin, lin, err, nerr, (double)solved, (double)d.success, (double)d.stop};
+        h->lm_trace.insert(h->lm_trace.end(), row, row + LM_TRACE_COLS);
+        if (P.verbosity > 0) {
+          if (solved && std::isfinite(lin)) std::fprintf(stderr, "[dynoba-lm] it %d inner %d lambda %.3e err %.12e -> %.12e lin %.6e %s\n", iterations, inner, lambda, err, nerr, lin, d.success ? "ok" : "rej");
+          else std::fprintf(stderr, "[dynoba-lm] it %d inner %d lambda %.3e solve failed (flag %.0f)\n", iterations, inner, lambda, sc[3]);
+        }
+        if (d.success) { std::swap(h->cur, h->cand); h->linearized = false; }
+        if (lm_update(d, nerr, P, lambda, err, iterations, inner)) break;
       }
       { float m2; cudaEventElapsedTime(&m2, ev[0], ev[1]); S.ms_linearize += m2; }
       newError = err;
-    } while (iterations < P.max_iterations &&
-             !((newError <= P.error_tol) ||
-               ((P.relative_error_tol != 0.0) && ((currentError - newError)/currentError <= P.relative_error_tol)) ||
-               ((currentError - newError) <= P.absolute_error_tol)) &&
-             std::isfinite(currentError));
+    } while (lm_continues(iterations, currentError, newError, P));
   }
   tick(7); cudaEventSynchronize(ev[7]); cudaEventElapsedTime(&ms, ev[6], ev[7]); S.ms_total = ms;
   S.iterations = iterations; S.inner_iterations = inner; S.error_final = err; S.lambda_final = lambda;
@@ -1467,6 +1468,20 @@ int dynoba_optimize(dynoba_handle h, const dynoba_lm_params* prm, dynoba_lm_stat
   if (iterations) cov_invalidate(h);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { h->err = cudaGetErrorString(e); return DYNOBA_ERR_CUDA; }
+  return DYNOBA_OK;
+}
+
+int dynoba_last_model(dynoba_handle h, double out[3]) {
+  ARG(h && out, "null argument");
+  for (int i = 0; i < 3; i++) out[i] = h->last_model[i];
+  return DYNOBA_OK;
+}
+
+int dynoba_get_lm_trace(dynoba_handle h, int64_t capacity, double* rows, int64_t* n) {
+  ARG(h && n && capacity >= 0 && (rows || capacity == 0), "null argument");
+  const int64_t have = (int64_t)h->lm_trace.size()/LM_TRACE_COLS;
+  std::copy(h->lm_trace.begin(), h->lm_trace.begin() + std::min(have, capacity)*LM_TRACE_COLS, rows);
+  *n = have;
   return DYNOBA_OK;
 }
 

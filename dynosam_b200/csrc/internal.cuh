@@ -9,24 +9,9 @@
 #include <vector>
 #include "../../include/dynoba.h"
 #include "factors.cuh"
+#include "lm_control.cuh"
 
 namespace dynoba {
-
-// The LM parameters every tryLambda loop (dynoba_optimize, the batch kernels' run_lm) is run with.  That loop ends on a
-// run of failed steps only once lambda reaches lambda_upper_bound, so it refuses (false) what could keep it from getting
-// there: lambda_initial not finite and > 0, lambda_factor not finite and > 1, a NaN upper bound.  It raises the lower
-// bound to DBL_MIN so that a long run of accepted steps cannot divide lambda down to 0; below DBL_MIN, lambda I changes
-// H + lambda I only where H has a diagonal entry below about 1e-290.  A factor so close to 1 that lambda needs more than
-// LM_MAX_CLIMB failed steps to climb from the lowest value it can take to the upper bound is refused as well: that loop
-// would end, but only after up to ~1e16 damped solves.
-constexpr double LM_MAX_CLIMB = 1e4;
-inline bool lm_params_usable(dynoba_lm_params& P) {
-  if (!(std::isfinite(P.lambda_initial) && P.lambda_initial > 0.0) || !(std::isfinite(P.lambda_factor) && P.lambda_factor > 1.0) ||
-      std::isnan(P.lambda_upper_bound)) return false;
-  if (!(P.lambda_lower_bound >= DBL_MIN)) P.lambda_lower_bound = DBL_MIN;
-  const double lo = std::min(P.lambda_initial, P.lambda_lower_bound), hi = std::min(P.lambda_upper_bound, DBL_MAX);
-  return !(hi > lo && std::log(hi) - std::log(lo) > LM_MAX_CLIMB*std::log(P.lambda_factor));
-}
 
 constexpr int TILE = 32;           // band-Cholesky tile edge
 constexpr int TILE2 = TILE*TILE;

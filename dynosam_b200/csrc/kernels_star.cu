@@ -12,8 +12,8 @@
 // One tiny LM (6 + 2N or 18 + 6N unknowns, N <= a few hundred) per object per frame.  Here every problem gets one CTA that runs
 // the WHOLE optimisation on the device (no host round trip per iteration or per outlier round): linearise, eliminate the
 // per-feature unknowns in registers, reduce the small pose system in a fixed order (deterministic), factor it, back-substitute,
-// retract, evaluate, and GTSAM's tryLambda control (LevenbergMarquardtOptimizer.cpp, SURVEY Appendix A.4) -- literally the
-// control loop of api.cu::dynoba_optimize.
+// retract, evaluate, and GTSAM's tryLambda control (LevenbergMarquardtOptimizer.cpp, SURVEY Appendix A.4) -- the decisions
+// of lm_control.cuh, which api.cu::dynoba_optimize takes as well.
 #include <cfloat>
 #include <algorithm>
 #include <mutex>
@@ -53,31 +53,19 @@ __device__ void run_lm(PB& pb, const dynoba_lm_params& P, double& err, int& iter
   err = pb.error_cur();
   double lambda = P.lambda_initial;
   int its = 0;
-  if (!(err <= P.error_tol) && P.max_iterations > 0) {
+  if (lm_starts(err, P)) {
     double newError = err, currentError;
     do {
       currentError = newError;
-      for (;;) {      // tryLambda
+      for (;;) {      // tryLambda (lm_control.cuh)
         double oldLin = 0, newLin = 0, nerr = INFINITY;
-        const bool solved0 = pb.try_step(lambda, oldLin, newLin, nerr);
-        const double lin = oldLin - newLin;
-        const bool solved = solved0 && isfinite(lin);
-        bool success = false, stop = false;
-        if (solved && lin >= 0) {
-          const double cost = err - nerr;
-          if (lin > DBL_EPSILON*oldLin) { const double fid = cost/lin; success = fid > P.min_model_fidelity; }
-          if (fabs(cost) < P.relative_error_tol*err) stop = true;
-        }
-        if (success) { pb.accept(); lambda = fmax(P.lambda_lower_bound, lambda/P.lambda_factor); err = nerr; its++; inner++; break; }
-        else if (!stop) { lambda *= P.lambda_factor; inner++; if (lambda >= P.lambda_upper_bound) break; }
-        else break;
+        const bool solved = pb.try_step(lambda, oldLin, newLin, nerr);
+        const LmDecision d = lm_decide(solved, oldLin, oldLin - newLin, err, nerr, P);
+        if (d.success) pb.accept();
+        if (lm_update(d, nerr, P, lambda, err, its, inner)) break;
       }
       newError = err;
-    } while (its < P.max_iterations &&
-             !((newError <= P.error_tol) ||
-               ((P.relative_error_tol != 0.0) && ((currentError - newError)/currentError <= P.relative_error_tol)) ||
-               ((currentError - newError) <= P.absolute_error_tol)) &&
-             isfinite(currentError));
+    } while (lm_continues(its, currentError, newError, P));
   }
   iterations += its;
 }

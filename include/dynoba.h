@@ -81,7 +81,12 @@ typedef enum {
  * of rejected steps ends only once lambda reaches lambda_upper_bound, which it could otherwise never do.  They also refuse a
  * lambda_factor under which that climb, from min(lambda_initial, lambda_lower_bound) to min(lambda_upper_bound, DBL_MAX),
  * takes more than 10^4 rejected steps.  lambda_lower_bound is raised to DBL_MIN where it is lower, so that lambda cannot
- * underflow to 0 after many accepted steps. */
+ * underflow to 0 after many accepted steps.
+ * They also refuse parameters under which the outer loop need not end.  A give-up (lambda at its upper bound without a
+ * step) leaves the iteration count and the error unchanged, so the loop ends there only if a decrease of exactly 0 counts
+ * as convergence: they require absolute_error_tol >= 0, or relative_error_tol > 0 together with error_tol >= 0 (an error
+ * of exactly 0 passes the relative test never and the error_tol test only then), or error_tol = +inf (the loop then does
+ * not start at a finite error).  NaN satisfies none of these. */
 typedef struct {
   double lambda_initial, lambda_factor, lambda_upper_bound, lambda_lower_bound;
   double min_model_fidelity;
@@ -231,6 +236,17 @@ int dynoba_solve(dynoba_handle h, double lambda, double* delta);
 int dynoba_get_reduced_system(dynoba_handle h, double lambda, double* S, double* g);
 /* values.retract(delta), same layout as dynoba_solve */
 int dynoba_retract(dynoba_handle h, const double* delta);
+/* {oldLin, lin, fail} of the latest trial step, of dynoba_solve or of the last trial of dynoba_optimize: oldLin =
+ * linear.error(0) of the linearised graph, lin = the linearised cost decrease 1/2 g^T delta + 1/2 lambda |delta|^2 (the
+ * decision's denominator), fail != 0 when the damped system was not positive definite (the other two are then
+ * meaningless). */
+int dynoba_last_model(dynoba_handle h, double out[3]);
+/* The trials of the latest dynoba_optimize, one row of 10 doubles each, in order: iterations and inner iterations before
+ * the trial, lambda, oldLin, lin, the current error, the error at the candidate (meaningful only for a valid step: solved,
+ * lin finite and >= 0), solved (1: positive definite; a non-finite lin is a failed solve all the same), success, stop
+ * (tryLambda's stopSearchingLambda).  Every dynoba_optimize call clears it first, a refused one included.  Copies
+ * min(capacity, *n) rows into rows[capacity][10] and sets *n to the number of rows recorded. */
+int dynoba_get_lm_trace(dynoba_handle h, int64_t capacity, double* rows, int64_t* n);
 
 /* ---- graph construction straight into SoA blocks (SURVEY.md 8f-3): what Formulation<MAP>::updateStaticObservations /
  * updateDynamicObservations + the hybrid formulation's callbacks do with the Map

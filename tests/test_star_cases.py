@@ -205,7 +205,10 @@ def test_projection_jacobian_equals_the_oracle():
 
 _BAD_LM = [dict(lambda_initial=0.0), dict(lambda_initial=-1e-5), dict(lambda_initial=float("nan")), dict(lambda_initial=float("inf")),
            dict(lambda_factor=1.0), dict(lambda_factor=0.9), dict(lambda_factor=float("nan")), dict(lambda_factor=float("inf")),
-           dict(lambda_upper_bound=float("nan")), dict(lambda_factor=float(np.nextafter(1.0, 2.0))), dict(lambda_factor=1.05)]
+           dict(lambda_upper_bound=float("nan")), dict(lambda_factor=float(np.nextafter(1.0, 2.0))), dict(lambda_factor=1.05),
+           # tolerances under which a give-up need not end the outer loop
+           dict(relative_error_tol=0.0, absolute_error_tol=-1.0), dict(relative_error_tol=float("nan"), absolute_error_tol=float("nan")),
+           dict(relative_error_tol=1e-5, absolute_error_tol=-1.0, error_tol=-1.0)]
 
 
 @pytest.mark.parametrize("bad", _BAD_LM, ids=lambda d: "-".join(f"{k}={v}" for k, v in d.items()))
