@@ -44,6 +44,9 @@ class GraphBuilder:
         L.dynoba_builder_block_info.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), c_i64p, C.POINTER(C.c_int32), c_i64p, c_dp, C.POINTER(C.c_int32)]
         L.dynoba_builder_get_block.argtypes = [C.c_void_p, C.c_int32, c_ip, c_dp, c_dp, c_ip]
         L.dynoba_builder_emit.argtypes = [C.c_void_p, C.c_void_p]
+        L.dynoba_builder_set_imu.argtypes = [C.c_void_p, C.c_int32, c_dp, c_dp]
+        L.dynoba_builder_nav_counts.argtypes = [C.c_void_p, c_i64p, c_i64p]
+        L.dynoba_builder_get_nav_variables.argtypes = [C.c_void_p, c_dp, c_dp, c_ip, c_ip, c_u64p, c_u64p]
         prm = BuilderParams(); L.dynoba_builder_default_params(C.byref(prm))
         for k, v in params.items():
             if k in ("odometry_sigma", "smoothing_sigma"):
@@ -89,6 +92,11 @@ class GraphBuilder:
     def set_keyframe_pose(self, obj, keyframe, L_e):
         L_e = np.ascontiguousarray(L_e, np.float64).reshape(12); self._ck(self.lib.dynoba_builder_set_keyframe_pose(self.h, int(obj), int(keyframe), _dp(L_e)))
 
+    def set_imu(self, frame, record, sqrt_info):
+        """the preintegrated measurement from the previous frame to `frame`: record[70] (COMBINED_IMU15 layout) and R[15, 15]"""
+        z = np.ascontiguousarray(record, np.float64).reshape(70); R = np.ascontiguousarray(sqrt_info, np.float64).reshape(225)
+        self._ck(self.lib.dynoba_builder_set_imu(self.h, int(frame), _dp(z), _dp(R)))
+
     def problem(self) -> Problem:
         """the emitted SoA problem as a Problem container"""
         L = self.lib
@@ -101,12 +109,21 @@ class GraphBuilder:
         for bi in range(nb.value):
             ty = C.c_int32(); n = C.c_int64(); sd = C.c_int32(); sc = C.c_int64(); k = C.c_double(); ha = C.c_int32()
             self._ck(L.dynoba_builder_block_info(self.h, bi, C.byref(ty), C.byref(n), C.byref(sd), C.byref(sc), C.byref(k), C.byref(ha)))
-            idx = np.zeros((n.value, ARITY[ty.value]), np.int32); meas = np.zeros((n.value, max(MEAS_DIM[ty.value], 1))); sig = np.zeros(sd.value)
+            idx = np.zeros((n.value, ARITY[ty.value]), np.int32); meas = np.zeros((n.value, max(MEAS_DIM[ty.value], 1)))
+            sig = np.zeros(sd.value) if sc.value == 1 else np.zeros((sc.value, sd.value))
             auxi = np.zeros(n.value, np.int32)
             self._ck(L.dynoba_builder_get_block(self.h, bi, idx.ctypes.data_as(c_ip), _dp(meas) if MEAS_DIM[ty.value] else C.cast(None, c_dp), _dp(sig),
                                                 auxi.ctypes.data_as(c_ip) if ha.value else C.cast(None, c_ip)))
             blocks.append(FactorBlock(ty.value, idx, meas if MEAS_DIM[ty.value] else None, sig, k.value, auxi if ha.value else None))
-        return Problem(pose, point, aux_pose=aux, blocks=blocks, pose_order=order, pose_keys=pk, point_keys=qk)
+        nv = C.c_int64(); nb6 = C.c_int64()
+        self._ck(L.dynoba_builder_nav_counts(self.h, C.byref(nv), C.byref(nb6)))
+        vel = np.zeros((nv.value, 3)); bias = np.zeros((nb6.value, 6))
+        vo = np.zeros(nv.value, np.int32); bo = np.zeros(nb6.value, np.int32)
+        self.nav_keys = (np.zeros(nv.value, np.uint64), np.zeros(nb6.value, np.uint64))
+        self._ck(L.dynoba_builder_get_nav_variables(self.h, _dp(vel), _dp(bias), vo.ctypes.data_as(c_ip), bo.ctypes.data_as(c_ip),
+                                                    self.nav_keys[0].ctypes.data_as(c_u64p), self.nav_keys[1].ctypes.data_as(c_u64p)))
+        nav = dict(vel=vel, bias=bias, vel_order=vo, bias_order=bo) if nv.value else {}
+        return Problem(pose, point, aux_pose=aux, blocks=blocks, pose_order=order, pose_keys=pk, point_keys=qk, **nav)
 
     def emit(self, solver):
         """hand the arrays to a dynosam_b200.binding.Solver handle (no Problem container in between)"""

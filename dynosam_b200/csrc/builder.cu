@@ -22,6 +22,13 @@
 //     object pose L_k per (object, frame) initialised motion * L_k-1 when the front end gave a motion and L_k-1 exists, else the
 //     centroid of the object's points at k with identity rotation (:205-232), LandmarkPoseSmoothingFactor over three consecutive
 //     frames (:259-306); no prior on the object poses.
+//   * IMU (dynoba_builder_set_imu; RegularBackendModule.cc:528-570, VisionImuBackendModule.hpp:114-290): when any frame has
+//     a preintegrated measurement, every frame after the first must have one and frame ids must be consecutive.  Velocity
+//     and bias variables V_k, b_k per frame; V_0 = 0, b_0 = 0 with PriorFactor<Vector3> (sigma 1e-5) and
+//     PriorFactor<ConstantBias> (sigma 0.1 x3, 0.01 x3); for k >= 1 (X_k, V_k) = predict(X_k-1, V_k-1, b_k-1) (the
+//     preintegrated measurement of frame k), b_k = b_k-1, CombinedImuFactor(X_k-1, V_k-1, X_k, V_k, b_k-1, b_k) in place of
+//     the odometry BetweenFactor, and the predicted X_k stands for the front end's pose everywhere: as the initial value of
+//     the camera pose and of every point (and key-frame centroid) initialised from frame k.  The first frame keeps its pose.
 // Host code only (no kernel): it lives in libdynoba.so because its output is the library's input.
 #include <algorithm>
 #include <array>
@@ -34,6 +41,7 @@
 
 #include "../../include/dynoba.h"
 #include "se3.cuh"
+#include "preint.cuh"
 
 using namespace dynoba;
 
@@ -41,7 +49,9 @@ namespace {
 
 struct Obs { int32_t frame; int64_t tracklet; int32_t object; double z[3]; };
 struct Block { int type = 0; std::vector<int32_t> idx, aux; std::vector<double> meas, sigma; int sigma_dim = 1; bool bcast = true; double k = 0; bool has_aux = false;
-               int64_t n() const { static const int ar[11] = {1, 2, 2, 2, 3, 3, 3, 4, 3, 3, 2}; return (int64_t)idx.size()/ar[type]; } };
+               int64_t sigma_count = 1;       // 1: one sigma for the block; n: one per factor (COMBINED_IMU15's R)
+               int64_t n() const { static const int ar[14] = {1, 2, 2, 2, 3, 3, 3, 4, 3, 3, 2, 1, 1, 6}; return (int64_t)idx.size()/ar[type]; } };
+struct ImuMeas { double z[70]; double R[225]; };
 
 Pose pose_from(const double* p) { Pose P; for (int i = 0; i < 9; i++) P.R[i] = p[i]; for (int i = 0; i < 3; i++) P.t[i] = p[9 + i]; return P; }
 void pose_to(const Pose& P, double* p) { for (int i = 0; i < 9; i++) p[i] = P.R[i]; for (int i = 0; i < 3; i++) p[9 + i] = P.t[i]; }
@@ -58,8 +68,10 @@ struct dynoba_builder {
   std::map<int32_t, Pose> odom;                                  // frame -> relative pose from the previous frame
   std::vector<Obs> stat, dyn;
   std::map<std::pair<int32_t, int32_t>, Pose> motion_init, keyframe_pose;    // (object, frame)
+  std::map<int32_t, ImuMeas> imu;                                // frame -> preintegrated measurement from the previous frame
   // products
   std::vector<double> pose, point, aux; std::vector<int32_t> order; std::vector<uint64_t> pose_keys, point_keys;
+  std::vector<double> vel, bias; std::vector<int32_t> nav_order; std::vector<uint64_t> vel_keys, bias_keys;
   std::vector<Block> blocks;
 };
 
@@ -108,17 +120,53 @@ int dynoba_builder_set_keyframe_pose(dynoba_builder_handle b, int32_t object, in
   BARG(b && L_e, "null"); b->keyframe_pose[{object, keyframe}] = pose_from(L_e); b->finalized = false; return DYNOBA_OK;
 }
 
+int dynoba_builder_set_imu(dynoba_builder_handle b, int32_t frame, const double* record, const double* sqrt_info) {
+  BARG(b && record && sqrt_info && frame >= 0, "bad IMU measurement");
+  for (int i = 0; i < 70; i++) BARG(std::isfinite(record[i]), "IMU record not finite");
+  BARG(record[15] > 0.0, "IMU record with deltaTij <= 0");
+  for (int i = 0; i < 225; i++) BARG(std::isfinite(sqrt_info[i]), "IMU square-root information not finite");
+  for (int i = 0; i < 15; i++) BARG(sqrt_info[16*i] > 0.0, "IMU square-root information with a non-positive diagonal");
+  ImuMeas& m = b->imu[frame];
+  std::copy(record, record + 70, m.z); std::copy(sqrt_info, sqrt_info + 225, m.R);
+  b->finalized = false; return DYNOBA_OK;
+}
+
 int dynoba_builder_finalize(dynoba_builder_handle b) {
   BARG(b, "null builder");
   if (b->finalized) return DYNOBA_OK;
   const dynoba_builder_params& P = b->prm;
   b->pose.clear(); b->point.clear(); b->aux.clear(); b->order.clear(); b->pose_keys.clear(); b->point_keys.clear(); b->blocks.clear();
+  b->vel.clear(); b->bias.clear(); b->nav_order.clear(); b->vel_keys.clear(); b->bias_keys.clear();
   BARG(!b->frames.empty(), "no frames");
+  // ---- initial camera poses: the front end's, or with IMU the prediction chain from the first frame
+  std::map<int32_t, Pose> X0;
+  for (auto& kv : b->frames) X0[kv.first] = kv.second.first;
+  const bool imu = !b->imu.empty();
+  if (imu) {
+    for (auto& kv : b->imu) BARG(b->frames.count(kv.first), "IMU measurement on a frame that was not added");
+    int32_t prev = -1; Pose X; double v[3] = {0, 0, 0}; const double bz[6] = {0, 0, 0, 0, 0, 0};
+    for (auto& kv : b->frames) {
+      const int32_t f = kv.first;
+      if (prev < 0) X = kv.second.first;
+      else {
+        BARG(f == prev + 1, "frame ids are not consecutive while IMU is present");
+        auto it = b->imu.find(f);
+        BARG(it != b->imu.end(), "IMU measurements on some frames but not on others");
+        Pose Xn; double vn[3];
+        preint_predict(it->second.z, X, v, bz, Xn, vn);             // b_k-1 = b_0 = 0
+        X = Xn; for (int a = 0; a < 3; a++) v[a] = vn[a];
+        X0[f] = X;
+      }
+      b->vel.insert(b->vel.end(), v, v + 3); b->bias.insert(b->bias.end(), bz, bz + 6);
+      b->nav_order.push_back(f); b->vel_keys.push_back(sym('V', (uint64_t)f)); b->bias_keys.push_back(sym('b', (uint64_t)f));
+      prev = f;
+    }
+  }
   // ---- camera poses, in frame order
   std::map<int32_t, int32_t> cam_index;
   for (auto& kv : b->frames) {
     cam_index[kv.first] = (int32_t)cam_index.size();
-    double p[12]; pose_to(kv.second.first, p); b->pose.insert(b->pose.end(), p, p + 12);
+    double p[12]; pose_to(X0[kv.first], p); b->pose.insert(b->pose.end(), p, p + 12);
     b->order.push_back(kv.first); b->pose_keys.push_back(sym('X', (uint64_t)kv.first));
   }
   auto cam = [&](int32_t f) -> int32_t { auto it = cam_index.find(f); return it == cam_index.end() ? -1 : it->second; };
@@ -151,7 +199,7 @@ int dynoba_builder_finalize(dynoba_builder_handle b) {
       auto& t = tracks[tid];
       const int32_t pi = (int32_t)(b->point.size()/3);
       const Obs& o0 = stat[t[0]];
-      double w[3]; se3_transform_from(b->frames[o0.frame].first, o0.z, w);          // initial value: X_k z of the first observation that enters
+      double w[3]; se3_transform_from(X0[o0.frame], o0.z, w);          // initial value: X_k z of the first observation that enters
       b->point.insert(b->point.end(), w, w + 3); b->point_keys.push_back(sym('l', (uint64_t)tid));
       for (size_t i : t) { const Obs& o = stat[i]; blk.idx.push_back(cam(o.frame)); blk.idx.push_back(pi); blk.meas.insert(blk.meas.end(), o.z, o.z + 3); }
     }
@@ -175,7 +223,7 @@ int dynoba_builder_finalize(dynoba_builder_handle b) {
       for (size_t k = 0; k < t.size(); k++) { const Obs& o = dyn[t[k]];
         if (k > 0) BARG(o.frame > dyn[t[k-1]].frame, "a tracklet is observed twice in one frame");
         if (wcpe || k > 0) var_index[{o.object, o.frame}] = -1;
-        double w[3]; se3_transform_from(b->frames[o.frame].first, o.z, w);
+        double w[3]; se3_transform_from(X0[o.frame], o.z, w);
         auto& c = centroid[{o.object, o.frame}]; for (int a = 0; a < 3; a++) c.first[a] += w[a]; c.second++; }
     }
     for (auto& kv : var_index) {                                       // std::map order: object-major, frames ascending
@@ -199,7 +247,7 @@ int dynoba_builder_finalize(dynoba_builder_handle b) {
       auto& t = tracks[key];
       for (size_t k = 0; k < t.size(); k++) { const Obs& o = dyn[t[k]];
         const int32_t pi = (int32_t)(b->point.size()/3);
-        double w[3]; se3_transform_from(b->frames[o.frame].first, o.z, w);                 // X_k z (dynamicPointUpdateCallback)
+        double w[3]; se3_transform_from(X0[o.frame], o.z, w);                 // X_k z (dynamicPointUpdateCallback)
         b->point.insert(b->point.end(), w, w + 3); b->point_keys.push_back(sym('m', cantor((uint64_t)o.tracklet, (uint64_t)o.frame)));
         ptp.idx.push_back(cam(o.frame)); ptp.idx.push_back(pi); ptp.meas.insert(ptp.meas.end(), o.z, o.z + 3);
         if (k > 0) { mot.idx.push_back(pi - 1); mot.idx.push_back(pi);
@@ -251,7 +299,7 @@ int dynoba_builder_finalize(dynoba_builder_handle b) {
       if (it != b->keyframe_pose.end()) Le = it->second;
       else {
         Le = identity_pose(); double c[3] = {0, 0, 0}; int cnt = 0;
-        for (auto& o : dyn) if (o.object == segs[s].object && o.frame == segs[s].keyframe) { double w[3]; se3_transform_from(b->frames[o.frame].first, o.z, w); for (int k = 0; k < 3; k++) c[k] += w[k]; cnt++; }
+        for (auto& o : dyn) if (o.object == segs[s].object && o.frame == segs[s].keyframe) { double w[3]; se3_transform_from(X0[o.frame], o.z, w); for (int k = 0; k < 3; k++) c[k] += w[k]; cnt++; }
         for (int k = 0; k < 3; k++) Le.t[k] = cnt ? c[k]/cnt : 0.0;
       }
       segs[s].aux = (int32_t)(b->aux.size()/12); double p[12]; pose_to(Le, p); b->aux.insert(b->aux.end(), p, p + 12);
@@ -267,7 +315,7 @@ int dynoba_builder_finalize(dynoba_builder_handle b) {
       const int32_t pi = (int32_t)(b->point.size()/3);
       // m_L = L_e^-1 (e_H_k)^-1 X_k z at the first observation (HybridObjectMotion::projectToObject3)
       const Pose Le = pose_from(&b->aux[(size_t)12*segs[s0].aux]); const Pose E = pose_from(&b->pose[(size_t)12*motion_index[{o0.object, o0.frame}]]);
-      double w[3], q[3], m[3]; se3_transform_from(b->frames[o0.frame].first, o0.z, w); se3_transform_to(E, w, q); se3_transform_to(Le, q, m);
+      double w[3], q[3], m[3]; se3_transform_from(X0[o0.frame], o0.z, w); se3_transform_to(E, w, q); se3_transform_to(Le, q, m);
       b->point.insert(b->point.end(), m, m + 3); b->point_keys.push_back(sym('m', cantor((uint64_t)key.second, 0)));
       for (size_t i : t) { const Obs& o = dyn[i];
         blk.idx.push_back(cam(o.frame)); blk.idx.push_back(motion_index[{o.object, o.frame}]); blk.idx.push_back(pi);
@@ -294,10 +342,28 @@ int dynoba_builder_finalize(dynoba_builder_handle b) {
     Block od; od.type = DYNOBA_BETWEEN6; od.sigma.assign(P.odometry_sigma, P.odometry_sigma + 6); od.sigma_dim = 6;
     int32_t prev = -1;
     for (auto& kv : b->frames) {
-      if (prev >= 0 && kv.second.second) { od.idx.push_back(cam(prev)); od.idx.push_back(cam(kv.first)); double p[12]; pose_to(b->odom[kv.first], p); od.meas.insert(od.meas.end(), p, p + 12); }
+      if (prev >= 0 && kv.second.second && !imu) { od.idx.push_back(cam(prev)); od.idx.push_back(cam(kv.first)); double p[12]; pose_to(b->odom[kv.first], p); od.meas.insert(od.meas.end(), p, p + 12); }
       prev = kv.first;
     }
     if (od.n()) b->blocks.push_back(std::move(od));
+  }
+  // ---- IMU chain: priors on V_0, b_0 and one CombinedImuFactor per later frame (velocity / bias index = camera index)
+  if (imu) {
+    Block pv; pv.type = DYNOBA_PRIOR_VEL3; pv.sigma = { 1e-5 }; pv.idx.push_back(0); pv.meas.assign(3, 0.0);
+    Block pb; pb.type = DYNOBA_PRIOR_BIAS6; pb.sigma = { 0.1, 0.1, 0.1, 0.01, 0.01, 0.01 }; pb.sigma_dim = 6; pb.idx.push_back(0); pb.meas.assign(6, 0.0);
+    b->blocks.push_back(std::move(pv)); b->blocks.push_back(std::move(pb));
+    Block im; im.type = DYNOBA_COMBINED_IMU15; im.sigma_dim = 225;
+    int32_t k = 0;
+    for (auto& kv : b->frames) {
+      if (k > 0) {
+        const int32_t q[6] = { k - 1, k - 1, k, k, k - 1, k };
+        const ImuMeas& m = b->imu[kv.first];
+        im.idx.insert(im.idx.end(), q, q + 6); im.meas.insert(im.meas.end(), m.z, m.z + 70); im.sigma.insert(im.sigma.end(), m.R, m.R + 225);
+      }
+      k++;
+    }
+    im.sigma_count = im.n();
+    if (im.n()) b->blocks.push_back(std::move(im));
   }
   b->finalized = true;
   return DYNOBA_OK;
@@ -320,7 +386,7 @@ int dynoba_builder_block_info(dynoba_builder_handle b, int32_t bi, int32_t* type
   BARG(b, "null builder"); int rc = dynoba_builder_finalize(b); if (rc) return rc;
   BARG(bi >= 0 && bi < (int32_t)b->blocks.size(), "bad block index");
   const Block& k = b->blocks[bi];
-  if (type) *type = k.type; if (n) *n = k.n(); if (sigma_dim) *sigma_dim = k.sigma_dim; if (sigma_count) *sigma_count = 1;
+  if (type) *type = k.type; if (n) *n = k.n(); if (sigma_dim) *sigma_dim = k.sigma_dim; if (sigma_count) *sigma_count = k.sigma_count;
   if (robust_k) *robust_k = k.k; if (has_aux) *has_aux = k.has_aux ? 1 : 0;
   return DYNOBA_OK;
 }
@@ -338,9 +404,33 @@ int dynoba_builder_emit(dynoba_builder_handle b, dynoba_handle h) {
   if ((rc = dynoba_set_variables(h, DYNOBA_POSE6, (int64_t)b->pose.size()/12, b->pose_keys.data(), b->pose.data()))) return rc;
   if ((rc = dynoba_set_variables(h, DYNOBA_POINT3, (int64_t)b->point.size()/3, b->point_keys.data(), b->point.data()))) return rc;
   if (!b->aux.empty() && (rc = dynoba_set_aux_poses(h, (int64_t)b->aux.size()/12, b->aux.data()))) return rc;
+  const int64_t nn = (int64_t)b->nav_order.size();
+  if (nn) {
+    if ((rc = dynoba_set_variables(h, DYNOBA_VEL3, nn, b->vel_keys.data(), b->vel.data()))) return rc;
+    if ((rc = dynoba_set_variables(h, DYNOBA_BIAS6, nn, b->bias_keys.data(), b->bias.data()))) return rc;
+  }
   for (auto& k : b->blocks)
-    if ((rc = dynoba_add_factors(h, k.type, k.n(), k.idx.data(), k.meas.empty() ? nullptr : k.meas.data(), k.sigma.data(), k.sigma_dim, 1, k.k, k.has_aux ? k.aux.data() : nullptr))) return rc;
-  return dynoba_set_pose_order(h, (int64_t)b->order.size(), b->order.data());
+    if ((rc = dynoba_add_factors(h, k.type, k.n(), k.idx.data(), k.meas.empty() ? nullptr : k.meas.data(), k.sigma.data(), k.sigma_dim, k.sigma_count, k.k, k.has_aux ? k.aux.data() : nullptr))) return rc;
+  if ((rc = dynoba_set_pose_order(h, (int64_t)b->order.size(), b->order.data()))) return rc;
+  if (nn) {
+    if ((rc = dynoba_set_variable_order(h, DYNOBA_VEL3, nn, b->nav_order.data()))) return rc;
+    if ((rc = dynoba_set_variable_order(h, DYNOBA_BIAS6, nn, b->nav_order.data()))) return rc;
+  }
+  return DYNOBA_OK;
+}
+int dynoba_builder_nav_counts(dynoba_builder_handle b, int64_t* n_vel, int64_t* n_bias) {
+  BARG(b, "null builder"); int rc = dynoba_builder_finalize(b); if (rc) return rc;
+  if (n_vel) *n_vel = (int64_t)b->vel.size()/3; if (n_bias) *n_bias = (int64_t)b->bias.size()/6;
+  return DYNOBA_OK;
+}
+int dynoba_builder_get_nav_variables(dynoba_builder_handle b, double* vel, double* bias, int32_t* vel_order, int32_t* bias_order,
+                                     uint64_t* vel_keys, uint64_t* bias_keys) {
+  BARG(b, "null builder"); int rc = dynoba_builder_finalize(b); if (rc) return rc;
+  if (vel) std::copy(b->vel.begin(), b->vel.end(), vel); if (bias) std::copy(b->bias.begin(), b->bias.end(), bias);
+  if (vel_order) std::copy(b->nav_order.begin(), b->nav_order.end(), vel_order);
+  if (bias_order) std::copy(b->nav_order.begin(), b->nav_order.end(), bias_order);
+  if (vel_keys) std::copy(b->vel_keys.begin(), b->vel_keys.end(), vel_keys); if (bias_keys) std::copy(b->bias_keys.begin(), b->bias_keys.end(), bias_keys);
+  return DYNOBA_OK;
 }
 
 }  // extern "C"

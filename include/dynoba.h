@@ -294,6 +294,21 @@ int dynoba_builder_block_info(dynoba_builder_handle b, int32_t block, int32_t* t
                               int64_t* sigma_count, double* robust_k, int32_t* has_aux);
 int dynoba_builder_get_block(dynoba_builder_handle b, int32_t block, int32_t* idx, double* meas, double* sigma, int32_t* aux_idx);
 int dynoba_builder_emit(dynoba_builder_handle b, dynoba_handle h);
+/* Visual-inertial graphs (RegularBackendModule.cc:528-570, VisionImuBackendModule.hpp:114-290): record[70] (the
+ * DYNOBA_COMBINED_IMU15 layout, e.g. from dynoba_imu_preintegrate_batch) and sqrt_info[225] (R, row-major) of the
+ * preintegrated measurement from the previous frame to `frame`.  Refused (DYNOBA_ERR_BAD_ARG): a non-finite record or R,
+ * deltaTij <= 0, a non-positive diagonal of R.  A builder that receives one builds the IMU chain at finalize: V_k, b_k per
+ * frame (V_0 = b_0 = 0 with PriorFactor<Vector3> sigma 1e-5 and PriorFactor<ConstantBias> sigma 0.1 x3, 0.01 x3), for each
+ * later frame (X_k, V_k) = predict(X_k-1, V_k-1, b_k-1), b_k = b_k-1, a COMBINED_IMU15 in place of the odometry
+ * BetweenFactor, and the predicted X_k as the initial value of the camera pose and of every point initialised from frame k.
+ * A measurement on the first frame only marks IMU as present.  finalize refuses (DYNOBA_ERR_BAD_ARG) a frame after the first
+ * without a measurement, non-consecutive frame ids, and a measurement on a frame that was not added.  Without set_imu the
+ * builder emits what it always did.  dynoba_builder_emit also sets the velocities / biases (keys Symbol('V', frame),
+ * Symbol('b', frame)) and their order hints (the frame id). */
+int dynoba_builder_set_imu(dynoba_builder_handle b, int32_t frame, const double* record, const double* sqrt_info);
+int dynoba_builder_nav_counts(dynoba_builder_handle b, int64_t* n_vel, int64_t* n_bias);
+int dynoba_builder_get_nav_variables(dynoba_builder_handle b, double* vel, double* bias, int32_t* vel_order, int32_t* bias_order,
+                                     uint64_t* vel_keys, uint64_t* bias_keys);
 
 /* ---- batched star problems (SURVEY.md 8f-2) --------------------------------------------------------------------------
  * The front end's per-object refinements, for ALL objects of a frame (or of many frames) in ONE launch: one CTA per problem
@@ -381,6 +396,35 @@ int dynoba_pnp_ransac_batch(int device, int32_t n_problems, const int32_t* offse
                             const double* points_world, const double* keypoints, const dynoba_pnp_ransac_params* prm,
                             double* pose_out, uint8_t* inlier_out, int32_t* n_inliers, int32_t* status, int32_t* iterations,
                             int32_t* skipped, int32_t* best_hypothesis, int32_t* hyp_counts);
+
+/* Combined IMU preintegration of many frame intervals in one launch: gtsam::PreintegratedCombinedMeasurements (GTSAM 4.2.0,
+ * ManifoldPreintegration, no Coriolis) integrateMeasurement once per sample, as ImuFrontend::preintegrateImuMeasurements
+ * (dynosam/src/frontend/imu/ImuFrontend.cc:121-143) does, then noiseModel::Gaussian::Covariance(preintMeasCov): the inputs of
+ * one DYNOBA_COMBINED_IMU15 factor per interval, without GTSAM.  The mathematics is stated in dynosam_b200/csrc/preint.cuh.
+ * All pointers are HOST memory.  Interval p owns the samples [offsets[p], offsets[p+1]) (offsets[0] = 0): stamps[m] in
+ * seconds and acc_gyr[m][6] (accelerometer then gyroscope, the sensor frame); it integrates m - 1 steps with
+ * dt = stamps[i+1] - stamps[i], so the last sample's values are not used.  bias_hat[p][6] (acc, gyro) may be NULL: zero.
+ * Outputs per interval: record[70] (the COMBINED_IMU15 layout, n_gravity in its last three doubles), cov[225] (preintMeasCov,
+ * rows theta, p, v, bias_acc, bias_gyro) and sqrt_info[225] (R upper triangular, positive diagonal, R^T R = cov^-1, row-major)
+ * and status (DYNOBA_PREINT_OK, or DYNOBA_PREINT_NOT_PD with sqrt_info zeroed: cov is not positive definite).
+ * Refused with DYNOBA_ERR_BAD_ARG before any device work: n_intervals < 0 or >= 2^24, NULL arrays, offsets[0] != 0, an
+ * interval with fewer than 2 samples, a dt <= 0 or not finite (the reference's CHECK_GT), non-finite samples, biases or
+ * parameters.  n_intervals = 0 is a no-op.  The call shares the batch entry points' per-device stream and workspace. */
+enum { DYNOBA_PREINT_OK = 0, DYNOBA_PREINT_NOT_PD = 1 };
+typedef struct {
+  double n_gravity[3];
+  double accelerometer_cov[9], gyroscope_cov[9], integration_cov[9];   /* 3x3 row-major */
+  double bias_acc_cov[9], bias_omega_cov[9];
+  double bias_acc_omega_int[36];                                        /* 6x6 row-major, (acc, gyro) */
+  double body_P_sensor[12];                                             /* R row-major | t, used when has_body_P_sensor */
+  int32_t has_body_P_sensor;
+} dynoba_imu_params;
+/* gtsam::PreintegrationCombinedParams(n_gravity) defaults of GTSAM 4.2.0 [GTSAM-ext]: every covariance the identity
+ * (accelerometer, gyroscope, integration, biasAcc, biasOmega, biasAccOmegaInt), body_P_sensor unset; n_gravity = 0 here. */
+void dynoba_imu_default_params(dynoba_imu_params* p);
+int dynoba_imu_preintegrate_batch(int device, const dynoba_imu_params* params, int32_t n_intervals, const int32_t* offsets,
+                                  const double* stamps, const double* acc_gyr, const double* bias_hat, double* record,
+                                  double* cov, double* sqrt_info, int32_t* status);
 
 #ifdef __cplusplus
 }
