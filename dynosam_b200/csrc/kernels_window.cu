@@ -31,9 +31,12 @@ __device__ __forceinline__ double acc_at(const double (&acc)[36], int e) {
   return v;
 }
 
-constexpr int STG_WARPS = 4;          // K4a: landmarks per CTA
+constexpr int STG_WARPS = 2;          // K4a: warps per CTA (NP = 2: 43 KB of slot images, five CTAs per SM)
 constexpr int ACC_THREADS = WIN_ACC_WARPS*32;
 constexpr int WSLOT = WIN_SLOT_DOUBLES;   // 42 doubles = 21 x 16 B: odd stride => conflict-free LDS.128 across slots
+// K4a: a lane's NP slots in the shared-memory image, in 16-byte units, padded to an odd count so that the lanes' STS.128
+// are conflict-free (NP = 2: 43 instead of 42)
+template <int NP> constexpr int STG_LANE16 = NP*(WSLOT/2) | 1;
 
 // slot meta word: bits 0-7 local variable (255 = not on the window path), 8-15 factor within the landmark, 16-47 group
 __device__ __forceinline__ double pack_meta(unsigned lvar, unsigned fac, unsigned g) {
@@ -41,10 +44,12 @@ __device__ __forceinline__ double pack_meta(unsigned lvar, unsigned fac, unsigne
 }
 
 // One landmark staged by a group of W = 32 or 16 lanes (`hl` = lane within the group, `mask` = the group's lanes): lane
-// `hl` owns factor `hl` of the landmark.
+// `hl` owns factor `hl` of the landmark.  The lanes build the landmark's slots in `img` (W lanes of STG_LANE16<NP>
+// 16-byte units), and the group then writes them as one contiguous range, 16 bytes per lane and store: a lane storing
+// its own 336-byte slot would touch 32 half-filled sectors per warp store.
 template <int NP, int PCOL0, int LCOL, int W>
 __device__ __forceinline__ void stage_landmark(const DevBlock& blk, const DevWindows& Wn, double lambda, int* __restrict__ fail,
-                                               int g, int hl, unsigned mask) {
+                                               int g, int hl, unsigned mask, double* __restrict__ img) {
   constexpr int JC = NP*6 + 3;
   auto gsum = [&](double x) {
 #pragma unroll
@@ -106,54 +111,65 @@ __device__ __forceinline__ void stage_landmark(const DevBlock& blk, const DevWin
     for (int i = hl; i < T*NP; i += W) slots[((size_t)f0*NP + i)*WSLOT + 39] = pack_meta(255u, 0u, (unsigned)g);
     return;
   }
-  if (!have) return;
-  const double m00 = 1.0/l00, m11 = 1.0/l11, m22 = 1.0/l22;
-  const double m10 = -l10*m00*m11, m21 = -l21*m11*m22, m20 = -(l20*m00 + l21*m10)*m22;
-  const double y0 = m00*gl[0], y1 = m10*gl[0] + m11*gl[1], y2 = m20*gl[0] + m21*gl[1] + m22*gl[2];   // y = M g_l
-  double Bh[9];                        // Bh = B M^T
+  if (have) {
+    const double m00 = 1.0/l00, m11 = 1.0/l11, m22 = 1.0/l22;
+    const double m10 = -l10*m00*m11, m21 = -l21*m11*m22, m20 = -(l20*m00 + l21*m10)*m22;
+    const double y0 = m00*gl[0], y1 = m10*gl[0] + m11*gl[1], y2 = m20*gl[0] + m21*gl[1] + m22*gl[2];   // y = M g_l
+    double Bh[9];                      // Bh = B M^T
 #pragma unroll
-  for (int r = 0; r < 3; r++) {
-    Bh[r*3 + 0] = Bm[r*3]*m00;
-    Bh[r*3 + 1] = Bm[r*3]*m10 + Bm[r*3 + 1]*m11;
-    Bh[r*3 + 2] = Bm[r*3]*m20 + Bm[r*3 + 1]*m21 + Bm[r*3 + 2]*m22;
+    for (int r = 0; r < 3; r++) {
+      Bh[r*3 + 0] = Bm[r*3]*m00;
+      Bh[r*3 + 1] = Bm[r*3]*m10 + Bm[r*3 + 1]*m11;
+      Bh[r*3 + 2] = Bm[r*3]*m20 + Bm[r*3 + 1]*m21 + Bm[r*3 + 2]*m22;
+    }
+    double rb[3];                      // rb = b - Bh y
+#pragma unroll
+    for (int r = 0; r < 3; r++) rb[r] = bb[r] - (Bh[r*3]*y0 + Bh[r*3 + 1]*y1 + Bh[r*3 + 2]*y2);
+#pragma unroll
+    for (int s = 0; s < NP; s++) {
+      double2* o = reinterpret_cast<double2*>(img) + hl*STG_LANE16<NP> + s*(WSLOT/2);
+      const double* A = Aall + s*18;
+      double w[18];                    // w[k*6 + c] = What[c][k] = sum_r A[r][c] Bh[r][k]
+#pragma unroll
+      for (int k = 0; k < 3; k++)
+#pragma unroll
+        for (int c = 0; c < 6; c++) w[k*6 + c] = A[c]*Bh[k] + A[6 + c]*Bh[3 + k] + A[12 + c]*Bh[6 + k];
+#pragma unroll
+      for (int i = 0; i < 9; i++) o[i] = make_double2(w[2*i], w[2*i + 1]);
+#pragma unroll
+      for (int i = 0; i < 9; i++) o[9 + i] = make_double2(A[2*i], A[2*i + 1]);
+      o[18] = make_double2(rb[0], rb[1]);
+      o[19] = make_double2(rb[2], pack_meta((unsigned)Wn.lvar[(size_t)s*blk.stride + f], (unsigned)hl, (unsigned)g));
+      o[20] = make_double2(0.0, 0.0);  // the pad too: every sector of the range is written whole
+    }
   }
-  double rb[3];                        // rb = b - Bh y
-#pragma unroll
-  for (int r = 0; r < 3; r++) rb[r] = bb[r] - (Bh[r*3]*y0 + Bh[r*3 + 1]*y1 + Bh[r*3 + 2]*y2);
-#pragma unroll
-  for (int s = 0; s < NP; s++) {
-    double2* o = reinterpret_cast<double2*>(slots + ((size_t)f*NP + s)*WSLOT);
-    const double* A = Aall + s*18;
-    double w[18];                      // w[k*6 + c] = What[c][k] = sum_r A[r][c] Bh[r][k]
-#pragma unroll
-    for (int k = 0; k < 3; k++)
-#pragma unroll
-      for (int c = 0; c < 6; c++) w[k*6 + c] = A[c]*Bh[k] + A[6 + c]*Bh[3 + k] + A[12 + c]*Bh[6 + k];
-#pragma unroll
-    for (int i = 0; i < 9; i++) o[i] = make_double2(w[2*i], w[2*i + 1]);
-#pragma unroll
-    for (int i = 0; i < 9; i++) o[9 + i] = make_double2(A[2*i], A[2*i + 1]);
-    o[18] = make_double2(rb[0], rb[1]);
-    o[19] = make_double2(rb[2], pack_meta((unsigned)Wn.lvar[(size_t)s*blk.stride + f], (unsigned)hl, (unsigned)g));
-  }
+  __syncwarp(mask);
+  const double2* src = reinterpret_cast<const double2*>(img);
+  double2* dst = reinterpret_cast<double2*>(slots + (size_t)f0*NP*WSLOT);
+  constexpr int PAD = STG_LANE16<NP> - NP*(WSLOT/2);   // 16-byte units after each lane's slots in the image
+  for (int i = hl; i < T*NP*(WSLOT/2); i += W) dst[i] = src[i + PAD*(i/(NP*(WSLOT/2)))];
+  __syncwarp(mask);                    // the image is read before the group's next landmark overwrites it
 }
 
 // A warp takes two consecutive landmarks: side by side on its two half-warps when both have at most 16 factors (the
 // common case: tracks average 8.5 / 11.4 observations), one after the other on all 32 lanes otherwise.
 template <int NP, int PCOL0, int LCOL>
-__global__ void __launch_bounds__(STG_WARPS*32, 3)
+__global__ void __launch_bounds__(STG_WARPS*32, NP == 2 ? 5 : 6)   // the CTAs per SM the slot images / registers allow
 schur_stage_kernel(DevBlock blk, DevWindows Wn, double lambda, int* __restrict__ fail) {
-  const int lane = threadIdx.x & 31;
-  const int g0 = 2*(blockIdx.x*STG_WARPS + (threadIdx.x >> 5));
+  __shared__ __align__(16) double img[STG_WARPS][32*2*STG_LANE16<NP>];   // a warp's slot images: 32 lanes' slots
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int g0 = 2*(blockIdx.x*STG_WARPS + warp);
   if (g0 >= blk.n_groups) return;
   const bool two = g0 + 1 < blk.n_groups;
   const int T0 = blk.grp_ptr[g0 + 1] - blk.grp_ptr[g0], T1 = two ? blk.grp_ptr[g0 + 2] - blk.grp_ptr[g0 + 1] : 0;
   if (two && T0 <= 16 && T1 <= 16) {
     const int half = lane >> 4;
-    stage_landmark<NP, PCOL0, LCOL, 16>(blk, Wn, lambda, fail, g0 + half, lane & 15, half ? 0xffff0000u : 0x0000ffffu);
+    stage_landmark<NP, PCOL0, LCOL, 16>(blk, Wn, lambda, fail, g0 + half, lane & 15, half ? 0xffff0000u : 0x0000ffffu,
+                                        img[warp] + half*16*2*STG_LANE16<NP>);
   } else {
 #pragma unroll 1
-    for (int k = 0; k < (two ? 2 : 1); k++) stage_landmark<NP, PCOL0, LCOL, 32>(blk, Wn, lambda, fail, g0 + k, lane, 0xffffffffu);
+    for (int k = 0; k < (two ? 2 : 1); k++)
+      stage_landmark<NP, PCOL0, LCOL, 32>(blk, Wn, lambda, fail, g0 + k, lane, 0xffffffffu, img[warp]);
   }
 }
 
@@ -350,6 +366,9 @@ int launch_schur_window(const DevBlock& blk, const DevWindows& Wn, const DevBand
   if (!attr) {
     cudaFuncSetAttribute(schur_accum_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)acc_smem());
     cudaFuncSetAttribute(schur_accum_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)acc_smem());
+    // the stage kernels' occupancy is set by their slot images: ask for the whole unified L1 as shared memory
+    cudaFuncSetAttribute(schur_stage_kernel<1, 0, 6>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(schur_stage_kernel<2, 0, 12>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
     attr = true;
   }
   const int sgrid = ((blk.n_groups + 1)/2 + STG_WARPS - 1)/STG_WARPS;
