@@ -13,6 +13,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdynoba.so")
 
 POSE6, POINT3, FLOW2, VEL3, BIAS6 = 0, 1, 2, 3, 4
+TANGENT_DIM = {POSE6: 6, VEL3: 3, BIAS6: 6}          # pose-like kinds: tangent dimension of a prior slot / kept variable
+LIN_DIM = {POSE6: 12, VEL3: 3, BIAS6: 6}             # doubles of a slot's linearisation point
 OK, ERR_BAD_ARG, ERR_STATE, ERR_CUDA, ERR_INDETERMINATE, ERR_UNSUPPORTED, ERR_COMM = 0, -1, -2, -3, -4, -5, -6
 
 c_dp = C.POINTER(C.c_double)
@@ -24,7 +26,7 @@ REDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.
 EXPORTS = [
     "dynoba_version", "dynoba_status_string", "dynoba_last_error", "dynoba_create", "dynoba_destroy",
     "dynoba_lm_default_params", "dynoba_set_variables", "dynoba_set_aux_poses", "dynoba_set_calibration",
-    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_marginal", "dynoba_marginal_covariance", "dynoba_finalize", "dynoba_error",
+    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_add_linear_prior_vars", "dynoba_marginal", "dynoba_marginal_vars", "dynoba_marginal_covariance", "dynoba_finalize", "dynoba_error",
     "dynoba_optimize", "dynoba_get_variables", "dynoba_get_keys", "dynoba_num_variables", "dynoba_problem_info", "dynoba_window_census",
     "dynoba_linearize", "dynoba_linearize_block", "dynoba_get_linearization", "dynoba_get_factor_errors", "dynoba_solve",
     "dynoba_get_reduced_system", "dynoba_retract", "dynoba_last_model", "dynoba_get_lm_trace", "dynoba_flow_pose_default_params", "dynoba_flow_pose_batch",
@@ -113,7 +115,9 @@ def load():
         L.dynoba_set_tuning.argtypes = [C.c_void_p, C.c_char_p, C.c_double]
         L.dynoba_fp64_rate.argtypes = [C.c_void_p, c_dp]
         L.dynoba_add_linear_prior.argtypes = [C.c_void_p, C.c_int32, c_ip, c_dp, c_dp, c_dp, C.c_double]
+        L.dynoba_add_linear_prior_vars.argtypes = [C.c_void_p, C.c_int32, c_ip, c_ip, c_dp, c_dp, c_dp, C.c_double]
         L.dynoba_marginal.argtypes = [C.c_void_p, C.c_int32, c_ip, c_dp, c_dp]
+        L.dynoba_marginal_vars.argtypes = [C.c_void_p, C.c_int32, c_ip, c_ip, c_dp, c_dp, c_dp]
         L.dynoba_marginal_covariance.argtypes = [C.c_void_p, C.c_int, C.c_int64, c_ip, c_dp]
         L.dynoba_finalize.argtypes = [C.c_void_p]
         L.dynoba_error.argtypes = [C.c_void_p, c_dp]
@@ -226,7 +230,10 @@ class Solver:
             if order is not None:
                 self._ck(L.dynoba_set_variable_order(self.h, kind, arr.shape[0], _ip(order)))
         for pr in getattr(p, "linear_priors", []):
-            self.add_linear_prior(pr["idx"], pr["lin"], pr["G"], pr["g"], pr.get("f", 0.0))
+            if "kind" in pr:
+                self.add_linear_prior_vars(pr["kind"], pr["idx"], pr["lin"], pr["G"], pr["g"], pr.get("f", 0.0))
+            else:
+                self.add_linear_prior(pr["idx"], pr["lin"], pr["G"], pr["g"], pr.get("f", 0.0))
 
     def add_factors(self, b):
         self._ck(self.lib.dynoba_add_factors(self.h, b.type, b.n, _ip(b.idx), _dp(b.meas) if b.meas is not None else C.cast(None, c_dp),
@@ -239,6 +246,37 @@ class Solver:
         G = np.ascontiguousarray(G, dtype=np.float64); g = np.ascontiguousarray(g, dtype=np.float64)
         assert G.shape == (6*idx.size, 6*idx.size) and g.shape == (6*idx.size,)
         self._ck(self.lib.dynoba_add_linear_prior(self.h, idx.size, _ip(idx), _dp(lin), _dp(G), _dp(g), float(f)))
+
+    def add_linear_prior_vars(self, kinds, idx, lin, G, g, f=0.0):
+        """add_linear_prior over pose-like variables of kinds POSE6 / VEL3 / BIAS6 (dynoba_add_linear_prior_vars).
+        lin: the slots' linearisation points packed in slot order (12 / 3 / 6 doubles each), or a list of one array per
+        slot; G [D, D], g [D] in the slots' tangent layout (6 / 3 / 6 scalars each).  Sizes that disagree with the kinds
+        raise DynobaError(ERR_BAD_ARG) before the call."""
+        kinds = np.ascontiguousarray(kinds, dtype=np.int32).reshape(-1); idx = np.ascontiguousarray(idx, dtype=np.int32).reshape(-1)
+        if isinstance(lin, (list, tuple)):
+            lin = np.concatenate([np.asarray(x, dtype=np.float64).reshape(-1) for x in lin]) if len(lin) else np.zeros(0)
+        lin = np.ascontiguousarray(lin, dtype=np.float64).reshape(-1)
+        G = np.ascontiguousarray(G, dtype=np.float64); g = np.ascontiguousarray(g, dtype=np.float64).reshape(-1)
+        if kinds.size != idx.size:
+            raise DynobaError(ERR_BAD_ARG, "kinds and idx differ in length")
+        if all(int(k) in TANGENT_DIM for k in kinds):       # (another kind is refused by the library itself)
+            D = sum(TANGENT_DIM[int(k)] for k in kinds); nl = sum(LIN_DIM[int(k)] for k in kinds)
+            if lin.size != nl or G.shape != (D, D) or g.shape != (D,):
+                raise DynobaError(ERR_BAD_ARG, f"lin ({lin.size}), G {G.shape} and g {g.shape} must have {nl}, ({D}, {D}) and ({D},) "
+                                               "elements for these kinds")
+        self._ck(self.lib.dynoba_add_linear_prior_vars(self.h, kinds.size, _ip(kinds), _ip(idx), _dp(lin), _dp(G), _dp(g), float(f)))
+
+    def marginal_vars(self, kinds, idx):
+        """(G, g, f): marginal information of the pose-like variables (kinds[k], idx[k]) -- poses, velocities and biases of
+        the last frames -- at the current values, in the caller's order and tangent layout, and the constant f of the
+        remaining HessianFactor (dynoba_marginal_vars)"""
+        kinds = np.ascontiguousarray(kinds, dtype=np.int32).reshape(-1); idx = np.ascontiguousarray(idx, dtype=np.int32).reshape(-1)
+        if kinds.size != idx.size:
+            raise DynobaError(ERR_BAD_ARG, "kinds and idx differ in length")
+        D = sum(TANGENT_DIM.get(int(k), 0) for k in kinds)
+        G = np.zeros((max(D, 1), max(D, 1))); g = np.zeros(max(D, 1)); f = C.c_double()
+        self._ck(self.lib.dynoba_marginal_vars(self.h, kinds.size, _ip(kinds), _ip(idx), _dp(G), _dp(g), C.byref(f)))
+        return G[:D, :D].copy(), g[:D].copy(), f.value
 
     def marginal(self, keep_idx):
         """(G, g): marginal information of the pose-like variables keep_idx (the last ones in frame order) at the current values"""

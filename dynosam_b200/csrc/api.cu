@@ -44,7 +44,8 @@ struct HostBlock {
 };
 
 struct HostPrior {      // gtsam::LinearContainerFactor(HessianFactor) over pose-like variables
-  std::vector<int32_t> idx; std::vector<double> lin, G, g; double f = 0;
+  std::vector<int32_t> kind, idx; std::vector<double> lin, G, g; double f = 0;
+  bool legacy = false;  // added through dynoba_add_linear_prior (pose-only graphs)
   DevPrior dev{}; int part_off = 0, bs_off = 0;
 };
 
@@ -285,6 +286,15 @@ static std::vector<uint64_t>* key_store(dynoba_solver* h, int kind) {
 }
 static int kind_width(int kind) { return kind == DYNOBA_POSE6 ? 12 : (kind == DYNOBA_POINT3 || kind == DYNOBA_VEL3 ? 3 : (kind == DYNOBA_BIAS6 ? 6 : 2)); }
 static bool has_nav(const dynoba_solver* h) { return !h->vel.empty() || !h->bias.empty(); }
+// tangent dimension of a pose-like kind (a prior slot / a kept variable of a marginal); 0 for the other kinds
+static int tangent_dim(int kind) { return kind == DYNOBA_POSE6 || kind == DYNOBA_BIAS6 ? 6 : (kind == DYNOBA_VEL3 ? 3 : 0); }
+// index of a pose-like variable among [poses | velocities | biases] (h->pos[] order), -1 when out of range
+static int64_t poselike_index(const dynoba_solver* h, int kind, int32_t ix) {
+  const int64_t np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3, nb = (int64_t)h->bias.size()/6;
+  const int64_t lim = kind == DYNOBA_POSE6 ? np : (kind == DYNOBA_VEL3 ? nv : nb);
+  if (ix < 0 || ix >= lim) return -1;
+  return kind == DYNOBA_POSE6 ? ix : (kind == DYNOBA_VEL3 ? np + ix : np + nv + ix);
+}
 
 int dynoba_set_variables(dynoba_handle h, int kind, int64_t n, const uint64_t* keys, const double* data) {
   ARG(h, "null handle"); ARG(n >= 0 && (n == 0 || data), "null data");
@@ -384,17 +394,42 @@ int dynoba_add_factors(dynoba_handle h, int type, int64_t n, const int32_t* idx,
   return DYNOBA_OK;
 }
 
-int dynoba_add_linear_prior(dynoba_handle h, int32_t n, const int32_t* pose_idx, const double* lin_poses, const double* G, const double* g, double f) {
-  ARG(h, "null handle"); ARG(n > 0 && n <= 512 && pose_idx && lin_poses && G && g, "bad prior");
-  if (has_nav(h)) { h->err = "dynoba_add_linear_prior is not available with velocity / bias variables"; return DYNOBA_ERR_UNSUPPORTED; }
-  HostPrior P; P.idx.assign(pose_idx, pose_idx + n); P.lin.assign(lin_poses, lin_poses + (size_t)12*n);
-  P.G.assign(G, G + (size_t)36*n*n); P.g.assign(g, g + (size_t)6*n); P.f = f;
-  { std::vector<int32_t> srt = P.idx; std::sort(srt.begin(), srt.end()); ARG(std::adjacent_find(srt.begin(), srt.end()) == srt.end(), "a prior lists a variable twice"); }
-  for (int r = 0; r < 6*n; r++) for (int c = 0; c < r; c++)
-    ARG(std::fabs(P.G[(size_t)r*6*n + c] - P.G[(size_t)c*6*n + r]) <= 1e-9*(std::fabs(P.G[(size_t)r*6*n + r]) + std::fabs(P.G[(size_t)c*6*n + c]) + 1e-300), "prior information matrix is not symmetric");
+}  // extern "C"
+
+// the one implementation behind dynoba_add_linear_prior and dynoba_add_linear_prior_vars (indices are checked at finalize,
+// where the variable counts are known)
+static int add_prior(dynoba_solver* h, int32_t n, const int32_t* kind, const int32_t* idx, const double* lin, const double* G,
+                     const double* g, double f, bool legacy) {
+  ARG(n > 0 && n <= 512 && kind && idx && lin && G && g, "bad prior");
+  HostPrior P; P.kind.assign(kind, kind + n); P.idx.assign(idx, idx + n); P.f = f; P.legacy = legacy;
+  size_t nlin = 0, dim = 0;
+  for (int i = 0; i < n; i++) {
+    const int d = tangent_dim(kind[i]);
+    ARG(d, "a prior slot must be of kind DYNOBA_POSE6, DYNOBA_VEL3 or DYNOBA_BIAS6");
+    dim += d; nlin += kind[i] == DYNOBA_POSE6 ? 12 : d;
+  }
+  P.lin.assign(lin, lin + nlin); P.G.assign(G, G + dim*dim); P.g.assign(g, g + dim);
+  { std::vector<std::pair<int32_t, int32_t>> srt(n); for (int i = 0; i < n; i++) srt[i] = { kind[i], idx[i] };
+    std::sort(srt.begin(), srt.end()); ARG(std::adjacent_find(srt.begin(), srt.end()) == srt.end(), "a prior lists a variable twice"); }
+  for (size_t r = 0; r < dim; r++) for (size_t c = 0; c < r; c++)
+    ARG(std::fabs(P.G[r*dim + c] - P.G[c*dim + r]) <= 1e-9*(std::fabs(P.G[r*dim + r]) + std::fabs(P.G[c*dim + c]) + 1e-300), "prior information matrix is not symmetric");
   h->priors.push_back(std::move(P));
   if (h->finalized) free_device(h);
   return DYNOBA_OK;
+}
+
+extern "C" {
+
+int dynoba_add_linear_prior(dynoba_handle h, int32_t n, const int32_t* pose_idx, const double* lin_poses, const double* G, const double* g, double f) {
+  ARG(h, "null handle"); ARG(n > 0 && n <= 512 && pose_idx && lin_poses && G && g, "bad prior");
+  if (has_nav(h)) { h->err = "dynoba_add_linear_prior is not available with velocity / bias variables"; return DYNOBA_ERR_UNSUPPORTED; }
+  const std::vector<int32_t> kind(n, DYNOBA_POSE6);
+  return add_prior(h, n, kind.data(), pose_idx, lin_poses, G, g, f, true);
+}
+int dynoba_add_linear_prior_vars(dynoba_handle h, int32_t n, const int32_t* kind, const int32_t* idx, const double* lin,
+                                 const double* G, const double* g, double f) {
+  ARG(h, "null handle");
+  return add_prior(h, n, kind, idx, lin, G, g, f, false);
 }
 
 int dynoba_set_pose_order(dynoba_handle h, int64_t n, const int32_t* rank) {
@@ -473,7 +508,8 @@ static int finalize_impl(dynoba_solver* h) {
   ARG(h->hint.empty() || (int64_t)h->hint.size() == np, "pose order hint length != number of poses");
   ARG(h->vhint.empty() || (int64_t)h->vhint.size() == nv, "velocity order hint length != number of velocities");
   ARG(h->bhint.empty() || (int64_t)h->bhint.size() == nb, "bias order hint length != number of biases");
-  if (NP > np && (!h->priors.empty() || h->world > 1 || h->reduce)) {
+  const bool legacy_prior = std::any_of(h->priors.begin(), h->priors.end(), [](const HostPrior& P) { return P.legacy; });
+  if (NP > np && (legacy_prior || h->world > 1 || h->reduce)) {
     h->err = "velocity / bias variables cannot be combined with dynoba_add_linear_prior, dynoba_set_shard or dynoba_set_reduce";
     return DYNOBA_ERR_UNSUPPORTED;
   }
@@ -562,7 +598,10 @@ static int finalize_impl(dynoba_solver* h) {
   for (int64_t g = 0; g < nl; g++) if (gmax[g] >= 0) spread = std::max(spread, gmax[g] - gmin[g]);
   for (auto& P : h->priors) {       // a prior couples all of its variables
     int lo = INT32_MAX, hi = -1;
-    for (int32_t ix : P.idx) { ARG(ix >= 0 && ix < np, "prior variable out of range"); lo = std::min(lo, h->pos[ix]); hi = std::max(hi, h->pos[ix]); }
+    for (size_t i = 0; i < P.idx.size(); i++) {
+      const int64_t v = poselike_index(h, P.kind[i], P.idx[i]);
+      ARG(v >= 0, "prior variable out of range"); lo = std::min(lo, h->pos[v]); hi = std::max(hi, h->pos[v]);
+    }
     spread = std::max(spread, hi - lo); pos_lo = std::min(pos_lo, lo); pos_hi = std::max(pos_hi, hi);
   }
   // group rank: by first pose position, then root id
@@ -831,12 +870,19 @@ static int finalize_impl(dynoba_solver* h) {
     h->gen.n_groups = (int)gl0.size(); h->gen.blocks = dblk; h->gen.gptr = dgptr; h->gen.refs = drefs; h->gen.gl0 = dgl0; h->gen.gnl = dgnl;
   }
   for (auto& P : h->priors) {
-    const int n = (int)P.idx.size(); std::vector<int32_t> ppos(n);
-    for (int i = 0; i < n; i++) ppos[i] = h->pos[P.idx[i]];
-    int* dpos; double *dlin, *dG, *dg, *dd, *dgc; int rc;
-    if ((rc = upload(h, &dpos, ppos)) || (rc = upload(h, &dlin, P.lin)) || (rc = upload(h, &dG, P.G)) || (rc = upload(h, &dg, P.g))) return rc;
-    if ((rc = dalloc(h, &dd, (size_t)6*n))) return rc; if ((rc = dalloc(h, &dgc, (size_t)6*n))) return rc;
-    P.dev = DevPrior{ n, dpos, dlin, dG, dg, P.f, dd, dgc };
+    const int n = (int)P.idx.size(); std::vector<int4> slot(n); std::vector<int32_t> sidx;
+    for (int i = 0, lo = 0; i < n; i++) {
+      const int p = h->pos[poselike_index(h, P.kind[i], P.idx[i])], d = tangent_dim(P.kind[i]);
+      slot[i] = make_int4(P.kind[i], p, lo, (int)sidx.size());
+      lo += P.kind[i] == DYNOBA_POSE6 ? 12 : d;
+      for (int c = 0; c < d; c++) sidx.push_back(6*p + c);      // (velocity: c < 3, never an inert scalar)
+    }
+    const int dim = (int)sidx.size();
+    int4* dslot; int* dsidx; double *dlin, *dG, *dg, *dd, *dgc; int rc;
+    if ((rc = upload(h, &dslot, slot)) || (rc = upload(h, &dsidx, sidx)) || (rc = upload(h, &dlin, P.lin)) || (rc = upload(h, &dG, P.G)) ||
+        (rc = upload(h, &dg, P.g))) return rc;
+    if ((rc = dalloc(h, &dd, (size_t)dim))) return rc; if ((rc = dalloc(h, &dgc, (size_t)dim))) return rc;
+    P.dev = DevPrior{ n, dim, dslot, dsidx, dlin, dG, dg, P.f, dd, dgc };
     P.part_off = part; part += 1; P.bs_off = bs; bs += 1;
   }
   h->n_nav = 0; h->d_nav = nullptr;
@@ -1218,28 +1264,36 @@ int dynoba_retract(dynoba_handle h, const double* delta) {
   return DYNOBA_OK;
 }
 
+}  // extern "C"
+
 // Marginal information of the LAST n_keep pose-like variables (solver order) at the current values: every landmark and
 // every other pose-like variable eliminated.  The band Cholesky already leaves a Schur complement in the columns it does
 // not factor, so this is one plain band factorisation that stops at the tile holding the first kept variable; the few
-// scalars of that tile that precede the kept block are eliminated on the host.
-int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_idx, double* G, double* g) {
-  int rc = check_ready(h, true); if (rc) return rc;
-  ARG(n_keep > 0 && keep_pose_idx && G && g, "bad arguments");
-  if (has_nav(h)) { h->err = "dynoba_marginal is not available with velocity / bias variables"; return DYNOBA_ERR_UNSUPPORTED; }
-  const int64_t np = h->cur.np;
-  ARG(n_keep <= np, "more variables than there are");
+// scalars of that tile that precede the kept block are eliminated on the host.  The one implementation behind
+// dynoba_marginal and dynoba_marginal_vars; f == nullptr skips the constant (and the full solve it takes).
+static int marginal_impl(dynoba_solver* h, int32_t n_keep, const int32_t* kind, const int32_t* idx, double* G, double* g, double* f) {
+  const int64_t NP = h->cur.np;
+  ARG(n_keep <= NP, "more variables than there are");
   if (h->world > 1) { h->err = "dynoba_marginal is a single-GPU entry point"; return DYNOBA_ERR_UNSUPPORTED; }
-  std::vector<int> slot(n_keep, -1);                    // kept variable k sits at solver position np - n_keep + slot
+  std::vector<int> slot(n_keep, -1), off(n_keep + 1, 0);   // kept variable k sits at solver position NP - n_keep + slot
   for (int k = 0; k < n_keep; k++) {
-    ARG(keep_pose_idx[k] >= 0 && keep_pose_idx[k] < np, "variable out of range");
-    const int p = h->pos[keep_pose_idx[k]] - (int)(np - n_keep);
+    ARG(tangent_dim(kind[k]), "a kept variable must be of kind DYNOBA_POSE6, DYNOBA_VEL3 or DYNOBA_BIAS6");
+    const int64_t v = poselike_index(h, kind[k], idx[k]);
+    ARG(v >= 0, "variable out of range");
+    const int p = h->pos[v] - (int)(NP - n_keep);
     if (p < 0) { h->err = "the kept variables must be the last ones of the elimination order (most recent frames)"; return DYNOBA_ERR_UNSUPPORTED; }
-    slot[k] = p;
+    slot[k] = p; off[k + 1] = off[k] + tangent_dim(kind[k]);
   }
   { std::vector<int> srt = slot; std::sort(srt.begin(), srt.end()); ARG(std::adjacent_find(srt.begin(), srt.end()) == srt.end(), "a variable is listed twice"); }
+  int rc;
   if (!h->linearized) do_linearize(h);
+  double lin_s[4] = {0, 0, 0, 0};
+  if (f) {   // undamped solve of the whole system: scalars[0] = 1/2 sum |b_w|^2, scalars[1] = 1/2 g^T H^-1 g
+    if ((rc = build_reduced(h, 0.0)) || (rc = solve_step(h, 0.0)) || (rc = read_scalars(h, lin_s, true))) return rc;
+    if (lin_s[3] != 0.0) { h->err = "the reduced system is not positive definite"; return DYNOBA_ERR_INDETERMINATE; }
+  }
   // a second, plain layout whose factorisation stops before the kept block
-  const int p0 = 6*(int)(np - n_keep), K0 = p0/TILE;
+  const int p0 = 6*(int)(NP - n_keep), K0 = p0/TILE;
   BandPlan mp;
   if ((rc = plain_plan_create(h, mp, K0))) return rc;
   const int NT = mp.band.NT, WBm = mp.band.WB;
@@ -1280,13 +1334,51 @@ int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_id
       rhs[i] -= l*rhs[k];
     }
   }
-  const int dim = 6*n_keep;
-  for (int a = 0; a < n_keep; a++) for (int r = 0; r < 6; r++) {
+  // caller's slot order and tangent layout; the inert scalars of a kept velocity are left out
+  const int dim = off[n_keep];
+  for (int a = 0; a < n_keep; a++) for (int r = 0; r < off[a + 1] - off[a]; r++) {
     const int qi = e + 6*slot[a] + r;
-    g[6*a + r] = rhs[qi];
-    for (int b = 0; b < n_keep; b++) for (int c = 0; c < 6; c++) G[(size_t)(6*a + r)*dim + 6*b + c] = M[(size_t)qi*m + e + 6*slot[b] + c];
+    g[off[a] + r] = rhs[qi];
+    for (int b = 0; b < n_keep; b++) for (int c = 0; c < off[b + 1] - off[b]; c++) G[(size_t)(off[a] + r)*dim + off[b] + c] = M[(size_t)qi*m + e + 6*slot[b] + c];
+  }
+  if (f) {
+    // f = sum |b_w|^2 - g_e^T H_ee^-1 g_e, and g_e^T H_ee^-1 g_e = g^T H^-1 g - g_m^T G_m^-1 g_m (block elimination of H):
+    // the last term by a dense Cholesky of the kept block
+    std::vector<double> L(G, G + (size_t)dim*dim), y(g, g + dim);
+    for (int j = 0; j < dim; j++) {
+      double d = L[(size_t)j*dim + j];
+      for (int k = 0; k < j; k++) d -= L[(size_t)j*dim + k]*L[(size_t)j*dim + k];
+      if (!(d > 0.0)) { h->err = "the marginal information is not positive definite"; return DYNOBA_ERR_INDETERMINATE; }
+      L[(size_t)j*dim + j] = std::sqrt(d);
+      for (int i = j + 1; i < dim; i++) {
+        double v = L[(size_t)i*dim + j];
+        for (int k = 0; k < j; k++) v -= L[(size_t)i*dim + k]*L[(size_t)j*dim + k];
+        L[(size_t)i*dim + j] = v/L[(size_t)j*dim + j];
+      }
+    }
+    double gGg = 0.0;
+    for (int i = 0; i < dim; i++) {
+      for (int k = 0; k < i; k++) y[i] -= L[(size_t)i*dim + k]*y[k];
+      y[i] /= L[(size_t)i*dim + i]; gGg += y[i]*y[i];
+    }
+    *f = 2.0*lin_s[0] - (2.0*lin_s[1] - gGg);
   }
   return DYNOBA_OK;
+}
+
+extern "C" {
+
+int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_idx, double* G, double* g) {
+  int rc = check_ready(h, true); if (rc) return rc;
+  ARG(n_keep > 0 && keep_pose_idx && G && g, "bad arguments");
+  if (has_nav(h)) { h->err = "dynoba_marginal is not available with velocity / bias variables"; return DYNOBA_ERR_UNSUPPORTED; }
+  const std::vector<int32_t> kind(n_keep, DYNOBA_POSE6);
+  return marginal_impl(h, n_keep, kind.data(), keep_pose_idx, G, g, nullptr);
+}
+int dynoba_marginal_vars(dynoba_handle h, int32_t n_keep, const int32_t* kind, const int32_t* idx, double* G, double* g, double* f) {
+  int rc = check_ready(h, true); if (rc) return rc;
+  ARG(n_keep > 0 && kind && idx && G && g, "bad arguments");
+  return marginal_impl(h, n_keep, kind, idx, G, g, f);
 }
 
 }  // extern "C"

@@ -232,12 +232,15 @@ struct DevWindows {
   double* slots;                 // [n*npose_slots][WIN_SLOT_DOUBLES] staged slots in factor order (HBM scratch)
 };
 
-// Dense quadratic prior over n pose-like variables (kernels_prior.cu): gtsam::LinearContainerFactor(HessianFactor)
+// Dense quadratic prior over n pose-like variables (kernels_prior.cu): gtsam::LinearContainerFactor(HessianFactor).
+// Slot i has kind POSE6, VEL3 or BIAS6 and tangent dimension 6, 3 or 6; dim = the sum, in slot order.
 struct DevPrior {
-  int n; const int* pos;          // solver positions of the variables
-  const double* lin;              // [n][12] linearisation point
-  const double* G; const double* g; double f;   // [6n][6n] row-major information, [6n] linear term, constant
-  double* delta; double* gcur;    // [6n] local coordinates / g - G delta at the current linearisation
+  int n, dim;
+  const int4* slot;               // [n] (kind, solver position, first element in lin, first tangent scalar)
+  const int* sidx;                // [dim] solver scalar index of every tangent scalar (position*6 + sub)
+  const double* lin;              // linearisation point, packed: 12 (pose) / 3 (velocity) / 6 (bias) doubles per slot
+  const double* G; const double* g; double f;   // [dim][dim] row-major information, [dim] linear term, constant
+  double* delta; double* gcur;    // [dim] local coordinates / g - G delta at the current linearisation
 };
 int launch_prior_eval(const DevPrior& P, const DevVars& v, double* partial, int store, cudaStream_t s);
 int launch_prior_accum(const DevPrior& P, const DevBand& B, cudaStream_t s);

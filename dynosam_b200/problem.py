@@ -82,7 +82,8 @@ class Problem:
     point_keys: Optional[np.ndarray] = None
     meta: dict = field(default_factory=dict)
     # gtsam::LinearContainerFactor(HessianFactor) priors over pose-like variables (sliding-window marginals): dicts with
-    # idx int32[n], lin [n,12], G [6n,6n], g [6n], f
+    # idx int32[n], lin [n,12], G [6n,6n], g [6n], f over poses; with a "kind" array (POSE6 / VEL3 / BIAS6 per slot) over
+    # any pose-like variables, lin packed 12 / 3 / 6 per slot and G, g in the slots' tangent layout (6 / 3 / 6)
     linear_priors: list = field(default_factory=list)
     # navigation variables of visual-inertial graphs: nav-frame velocities [n_vel, 3], IMU biases [n_bias, 6] (acc | gyro),
     # and their ordering hints (frame id), as pose_order is for the poses
@@ -121,7 +122,8 @@ class Problem:
     def copy(self) -> "Problem":
         return Problem(self.pose.copy(), self.point.copy(), self.flow.copy(), self.aux_pose, self.calib, self.blocks,
                        self.pose_order, self.pose_keys, self.point_keys, dict(self.meta), vel=self.vel.copy(),
-                       bias=self.bias.copy(), vel_order=self.vel_order, bias_order=self.bias_order)
+                       bias=self.bias.copy(), vel_order=self.vel_order, bias_order=self.bias_order,
+                       linear_priors=list(self.linear_priors))
 
     def jacobian_bytes(self) -> int:
         """Algorithmic bytes of one materialising linearize() (SURVEY.md 8d): every factor record read once,

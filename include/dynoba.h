@@ -142,17 +142,45 @@ int dynoba_add_factors(dynoba_handle h, int type, int64_t n, const int32_t* idx,
  * (row-major, symmetric) and g[6n] = information matrix / vector in the tangent space at the linearisation point
  * ([omega; v] per pose), f = constant:  error(x) = 1/2 d^T G d - g^T d + 1/2 f  with d_i = Logmap(lin_i^-1 x_i);
  * linearising at x gives HessianFactor(G, g - G d, ...) as GTSAM does.  A variable may appear once per prior.  With
- * several ranks, give a prior to exactly one of them. */
+ * several ranks, give a prior to exactly one of them.  Poses only: refused (DYNOBA_ERR_UNSUPPORTED) once the graph has
+ * velocity / bias variables, also when they are set after the prior (then at finalize); dynoba_add_linear_prior_vars
+ * takes those graphs. */
 int dynoba_add_linear_prior(dynoba_handle h, int32_t n, const int32_t* pose_idx, const double* lin_poses,
                             const double* G, const double* g, double f);
+/* The same factor over n pose-like variables of any of the kinds DYNOBA_POSE6, DYNOBA_VEL3 and DYNOBA_BIAS6 (slot i:
+ * kind[i], index idx[i] among the variables of that kind), on any graph, visual-inertial ones included.  Slot i has the
+ * tangent dimension d_i = 6 / 3 / 6 and its linearisation point takes 12 (R row-major | t) / 3 / 6 (acc, gyro) doubles
+ * of lin, packed in slot order; G[D][D] and g[D], D = sum d_i, follow the slots' tangent layout.  Local coordinates are
+ * those of gtsam::Values::localCoordinates: Logmap(lin_i^-1 x_i) for a pose, x_i - lin_i for a velocity or a bias.
+ * DYNOBA_ERR_BAD_ARG: n outside [1, 512], a NULL array, another kind, a variable listed twice, an asymmetric G; an index
+ * out of range is refused when the graph is built (finalize or the first compute call).  The caller must size lin, G
+ * and g by the kinds; nothing else can check that. */
+int dynoba_add_linear_prior_vars(dynoba_handle h, int32_t n, const int32_t* kind, const int32_t* idx, const double* lin,
+                                 const double* G, const double* g, double f);
 /* Marginal information (G[6k][6k], g[6k]) of the k pose-like variables keep_pose_idx at the current values, every other
  * variable -- all landmarks and the older pose-like variables -- eliminated: what SlidingWindowOptimization::
  * CalculateMarginalFactors computes with eliminatePartialMultifrontal (:165-190), ready to be passed to
  * dynoba_add_linear_prior of the next window together with the current values of the kept variables as linearisation
  * point.  The kept variables must be the last ones of the elimination order (the most recent frames) and span no more
  * than the band of the reduced system (else DYNOBA_ERR_UNSUPPORTED).  Difference from the reference: it retains recent
- * LANDMARKS as well; here every landmark is eliminated into the prior.  Single GPU. */
+ * LANDMARKS as well; here every landmark is eliminated into the prior.  Single GPU.  Poses only: refused
+ * (DYNOBA_ERR_UNSUPPORTED) on a graph with velocity / bias variables; dynoba_marginal_vars takes those graphs. */
 int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_idx, double* G, double* g);
+/* dynoba_marginal for a kept set of any pose-like kinds (kind[k], idx[k] as in dynoba_add_linear_prior_vars): poses,
+ * object motions, velocities and biases mixed, e.g. X_k, H_k, V_k, b_k of the last frames.  G[D][D] and g[D] are in the
+ * caller's slot order and tangent layout (D = sum of 6 / 3 / 6; a velocity's inert scalars are left out) -- ready for
+ * dynoba_add_linear_prior_vars of the next window with the kept variables' current values as linearisation point.  The
+ * same DYNOBA_ERR_UNSUPPORTED statuses: kept variables that are not the last of the elimination order (with frame ids as
+ * order hints, (rank, kind, index) puts the last frames' variables there), a kept block wider than the band, world > 1.
+ * f (may be NULL) receives the constant of GTSAM's remaining HessianFactor,
+ *     f = sum |b_w|^2 - g_e^T H_ee^-1 g_e,
+ * b_w the whitened, Huber-re-weighted right-hand sides of the linearised factors plus the priors' relinearised constants,
+ * e every eliminated scalar.  It is computed as 2 oldLin - (g^T H^-1 g - g_m^T G_m^-1 g_m) from one more undamped solve of
+ * the whole system: exact at the optimum (g = 0, the point the reference marginalises at), elsewhere the subtraction
+ * loses about kappa(H) eps of g^T H^-1 g, i.e. f is accurate to about kappa(H) eps sum |b_w|^2.  With f the call takes
+ * that solve's time on top of the marginal's. */
+int dynoba_marginal_vars(dynoba_handle h, int32_t n_keep, const int32_t* kind, const int32_t* idx, double* G, double* g,
+                         double* f);
 /* gtsam::Marginals(graph, values, Marginals::CHOLESKY).marginalCovariance(key) for many variables of one kind:
  * the graph linearised at the current values (robust re-weighting as linearize does, no damping), H = J^T J,
  * cov[i] = the diagonal block of H^-1 of variable idx[i] (caller order; idx == NULL: all n variables of the kind).
@@ -171,7 +199,8 @@ int dynoba_set_pose_order(dynoba_handle h, int64_t n, const int32_t* rank);
  * (rank, kind: pose < velocity < bias, index); a kind without a hint ranks by index.  Passing the frame id as the rank of
  * X_k, V_k and b_k puts them next to each other, which keeps the reduced system banded.
  * Velocity / bias variables cannot be combined with dynoba_add_linear_prior, dynoba_marginal, dynoba_set_shard (world > 1)
- * or dynoba_set_reduce: those return DYNOBA_ERR_UNSUPPORTED. */
+ * or dynoba_set_reduce: those return DYNOBA_ERR_UNSUPPORTED.  The sliding window's prior and marginal take them through
+ * dynoba_add_linear_prior_vars and dynoba_marginal_vars. */
 int dynoba_set_variable_order(dynoba_handle h, int kind, int64_t n, const int32_t* rank);
 /* Multi-GPU: rank/world of the landmark shard held by this handle and the all-reduce used for the reduced
  * system and the scalar sums.  min_bandwidth forces a common band layout on all ranks (0 = local). */
