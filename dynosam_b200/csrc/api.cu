@@ -24,6 +24,7 @@
 
 #include "../../include/dynoba.h"
 #include "internal.cuh"
+#include "var_layout.cuh"
 #include "window_plan.cuh"
 
 using namespace dynoba;
@@ -55,16 +56,15 @@ constexpr int LM_TRACE_COLS = 10;   // columns of a dynoba_get_lm_trace row
 
 struct dynoba_solver {
   int device = 0; cudaStream_t stream = nullptr; cudaStream_t stream2 = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr; std::string err;
-  std::vector<double> pose, point, flow, aux; std::vector<uint64_t> kpose, kpoint, kflow;
+  // values [n][KINDS[kind].width] and keys of every variable kind, in caller order
+  std::vector<double> vals[NUM_KINDS], aux; std::vector<uint64_t> keys[NUM_KINDS];
   double calib[6] = { 721.5377, 721.5377, 0.0, 609.5593, 172.854, 0.5372 };
-  std::vector<int32_t> hint;
-  // navigation variables (DYNOBA_VEL3 / DYNOBA_BIAS6): pose-like, solver positions pos[np + i] / pos[np + nv + i]
-  std::vector<double> vel, bias; std::vector<uint64_t> kvel, kbias; std::vector<int32_t> vhint, bhint;
+  std::vector<int32_t> hints[NUM_KINDS];   // order hints of the pose-like kinds
   int2* d_nav = nullptr; int n_nav = 0;   // device (position, dimension) of every velocity and bias
   std::vector<HostBlock> blocks;
   std::vector<HostPrior> priors;
   bool finalized = false, linearized = false, supported = true;
-  std::vector<int32_t> pos, pt_new, fl_new;
+  VarLayout layout;      // where every variable sits, from finalize on
   DevVars cur{}, cand{}; BandPlan plan{}; DevBand& band = plan.band; int ncell_request = 0;
   double *dl_point = nullptr, *dl_flow = nullptr, *partials = nullptr, *scalars = nullptr;
   int* fail = nullptr; int n_partials = 0, n_lin_partials = 0, n_bs_partials = 0;
@@ -86,8 +86,6 @@ struct dynoba_solver {
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return DYNOBA_ERR_CUDA; } } while (0)
 #define ARG(cond, msg) do { if (!(cond)) { if (h) h->err = msg; return DYNOBA_ERR_BAD_ARG; } } while (0)
-
-static int pad32(int64_t n) { return (int)((n + 31)/32*32); }
 
 // Process-wide pinned staging arena for the SoA images of the factor blocks: host->device copies from it run at PCIe
 // speed and asynchronously, so the upload of one block overlaps the host-side preparation of the next.  Grow-only.
@@ -163,10 +161,11 @@ template <class T> static int dalloc(dynoba_solver* h, T** p, size_t count, bool
   h->allocs.emplace_back(q, got);
   return DYNOBA_OK;
 }
-// device copy of a host array: a clean dalloc (an empty array gets one zero element) and a synchronous copy
+// device copy of a host array: a clean dalloc (an empty array gets one zero element) and a copy on the handle's stream,
+// waited for
 template <class T> static int upload(dynoba_solver* h, T** p, const T* src, size_t count) {
   if (int rc = dalloc(h, p, count)) return rc;
-  if (count) CK(cudaMemcpy(*p, src, count*sizeof(T), cudaMemcpyHostToDevice));
+  if (count) { CK(cudaMemcpyAsync(*p, src, count*sizeof(T), cudaMemcpyHostToDevice, h->stream)); CK(cudaStreamSynchronize(h->stream)); }
   return DYNOBA_OK;
 }
 template <class V> static int upload(dynoba_solver* h, typename V::value_type** p, const V& v) { return upload(h, p, v.data(), v.size()); }
@@ -272,74 +271,26 @@ int dynoba_destroy(dynoba_handle h) {
   return DYNOBA_OK;
 }
 
-static std::vector<double>* var_store(dynoba_solver* h, int kind) {
-  switch (kind) {
-    case DYNOBA_POSE6: return &h->pose; case DYNOBA_POINT3: return &h->point; case DYNOBA_FLOW2: return &h->flow;
-    case DYNOBA_VEL3: return &h->vel; case DYNOBA_BIAS6: return &h->bias; default: return nullptr;
-  }
-}
-static std::vector<uint64_t>* key_store(dynoba_solver* h, int kind) {
-  switch (kind) {
-    case DYNOBA_POSE6: return &h->kpose; case DYNOBA_POINT3: return &h->kpoint; case DYNOBA_FLOW2: return &h->kflow;
-    case DYNOBA_VEL3: return &h->kvel; case DYNOBA_BIAS6: return &h->kbias; default: return nullptr;
-  }
-}
-static int kind_width(int kind) { return kind == DYNOBA_POSE6 ? 12 : (kind == DYNOBA_POINT3 || kind == DYNOBA_VEL3 ? 3 : (kind == DYNOBA_BIAS6 ? 6 : 2)); }
-static bool has_nav(const dynoba_solver* h) { return !h->vel.empty() || !h->bias.empty(); }
-// tangent dimension of a pose-like kind (a prior slot / a kept variable of a marginal); 0 for the other kinds
-static int tangent_dim(int kind) { return kind == DYNOBA_POSE6 || kind == DYNOBA_BIAS6 ? 6 : (kind == DYNOBA_VEL3 ? 3 : 0); }
-// index of a pose-like variable among [poses | velocities | biases] (h->pos[] order), -1 when out of range
-static int64_t poselike_index(const dynoba_solver* h, int kind, int32_t ix) {
-  const int64_t np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3, nb = (int64_t)h->bias.size()/6;
-  const int64_t lim = kind == DYNOBA_POSE6 ? np : (kind == DYNOBA_VEL3 ? nv : nb);
-  if (ix < 0 || ix >= lim) return -1;
-  return kind == DYNOBA_POSE6 ? ix : (kind == DYNOBA_VEL3 ? np + ix : np + nv + ix);
-}
+static int64_t n_vars(const dynoba_solver* h, int kind) { return (int64_t)h->vals[kind].size()/KINDS[kind].width; }
+static bool has_nav(const dynoba_solver* h) { return !h->vals[DYNOBA_VEL3].empty() || !h->vals[DYNOBA_BIAS6].empty(); }
 
 int dynoba_set_variables(dynoba_handle h, int kind, int64_t n, const uint64_t* keys, const double* data) {
-  ARG(h, "null handle"); ARG(n >= 0 && (n == 0 || data), "null data");
-  const int w = kind_width(kind);
-  std::vector<double>* dst = var_store(h, kind);
-  std::vector<uint64_t>* kd = key_store(h, kind);
-  ARG(dst, "bad variable kind");
+  ARG(h, "null handle"); ARG(n >= 0 && (n == 0 || data), "null data"); ARG(valid_kind(kind), "bad variable kind");
+  std::vector<double>* dst = &h->vals[kind];
+  const int w = KINDS[kind].width;
   const bool same_shape = dst->size() == (size_t)n*w;
   dst->assign(data, data + (size_t)n*w);
-  if (keys) kd->assign(keys, keys + n); else if (!same_shape) kd->clear();   // a value refresh keeps the keys
-  if (h->finalized && same_shape && (has_nav(h) || kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6)) {
-    // pose-like values of a visual-inertial graph: the pose SoA holds poses, velocities and biases, so only the rows of
-    // the refreshed kind are replaced in the current device image
-    const int64_t np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3;
-    const int64_t base = kind == DYNOBA_POSE6 ? 0 : (kind == DYNOBA_VEL3 ? np : np + nv);
-    const int st = h->cur.np_stride;
-    if (kind == DYNOBA_POSE6 || kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6) {
-      if (n == 0) return DYNOBA_OK;
-      cudaSetDevice(h->device);
-      std::vector<double> soa((size_t)12*st);
-      CK(cudaMemcpy(soa.data(), h->cur.pose, soa.size()*8, cudaMemcpyDeviceToHost));
-      for (int64_t i = 0; i < n; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*st + h->pos[base + i]] = k < w ? data[i*w + k] : 0.0;
-      CK(cudaMemcpy(h->cur.pose, soa.data(), soa.size()*8, cudaMemcpyHostToDevice));
-      h->linearized = false; cov_invalidate(h);
-      return DYNOBA_OK;
-    }
-  }
+  if (keys) h->keys[kind].assign(keys, keys + n); else if (!same_shape) h->keys[kind].clear();   // a value refresh keeps the keys
   if (h->finalized && same_shape) {
-    // refresh device values only (layout unchanged)
+    // refresh device values only (layout unchanged).  When the kind shares the pose SoA with other pose-like kinds, only
+    // its columns are replaced in the current device image.
     cudaSetDevice(h->device);
-    std::vector<double> soa;
-    if (kind == DYNOBA_POSE6) {
-      soa.assign((size_t)12*h->cur.np_stride, 0.0);
-      for (int64_t i = 0; i < n; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*h->cur.np_stride + h->pos[i]] = data[i*12 + k];
-      for (int p = (int)n; p < h->cur.np_stride; p++) { soa[(size_t)0*h->cur.np_stride + p] = soa[(size_t)4*h->cur.np_stride + p] = soa[(size_t)8*h->cur.np_stride + p] = 1.0; }
-      CK(cudaMemcpyAsync(h->cur.pose, soa.data(), soa.size()*8, cudaMemcpyHostToDevice, h->stream));
-    } else if (kind == DYNOBA_POINT3) {
-      soa.assign((size_t)3*h->cur.nl_stride, 0.0);
-      for (int64_t i = 0; i < n; i++) for (int k = 0; k < 3; k++) soa[(size_t)k*h->cur.nl_stride + h->pt_new[i]] = data[i*3 + k];
-      CK(cudaMemcpyAsync(h->cur.point, soa.data(), soa.size()*8, cudaMemcpyHostToDevice, h->stream));
-    } else {
-      soa.assign((size_t)2*h->cur.nf_stride, 0.0);
-      for (int64_t i = 0; i < n; i++) for (int k = 0; k < 2; k++) soa[(size_t)k*h->cur.nf_stride + h->fl_new[i]] = data[i*2 + k];
-      CK(cudaMemcpyAsync(h->cur.flow, soa.data(), soa.size()*8, cudaMemcpyHostToDevice, h->stream));
-    }
+    const VarLayout& L = h->layout;
+    double* img_d = image_of(h->cur, kind);
+    std::vector<double> img = L.blank_image(kind);
+    if (KINDS[kind].poselike && L.NP() > L.count(kind)) { CK(cudaMemcpyAsync(img.data(), img_d, img.size()*8, cudaMemcpyDeviceToHost, h->stream)); CK(cudaStreamSynchronize(h->stream)); }
+    L.scatter_values(kind, data, img.data());
+    CK(cudaMemcpyAsync(img_d, img.data(), img.size()*8, cudaMemcpyHostToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     h->linearized = false; cov_invalidate(h);
   } else if (h->finalized) {
@@ -404,9 +355,8 @@ static int add_prior(dynoba_solver* h, int32_t n, const int32_t* kind, const int
   HostPrior P; P.kind.assign(kind, kind + n); P.idx.assign(idx, idx + n); P.f = f; P.legacy = legacy;
   size_t nlin = 0, dim = 0;
   for (int i = 0; i < n; i++) {
-    const int d = tangent_dim(kind[i]);
-    ARG(d, "a prior slot must be of kind DYNOBA_POSE6, DYNOBA_VEL3 or DYNOBA_BIAS6");
-    dim += d; nlin += kind[i] == DYNOBA_POSE6 ? 12 : d;
+    ARG(poselike_kind(kind[i]), "a prior slot must be of kind DYNOBA_POSE6, DYNOBA_VEL3 or DYNOBA_BIAS6");
+    dim += KINDS[kind[i]].tdim; nlin += KINDS[kind[i]].width;
   }
   P.lin.assign(lin, lin + nlin); P.G.assign(G, G + dim*dim); P.g.assign(g, g + dim);
   { std::vector<std::pair<int32_t, int32_t>> srt(n); for (int i = 0; i < n; i++) srt[i] = { kind[i], idx[i] };
@@ -434,7 +384,7 @@ int dynoba_add_linear_prior_vars(dynoba_handle h, int32_t n, const int32_t* kind
 
 int dynoba_set_pose_order(dynoba_handle h, int64_t n, const int32_t* rank) {
   ARG(h, "null handle"); ARG(n >= 0 && (n == 0 || rank), "null rank");
-  h->hint.assign(rank, rank + n);
+  h->hints[DYNOBA_POSE6].assign(rank, rank + n);
   if (h->finalized) free_device(h);
   return DYNOBA_OK;
 }
@@ -442,7 +392,7 @@ int dynoba_set_pose_order(dynoba_handle h, int64_t n, const int32_t* rank) {
 int dynoba_set_variable_order(dynoba_handle h, int kind, int64_t n, const int32_t* rank) {
   ARG(h, "null handle"); ARG(kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6, "variable order hints are for DYNOBA_VEL3 / DYNOBA_BIAS6 (poses: dynoba_set_pose_order)");
   ARG(n >= 0 && (n == 0 || rank), "null rank");
-  (kind == DYNOBA_VEL3 ? h->vhint : h->bhint).assign(rank, rank + n);
+  h->hints[kind].assign(rank, rank + n);
   if (h->finalized) free_device(h);
   return DYNOBA_OK;
 }
@@ -487,6 +437,11 @@ int dynoba_set_shard(dynoba_handle h, int rank, int world, dynoba_allreduce_fn f
 }  // extern "C"
 
 // ------------------------------------------------------------------------------------------------ finalize
+// algorithmic bytes of a block's linearize: factor record read once + whitened tiles written once (variable reads left out)
+static int64_t block_bytes(const HostBlock& b) {
+  const TypeInfo ti = type_info(b.type);
+  return b.n*(4*ti.arity + 8*ti.meas + 8*b.sigma_dim + (b.has_aux ? 4 : 0) + 8*(ti.dim*ti.jcols + ti.dim));
+}
 static int uf_find(std::vector<int32_t>& p, int x) { while (p[x] != x) { p[x] = p[p[x]]; x = p[x]; } return x; }
 // x = v where better(v, x), atomically with relaxed ordering (a min / max the parallel loops over factors share)
 template <class Better> static void atomic_keep(int32_t& x, int32_t v, Better better) {
@@ -503,29 +458,29 @@ static int finalize_impl(dynoba_solver* h) {
   auto t_last = std::chrono::steady_clock::now();
   auto lap = [&](const char* what) { if (!timing) return; auto t = std::chrono::steady_clock::now();
     std::fprintf(stderr, "[dynoba finalize] %-28s %8.1f ms\n", what, std::chrono::duration<double, std::milli>(t - t_last).count()); t_last = t; };
-  const int64_t np = (int64_t)h->pose.size()/12, npt = (int64_t)h->point.size()/3, nfl = (int64_t)h->flow.size()/2, naux = (int64_t)h->aux.size()/12;
-  const int64_t nv = (int64_t)h->vel.size()/3, nb = (int64_t)h->bias.size()/6, NP = np + nv + nb;   // NP: pose-like variables
-  ARG(h->hint.empty() || (int64_t)h->hint.size() == np, "pose order hint length != number of poses");
-  ARG(h->vhint.empty() || (int64_t)h->vhint.size() == nv, "velocity order hint length != number of velocities");
-  ARG(h->bhint.empty() || (int64_t)h->bhint.size() == nb, "bias order hint length != number of biases");
+  h->layout = VarLayout{n_vars(h, DYNOBA_POSE6), n_vars(h, DYNOBA_POINT3), n_vars(h, DYNOBA_FLOW2), n_vars(h, DYNOBA_VEL3), n_vars(h, DYNOBA_BIAS6)};
+  VarLayout& L = h->layout;
+  const int64_t np = L.np, npt = L.npt, nfl = L.nfl, nv = L.nv, nb = L.nb, NP = L.NP();   // NP: pose-like variables
+  const int64_t naux = (int64_t)h->aux.size()/KINDS[DYNOBA_POSE6].width;
+  ARG(h->hints[DYNOBA_POSE6].empty() || (int64_t)h->hints[DYNOBA_POSE6].size() == np, "pose order hint length != number of poses");
+  ARG(h->hints[DYNOBA_VEL3].empty() || (int64_t)h->hints[DYNOBA_VEL3].size() == nv, "velocity order hint length != number of velocities");
+  ARG(h->hints[DYNOBA_BIAS6].empty() || (int64_t)h->hints[DYNOBA_BIAS6].size() == nb, "bias order hint length != number of biases");
   const bool legacy_prior = std::any_of(h->priors.begin(), h->priors.end(), [](const HostPrior& P) { return P.legacy; });
   if (NP > np && (legacy_prior || h->world > 1 || h->reduce)) {
     h->err = "velocity / bias variables cannot be combined with dynoba_add_linear_prior, dynoba_set_shard or dynoba_set_reduce";
     return DYNOBA_ERR_UNSUPPORTED;
   }
-  // pose-like index of a key slot: poses [0, np), velocities [np, np + nv), biases [np + nv, NP)
-  auto plx = [&](int cls, int32_t ix) -> int64_t { return cls == VC_POSE ? ix : (cls == VC_VEL ? np + ix : np + nv + ix); };
   // ---- validate indices
   for (auto& b : h->blocks) {
     const TypeInfo ti = type_info(b.type);
     int bad = 0;
+    int64_t lim[6];
+    for (int k = 0; k < ti.arity; k++) lim[k] = L.count(ti.cls[k]);
 #pragma omp parallel for schedule(static) reduction(|:bad)
     for (int64_t i = 0; i < b.n; i++) {
       for (int k = 0; k < ti.arity; k++) {
         const int32_t ix = b.idx[i*ti.arity + k];
-        const int c = ti.cls[k];
-        const int64_t lim = c == VC_POSE ? np : (c == VC_POINT ? npt : (c == VC_FLOW ? nfl : (c == VC_VEL ? nv : nb)));
-        if (!(ix >= 0 && ix < lim)) bad |= 1;
+        if (!(ix >= 0 && ix < lim[k])) bad |= 1;
       }
       if (b.has_aux && !(b.aux[i] >= 0 && b.aux[i] < naux)) bad |= 2;
     }
@@ -533,22 +488,7 @@ static int finalize_impl(dynoba_solver* h) {
   }
   lap("validate");
   // ---- pose ordering
-  h->pos.resize(NP);
-  if (NP == np) {
-    std::vector<int32_t> ord(np); std::iota(ord.begin(), ord.end(), 0);
-    if (!h->hint.empty()) std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return h->hint[a] < h->hint[b]; });
-    for (int64_t i = 0; i < np; i++) h->pos[ord[i]] = (int32_t)i;
-  } else {
-    // visual-inertial graph: ordered by (rank, kind: pose < velocity < bias, index); a kind without a hint ranks by index,
-    // so X_k, V_k, b_k with the frame as rank sit next to each other and the system stays banded
-    std::vector<int32_t> ord(NP), rk(NP);
-    std::iota(ord.begin(), ord.end(), 0);
-    for (int64_t i = 0; i < np; i++) rk[i] = h->hint.empty() ? (int32_t)i : h->hint[i];
-    for (int64_t i = 0; i < nv; i++) rk[np + i] = h->vhint.empty() ? (int32_t)i : h->vhint[i];
-    for (int64_t i = 0; i < nb; i++) rk[np + nv + i] = h->bhint.empty() ? (int32_t)i : h->bhint[i];
-    std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return rk[a] < rk[b]; });
-    for (int64_t i = 0; i < NP; i++) h->pos[ord[i]] = (int32_t)i;
-  }
+  L.pos = L.poselike_positions(h->hints);
   // ---- landmark groups (union-find across factors that touch two landmarks)
   const int64_t nl = npt + nfl;
   std::vector<int32_t> uf(nl); std::iota(uf.begin(), uf.end(), 0);
@@ -578,7 +518,7 @@ static int finalize_impl(dynoba_solver* h) {
 #pragma omp parallel for schedule(static) reduction(max:bspread) reduction(min:blo) reduction(max:bhi)
     for (int64_t i = 0; i < b.n; i++) {
       int lo = INT32_MAX, hi = -1;
-      for (int k = 0; k < ti.arity; k++) if (is_poselike(ti.cls[k])) { const int p = h->pos[plx(ti.cls[k], b.idx[i*ti.arity + k])]; lo = std::min(lo, p); hi = std::max(hi, p); }
+      for (int k = 0; k < ti.arity; k++) if (is_poselike(ti.cls[k])) { const int p = L.column(ti.cls[k], b.idx[i*ti.arity + k]); lo = std::min(lo, p); hi = std::max(hi, p); }
       blo = std::min(blo, lo); bhi = std::max(bhi, hi);
       if (lslot < 0) { bspread = std::max(bspread, hi - lo); continue; }
       const int g = root[lmk_id(ti.cls[lslot], b.idx[i*ti.arity + lslot])];
@@ -599,8 +539,8 @@ static int finalize_impl(dynoba_solver* h) {
   for (auto& P : h->priors) {       // a prior couples all of its variables
     int lo = INT32_MAX, hi = -1;
     for (size_t i = 0; i < P.idx.size(); i++) {
-      const int64_t v = poselike_index(h, P.kind[i], P.idx[i]);
-      ARG(v >= 0, "prior variable out of range"); lo = std::min(lo, h->pos[v]); hi = std::max(hi, h->pos[v]);
+      const int p = L.column_checked(P.kind[i], P.idx[i]);
+      ARG(p >= 0, "prior variable out of range"); lo = std::min(lo, p); hi = std::max(hi, p);
     }
     spread = std::max(spread, hi - lo); pos_lo = std::min(pos_lo, lo); pos_hi = std::max(pos_hi, hi);
   }
@@ -626,20 +566,9 @@ static int finalize_impl(dynoba_solver* h) {
   std::vector<int32_t> lrank(nl);                       // group rank of every landmark (one gather per factor later)
 #pragma omp parallel for schedule(static)
   for (int64_t i = 0; i < nl; i++) lrank[i] = grank[root[i]];
-  // landmark device indices
-  h->pt_new.assign(npt, 0); h->fl_new.assign(nfl, 0);
-  {
-    std::vector<int32_t> ord(npt); std::iota(ord.begin(), ord.end(), 0);
-    int unsorted = 0;
-#pragma omp parallel for schedule(static) reduction(|:unsorted)
-    for (int64_t i = 1; i < npt; i++) unsorted |= grank[root[i-1]] > grank[root[i]];
-    if (unsorted) __gnu_parallel::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return grank[root[a]] < grank[root[b]]; });
-#pragma omp parallel for schedule(static)
-    for (int64_t i = 0; i < npt; i++) h->pt_new[ord[i]] = (int32_t)i;
-    std::vector<int32_t> of(nfl); std::iota(of.begin(), of.end(), 0);
-    std::stable_sort(of.begin(), of.end(), [&](int a, int b) { return grank[root[npt + a]] < grank[root[npt + b]]; });
-    for (int64_t i = 0; i < nfl; i++) h->fl_new[of[i]] = (int32_t)i;
-  }
+  // landmark device indices: group order
+  L.pt_new = positions_by(npt, [&](int32_t a, int32_t b) { return lrank[a] < lrank[b]; });
+  L.fl_new = positions_by(nfl, [&](int32_t a, int32_t b) { return lrank[npt + a] < lrank[npt + b]; });
   lap("groups + landmark order");
   // ---- band structure: cell decomposition of the reduced system (kernels_band.cu)
   {
@@ -682,23 +611,18 @@ static int finalize_impl(dynoba_solver* h) {
   DevBand& B = h->band;
   // ---- variables
   DevVars& V = h->cur;
-  V.np = (int)NP; V.np_stride = pad32(NP); V.nl = (int)npt; V.nl_stride = pad32(npt); V.nf = (int)nfl; V.nf_stride = pad32(nfl);
+  V.np = (int)NP; V.np_stride = L.stride(DYNOBA_POSE6); V.nl = (int)npt; V.nl_stride = L.stride(DYNOBA_POINT3); V.nf = (int)nfl; V.nf_stride = L.stride(DYNOBA_FLOW2);
   V.naux = (int)naux; V.naux_stride = pad32(naux);
   for (int i = 0; i < 6; i++) V.K[i] = h->calib[i];
   h->cand = V;
   {
-    std::vector<double> soa((size_t)12*V.np_stride, 0.0);
-    for (int p = 0; p < V.np_stride; p++) soa[(size_t)0*V.np_stride + p] = soa[(size_t)4*V.np_stride + p] = soa[(size_t)8*V.np_stride + p] = 1.0;
-    for (int64_t i = 0; i < np; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.np_stride + h->pos[i]] = h->pose[i*12 + k];
-    for (int64_t i = 0; i < nv; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.np_stride + h->pos[np + i]] = k < 3 ? h->vel[i*3 + k] : 0.0;
-    for (int64_t i = 0; i < nb; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.np_stride + h->pos[np + nv + i]] = k < 6 ? h->bias[i*6 + k] : 0.0;
+    std::vector<double> soa = L.blank_image(DYNOBA_POSE6);
+    for (int kind : {DYNOBA_POSE6, DYNOBA_VEL3, DYNOBA_BIAS6}) L.scatter_values(kind, h->vals[kind].data(), soa.data());
     int rc;
     if ((rc = upload(h, &h->cur.pose, soa)) || (rc = upload(h, &h->cand.pose, soa))) return rc;
-    soa.assign((size_t)3*V.nl_stride, 0.0);
-    for (int64_t i = 0; i < npt; i++) for (int k = 0; k < 3; k++) soa[(size_t)k*V.nl_stride + h->pt_new[i]] = h->point[i*3 + k];
+    soa = L.blank_image(DYNOBA_POINT3); L.scatter_values(DYNOBA_POINT3, h->vals[DYNOBA_POINT3].data(), soa.data());
     if ((rc = upload(h, &h->cur.point, soa)) || (rc = dalloc(h, &h->cand.point, soa.size())) || (rc = dalloc(h, &h->dl_point, soa.size()))) return rc;
-    soa.assign((size_t)2*V.nf_stride, 0.0);
-    for (int64_t i = 0; i < nfl; i++) for (int k = 0; k < 2; k++) soa[(size_t)k*V.nf_stride + h->fl_new[i]] = h->flow[i*2 + k];
+    soa = L.blank_image(DYNOBA_FLOW2); L.scatter_values(DYNOBA_FLOW2, h->vals[DYNOBA_FLOW2].data(), soa.data());
     if ((rc = upload(h, &h->cur.flow, soa)) || (rc = dalloc(h, &h->cand.flow, soa.size())) || (rc = dalloc(h, &h->dl_flow, soa.size()))) return rc;
     soa.assign((size_t)12*V.naux_stride, 0.0);
     for (int64_t i = 0; i < naux; i++) for (int k = 0; k < 12; k++) soa[(size_t)k*V.naux_stride + i] = h->aux[i*12 + k];
@@ -734,7 +658,7 @@ static int finalize_impl(dynoba_solver* h) {
 #pragma omp parallel for schedule(static)
       for (int64_t i = 0; i < n; i++) {
         frank[i] = lrank[lmk_id(ti.cls[lslot], b.idx[i*ti.arity + lslot])];
-        key[i] = ((int64_t)frank[i] << 32) | (uint32_t)h->pos[b.idx[i*ti.arity + pslot]];
+        key[i] = ((int64_t)frank[i] << 32) | (uint32_t)L.column(VC_POSE, b.idx[i*ti.arity + pslot]);
       }
       order_block_factors(b.perm.data(), frank, key, n, gorder.size());
     }
@@ -765,7 +689,7 @@ static int finalize_impl(dynoba_solver* h) {
       const int64_t o = b.perm[s];
       for (int k = 0; k < ti.arity; k++) {
         const int32_t ix = b.idx[o*ti.arity + k];
-        hidx[(size_t)k*stride + s] = is_poselike(ti.cls[k]) ? h->pos[plx(ti.cls[k], ix)] : (ti.cls[k] == VC_POINT ? h->pt_new[ix] : h->fl_new[ix]);
+        hidx[(size_t)k*stride + s] = L.column(ti.cls[k], ix);
       }
       for (int k = 0; k < ti.meas; k++) hmeas[(size_t)k*stride + s] = b.meas[o*ti.meas + k];
       if (b.type == F_COMBINED_IMU15)   // square-root information, used as given
@@ -836,8 +760,7 @@ static int finalize_impl(dynoba_solver* h) {
     lap("  blk groups+windows");
     b.part_off = part; part += is_nav_type(b.type) ? nav_grid(b.type, (int)n) : linearize_grid((int)n);
     b.bs_off = bs; bs += b.pose_only ? (int)((n + 127)/128) : backsub_grid(d.n_groups);
-    const int64_t rd = 4*ti.arity + 8*ti.meas + 8*b.sigma_dim + (b.has_aux ? 4 : 0), wr = 8*(ti.dim*ti.jcols + ti.dim);
-    h->jac_bytes += n*(rd + wr);
+    h->jac_bytes += block_bytes(b);
   }
   lap("factor blocks");
   // ---- general landmark groups
@@ -861,7 +784,7 @@ static int finalize_impl(dynoba_solver* h) {
     {
       std::vector<int32_t> rank2g(gorder.size(), -1);
       for (size_t g = 0; g + 1 < gptr.size(); g++) rank2g[gen_refs[gptr[g]].rank] = (int32_t)g;
-      for (int64_t i = 0; i < nl; i++) { const int g = rank2g[grank[root[i]]]; if (g >= 0) { if (i >= npt) { h->supported = false; continue; } gl0[g] = std::min(gl0[g], h->pt_new[i]); } }
+      for (int64_t i = 0; i < nl; i++) { const int g = rank2g[grank[root[i]]]; if (g >= 0) { if (i >= npt) { h->supported = false; continue; } gl0[g] = std::min(gl0[g], L.column(DYNOBA_POINT3, i)); } }
     }
     std::vector<DevBlock> hb; for (auto& b : h->blocks) hb.push_back(b.dev);
     DevBlock* dblk; int* dgptr; int* drefs; int* dgl0; int* dgnl; int rc;
@@ -870,13 +793,8 @@ static int finalize_impl(dynoba_solver* h) {
     h->gen.n_groups = (int)gl0.size(); h->gen.blocks = dblk; h->gen.gptr = dgptr; h->gen.refs = drefs; h->gen.gl0 = dgl0; h->gen.gnl = dgnl;
   }
   for (auto& P : h->priors) {
-    const int n = (int)P.idx.size(); std::vector<int4> slot(n); std::vector<int32_t> sidx;
-    for (int i = 0, lo = 0; i < n; i++) {
-      const int p = h->pos[poselike_index(h, P.kind[i], P.idx[i])], d = tangent_dim(P.kind[i]);
-      slot[i] = make_int4(P.kind[i], p, lo, (int)sidx.size());
-      lo += P.kind[i] == DYNOBA_POSE6 ? 12 : d;
-      for (int c = 0; c < d; c++) sidx.push_back(6*p + c);      // (velocity: c < 3, never an inert scalar)
-    }
+    const int n = (int)P.idx.size(); std::vector<int4> slot; std::vector<int32_t> sidx;
+    L.prior_table(n, P.kind.data(), P.idx.data(), slot, sidx);
     const int dim = (int)sidx.size();
     int4* dslot; int* dsidx; double *dlin, *dG, *dg, *dd, *dgc; int rc;
     if ((rc = upload(h, &dslot, slot)) || (rc = upload(h, &dsidx, sidx)) || (rc = upload(h, &dlin, P.lin)) || (rc = upload(h, &dG, P.G)) ||
@@ -887,9 +805,7 @@ static int finalize_impl(dynoba_solver* h) {
   }
   h->n_nav = 0; h->d_nav = nullptr;
   if (NP > np) {
-    std::vector<int2> nav(nv + nb);
-    for (int64_t i = 0; i < nv; i++) nav[i] = make_int2(h->pos[np + i], 3);
-    for (int64_t i = 0; i < nb; i++) nav[nv + i] = make_int2(h->pos[np + nv + i], 6);
+    const std::vector<int2> nav = L.nav_table();
     if (int rc = upload(h, &h->d_nav, nav)) return rc;
     h->n_nav = (int)nav.size();
   }
@@ -1071,16 +987,14 @@ int dynoba_finalize(dynoba_handle h) { if (!h) return DYNOBA_ERR_BAD_ARG; return
 
 int dynoba_num_variables(dynoba_handle h, int kind, int64_t* out) {
   ARG(h && out, "null");
-  const std::vector<double>* v = var_store(h, kind);
-  ARG(v, "bad variable kind");
-  *out = (int64_t)v->size()/kind_width(kind);
+  ARG(valid_kind(kind), "bad variable kind");
+  *out = n_vars(h, kind);
   return DYNOBA_OK;
 }
 int dynoba_get_keys(dynoba_handle h, int kind, int64_t n, uint64_t* out) {
   ARG(h && out, "null");
-  const std::vector<uint64_t>* kp = key_store(h, kind);
-  ARG(kp, "bad variable kind");
-  const auto& k = *kp;
+  ARG(valid_kind(kind), "bad variable kind");
+  const auto& k = h->keys[kind];
   ARG((int64_t)k.size() == n, "no keys stored / size mismatch");
   std::copy(k.begin(), k.end(), out);
   return DYNOBA_OK;
@@ -1125,16 +1039,13 @@ int dynoba_linearize(dynoba_handle h, float* ms) {
 int dynoba_linearize_block(dynoba_handle h, int bi, float* ms, int64_t* bytes) {
   int rc = check_ready(h, false); if (rc) return rc;
   ARG(bi >= 0 && bi < (int)h->blocks.size(), "bad block index");
-  auto& b = h->blocks[bi]; const TypeInfo ti = type_info(b.type);
+  auto& b = h->blocks[bi];
   CK(cudaEventRecord(h->ev[0], h->stream));
   h->launches += launch_linearize(b.dev, h->cur, h->partials + b.part_off, h->stream);
   CK(cudaEventRecord(h->ev[1], h->stream));
   CK(cudaStreamSynchronize(h->stream));
   if (ms) CK(cudaEventElapsedTime(ms, h->ev[0], h->ev[1]));
-  if (bytes) {   // factor record read once + whitened tiles written once (variable reads left out: conservative)
-    const int64_t rd = 4*ti.arity + 8*ti.meas + 8*b.sigma_dim + (b.has_aux ? 4 : 0), wr = 8*(ti.dim*ti.jcols + ti.dim);
-    *bytes = b.n*(rd + wr);
-  }
+  if (bytes) *bytes = block_bytes(b);
   CK(cudaGetLastError());
   return DYNOBA_OK;
 }
@@ -1165,8 +1076,7 @@ int dynoba_get_factor_errors(dynoba_handle h, int bi, double* err) {
   CK(cudaMemcpyAsync(he.data(), d, he.size()*8, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   for (int64_t s = 0; s < b.n; s++) err[b.perm[s]] = he[s];
-  { auto it = std::find_if(h->allocs.begin(), h->allocs.end(), [&](const std::pair<void*, size_t>& a) { return a.first == (void*)d; });
-    g_devcache.give(h->device, it->first, it->second); h->allocs.erase(it); }
+  release(h, d);
   return DYNOBA_OK;
 }
 
@@ -1184,44 +1094,17 @@ int dynoba_get_reduced_system(dynoba_handle h, double lambda, double* S, double*
     if (p.ff) p.ff = hacc.data() + (p.ff - B.acc); if (p.gf) p.gf = hacc.data() + (p.gf - B.acc);
   }
   DevBand HB = B; HB.chains = hch.data(); HB.cells = h->plan.cells.data();
-  // caller layout [poses 6 | velocities 3 | biases 6]; the inert scalars of the velocity blocks are left out
-  const int nb_ = B.n; const int64_t NP = nb_/6, np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3;
-  std::vector<int32_t> usr(nb_, -1);
-  for (int64_t i = 0; i < NP; i++) {
-    const int64_t off = i < np ? 6*i : (i < np + nv ? 6*np + 3*(i - np) : 6*np + 3*nv + 6*(i - np - nv));
-    const int d = i >= np && i < np + nv ? 3 : 6;
-    for (int c = 0; c < d; c++) usr[6*(size_t)h->pos[i] + c] = (int32_t)(off + c);
-  }
-  const int n = (int)(nb_ - 3*nv);
+  const std::vector<int32_t> usr = h->layout.reduced_map();
+  const int n = (int)h->layout.reduced_dim();
   if (S) {
     std::fill(S, S + (size_t)n*n, 0.0);
-    for (int j = 0; j < nb_; j++) for (int i = j; i < nb_ && i <= j + B.bw; i++) {
+    for (int j = 0; j < B.n; j++) for (int i = j; i < B.n && i <= j + B.bw; i++) {
       if (usr[i] < 0 || usr[j] < 0) continue;
       const double v = *band_at(HB, i, j);
       S[(size_t)usr[i]*n + usr[j]] = v; S[(size_t)usr[j]*n + usr[i]] = v;
     }
   }
-  if (g) for (int i = 0; i < nb_; i++) if (usr[i] >= 0) g[usr[i]] = *rhs_at(HB, i);
-  return DYNOBA_OK;
-}
-
-static int download_delta(dynoba_solver* h, double* delta) {
-  const DevBand& B = h->band; const int64_t np = (int64_t)h->pose.size()/12, npt = h->cur.nl, nfl = h->cur.nf;
-  std::vector<double> hr(B.n_pad), hp((size_t)3*h->cur.nl_stride), hf((size_t)2*h->cur.nf_stride);
-  CK(cudaMemcpyAsync(hr.data(), B.dp, hr.size()*8, cudaMemcpyDeviceToHost, h->stream));
-  if (npt) CK(cudaMemcpyAsync(hp.data(), h->dl_point, hp.size()*8, cudaMemcpyDeviceToHost, h->stream));
-  if (nfl) CK(cudaMemcpyAsync(hf.data(), h->dl_flow, hf.size()*8, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  for (int64_t i = 0; i < np; i++) for (int c = 0; c < 6; c++) delta[6*i + c] = hr[6*(size_t)h->pos[i] + c];
-  double* dp = delta + 6*np;
-  for (int64_t i = 0; i < npt; i++) for (int c = 0; c < 3; c++) dp[3*i + c] = hp[(size_t)c*h->cur.nl_stride + h->pt_new[i]];
-  double* df = dp + 3*npt;
-  for (int64_t i = 0; i < nfl; i++) for (int c = 0; c < 2; c++) df[2*i + c] = hf[(size_t)c*h->cur.nf_stride + h->fl_new[i]];
-  double* dn = df + 2*nfl;          // velocities (3), then biases (6)
-  for (int64_t i = np; i < (int64_t)h->pos.size(); i++) {
-    const int d = i < np + (int64_t)h->vel.size()/3 ? 3 : 6;
-    for (int c = 0; c < d; c++) *dn++ = hr[6*(size_t)h->pos[i] + c];
-  }
+  if (g) for (int i = 0; i < B.n; i++) if (usr[i] >= 0) g[usr[i]] = *rhs_at(HB, i);
   return DYNOBA_OK;
 }
 
@@ -1235,27 +1118,25 @@ int dynoba_solve(dynoba_handle h, double lambda, double* delta) {
   h->last_model[0] = s[0]; h->last_model[1] = s[1]; h->last_model[2] = s[3];
   CK(cudaGetLastError());
   if (s[3] != 0.0) { h->err = "reduced system not positive definite"; return DYNOBA_ERR_INDETERMINATE; }
-  return download_delta(h, delta);
+  const VarLayout& L = h->layout;
+  std::vector<double> hr(h->band.n_pad), hp(L.image_size(DYNOBA_POINT3)), hf(L.image_size(DYNOBA_FLOW2));
+  CK(cudaMemcpyAsync(hr.data(), h->band.dp, hr.size()*8, cudaMemcpyDeviceToHost, h->stream));
+  if (L.npt) CK(cudaMemcpyAsync(hp.data(), h->dl_point, hp.size()*8, cudaMemcpyDeviceToHost, h->stream));
+  if (L.nfl) CK(cudaMemcpyAsync(hf.data(), h->dl_flow, hf.size()*8, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  L.walk_delta(hr.data(), hp.data(), hf.data(), [&](size_t u, double& v) { delta[u] = v; });
+  return DYNOBA_OK;
 }
 
 int dynoba_retract(dynoba_handle h, const double* delta) {
   int rc = check_ready(h, false); if (rc) return rc;
   ARG(delta, "null delta");
-  const DevBand& B = h->band; const int64_t np = (int64_t)h->pose.size()/12, npt = h->cur.nl, nfl = h->cur.nf;
-  std::vector<double> hr(B.n_pad, 0.0), hp((size_t)3*h->cur.nl_stride, 0.0), hf((size_t)2*h->cur.nf_stride, 0.0);
-  for (int64_t i = 0; i < np; i++) for (int c = 0; c < 6; c++) hr[6*(size_t)h->pos[i] + c] = delta[6*i + c];
-  const double* dp = delta + 6*np;
-  for (int64_t i = 0; i < npt; i++) for (int c = 0; c < 3; c++) hp[(size_t)c*h->cur.nl_stride + h->pt_new[i]] = dp[3*i + c];
-  const double* df = dp + 3*npt;
-  for (int64_t i = 0; i < nfl; i++) for (int c = 0; c < 2; c++) hf[(size_t)c*h->cur.nf_stride + h->fl_new[i]] = df[2*i + c];
-  const double* dn = df + 2*nfl;    // velocities (3), then biases (6)
-  for (int64_t i = np; i < (int64_t)h->pos.size(); i++) {
-    const int d = i < np + (int64_t)h->vel.size()/3 ? 3 : 6;
-    for (int c = 0; c < d; c++) hr[6*(size_t)h->pos[i] + c] = *dn++;
-  }
-  CK(cudaMemcpyAsync(B.dp, hr.data(), hr.size()*8, cudaMemcpyHostToDevice, h->stream));
-  if (npt) CK(cudaMemcpyAsync(h->dl_point, hp.data(), hp.size()*8, cudaMemcpyHostToDevice, h->stream));
-  if (nfl) CK(cudaMemcpyAsync(h->dl_flow, hf.data(), hf.size()*8, cudaMemcpyHostToDevice, h->stream));
+  const VarLayout& L = h->layout;
+  std::vector<double> hr(h->band.n_pad, 0.0), hp(L.image_size(DYNOBA_POINT3), 0.0), hf(L.image_size(DYNOBA_FLOW2), 0.0);
+  L.walk_delta(hr.data(), hp.data(), hf.data(), [&](size_t u, double& v) { v = delta[u]; });
+  CK(cudaMemcpyAsync(h->band.dp, hr.data(), hr.size()*8, cudaMemcpyHostToDevice, h->stream));
+  if (L.npt) CK(cudaMemcpyAsync(h->dl_point, hp.data(), hp.size()*8, cudaMemcpyHostToDevice, h->stream));
+  if (L.nfl) CK(cudaMemcpyAsync(h->dl_flow, hf.data(), hf.size()*8, cudaMemcpyHostToDevice, h->stream));
   h->launches += launch_retract(h->cur, h->cand, h->band, h->dl_point, h->dl_flow, h->stream);
   h->launches += launch_nav_retract(h->cur, h->cand, h->band, h->d_nav, h->n_nav, h->stream);
   CK(cudaStreamSynchronize(h->stream));
@@ -1277,12 +1158,12 @@ static int marginal_impl(dynoba_solver* h, int32_t n_keep, const int32_t* kind, 
   if (h->world > 1) { h->err = "dynoba_marginal is a single-GPU entry point"; return DYNOBA_ERR_UNSUPPORTED; }
   std::vector<int> slot(n_keep, -1), off(n_keep + 1, 0);   // kept variable k sits at solver position NP - n_keep + slot
   for (int k = 0; k < n_keep; k++) {
-    ARG(tangent_dim(kind[k]), "a kept variable must be of kind DYNOBA_POSE6, DYNOBA_VEL3 or DYNOBA_BIAS6");
-    const int64_t v = poselike_index(h, kind[k], idx[k]);
-    ARG(v >= 0, "variable out of range");
-    const int p = h->pos[v] - (int)(NP - n_keep);
+    ARG(poselike_kind(kind[k]), "a kept variable must be of kind DYNOBA_POSE6, DYNOBA_VEL3 or DYNOBA_BIAS6");
+    const int32_t c = h->layout.column_checked(kind[k], idx[k]);
+    ARG(c >= 0, "variable out of range");
+    const int p = c - (int)(NP - n_keep);
     if (p < 0) { h->err = "the kept variables must be the last ones of the elimination order (most recent frames)"; return DYNOBA_ERR_UNSUPPORTED; }
-    slot[k] = p; off[k + 1] = off[k] + tangent_dim(kind[k]);
+    slot[k] = p; off[k + 1] = off[k] + KINDS[kind[k]].tdim;
   }
   { std::vector<int> srt = slot; std::sort(srt.begin(), srt.end()); ARG(std::adjacent_find(srt.begin(), srt.end()) == srt.end(), "a variable is listed twice"); }
   int rc;
@@ -1441,25 +1322,20 @@ extern "C" {
 int dynoba_marginal_covariance(dynoba_handle h, int kind, int64_t n, const int32_t* idx, double* cov) {
   int rc = check_ready(h, true); if (rc) return rc;
   if (h->world > 1) { h->err = "dynoba_marginal_covariance is a single-GPU entry point"; return DYNOBA_ERR_UNSUPPORTED; }
-  const std::vector<double>* store = var_store(h, kind);
-  ARG(store, "bad variable kind");
-  const int64_t nk = (int64_t)store->size()/kind_width(kind);
+  ARG(valid_kind(kind), "bad variable kind");
+  const VarLayout& L = h->layout;
+  const int64_t nk = L.count(kind);
   ARG(idx ? n >= 0 : n == nk, "idx == NULL asks for every variable of the kind: n must be their number");
   ARG(n == 0 || cov, "null cov");
   for (int64_t i = 0; idx && i < n; i++) ARG(idx[i] >= 0 && idx[i] < nk, "variable out of range");
   if (n == 0) return DYNOBA_OK;
   if (!h->cov_ready && (rc = cov_band(h))) return rc;
-  const bool poselike = kind == DYNOBA_POSE6 || kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6;
+  const bool poselike = KINDS[kind].poselike;
   if (!poselike && !h->cov_lmk_ready && (rc = cov_landmarks(h))) return rc;
-  const int d = kind == DYNOBA_POSE6 || kind == DYNOBA_BIAS6 ? 6 : (kind == DYNOBA_FLOW2 ? 2 : 3);
+  const int d = KINDS[kind].tdim;
   // caller order -> scalar position of the block (pose-like) / device landmark index
   std::vector<int32_t> at(n);
-  const int64_t np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3;
-  const int64_t base = kind == DYNOBA_VEL3 ? np : (kind == DYNOBA_BIAS6 ? np + nv : 0);
-  for (int64_t i = 0; i < n; i++) {
-    const int64_t v = idx ? idx[i] : i;
-    at[i] = poselike ? 6*h->pos[base + v] : (kind == DYNOBA_POINT3 ? h->pt_new[v] : h->fl_new[v]);
-  }
+  for (int64_t i = 0; i < n; i++) at[i] = (poselike ? 6 : 1)*L.column(kind, idx ? idx[i] : i);
   int* dat; double* dout;
   if ((rc = dalloc(h, &dat, (size_t)n, false))) return rc;
   if ((rc = dalloc(h, &dout, (size_t)n*d*d, false))) { release(h, dat); return rc; }
@@ -1477,26 +1353,13 @@ int dynoba_marginal_covariance(dynoba_handle h, int kind, int64_t n, const int32
 
 int dynoba_get_variables(dynoba_handle h, int kind, int64_t n, double* out) {
   int rc = check_ready(h, false); if (rc) return rc;
-  ARG(out, "null out");
-  const DevVars& V = h->cur;
-  if (kind == DYNOBA_POSE6 || kind == DYNOBA_VEL3 || kind == DYNOBA_BIAS6) {
-    const int64_t np = (int64_t)h->pose.size()/12, nv = (int64_t)h->vel.size()/3, w = kind_width(kind);
-    ARG(n == (int64_t)var_store(h, kind)->size()/w, "size mismatch");
-    const int64_t base = kind == DYNOBA_POSE6 ? 0 : (kind == DYNOBA_VEL3 ? np : np + nv);
-    std::vector<double> soa((size_t)12*V.np_stride);
-    CK(cudaMemcpy(soa.data(), V.pose, soa.size()*8, cudaMemcpyDeviceToHost));
-    for (int64_t i = 0; i < n; i++) for (int k = 0; k < w; k++) out[i*w + k] = soa[(size_t)k*V.np_stride + h->pos[base + i]];
-  } else if (kind == DYNOBA_POINT3) {
-    ARG(n == V.nl, "size mismatch");
-    std::vector<double> soa((size_t)3*V.nl_stride);
-    CK(cudaMemcpy(soa.data(), V.point, soa.size()*8, cudaMemcpyDeviceToHost));
-    for (int64_t i = 0; i < n; i++) for (int k = 0; k < 3; k++) out[i*3 + k] = soa[(size_t)k*V.nl_stride + h->pt_new[i]];
-  } else if (kind == DYNOBA_FLOW2) {
-    ARG(n == V.nf, "size mismatch");
-    std::vector<double> soa((size_t)2*V.nf_stride);
-    CK(cudaMemcpy(soa.data(), V.flow, soa.size()*8, cudaMemcpyDeviceToHost));
-    for (int64_t i = 0; i < n; i++) for (int k = 0; k < 2; k++) out[i*2 + k] = soa[(size_t)k*V.nf_stride + h->fl_new[i]];
-  } else ARG(false, "bad kind");
+  ARG(out, "null out"); ARG(valid_kind(kind), "bad kind");
+  const VarLayout& L = h->layout;
+  ARG(n == L.count(kind), "size mismatch");
+  std::vector<double> img(L.image_size(kind));
+  CK(cudaMemcpyAsync(img.data(), image_of(h->cur, kind), img.size()*8, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  L.gather_values(kind, img.data(), out);
   return DYNOBA_OK;
 }
 
