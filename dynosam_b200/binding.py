@@ -7,7 +7,7 @@ import os
 
 import numpy as np
 
-from .problem import ARITY, DIM, JCOLS, MEAS_DIM, Problem
+from .problem import ARITY, DIM, JCOLS, LINEAR_PP3, MEAS_DIM, Problem, linear_block
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdynoba.so")
@@ -26,7 +26,7 @@ REDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.
 EXPORTS = [
     "dynoba_version", "dynoba_status_string", "dynoba_last_error", "dynoba_create", "dynoba_destroy",
     "dynoba_lm_default_params", "dynoba_set_variables", "dynoba_set_aux_poses", "dynoba_set_calibration",
-    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_add_linear_prior_vars", "dynoba_marginal", "dynoba_marginal_vars", "dynoba_marginal_covariance", "dynoba_finalize", "dynoba_error",
+    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_add_linear_prior_vars", "dynoba_marginal", "dynoba_marginal_vars", "dynoba_marginal_keep_points", "dynoba_marginal_covariance", "dynoba_finalize", "dynoba_error",
     "dynoba_optimize", "dynoba_get_variables", "dynoba_get_keys", "dynoba_num_variables", "dynoba_problem_info", "dynoba_window_census",
     "dynoba_linearize", "dynoba_linearize_block", "dynoba_get_linearization", "dynoba_get_factor_errors", "dynoba_solve",
     "dynoba_get_reduced_system", "dynoba_retract", "dynoba_last_model", "dynoba_get_lm_trace", "dynoba_flow_pose_default_params", "dynoba_flow_pose_batch",
@@ -119,6 +119,8 @@ def load():
         L.dynoba_marginal.argtypes = [C.c_void_p, C.c_int32, c_ip, c_dp, c_dp]
         L.dynoba_marginal_vars.argtypes = [C.c_void_p, C.c_int32, c_ip, c_ip, c_dp, c_dp, c_dp]
         L.dynoba_marginal_covariance.argtypes = [C.c_void_p, C.c_int, C.c_int64, c_ip, c_dp]
+        L.dynoba_marginal_keep_points.argtypes = [C.c_void_p, C.c_int32, c_ip, c_ip, C.c_int32, c_ip, c_ip, c_dp, c_dp, c_dp,
+                                                  C.c_int64, C.POINTER(C.c_int64), c_ip, c_ip, c_dp]
         L.dynoba_finalize.argtypes = [C.c_void_p]
         L.dynoba_error.argtypes = [C.c_void_p, c_dp]
         L.dynoba_optimize.argtypes = [C.c_void_p, C.POINTER(LmParams), C.POINTER(LmStats)]
@@ -277,6 +279,40 @@ class Solver:
         G = np.zeros((max(D, 1), max(D, 1))); g = np.zeros(max(D, 1)); f = C.c_double()
         self._ck(self.lib.dynoba_marginal_vars(self.h, kinds.size, _ip(kinds), _ip(idx), _dp(G), _dp(g), C.byref(f)))
         return G[:D, :D].copy(), g[:D].copy(), f.value
+
+    def marginal_keep_points(self, kinds, idx, pts, pt_kinds=None):
+        """(G, g, f, blocks): marginal_vars of the pose-like variables (kinds[k], idx[k]) that also keeps the POINT3
+        landmarks pts (dynoba_marginal_keep_points).  G, g, f hold every factor except those of the kept points; blocks
+        holds those factors as LINEAR_PP3 / LINEAR_PPP3 FactorBlocks, linearised and with the current values as
+        linearisation point, in export order (consecutive factors of one type share a block) -- ready for the next window.
+        pt_kinds: a kind per kept landmark (default POINT3; anything else is refused)."""
+        kinds = np.ascontiguousarray(kinds, dtype=np.int32).reshape(-1); idx = np.ascontiguousarray(idx, dtype=np.int32).reshape(-1)
+        pts = np.ascontiguousarray(pts, dtype=np.int32).reshape(-1)
+        pk = None if pt_kinds is None else np.ascontiguousarray(pt_kinds, dtype=np.int32).reshape(-1)
+        if kinds.size != idx.size or (pk is not None and pk.size != pts.size):
+            raise DynobaError(ERR_BAD_ARG, "kinds and idx (or pt_kinds and pts) differ in length")
+        D = sum(TANGENT_DIM.get(int(k), 0) for k in kinds)
+        G = np.zeros((max(D, 1), max(D, 1))); g = np.zeros(max(D, 1)); f = C.c_double(); n = C.c_int64()
+        args = (self.h, kinds.size, _ip(kinds), _ip(idx), pts.size, _ip(pk), _ip(pts), _dp(G), _dp(g), C.byref(f))
+        st = self.lib.dynoba_marginal_keep_points(*args, 0, C.byref(n), C.cast(None, c_ip), C.cast(None, c_ip), C.cast(None, c_dp))
+        if st == ERR_BAD_ARG and n.value > 0:          # the capacity query: call again with room for every exported factor
+            cnt = n.value
+            typ = np.zeros(cnt, np.int32); vid = np.zeros((cnt, 3), np.int32); Ab = np.zeros((cnt, 3, 16))
+            st = self.lib.dynoba_marginal_keep_points(*args, cnt, C.byref(n), _ip(typ), _ip(vid), _dp(Ab))
+        else:
+            typ = np.zeros(0, np.int32); vid = np.zeros((0, 3), np.int32); Ab = np.zeros((0, 3, 16))
+        self._ck(st)
+        pose, point, _ = self.values()
+        blocks, a = [], 0
+        while a < typ.size:
+            e = a
+            while e < typ.size and typ[e] == typ[a]:
+                e += 1
+            t = int(typ[a]); npose = 1 if t == LINEAR_PP3 else 2; jc = JCOLS[t]
+            bidx = vid[a:e, :npose + 1]
+            blocks.append(linear_block(t, bidx, Ab[a:e, :, :jc], Ab[a:e, :, 15], pose[bidx[:, :npose]], point[bidx[:, npose]]))
+            a = e
+        return G[:D, :D].copy(), g[:D].copy(), f.value, blocks
 
     def marginal(self, keep_idx):
         """(G, g): marginal information of the pose-like variables keep_idx (the last ones in frame order) at the current values"""

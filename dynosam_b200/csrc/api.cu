@@ -337,6 +337,10 @@ int dynoba_add_factors(dynoba_handle h, int type, int64_t n, const int32_t* idx,
     for (size_t o = 0; o < b.sigma.size(); o += IMU_SQRT_INFO) for (int k = 0; k < 15; k++) ARG(b.sigma[o + 16*k] > 0, "square-root information must have a positive diagonal");
   }
   else for (double s : b.sigma) ARG(s > 0, "sigma must be positive");
+  if (is_linear_type(type)) {   // a linearised factor is already whitened: no noise model
+    for (double s : b.sigma) ARG(s == 1.0, "LINEAR_PP3 / LINEAR_PPP3 take no noise model: sigma must be 1");
+    ARG(robust_k == 0.0, "LINEAR_PP3 / LINEAR_PPP3 take no noise model: robust_k must be 0");
+  }
   if (imu) for (size_t i = 0; i < b.meas.size(); i++) ARG(std::isfinite(b.meas[i]), "IMU measurement must be finite");
   b.robust_k = robust_k;
   if (aux_idx) { par_assign(b.aux, aux_idx, (size_t)n); b.has_aux = true; }
@@ -1260,6 +1264,101 @@ int dynoba_marginal_vars(dynoba_handle h, int32_t n_keep, const int32_t* kind, c
   int rc = check_ready(h, true); if (rc) return rc;
   ARG(n_keep > 0 && kind && idx && G && g, "bad arguments");
   return marginal_impl(h, n_keep, kind, idx, G, g, f);
+}
+
+// The host finds the factors of the kept points and checks them against the kept pose-like set.  The device then copies
+// their linearisation out (linear_gather_kernel) and zeroes their pose columns and rhs (linear_mask_kernel), so that they
+// add exactly 0 to S, g_S and g_l in the one marginal_impl call that follows.  Linearising again afterwards restores every
+// Jacobian and rhs bit for bit.  The constant f of marginal_impl counts 1/2 |b|^2 from the linearize pass, which still
+// holds the kept factors: their sum |b|^2 is taken off on the host.
+int dynoba_marginal_keep_points(dynoba_handle h, int32_t n_keep, const int32_t* kind, const int32_t* idx, int32_t n_pts,
+                                const int32_t* pt_kind, const int32_t* pt_idx, double* G, double* g, double* f,
+                                int64_t capacity, int64_t* n_out, int32_t* out_type, int32_t* out_idx, double* out_Ab) {
+  int rc = check_ready(h, true); if (rc) return rc;
+  ARG(n_keep > 0 && kind && idx && G && g && n_out, "bad arguments");
+  ARG(n_pts >= 0 && (n_pts == 0 || pt_idx), "bad kept points");
+  *n_out = 0;
+  if (n_pts == 0) return marginal_impl(h, n_keep, kind, idx, G, g, f);
+  if (h->world > 1) { h->err = "dynoba_marginal_keep_points is a single-GPU entry point"; return DYNOBA_ERR_UNSUPPORTED; }
+  const VarLayout& L = h->layout;
+  std::vector<char> kept_pt(L.npt, 0), kept_pose(L.np, 0);
+  for (int32_t i = 0; i < n_pts; i++) {
+    ARG(!pt_kind || pt_kind[i] == DYNOBA_POINT3, "only POINT3 landmarks can be kept: a flow variable is always eliminated");
+    ARG(pt_idx[i] >= 0 && pt_idx[i] < L.npt, "kept point out of range");
+    ARG(!kept_pt[pt_idx[i]], "a point is listed twice"); kept_pt[pt_idx[i]] = 1;
+  }
+  for (int32_t k = 0; k < n_keep; k++) {
+    ARG(poselike_kind(kind[k]) && L.column_checked(kind[k], idx[k]) >= 0, "a kept variable must be a pose-like variable in range");
+    if (kind[k] == DYNOBA_POSE6) kept_pose[idx[k]] = 1;
+  }
+  // the kept points' factors, block by block in caller order
+  struct Export { int bi; std::vector<int32_t> orig; };
+  std::vector<Export> ex; int64_t count = 0;
+  for (size_t bi = 0; bi < h->blocks.size(); bi++) {
+    const HostBlock& b = h->blocks[bi]; const TypeInfo ti = type_info(b.type);
+    if (ti.nlmk == 0) continue;
+    std::vector<int32_t> orig;
+    for (int64_t i = 0; i < b.n; i++) {
+      const int32_t* ix = b.idx.data() + i*ti.arity;
+      bool touches = false;
+      for (int k = 0; k < ti.arity; k++) touches |= ti.cls[k] == VC_POINT && kept_pt[ix[k]];
+      if (!touches) continue;
+      if (ti.nlmk > 1) { h->err = "a kept point belongs to a group of more than one point (a WCME / WCPE chain)"; return DYNOBA_ERR_UNSUPPORTED; }
+      if (!(b.type == F_POSE2POINT3 || b.type == F_STEREO3 || b.type == F_HYBRID3 || b.type == F_HYBRID_STEREO3 || is_linear_type(b.type))) {
+        h->err = "a kept point has a factor of a type that is not kept (POSE2POINT3, STEREO3, HYBRID3, HYBRID_STEREO3, LINEAR_PP3, LINEAR_PPP3)";
+        return DYNOBA_ERR_UNSUPPORTED;
+      }
+      for (int k = 0; k < ti.arity; k++) if (ti.cls[k] == VC_POSE && !kept_pose[ix[k]]) {
+        h->err = "a kept point has a factor on a pose that is not kept (a backtracked tracklet would couple the kept landmarks densely)";
+        return DYNOBA_ERR_UNSUPPORTED;
+      }
+      orig.push_back((int32_t)i);
+    }
+    if (!orig.empty()) { count += (int64_t)orig.size(); ex.push_back({ (int)bi, std::move(orig) }); }
+  }
+  *n_out = count;
+  ARG(capacity >= count, "capacity is smaller than the number of exported factors (*n_out)");
+  ARG(count == 0 || (out_type && out_idx && out_Ab), "null output array");
+  if (count == 0) return marginal_impl(h, n_keep, kind, idx, G, g, f);
+  std::vector<int32_t> pos; pos.reserve(count);
+  {
+    int64_t k = 0;
+    for (const Export& e : ex) {
+      const HostBlock& b = h->blocks[e.bi]; const TypeInfo ti = type_info(b.type);
+      std::vector<int32_t> sorted_of(b.n);
+      for (int64_t s = 0; s < b.n; s++) sorted_of[b.perm[s]] = (int32_t)s;
+      for (int32_t o : e.orig) {
+        pos.push_back(sorted_of[o]);
+        out_type[k] = ti.npose == 1 ? DYNOBA_LINEAR_PP3 : DYNOBA_LINEAR_PPP3;
+        for (int c = 0; c < 3; c++) out_idx[3*k + c] = c < ti.arity ? b.idx[(int64_t)o*ti.arity + c] : -1;
+        k++;
+      }
+    }
+  }
+  int* dpos; double* dout;
+  if ((rc = upload(h, &dpos, pos))) return rc;
+  if ((rc = dalloc(h, &dout, (size_t)count*3*LINEAR_EXPORT_COLS, false))) { release(h, dpos); return rc; }
+  if (!h->linearized) do_linearize(h);
+  {
+    int64_t off = 0;
+    for (const Export& e : ex) {
+      h->launches += launch_linear_export(h->blocks[e.bi].dev, dpos + off, (int)e.orig.size(), dout + off*3*LINEAR_EXPORT_COLS, h->stream);
+      off += (int64_t)e.orig.size();
+    }
+  }
+  CK(cudaMemcpyAsync(out_Ab, dout, (size_t)count*3*LINEAR_EXPORT_COLS*8, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  release(h, dpos); release(h, dout);
+  rc = marginal_impl(h, n_keep, kind, idx, G, g, f);
+  do_linearize(h);                                      // the masked factors get their Jacobians and rhs back
+  CK(cudaStreamSynchronize(h->stream)); CK(cudaGetLastError());
+  if (rc) return rc;
+  if (f) {
+    double sb2 = 0.0;
+    for (int64_t k = 0; k < count*3; k++) { const double bk = out_Ab[k*LINEAR_EXPORT_COLS + LINEAR_EXPORT_COLS - 1]; sb2 += bk*bk; }
+    *f -= sb2;
+  }
+  return DYNOBA_OK;
 }
 
 }  // extern "C"

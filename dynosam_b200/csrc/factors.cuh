@@ -10,16 +10,20 @@ namespace dynoba {
 enum : int {
   F_PRIOR6 = 0, F_BETWEEN6 = 1, F_POSE2POINT3 = 2, F_STEREO3 = 3, F_TERNARY3 = 4, F_HYBRID3 = 5,
   F_HYBRID_STEREO3 = 6, F_MOTIONPOSE3 = 7, F_SMOOTH_HYBRID6 = 8, F_SMOOTH_POSE6 = 9, F_FLOWPROJ2 = 10,
-  F_PRIOR_VEL3 = 11, F_PRIOR_BIAS6 = 12, F_COMBINED_IMU15 = 13,
-  F_NUM_TYPES = 14
+  F_PRIOR_VEL3 = 11, F_PRIOR_BIAS6 = 12, F_COMBINED_IMU15 = 13, F_LINEAR_PP3 = 14, F_LINEAR_PPP3 = 15,
+  F_NUM_TYPES = 16
 };
 // VC_VEL / VC_BIAS: the navigation variables of the visual-inertial graphs.  Like poses they live in the reduced system,
 // each in a 6-wide block (a velocity's last three scalars are inert), and are stored in the pose SoA at their position.
 enum : int { VC_POSE = 0, VC_POINT = 1, VC_FLOW = 2, VC_VEL = 3, VC_BIAS = 4 };
 __host__ __device__ constexpr bool is_poselike(int c) { return c == VC_POSE || c == VC_VEL || c == VC_BIAS; }
 __host__ __device__ constexpr bool is_nav_type(int t) { return t == F_PRIOR_VEL3 || t == F_PRIOR_BIAS6 || t == F_COMBINED_IMU15; }
+// linearised landmark factors (gtsam::LinearContainerFactor holding a 3-row JacobianFactor): kernels_linear.cu
+__host__ __device__ constexpr bool is_linear_type(int t) { return t == F_LINEAR_PP3 || t == F_LINEAR_PPP3; }
 constexpr int IMU_MEAS = 70;       // meas record of COMBINED_IMU15 (include/dynoba.h)
 constexpr int IMU_SQRT_INFO = 225; // its 15 x 15 square-root information, row-major
+constexpr int LINEAR_PP3_MEAS = 45;  // A (3 x 9) | b (3) | lin pose (12) | lin point (3)
+constexpr int LINEAR_PPP3_MEAS = 75; // A (3 x 15) | b (3) | lin poses (2 x 12) | lin point (3)
 
 // static type tables (host + device constexpr)
 struct TypeInfo {
@@ -44,6 +48,8 @@ __host__ __device__ constexpr TypeInfo type_info(int t) {
     case F_PRIOR_VEL3:     return { 1, 3, 3, 3, 0, 0, 0, { VC_VEL, -1, -1, -1, -1, -1 }, { 0, 0, 0, 0, 0, 0 }, false };
     case F_PRIOR_BIAS6:    return { 1, 6, 6, 6, 0, 0, 0, { VC_BIAS, -1, -1, -1, -1, -1 }, { 0, 0, 0, 0, 0, 0 }, false };
     case F_COMBINED_IMU15: return { 6, 15, IMU_MEAS, 30, 2, 0, 0, { VC_POSE, VC_VEL, VC_POSE, VC_VEL, VC_BIAS, VC_BIAS }, { 0, 6, 9, 15, 18, 24 }, false };
+    case F_LINEAR_PP3:     return { 2, 3, LINEAR_PP3_MEAS, 9, 1, 1, 3, { VC_POSE, VC_POINT, -1, -1 }, { 0, 6, 0, 0 }, false };
+    case F_LINEAR_PPP3:    return { 3, 3, LINEAR_PPP3_MEAS, 15, 2, 1, 3, { VC_POSE, VC_POSE, VC_POINT, -1 }, { 0, 6, 12, 0 }, false };
     default:               return { 0, 0, 0, 0, 0, 0, 0, { -1, -1, -1, -1 }, { 0, 0, 0, 0 }, false };
   }
 }

@@ -316,6 +316,14 @@ int launch_nav_factors(const DevBlock& blk, const DevBand& B, cudaStream_t s);
 int launch_nav_model(const DevBlock& blk, const DevBand& B, double* partials, cudaStream_t s);
 int launch_nav_retract(const DevVars& cur, const DevVars& cand, const DevBand& B, const int2* nav, int n, cudaStream_t s);
 int launch_nav_inert(const DevBand& B, const int2* nav, int n, cudaStream_t s);
+// ---- linearised landmark factors (kernels_linear.cu).  with_jacobian: J = A, b - A d into the block (linearize); else the
+// errors alone.  Writes linearize_grid(n) partial sums.
+int launch_linear_factors(const DevBlock& blk, const DevVars& v, bool with_jacobian, double* partials, double* per_factor,
+                          cudaStream_t s);
+// export of the factors at sorted positions pos[n] of a landmark block: out[i] = 3 rows of [A | 0 | b]
+// (LINEAR_EXPORT_COLS doubles each); then their pose columns and rhs are zeroed in the block
+constexpr int LINEAR_EXPORT_COLS = 16;
+int launch_linear_export(const DevBlock& blk, const int* pos, int n, double* out, cudaStream_t s);
 
 // ---- per-frame batch entry points (kernels_star.cu, kernels_ransac.cu).  Per-device state kept between calls (these entry
 // points run every frame): one stream and one grow-only workspace, so a call costs copies + one launch -- no cudaMalloc /

@@ -295,9 +295,9 @@ int launch_cov_simple(const DevBlock& blk, const double* sig, int TPC, double* o
   if (blk.n_groups == 0) return 0;
   const int grid = (blk.n_groups + COV_WARPS - 1)/COV_WARPS;
   switch (blk.type) {
-    case F_POSE2POINT3: case F_STEREO3:
+    case F_POSE2POINT3: case F_STEREO3: case F_LINEAR_PP3:
       cov_simple_kernel<1, 3, 3, 0, 6, 0><<<grid, COV_WARPS*32, 0, s>>>(blk, sig, TPC, out_point, fail); return 1;
-    case F_HYBRID3: case F_HYBRID_STEREO3:
+    case F_HYBRID3: case F_HYBRID_STEREO3: case F_LINEAR_PPP3:
       cov_simple_kernel<2, 3, 3, 0, 12, 0><<<grid, COV_WARPS*32, 0, s>>>(blk, sig, TPC, out_point, fail); return 1;
     case F_FLOWPROJ2:
       cov_simple_kernel<1, 2, 2, 2, 0, 1><<<grid, COV_WARPS*32, 0, s>>>(blk, sig, TPC, out_flow, fail); return 1;

@@ -235,6 +235,7 @@ __global__ void fold_partials_kernel(const double* __restrict__ in, int nin, dou
 int launch_linearize(const DevBlock& blk, const DevVars& v, double* partials, cudaStream_t s) {
   if (blk.n == 0) return 0;
   if (is_nav_type(blk.type)) return launch_nav_linearize(blk, v, partials, s);
+  if (is_linear_type(blk.type)) return launch_linear_factors(blk, v, true, partials, nullptr, s);
   const int grid = linearize_grid(blk.n);
   if (blk.type == F_MOTIONPOSE3 || blk.type == F_SMOOTH_HYBRID6 || blk.type == F_SMOOTH_POSE6) {
     const int g2 = numeric_grid(blk.type, blk.n);
@@ -254,6 +255,7 @@ int launch_linearize(const DevBlock& blk, const DevVars& v, double* partials, cu
 int launch_error(const DevBlock& blk, const DevVars& v, double* partials, double* per_factor, cudaStream_t s) {
   if (blk.n == 0) return 0;
   if (is_nav_type(blk.type)) return launch_nav_error(blk, v, partials, per_factor, s);
+  if (is_linear_type(blk.type)) return launch_linear_factors(blk, v, false, partials, per_factor, s);
   const int grid = linearize_grid(blk.n);
 #define CALL_ERR(TT) error_kernel<TT><<<grid, LIN_THREADS, 0, s>>>(blk, v, partials, per_factor)
   DISPATCH_TYPE(blk.type, CALL_ERR)

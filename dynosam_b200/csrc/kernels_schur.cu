@@ -218,8 +218,8 @@ static int launch_schur_t(const DevBlock& blk, const unsigned char* grp_win, con
 int launch_schur_simple(const DevBlock& blk, const unsigned char* grp_win, const DevBand& B, double lambda, int* fail, cudaStream_t s) {
   if (blk.n_groups == 0) return 0;
   switch (blk.type) {
-    case F_POSE2POINT3: case F_STEREO3: return launch_schur_t<1, 3, 3, 0, 6, 0>(blk, grp_win, B, lambda, fail, s);
-    case F_HYBRID3: case F_HYBRID_STEREO3: return launch_schur_t<2, 3, 3, 0, 12, 0>(blk, grp_win, B, lambda, fail, s);
+    case F_POSE2POINT3: case F_STEREO3: case F_LINEAR_PP3: return launch_schur_t<1, 3, 3, 0, 6, 0>(blk, grp_win, B, lambda, fail, s);
+    case F_HYBRID3: case F_HYBRID_STEREO3: case F_LINEAR_PPP3: return launch_schur_t<2, 3, 3, 0, 12, 0>(blk, grp_win, B, lambda, fail, s);
     case F_FLOWPROJ2: return launch_schur_t<1, 2, 2, 2, 0, 1>(blk, grp_win, B, lambda, fail, s);
     default: return 0;
   }
@@ -354,9 +354,9 @@ int launch_backsub_simple(const DevBlock& blk, const DevBand& B, double lambda, 
   if (blk.n_groups == 0) return 0;
   const int grid = backsub_grid(blk.n_groups);
   switch (blk.type) {
-    case F_POSE2POINT3: case F_STEREO3:
+    case F_POSE2POINT3: case F_STEREO3: case F_LINEAR_PP3:
       backsub_simple_kernel<1, 3, 3, 0, 6, 0><<<grid, SCHUR_WARPS*32, 0, s>>>(blk, B, lambda, dl_point, nl_stride, partials); return 1;
-    case F_HYBRID3: case F_HYBRID_STEREO3:
+    case F_HYBRID3: case F_HYBRID_STEREO3: case F_LINEAR_PPP3:
       backsub_simple_kernel<2, 3, 3, 0, 12, 0><<<grid, SCHUR_WARPS*32, 0, s>>>(blk, B, lambda, dl_point, nl_stride, partials); return 1;
     case F_FLOWPROJ2:
       backsub_simple_kernel<1, 2, 2, 2, 0, 1><<<grid, SCHUR_WARPS*32, 0, s>>>(blk, B, lambda, dl_flow, nf_stride, partials); return 1;

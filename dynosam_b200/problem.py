@@ -15,21 +15,34 @@ import numpy as np
 
 # factor type ids == include/dynoba.h enum dynoba_factor_type
 PRIOR6, BETWEEN6, POSE2POINT3, STEREO3, TERNARY3, HYBRID3, HYBRID_STEREO3, MOTIONPOSE3, \
-    SMOOTH_HYBRID6, SMOOTH_POSE6, FLOWPROJ2, PRIOR_VEL3, PRIOR_BIAS6, COMBINED_IMU15 = range(14)
+    SMOOTH_HYBRID6, SMOOTH_POSE6, FLOWPROJ2, PRIOR_VEL3, PRIOR_BIAS6, COMBINED_IMU15, LINEAR_PP3, LINEAR_PPP3 = range(16)
 TYPE_NAMES = ["PRIOR6", "BETWEEN6", "POSE2POINT3", "STEREO3", "TERNARY3", "HYBRID3", "HYBRID_STEREO3",
-              "MOTIONPOSE3", "SMOOTH_HYBRID6", "SMOOTH_POSE6", "FLOWPROJ2", "PRIOR_VEL3", "PRIOR_BIAS6", "COMBINED_IMU15"]
-ARITY = [1, 2, 2, 2, 3, 3, 3, 4, 3, 3, 2, 1, 1, 6]
-DIM = [6, 6, 3, 3, 3, 3, 3, 3, 6, 6, 2, 3, 6, 15]
-MEAS_DIM = [12, 12, 3, 3, 0, 3, 3, 0, 0, 0, 15, 3, 6, 70]
+              "MOTIONPOSE3", "SMOOTH_HYBRID6", "SMOOTH_POSE6", "FLOWPROJ2", "PRIOR_VEL3", "PRIOR_BIAS6", "COMBINED_IMU15",
+              "LINEAR_PP3", "LINEAR_PPP3"]
+ARITY = [1, 2, 2, 2, 3, 3, 3, 4, 3, 3, 2, 1, 1, 6, 2, 3]
+DIM = [6, 6, 3, 3, 3, 3, 3, 3, 6, 6, 2, 3, 6, 15, 3, 3]
+# LINEAR_PP3 / LINEAR_PPP3 (linearised landmark factors, no noise model: sigma 1): A [3, jcols] row-major | b [3] |
+# linearisation point of each pose slot [12] | of the point [3]
+MEAS_DIM = [12, 12, 3, 3, 0, 3, 3, 0, 0, 0, 15, 3, 6, 70, 45, 75]
 # variable class per key slot: 0 pose(6), 1 point(3), 2 flow(2), 3 velocity(3), 4 IMU bias(6)
 SLOT_CLASS = [
     [0], [0, 0], [0, 1], [0, 1], [1, 1, 0], [0, 0, 1], [0, 0, 1], [1, 1, 0, 0], [0, 0, 0], [0, 0, 0], [2, 0],
-    [3], [4], [0, 3, 0, 3, 4, 4],
+    [3], [4], [0, 3, 0, 3, 4, 4], [0, 1], [0, 0, 1],
 ]
 CLASS_DIM = [6, 3, 2, 3, 6]
 JCOLS = [sum(CLASS_DIM[c] for c in s) for s in SLOT_CLASS]
-NEEDS_AUX = [False, False, False, False, False, True, True, False, True, False, False, False, False, False]
+NEEDS_AUX = [False, False, False, False, False, True, True, False, True, False, False, False, False, False, False, False]
 IMU_SQRT_INFO_DIM = 225   # COMBINED_IMU15's sigma: the 15x15 square-root information R, row-major
+LINEAR_TYPES = (LINEAR_PP3, LINEAR_PPP3)
+
+
+def linear_block(type_, idx, A, b, lin_pose, lin_point) -> "FactorBlock":
+    """A LINEAR_PP3 / LINEAR_PPP3 block: idx [n, arity], A [n, 3, jcols], b [n, 3], lin_pose [n, npose, 12] (or
+    [n, 12] for one pose slot), lin_point [n, 3].  error = 1/2 |A d - b|^2, d = localCoordinates(lin, x)."""
+    n, npose = np.asarray(idx).reshape(-1, ARITY[type_]).shape[0], ARITY[type_] - 1
+    meas = np.concatenate([np.asarray(A, np.float64).reshape(n, 3*JCOLS[type_]), np.asarray(b, np.float64).reshape(n, 3),
+                           np.asarray(lin_pose, np.float64).reshape(n, 12*npose), np.asarray(lin_point, np.float64).reshape(n, 3)], 1)
+    return FactorBlock(type_, idx, meas, np.ones(1))
 
 
 @dataclass

@@ -61,8 +61,20 @@ typedef enum {
   DYNOBA_PRIOR_VEL3 = 11,   /* gtsam::PriorFactor<Vector3> (VisionImuBackendModule.hpp:114-166)      vel                  prior (3)         */
   DYNOBA_PRIOR_BIAS6 = 12,  /* gtsam::PriorFactor<imuBias::ConstantBias> (same)                      bias                 prior (6)         */
   DYNOBA_COMBINED_IMU15 = 13,/* gtsam::CombinedImuFactor   (VisionImuBackendModule.hpp:168-243)      pose_i, vel_i, pose_j, vel_j, bias_i, bias_j   pim (70) */
-  DYNOBA_NUM_FACTOR_TYPES = 14
+  DYNOBA_LINEAR_PP3 = 14,   /* gtsam::LinearContainerFactor(JacobianFactor) (SlidingWindowOptimization.cc:170-188) pose, point  A | b | lin (45) */
+  DYNOBA_LINEAR_PPP3 = 15,  /* the same over a camera pose, an object motion and a point              pose, motion, point  A | b | lin (75) */
+  DYNOBA_NUM_FACTOR_TYPES = 16
 } dynoba_factor_type;
+/* LINEAR_PP3 / LINEAR_PPP3: the linearised observation factor of a landmark that the previous sliding window kept
+ * (dynoba_marginal_keep_points exports them).  A 3-row JacobianFactor(keys, A, b) with no noise model -- A and b already
+ * whitened and Huber re-weighted, as NoiseModelFactor::linearize leaves them -- held by a LinearContainerFactor with
+ * linearisation point lin [GTSAM-ext LinearContainerFactor]:
+ *     d = lin.localCoordinates(x): Logmap(lin_i^-1 x_i) per pose slot, x - lin for the point;
+ *     error(x) = 1/2 |A d - b|^2;   linearize(x) = JacobianFactor(A, b - A d)   (A is used as is, as GTSAM does).
+ * meas: A (3 x jcols, row-major, columns in key order: 6 per pose slot, 3 for the point) | b (3) | lin of each pose slot
+ * (12: R row-major | t) | lin of the point (3): 27 + 3 + 12 + 3 = 45 for PP3, 45 + 3 + 24 + 3 = 75 for PPP3.  The pose
+ * slots take POSE6 variables.  No noise model: sigma must be 1 (sigma_dim 1 or 3) and robust_k 0, else DYNOBA_ERR_BAD_ARG.
+ * dynoba_get_linearization returns A bit for bit as the Jacobian and b - A d as the rhs. */
 /* PRIOR_VEL3 / PRIOR_BIAS6: e = x - prior, H = I.
  * COMBINED_IMU15: CombinedImuFactor::evaluateError of GTSAM 4.2.0 with ManifoldPreintegration and no Coriolis term,
  * r = [PreintegrationBase::computeErrorAndJacobians (9: rotation, position, velocity), b_i - b_j (6)], 15 rows.
@@ -163,7 +175,7 @@ int dynoba_add_linear_prior_vars(dynoba_handle h, int32_t n, const int32_t* kind
  * dynoba_add_linear_prior of the next window together with the current values of the kept variables as linearisation
  * point.  The kept variables must be the last ones of the elimination order (the most recent frames) and span no more
  * than the band of the reduced system (else DYNOBA_ERR_UNSUPPORTED).  Difference from the reference: it retains recent
- * LANDMARKS as well; here every landmark is eliminated into the prior.  Single GPU.  Poses only: refused
+ * LANDMARKS as well; here every landmark is eliminated into the prior (dynoba_marginal_keep_points keeps them).  Single GPU.  Poses only: refused
  * (DYNOBA_ERR_UNSUPPORTED) on a graph with velocity / bias variables; dynoba_marginal_vars takes those graphs. */
 int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_idx, double* G, double* g);
 /* dynoba_marginal for a kept set of any pose-like kinds (kind[k], idx[k] as in dynoba_add_linear_prior_vars): poses,
@@ -181,6 +193,27 @@ int dynoba_marginal(dynoba_handle h, int32_t n_keep, const int32_t* keep_pose_id
  * that solve's time on top of the marginal's. */
 int dynoba_marginal_vars(dynoba_handle h, int32_t n_keep, const int32_t* kind, const int32_t* idx, double* G, double* g,
                          double* f);
+/* dynoba_marginal_vars that also keeps n_pts landmarks (pt_idx[i], POINT3 indices; pt_kind NULL or every entry
+ * DYNOBA_POINT3), as the reference's sliding window keeps every key inserted in its last frames, landmarks included
+ * (SlidingWindowOptimization.cc:64-130).  What eliminatePartialMultifrontal leaves of the linearised graph is then
+ *   (i)  every factor that touches a kept point, as it is linearised at the current values: exported, one per factor,
+ *        block by block in dynoba_add_factors order and in the caller's factor order within a block;
+ *   (ii) the Schur marginal (G, g, f) of every OTHER factor onto the kept pose-like variables -- dynoba_marginal_vars of
+ *        the graph without the factors of (i), which therefore are not counted twice.
+ * Exported factor k: out_type[k] = DYNOBA_LINEAR_PP3 for a POSE2POINT3, STEREO3 or LINEAR_PP3 factor, DYNOBA_LINEAR_PPP3
+ * for a HYBRID3, HYBRID_STEREO3 or LINEAR_PPP3 factor; out_idx[3k..3k+2] = its variable indices in key order (pose,
+ * point, -1 or pose, motion, point); out_Ab[48k..48k+47] = 3 rows of 16 doubles: A in columns [0, jcols), zeros, b in
+ * column 15, so that error = 1/2 |A delta - b|^2.  With the current values of those variables as linearisation point
+ * they are the meas records of dynoba_add_factors for the next window.  *n_out receives the number of exported factors
+ * also when capacity is too small (then DYNOBA_ERR_BAD_ARG and nothing else happens).
+ * n_pts = 0 is dynoba_marginal_vars exactly.  DYNOBA_ERR_UNSUPPORTED, before any device work: a kept point with a factor on
+ * a pose-like variable that is not kept (a backtracked tracklet: GTSAM's separator would couple landmarks densely), with a
+ * factor of another type, or in a group of more than one point (WCME / WCPE chains); world > 1.  DYNOBA_ERR_BAD_ARG: a
+ * point listed twice or out of range, a flow variable, capacity < *n_out.  Every other refusal of dynoba_marginal_vars
+ * applies.  The handle's state after the call, successful or not, is that of a fresh linearisation at the same values. */
+int dynoba_marginal_keep_points(dynoba_handle h, int32_t n_keep, const int32_t* kind, const int32_t* idx, int32_t n_pts,
+                                const int32_t* pt_kind, const int32_t* pt_idx, double* G, double* g, double* f,
+                                int64_t capacity, int64_t* n_out, int32_t* out_type, int32_t* out_idx, double* out_Ab);
 /* gtsam::Marginals(graph, values, Marginals::CHOLESKY).marginalCovariance(key) for many variables of one kind:
  * the graph linearised at the current values (robust re-weighting as linearize does, no damping), H = J^T J,
  * cov[i] = the diagonal block of H^-1 of variable idx[i] (caller order; idx == NULL: all n variables of the kind).
