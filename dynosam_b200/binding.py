@@ -26,7 +26,7 @@ REDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.
 EXPORTS = [
     "dynoba_version", "dynoba_status_string", "dynoba_last_error", "dynoba_create", "dynoba_destroy",
     "dynoba_lm_default_params", "dynoba_set_variables", "dynoba_set_aux_poses", "dynoba_set_calibration",
-    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_add_linear_prior_vars", "dynoba_marginal", "dynoba_marginal_vars", "dynoba_marginal_keep_points", "dynoba_marginal_covariance", "dynoba_finalize", "dynoba_error",
+    "dynoba_add_factors", "dynoba_set_pose_order", "dynoba_set_variable_order", "dynoba_set_shard", "dynoba_set_reduce", "dynoba_set_partition", "dynoba_plan_partition", "dynoba_set_tuning", "dynoba_fp64_rate", "dynoba_add_linear_prior", "dynoba_add_linear_prior_vars", "dynoba_marginal", "dynoba_marginal_vars", "dynoba_marginal_keep_points", "dynoba_marginal_covariance", "dynoba_joint_marginal_covariance", "dynoba_finalize", "dynoba_error",
     "dynoba_optimize", "dynoba_get_variables", "dynoba_get_keys", "dynoba_num_variables", "dynoba_problem_info", "dynoba_window_census",
     "dynoba_linearize", "dynoba_linearize_block", "dynoba_get_linearization", "dynoba_get_factor_errors", "dynoba_solve",
     "dynoba_get_reduced_system", "dynoba_retract", "dynoba_last_model", "dynoba_get_lm_trace", "dynoba_flow_pose_default_params", "dynoba_flow_pose_batch",
@@ -119,6 +119,7 @@ def load():
         L.dynoba_marginal.argtypes = [C.c_void_p, C.c_int32, c_ip, c_dp, c_dp]
         L.dynoba_marginal_vars.argtypes = [C.c_void_p, C.c_int32, c_ip, c_ip, c_dp, c_dp, c_dp]
         L.dynoba_marginal_covariance.argtypes = [C.c_void_p, C.c_int, C.c_int64, c_ip, c_dp]
+        L.dynoba_joint_marginal_covariance.argtypes = [C.c_void_p, C.c_int32, c_ip, c_ip, c_dp]
         L.dynoba_marginal_keep_points.argtypes = [C.c_void_p, C.c_int32, c_ip, c_ip, C.c_int32, c_ip, c_ip, c_dp, c_dp, c_dp,
                                                   C.c_int64, C.POINTER(C.c_int64), c_ip, c_ip, c_dp]
         L.dynoba_finalize.argtypes = [C.c_void_p]
@@ -335,6 +336,20 @@ class Solver:
         cov = np.zeros((n, d, d))
         self._ck(self.lib.dynoba_marginal_covariance(self.h, kind, n, ip, _dp(cov)))
         return cov
+
+    def joint_marginal_covariance(self, kinds, idx):
+        """(cov, offsets): the joint marginal covariance of the variables (kinds[k], idx[k]) of any kinds at the current
+        values -- gtsam::Marginals(graph, values, CHOLESKY).jointMarginalCovariance in the caller's order -- as one D x D
+        array, and the first row of every variable's block (dynoba_joint_marginal_covariance)"""
+        kinds = np.ascontiguousarray(kinds, dtype=np.int32).reshape(-1); idx = np.ascontiguousarray(idx, dtype=np.int32).reshape(-1)
+        if kinds.size != idx.size:
+            raise DynobaError(ERR_BAD_ARG, "kinds and idx differ in length")
+        dims = [{POSE6: 6, BIAS6: 6, POINT3: 3, VEL3: 3, FLOW2: 2}.get(int(k), 0) for k in kinds]
+        offsets = np.concatenate([[0], np.cumsum(dims, dtype=np.int64)])
+        D = int(offsets[-1])
+        cov = np.zeros((max(D, 1), max(D, 1)))
+        self._ck(self.lib.dynoba_joint_marginal_covariance(self.h, kinds.size, _ip(kinds), _ip(idx), _dp(cov)))
+        return cov[:D, :D].copy(), offsets[:-1].copy()
 
     def set_shard(self, rank, world, allreduce, min_bandwidth=0):
         """allreduce(dev_ptr:int, n:int, stream:int) -> None sums n doubles in place across ranks."""

@@ -51,6 +51,7 @@ struct HostPrior {      // gtsam::LinearContainerFactor(HessianFactor) over pose
 };
 
 constexpr int LM_TRACE_COLS = 10;   // columns of a dynoba_get_lm_trace row
+enum CovTiles { COV_NONE, COV_FACTOR, COV_SIGMA };   // what the covariance layout's tiles hold
 
 }  // namespace
 
@@ -78,10 +79,11 @@ struct dynoba_solver {
   // (LM_TRACE_COLS doubles: iterations, inner, lambda, oldLin, lin, err, nerr, solved, success, stop)
   double last_model[3] = {0.0, 0.0, 0.0};
   std::vector<double> lm_trace;
-  // dynoba_marginal_covariance: Sigma = S^-1 on the band of a plain layout of its own, and the landmark tables, kept from
-  // the first call at a linearisation point until the values change
+  // dynoba_marginal_covariance / dynoba_joint_marginal_covariance: a plain layout of their own whose tiles hold nothing,
+  // the factor L of the undamped reduced system or Sigma = S^-1 on its band (cov_tiles), and the landmark tables, kept
+  // from the first call at a linearisation point until the values change
   BandPlan cov_plan{}; double* cov_stage = nullptr; double* cov_lmk = nullptr;
-  bool cov_live = false, cov_ready = false, cov_lmk_ready = false;
+  bool cov_live = false, cov_lmk_ready = false; int cov_tiles = 0; float cov_ms[2] = {0.0f, 0.0f};
 };
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return DYNOBA_ERR_CUDA; } } while (0)
@@ -174,7 +176,7 @@ static void free_device(dynoba_solver* h) {
   for (auto& a : h->allocs) g_devcache.give(h->device, a.first, a.second);
   h->allocs.clear();
   h->finalized = false; h->linearized = false;
-  h->cov_live = h->cov_ready = h->cov_lmk_ready = false; h->cov_stage = nullptr; h->cov_lmk = nullptr;
+  h->cov_live = h->cov_lmk_ready = false; h->cov_tiles = COV_NONE; h->cov_stage = nullptr; h->cov_lmk = nullptr;
 }
 // hands one allocation of the handle back to the cache
 static void release(dynoba_solver* h, void* q) {
@@ -201,7 +203,7 @@ static void plain_plan_release(dynoba_solver* h, BandPlan& mp) {
 static void cov_invalidate(dynoba_solver* h) {
   if (h->cov_live) { cudaStreamSynchronize(h->stream); plain_plan_release(h, h->cov_plan); release(h, h->cov_stage); }
   if (h->cov_lmk) release(h, h->cov_lmk);
-  h->cov_live = h->cov_ready = h->cov_lmk_ready = false; h->cov_stage = nullptr; h->cov_lmk = nullptr;
+  h->cov_live = h->cov_lmk_ready = false; h->cov_tiles = COV_NONE; h->cov_stage = nullptr; h->cov_lmk = nullptr;
 }
 
 // copy of a caller's array into the handle: parallel, so that the first touch of the fresh pages (the expensive part of a
@@ -1363,9 +1365,9 @@ int dynoba_marginal_keep_points(dynoba_handle h, int32_t n_keep, const int32_t* 
 
 }  // extern "C"
 
-// Sigma = S^-1 on the band of the plain layout, S the undamped reduced system at the current values: build, factor,
-// selected inversion.  DYNOBA_TIMING=1 prints the CUDA-event times of the stages.
-static int cov_band(dynoba_solver* h) {
+// The factor L of S, the undamped reduced system at the current values, in the covariance layout's tiles: build and
+// factor (over whatever the tiles held).  The stage times are kept for the DYNOBA_TIMING lines.
+static int cov_factor(dynoba_solver* h) {
   int rc;
   if (!h->linearized) do_linearize(h);
   if (!h->cov_live) {
@@ -1373,6 +1375,7 @@ static int cov_band(dynoba_solver* h) {
     if ((rc = dalloc(h, &h->cov_stage, selinv_stage_count(h->cov_plan.band.WB), false))) { plain_plan_release(h, h->cov_plan); return rc; }
     h->cov_live = true;
   }
+  h->cov_tiles = COV_NONE;
   std::swap(h->plan, h->cov_plan);                      // (h->band refers to h->plan.band)
   cudaEventRecord(h->ev[0], h->stream);
   rc = build_reduced(h, 0.0);
@@ -1383,16 +1386,24 @@ static int cov_band(dynoba_solver* h) {
   if (rc) return rc;
   int failed = 0;
   CK(cudaMemcpyAsync(&failed, h->fail, 4, cudaMemcpyDeviceToHost, h->stream)); CK(cudaStreamSynchronize(h->stream));
+  for (int k = 0; k < 2; k++) cudaEventElapsedTime(&h->cov_ms[k], h->ev[k], h->ev[k + 1]);
   if (failed) { h->err = "the reduced system is not positive definite"; return DYNOBA_ERR_INDETERMINATE; }
+  h->cov_tiles = COV_FACTOR;
+  return DYNOBA_OK;
+}
+// Sigma = S^-1 on the band, over L in place (selected inversion).  DYNOBA_TIMING=1 prints the CUDA-event times of the
+// stages, build and factor from the call that factored.
+static int cov_selinv(dynoba_solver* h) {
+  cudaEventRecord(h->ev[2], h->stream);
   h->launches += launch_band_selinv(h->cov_plan.chains[0], h->cov_plan.band.WB, h->cov_stage, h->stream);
   cudaEventRecord(h->ev[3], h->stream);
   CK(cudaStreamSynchronize(h->stream)); CK(cudaGetLastError());
   if (getenv("DYNOBA_TIMING")) {
-    float t[3]; for (int k = 0; k < 3; k++) cudaEventElapsedTime(&t[k], h->ev[k], h->ev[k + 1]);
+    float t; cudaEventElapsedTime(&t, h->ev[2], h->ev[3]);
     std::fprintf(stderr, "[dynoba covariance] reduced system %.3f ms  factor %.3f ms  selected inversion %.3f ms  (n %d, WB %d)\n",
-                 t[0], t[1], t[2], h->cov_plan.band.n, h->cov_plan.band.WB);
+                 h->cov_ms[0], h->cov_ms[1], t, h->cov_plan.band.n, h->cov_plan.band.WB);
   }
-  h->cov_ready = true;
+  h->cov_tiles = COV_SIGMA;
   return DYNOBA_OK;
 }
 // covariances of every point ([npt][9]) and flow ([nfl][4]) in device order, from Sigma on the band.  A landmark that no
@@ -1428,7 +1439,10 @@ int dynoba_marginal_covariance(dynoba_handle h, int kind, int64_t n, const int32
   ARG(n == 0 || cov, "null cov");
   for (int64_t i = 0; idx && i < n; i++) ARG(idx[i] >= 0 && idx[i] < nk, "variable out of range");
   if (n == 0) return DYNOBA_OK;
-  if (!h->cov_ready && (rc = cov_band(h))) return rc;
+  if (h->cov_tiles != COV_SIGMA) {
+    if (h->cov_tiles != COV_FACTOR && (rc = cov_factor(h))) return rc;
+    if ((rc = cov_selinv(h))) return rc;
+  }
   const bool poselike = KINDS[kind].poselike;
   if (!poselike && !h->cov_lmk_ready && (rc = cov_landmarks(h))) return rc;
   const int d = KINDS[kind].tdim;
@@ -1448,6 +1462,208 @@ int dynoba_marginal_covariance(dynoba_handle h, int kind, int64_t n, const int32
   for (int64_t e = 0; e < n*d*d; e++)
     if (std::isnan(cov[e])) { h->err = "a requested landmark is not touched by any factor"; return DYNOBA_ERR_INDETERMINATE; }
   return DYNOBA_OK;
+}
+
+}  // extern "C"
+
+// Joint marginal covariance of n variables (DESIGN.md §4 "Joint marginal covariances").  C = the requested pose-like
+// variables and every pose a factor of a requested landmark's group touches; X = S^-1 E_C by the span-restricted band
+// sweeps over L; the requested landmark groups' strips from X[C, C]; the D x D result assembled here.
+static int joint_impl(dynoba_solver* h, int32_t n, const int32_t* kind, const int32_t* idx, double* cov) {
+  const VarLayout& L = h->layout;
+  const int64_t NP = L.NP();
+  // ---- requested landmark groups: points chained by a factor with several landmarks form one group
+  std::vector<int32_t> uf;                              // union-find over points (empty: every point alone)
+  auto root = [&](int32_t a) { if (uf.empty()) return a; while (uf[a] != a) a = uf[a] = uf[uf[a]]; return a; };
+  bool any_lmk = false;
+  for (int32_t i = 0; i < n; i++) any_lmk |= !KINDS[kind[i]].poselike;
+  if (any_lmk)
+    for (const HostBlock& b : h->blocks) {
+      const TypeInfo ti = type_info(b.type);
+      if (ti.nlmk < 2) continue;
+      if (uf.empty()) { uf.resize(L.npt); std::iota(uf.begin(), uf.end(), 0); }
+      for (int64_t o = 0; o < b.n; o++) {
+        int32_t r0 = -1;
+        for (int k = 0; k < ti.arity; k++) if (ti.cls[k] == VC_POINT) {
+          const int32_t r = root(b.idx[o*ti.arity + k]);
+          if (r0 < 0) r0 = r; else if (r != r0) uf[r] = r0;
+        }
+      }
+    }
+  // group of every requested landmark, in order of first request; key: root point, or npt + flow index
+  std::vector<int32_t> gkey_of((size_t)(L.npt + L.nfl), -1), gkey;
+  struct Req { int i, g; };
+  std::vector<Req> req;
+  for (int32_t i = 0; i < n; i++) {
+    if (KINDS[kind[i]].poselike) continue;
+    const int64_t key = kind[i] == DYNOBA_POINT3 ? root(idx[i]) : L.npt + idx[i];
+    if (gkey_of[key] < 0) { gkey_of[key] = (int32_t)gkey.size(); gkey.push_back((int32_t)key); }
+    req.push_back({ i, gkey_of[key] });
+  }
+  const int ng = (int)gkey.size();
+  // every factor of a requested group (block, sorted position), and the poses they touch
+  std::vector<std::vector<int32_t>> grefs(ng);
+  std::vector<char> in_c((size_t)NP, 0);
+  for (int32_t i = 0; i < n; i++) if (KINDS[kind[i]].poselike) in_c[L.column(kind[i], idx[i])] = 1;
+  for (size_t bi = 0; ng && bi < h->blocks.size(); bi++) {
+    const HostBlock& b = h->blocks[bi]; const TypeInfo ti = type_info(b.type);
+    if (ti.nlmk == 0) continue;
+    std::vector<std::pair<int32_t, int32_t>> hit;       // (original index, group)
+    for (int64_t o = 0; o < b.n; o++) {
+      const int32_t* ix = b.idx.data() + o*ti.arity;
+      for (int k = 0; k < ti.arity; k++) {
+        if (is_poselike(ti.cls[k])) continue;
+        const int32_t g = gkey_of[ti.cls[k] == VC_POINT ? root(ix[k]) : L.npt + ix[k]];
+        if (g >= 0) { hit.push_back({ (int32_t)o, g }); break; }
+      }
+    }
+    if (hit.empty()) continue;
+    std::vector<int32_t> sorted_of(b.n);
+    for (int64_t s = 0; s < b.n; s++) sorted_of[b.perm[s]] = (int32_t)s;
+    for (const auto& e : hit) {
+      grefs[e.second].push_back((int32_t)bi); grefs[e.second].push_back(sorted_of[e.first]);
+      for (int k = 0; k < ti.arity; k++) if (ti.cls[k] == VC_POSE) in_c[L.column(VC_POSE, b.idx[(int64_t)e.first*ti.arity + k])] = 1;
+    }
+  }
+  for (int g = 0; g < ng; g++) if (grefs[g].empty()) { h->err = "a requested landmark is not touched by any factor"; return DYNOBA_ERR_INDETERMINATE; }
+  // first device index and size of every group (a chain's points are contiguous in device order)
+  std::vector<int4> groups(ng);
+  {
+    std::vector<int32_t> lo(ng, INT32_MAX), hi(ng, -1), cnt(ng, 0);
+    auto add = [&](int g, int32_t d) { lo[g] = std::min(lo[g], d); hi[g] = std::max(hi[g], d); cnt[g]++; };
+    if (!uf.empty()) { for (int64_t p = 0; p < L.npt; p++) { const int32_t g = gkey_of[root((int32_t)p)]; if (g >= 0) add(g, L.pt_new[p]); } }
+    for (int g = 0; g < ng; g++) {
+      if (gkey[g] >= L.npt) { lo[g] = L.fl_new[gkey[g] - L.npt]; cnt[g] = 0; continue; }
+      if (uf.empty()) { lo[g] = hi[g] = L.pt_new[gkey[g]]; cnt[g] = 1; }
+      if (3*cnt[g] > STRIP_LD || hi[g] - lo[g] + 1 != cnt[g]) { h->err = "a requested landmark belongs to a group of more than 21 chained points"; return DYNOBA_ERR_UNSUPPORTED; }
+    }
+    int32_t r = 0;
+    for (int g = 0; g < ng; g++) { groups[g] = make_int4(r, r + (int)grefs[g].size()/2, lo[g], cnt[g]); r = groups[g].y; }
+  }
+  // C: ascending solver positions, the live scalars of each (a velocity's 3)
+  std::vector<char> is_vel((size_t)NP, 0);
+  for (int64_t i = 0; i < L.nv; i++) is_vel[L.column(DYNOBA_VEL3, i)] = 1;
+  std::vector<int32_t> cmap((size_t)NP, -1), cs;
+  for (int64_t p = 0; p < NP; p++) if (in_c[p]) { cmap[p] = (int32_t)cs.size(); for (int c = 0; c < (is_vel[p] ? 3 : 6); c++) cs.push_back((int32_t)(6*p + c)); }
+  const int nc = (int)cs.size(), J0 = cs[0]/TILE;
+  // requested landmarks grouped: rptr / rl, and each one's slot there
+  std::vector<int32_t> rptr(ng + 1, 0), rl(req.size()), rslot(req.size());
+  for (const Req& q : req) rptr[q.g + 1]++;
+  for (int g = 0; g < ng; g++) rptr[g + 1] += rptr[g];
+  {
+    std::vector<int32_t> fill(rptr.begin(), rptr.end() - 1);
+    for (size_t k = 0; k < req.size(); k++) {
+      const int s = fill[req[k].g]++;
+      rslot[k] = s; rl[s] = L.column(kind[req[k].i], idx[req[k].i]);
+    }
+  }
+  // ---- device: L, sweeps, X[C, C], strips
+  int rc;
+  const bool fresh = h->cov_tiles != COV_FACTOR;        // L is built here (else an earlier call left it)
+  if (fresh && (rc = cov_factor(h))) return rc;
+  const BandProb& ch = h->cov_plan.chains[0];
+  const size_t nreq = req.size();
+  std::vector<void*> owned;
+  auto done = [&](int r) { for (void* q : owned) release(h, q); return r; };
+  int* dcs; double *dpanel, *dxcc;
+  if ((rc = upload(h, &dcs, cs))) return rc;
+  owned.push_back(dcs);
+  if ((rc = dalloc(h, &dpanel, joint_panel_count(ch.NT, J0, nc), false))) return done(rc);
+  owned.push_back(dpanel);
+  if ((rc = dalloc(h, &dxcc, (size_t)nc*nc, false))) return done(rc);
+  owned.push_back(dxcc);
+  cudaEventRecord(h->ev[3], h->stream);
+  h->launches += launch_band_sweeps(ch, h->cov_plan.band.WB, dcs, nc, J0, dpanel, h->stream);
+  cudaEventRecord(h->ev[4], h->stream);
+  h->launches += launch_joint_gather(dpanel, J0, dcs, nc, dxcc, h->stream);
+  std::vector<double> xcc((size_t)nc*nc), m(nreq*nc*3), z(nreq*3*nc), vinv((size_t)ng*STRIP_LD*STRIP_LD);
+  if (ng) {
+    StripJob j{};
+    std::vector<DevBlock> hb; for (const HostBlock& b : h->blocks) hb.push_back(b.dev);
+    std::vector<int32_t> refs; for (const auto& r : grefs) refs.insert(refs.end(), r.begin(), r.end());
+    DevBlock* dblk; int32_t *drefs, *drptr, *drl, *dcmap; int4* dgroups; double *dm, *dz, *dvinv;
+    if ((rc = upload(h, &dblk, hb))) return done(rc);
+    owned.push_back(dblk);
+    if ((rc = upload(h, &drefs, refs))) return done(rc);
+    owned.push_back(drefs);
+    if ((rc = upload(h, &dgroups, groups))) return done(rc);
+    owned.push_back(dgroups);
+    if ((rc = upload(h, &drptr, rptr))) return done(rc);
+    owned.push_back(drptr);
+    if ((rc = upload(h, &drl, rl))) return done(rc);
+    owned.push_back(drl);
+    if ((rc = upload(h, &dcmap, cmap))) return done(rc);
+    owned.push_back(dcmap);
+    if ((rc = dalloc(h, &dm, m.size()))) return done(rc);        // zeroed: the strips add into it
+    owned.push_back(dm);
+    if ((rc = dalloc(h, &dz, z.size(), false))) return done(rc);
+    owned.push_back(dz);
+    if ((rc = dalloc(h, &dvinv, vinv.size(), false))) return done(rc);
+    owned.push_back(dvinv);
+    j.blocks = dblk; j.refs = drefs; j.groups = dgroups; j.rptr = drptr; j.rl = drl; j.cmap = dcmap; j.xcc = dxcc; j.nc = nc;
+    j.m = dm; j.z = dz; j.vinv = dvinv; j.ng = ng; j.fail = h->fail;
+    if (cudaMemsetAsync(h->fail, 0, 4, h->stream) != cudaSuccess) return done(DYNOBA_ERR_CUDA);
+    h->launches += launch_cov_strips(j, h->stream);
+    cudaEventRecord(h->ev[5], h->stream);
+    cudaMemcpyAsync(m.data(), dm, m.size()*8, cudaMemcpyDeviceToHost, h->stream);
+    cudaMemcpyAsync(z.data(), dz, z.size()*8, cudaMemcpyDeviceToHost, h->stream);
+    cudaMemcpyAsync(vinv.data(), dvinv, vinv.size()*8, cudaMemcpyDeviceToHost, h->stream);
+  } else {
+    cudaEventRecord(h->ev[5], h->stream);
+  }
+  int failed = 0;
+  cudaMemcpyAsync(xcc.data(), dxcc, xcc.size()*8, cudaMemcpyDeviceToHost, h->stream);
+  if (ng) cudaMemcpyAsync(&failed, h->fail, 4, cudaMemcpyDeviceToHost, h->stream);
+  const cudaError_t e = cudaStreamSynchronize(h->stream);
+  rc = done(DYNOBA_OK);
+  if (e != cudaSuccess || cudaGetLastError() != cudaSuccess) { h->err = std::string("joint covariance: ") + cudaGetErrorString(e); return DYNOBA_ERR_CUDA; }
+  if (getenv("DYNOBA_TIMING")) {
+    float t[2]; cudaEventElapsedTime(&t[0], h->ev[3], h->ev[4]); cudaEventElapsedTime(&t[1], h->ev[4], h->ev[5]);
+    std::fprintf(stderr, "[dynoba joint covariance] reduced system %.3f ms  factor %.3f ms%s  sweeps %.3f ms  strips %.3f ms  (span %d tiles, |C| %d, %d landmark groups, n %d, WB %d)\n",
+                 h->cov_ms[0], h->cov_ms[1], fresh ? "" : " (earlier call)", t[0], t[1], ch.NT - J0, nc, ng, h->cov_plan.band.n, h->cov_plan.band.WB);
+  }
+  if (failed) { h->err = "a requested landmark's information block is not positive definite"; return DYNOBA_ERR_INDETERMINATE; }
+  // ---- assembly: scalar a of the result = (variable, tangent index); the lower triangle, mirrored
+  std::vector<int32_t> var_of, sub_of, slot_of(n, -1);
+  for (size_t k = 0; k < req.size(); k++) slot_of[req[k].i] = rslot[k];
+  std::vector<int32_t> grp_of(n, -1);
+  for (const Req& q : req) grp_of[q.i] = q.g;
+  for (int32_t i = 0; i < n; i++) for (int c = 0; c < KINDS[kind[i]].tdim; c++) { var_of.push_back(i); sub_of.push_back(c); }
+  const int64_t D = (int64_t)var_of.size();
+  auto cidx = [&](int32_t i, int c) { return (size_t)cmap[L.column(kind[i], idx[i])] + c; };
+  auto loff = [&](int32_t i) { const int g = grp_of[i]; return (groups[g].w ? 3 : 2)*(L.column(kind[i], idx[i]) - groups[g].z); };
+  for (int64_t a = 0; a < D; a++) for (int64_t b = 0; b <= a; b++) {
+    const int32_t i = var_of[a], k = var_of[b]; const int r = sub_of[a], c = sub_of[b];
+    const bool pi = KINDS[kind[i]].poselike, pk = KINDS[kind[k]].poselike;
+    double v;
+    if (pi && pk) v = xcc[cidx(i, r)*nc + cidx(k, c)];
+    else if (!pi && pk) v = z[((size_t)slot_of[i]*3 + r)*nc + cidx(k, c)];
+    else if (pi && !pk) v = z[((size_t)slot_of[k]*3 + c)*nc + cidx(i, r)];
+    else {
+      v = grp_of[i] == grp_of[k] ? vinv[(size_t)grp_of[i]*STRIP_LD*STRIP_LD + (size_t)(loff(i) + r)*STRIP_LD + loff(k) + c] : 0.0;
+      const double* zi = z.data() + ((size_t)slot_of[i]*3 + r)*nc; const double* mk = m.data() + (size_t)slot_of[k]*nc*3 + c;
+      for (int q = 0; q < nc; q++) v -= zi[q]*mk[(size_t)q*3];
+    }
+    cov[a*D + b] = v; cov[b*D + a] = v;
+  }
+  return rc;
+}
+
+extern "C" {
+
+int dynoba_joint_marginal_covariance(dynoba_handle h, int32_t n, const int32_t* kind, const int32_t* idx, double* cov) {
+  int rc = check_ready(h, true); if (rc) return rc;
+  if (h->world > 1) { h->err = "dynoba_joint_marginal_covariance is a single-GPU entry point"; return DYNOBA_ERR_UNSUPPORTED; }
+  ARG(n > 0, "n must be positive"); ARG(kind && idx, "null kind or idx"); ARG(cov, "null cov");
+  std::vector<std::pair<int32_t, int32_t>> seen(n);
+  for (int32_t i = 0; i < n; i++) {
+    ARG(valid_kind(kind[i]), "bad variable kind");
+    ARG(h->layout.column_checked(kind[i], idx[i]) >= 0, "variable out of range");
+    seen[i] = { kind[i], idx[i] };
+  }
+  std::sort(seen.begin(), seen.end());
+  ARG(std::adjacent_find(seen.begin(), seen.end()) == seen.end(), "a variable is listed twice");
+  return joint_impl(h, n, kind, idx, cov);
 }
 
 int dynoba_get_variables(dynoba_handle h, int kind, int64_t n, double* out) {

@@ -102,6 +102,14 @@ __device__ __forceinline__ void frag16_load(const double* t, double (&f)[KF16], 
 #pragma unroll
     for (int j = 0; j < 4; j++) f[cb*4 + j] = __ldcg(p + 4*j*TILE + 8*cb);
 }
+// the same of the tile's TRANSPOSE: f[cb*4 + j] = L[16kb + q + 4j][8cb + g] (the joint covariance's backward sweep)
+__device__ __forceinline__ void frag16_load_t(const double* t, double (&f)[KF16], int kb, int lane) {
+  const double* p = t + (lane >> 2)*TILE + 16*kb + (lane & 3);
+#pragma unroll
+  for (int cb = 0; cb < 4; cb++)
+#pragma unroll
+    for (int j = 0; j < 4; j++) f[cb*4 + j] = __ldcg(p + 8*cb*TILE + 4*j);
+}
 // Shared-memory stage of a tile: 32 columns of 32 doubles (stride 32, 8 KB, no padding), rows XOR-swizzled per column:
 // element (r, c) at c*32 + (r ^ 4(c & 3)).  The swizzle flips row bits 2-3 only, so every 16-byte pair of rows (2p, 2p+1)
 // stays together and cp.async fills a stage with 16-byte copies (stage16_prefetch).

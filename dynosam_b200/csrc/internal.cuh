@@ -307,6 +307,26 @@ int launch_cov_pose_gather(const double* tiles, int TPC, const int* spos, int n,
 int launch_cov_rows_gather(const double* src, const int* rows, int n, int w, double* out, cudaStream_t s);
 int launch_cov_simple(const DevBlock& blk, const double* sig, int TPC, double* out_point, double* out_flow, int* fail, cudaStream_t s);
 int launch_cov_general(const GeneralGroups& G, const double* sig, int TPC, double* out_point, int* fail, cudaStream_t s);
+// ---- joint marginal covariances (kernels_cov.cu: the sweeps; kernels_chain.cu: the landmark strips).  P is the plain
+// chain holding the factor L.  The sweeps solve S X = E_C over tile columns [J0, NT) into a panel of
+// joint_panel_count(NT, J0, nc) doubles, cs[nc] the band scalars of C (ascending, J0 = cs[0] / 32); the gather writes X[C, C].
+size_t joint_panel_count(int NT, int J0, int nc);
+int launch_band_sweeps(const BandProb& P, int WB, const int* cs, int nc, int J0, double* panel, cudaStream_t s);
+int launch_joint_gather(const double* panel, int J0, const int* cs, int nc, double* out, cudaStream_t s);
+constexpr int STRIP_LD = 63;      // leading dimension of a group's V^-1 in the strip output (3 x 21 chained points)
+struct StripJob {
+  const DevBlock* blocks; const void* refs;   // every factor block descriptor; (int blk, int sorted idx) per group factor
+  const int4* groups;   // [ng] (first ref, end ref, first device landmark index, points of the group; 0: one flow)
+  const int* rptr;      // [ng + 1] requested landmarks of each group, into rl
+  const int* rl;        // [nreq] device index of every requested landmark, grouped
+  const int* cmap;      // [pose-like positions] index in C of the position's first scalar, -1 outside C
+  const double* xcc; int nc;   // X[C, C], row-major
+  double* m;            // [nreq][nc][3] (W V^-1)[C, l], zeroed by the caller
+  double* z;            // [nreq][3][nc] Sigma(l, C)
+  double* vinv;         // [ng][STRIP_LD][STRIP_LD] V_g^-1
+  int ng; int* fail;
+};
+int launch_cov_strips(const StripJob& j, cudaStream_t s);
 // ---- navigation variables and visual-inertial factors (kernels_imu.cu).  nav[i] = (solver position, dimension) of every
 // velocity (3) and bias (6).
 int nav_grid(int type, int n);      // partial sums a linearize / error launch of a navigation factor block writes

@@ -297,6 +297,93 @@ cov_general_kernel(const DevBlock* __restrict__ blocks, const int* __restrict__ 
 
 static size_t gg_smem() { return (size_t)2*(2*GG_N*GG_LD + 2*GG_N)*sizeof(double); }
 
+// Requested-landmark strips of dynoba_joint_marginal_covariance (here because it shares group_inverse), one warp per
+// requested landmark group g (a point alone, a WCME / WCPE chain, or a flow).  With V_g^-1 the group's undamped inverse
+// and W the pose-landmark block of H, for every requested landmark l of the group:
+//     M_l = (W V_g^-1)[C, l]   = sum over the (factor, pose slot) terms b of U_b^T (V_g^-1)[., l],  U_b = B_f^T A_{f,s}
+//     Z_l = Sigma(l, C)        = -M_l^T X[C, C]    (= -V_g^-1 W^T S^-1 restricted to C: every pose of W[., g] is in C)
+// and V_g^-1 itself; the host then forms Sigma(l1, l2) = delta_g (V_g^-1)(l1, l2) - Z_l1 M_l2.
+static_assert(STRIP_LD == GG_N, "a group's V^-1 is returned with the leading dimension of the largest group");
+__global__ void __launch_bounds__(64) cov_strip_kernel(StripJob j) {
+  extern __shared__ double sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = blockIdx.x*2 + warp;
+  if (g >= j.ng) return;
+  double* V = sm + (size_t)warp*(2*GG_N*GG_LD + 2*GG_N);
+  double* W = V + GG_N*GG_LD; double* gl = W + GG_N*GG_LD;
+  const int4 G = j.groups[g];
+  const FRef* rf = (const FRef*)j.refs + G.x;
+  const int nf = G.y - G.x, l0 = G.z;
+  const bool flow = G.w == 0;
+  const int ld = flow ? 2 : 3, rows = flow ? 2 : 3, n = flow ? 2 : 3*G.w;
+  if (flow) {                 // one flow: V = sum_f B_f^T B_f (2x2)
+    double v[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int q = lane; q < nf; q += 32) {
+      const FView f = make_view(j.blocks, rf[q]);
+      for (int r = 0; r < 2; r++) { const double b0 = f.J(r, f.lcol[0]), b1 = f.J(r, f.lcol[0] + 1); v[0] += b0*b0; v[1] += b0*b1; v[3] += b1*b1; }
+    }
+    for (int e = 0; e < 4; e++) v[e] = warp_sum(v[e]);
+    v[2] = v[1];
+    double vi[4];
+    if (!spd_inverse<2>(v, vi)) { if (lane == 0) atomicOr(j.fail, 1); return; }
+    if (lane == 0) { V[0] = vi[0]; V[1] = vi[1]; V[GG_LD] = vi[2]; V[GG_LD + 1] = vi[3]; }
+    __syncwarp();
+  } else if (!group_inverse(j.blocks, rf, nf, l0, n, 0.0, V, gl, W, lane)) { if (lane == 0) atomicOr(j.fail, 1); return; }
+  for (int e = lane; e < n*n; e += 32) j.vinv[(size_t)g*STRIP_LD*STRIP_LD + (size_t)(e/n)*STRIP_LD + e%n] = V[(e/n)*GG_LD + e%n];
+  for (int q = j.rptr[g]; q < j.rptr[g + 1]; q++) {
+    const int o = ld*(j.rl[q] - l0);
+    double* mq = j.m + (size_t)q*j.nc*3;
+    for (int p = lane; p < 2*nf; p += 32) {   // terms (factor p/2, pose slot p%2) over the lanes
+      const FView f = make_view(j.blocks, rf[p >> 1]);
+      const int s = p & 1;
+      if (s >= f.np) continue;
+      const int c0 = j.cmap[f.pose(s)];
+      double acc[6][3];
+#pragma unroll
+      for (int c = 0; c < 6; c++)
+#pragma unroll
+        for (int k = 0; k < 3; k++) acc[c][k] = 0.0;
+      for (int t = 0; t < f.nl; t++) {
+        const int ot = ld*(f.lmk(t) - l0);
+        for (int a = 0; a < ld; a++) {
+          double vk[3];
+#pragma unroll
+          for (int k = 0; k < 3; k++) vk[k] = k < ld ? V[(ot + a)*GG_LD + o + k] : 0.0;
+#pragma unroll
+          for (int c = 0; c < 6; c++) {
+            double u = 0.0;
+            for (int r = 0; r < rows; r++) u += f.J(r, f.lcol[t] + a)*f.J(r, f.pcol[s] + c);
+#pragma unroll
+            for (int k = 0; k < 3; k++) acc[c][k] += u*vk[k];
+          }
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < 6; c++)
+#pragma unroll
+        for (int k = 0; k < 3; k++) if (k < ld) atomicAdd(mq + (size_t)(c0 + c)*3 + k, acc[c][k]);
+    }
+    __threadfence_block();
+    __syncwarp();
+    for (int col = lane; col < j.nc; col += 32) {
+      double zk[3] = {0.0, 0.0, 0.0};
+      for (int r = 0; r < j.nc; r++) {
+        const double x = j.xcc[(size_t)r*j.nc + col];
+#pragma unroll
+        for (int k = 0; k < 3; k++) zk[k] += __ldcg(mq + (size_t)r*3 + k)*x;
+      }
+      for (int k = 0; k < ld; k++) j.z[((size_t)q*3 + k)*j.nc + col] = -zk[k];
+    }
+  }
+}
+int launch_cov_strips(const StripJob& j, cudaStream_t s) {
+  if (j.ng == 0) return 0;
+  static bool attr = false;
+  if (!attr) { cudaFuncSetAttribute(cov_strip_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gg_smem()); attr = true; }
+  cov_strip_kernel<<<general_grid(j.ng), 64, gg_smem(), s>>>(j);
+  return 1;
+}
+
 int launch_cov_general(const GeneralGroups& G, const double* sig, int TPC, double* out_point, int* fail, cudaStream_t s) {
   if (G.n_groups == 0) return 0;
   static bool attr = false;

@@ -163,6 +163,121 @@ int launch_band_selinv(const BandProb& P, int WB, double* stage, cudaStream_t s)
   return 2;
 }
 
+// ---- joint marginal covariances (dynoba_joint_marginal_covariance): X = S^-1 E_C over the plain band factor L, E_C the
+// unit columns of the requested scalars C.  L^-1 E_C is zero above the first requested scalar, so both sweeps run over the
+// tile columns [J0, NT) only, J0 the tile of min(C):
+//     forward   Y_J = L_JJ^-1 (E_J - sum_{t=1..WB} L(J, J-t) Y_{J-t})          J = J0 .. NT-1
+//     backward  X_J = L_JJ^-T (Y_J - sum_{t=1..WB} L(J+t, J)^T X_{J+t})      J = NT-1 .. J0
+// (tests/joint_reference.py is the executable statement).  The panel of right-hand sides is cut into chunks of
+// SWEEP_COLS columns, one CTA each; a chunk's panel tiles are square and hold the TRANSPOSE (tile (J, k) element (r, c) =
+// X[32J + c][32k + r]), so every product is T -= A B^T of two 32x32 tiles on the m16n8k16 loaders of band_tile.cuh:
+//     forward   Y^T_J -= Y^T_{J-t} L(J, J-t)^T        backward  X^T_J -= X^T_{J+t} L(J+t, J)
+// The WB products of a tile column are dealt over the CTA's warps, their partial sums added in shared memory, and one
+// warp multiplies by the factorisation's diagonal-tile inverse.  Work and memory: (NT - J0) WB |C| / 32 tile products and
+// (NT - J0) |C| / 32 panel tiles.
+constexpr int SWEEP_COLS = 32;    // right-hand sides per chunk (a multiple of 8: one n8 block per 8 columns)
+constexpr int SWEEP_WARPS = 8;    // warps sharing a tile column's WB products
+static_assert(SWEEP_COLS == TILE, "the panel's tiles are square");
+
+struct SweepJob {
+  const double* tiles; const double* linv; int TPC, NT, WB, J0;
+  const int* cs; int nc;          // [nc] band scalar of each right-hand side's unit entry
+  double* panel; int nchunk;      // [NT - J0][nchunk][TILE2]
+};
+// operand fragment (frag16_load's map) of a tile this CTA wrote: plain loads, global or shared memory
+__device__ __forceinline__ void frag16_load_p(const double* t, double (&f)[KF16], int kb, int lane) {
+  const double* p = t + (16*kb + (lane & 3))*TILE + (lane >> 2);
+#pragma unroll
+  for (int cb = 0; cb < 4; cb++)
+#pragma unroll
+    for (int j = 0; j < 4; j++) f[cb*4 + j] = p[4*j*TILE + 8*cb];
+}
+
+template <bool FWD>
+__device__ __forceinline__ void sweep_column(const SweepJob& j, int J, const int* cs, double* sm, int warp, int lane) {
+  const int k = blockIdx.x;
+  double* part = sm + (size_t)warp*TILE2;
+  double* z = sm + (size_t)SWEEP_WARPS*TILE2;
+  double* pj = j.panel + ((size_t)(J - j.J0)*j.nchunk + k)*TILE2;
+  double acc[TILE];
+#pragma unroll
+  for (int e = 0; e < TILE; e++) acc[e] = 0.0;
+  const int m = FWD ? min(j.WB, J - j.J0) : min(j.WB, j.NT - 1 - J);
+  for (int t = 1 + warp; t <= m; t += SWEEP_WARPS) {
+    const int I = FWD ? J - t : J + t;
+    const double* Lt = FWD ? j.tiles + ((size_t)I*j.TPC + t)*TILE2 : j.tiles + ((size_t)J*j.TPC + t)*TILE2;
+    const double* Pt = j.panel + ((size_t)(I - j.J0)*j.nchunk + k)*TILE2;
+    double fa[2][KF16], fb[2][KF16];
+#pragma unroll
+    for (int kb = 0; kb < 2; kb++) {
+      if (FWD) frag16_load(Lt, fb[kb], kb, lane); else frag16_load_t(Lt, fb[kb], kb, lane);
+      frag16_load_p(Pt, fa[kb], kb, lane);
+    }
+#pragma unroll
+    for (int kb = 0; kb < 2; kb++) frag16_gemm_sub(acc, fa[kb], fb[kb]);
+  }
+  cfrag16_store(part, acc, lane);
+  __syncthreads();
+  for (int e = threadIdx.x; e < TILE2; e += SWEEP_WARPS*32) {   // Z^T = E^T_J (forward) / Y^T_J (backward) + partial sums
+    double s = FWD ? (cs[e & 31] == J*TILE + (e >> 5) ? 1.0 : 0.0) : pj[e];
+#pragma unroll
+    for (int w = 0; w < SWEEP_WARPS; w++) s += sm[(size_t)w*TILE2 + e];
+    z[e] = s;
+  }
+  __syncthreads();
+  if (warp == 0) {            // Y^T_J = Z^T L_JJ^-T,  X^T_J = Z^T L_JJ^-1
+    const double* li = j.linv + (size_t)J*TILE2;
+#pragma unroll
+    for (int e = 0; e < TILE; e++) acc[e] = 0.0;
+#pragma unroll
+    for (int kb = 0; kb < 2; kb++) {
+      double fa[KF16], fb[KF16];
+      frag16_load_p(z, fa, kb, lane);
+      if (FWD) frag16_load(li, fb, kb, lane); else frag16_load_t(li, fb, kb, lane);
+      frag16_gemm_sub(acc, fa, fb);
+    }
+#pragma unroll
+    for (int e = 0; e < TILE; e++) acc[e] = -acc[e];
+    cfrag16_store(pj, acc, lane);
+  }
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(SWEEP_WARPS*32) band_sweep_kernel(SweepJob j) {
+  extern __shared__ double sw_sm[];     // [SWEEP_WARPS] partial sums | Z
+  __shared__ int cs[SWEEP_COLS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x < SWEEP_COLS) { const int c = blockIdx.x*SWEEP_COLS + threadIdx.x; cs[threadIdx.x] = c < j.nc ? j.cs[c] : -1; }
+  __syncthreads();
+  for (int J = j.J0; J < j.NT; J++) sweep_column<true>(j, J, cs, sw_sm, warp, lane);
+  for (int J = j.NT - 1; J >= j.J0; J--) sweep_column<false>(j, J, cs, sw_sm, warp, lane);
+}
+
+size_t joint_panel_count(int NT, int J0, int nc) { return (size_t)(NT - J0)*((nc + SWEEP_COLS - 1)/SWEEP_COLS)*TILE2; }
+
+int launch_band_sweeps(const BandProb& P, int WB, const int* cs, int nc, int J0, double* panel, cudaStream_t s) {
+  const size_t smem = (size_t)(SWEEP_WARPS + 1)*TILE2*sizeof(double);
+  static bool attr = false;
+  if (!attr) { cudaFuncSetAttribute(band_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr = true; }
+  const int nchunk = (nc + SWEEP_COLS - 1)/SWEEP_COLS;
+  SweepJob j{ P.tiles, P.linv, P.TPC, P.NT, WB, J0, cs, nc, panel, nchunk };
+  band_sweep_kernel<<<nchunk, SWEEP_WARPS*32, smem, s>>>(j);
+  return 1;
+}
+// X[C, C] row-major from the panel: out[a*nc + b] = X[cs[a]][b]
+__global__ void joint_gather_kernel(const double* __restrict__ panel, int nchunk, int J0, const int* __restrict__ cs, int nc,
+                                    double* __restrict__ out) {
+  const long long e = (long long)blockIdx.x*blockDim.x + threadIdx.x;
+  if (e >= (long long)nc*nc) return;
+  const int a = (int)(e/nc), b = (int)(e%nc), s = cs[a];
+  out[e] = panel[((size_t)((s >> 5) - J0)*nchunk + b/SWEEP_COLS)*TILE2 + (size_t)(s & 31)*TILE + (b % SWEEP_COLS)];
+}
+int launch_joint_gather(const double* panel, int J0, const int* cs, int nc, double* out, cudaStream_t s) {
+  const long long ne = (long long)nc*nc;
+  joint_gather_kernel<<<(unsigned)((ne + 255)/256), 256, 0, s>>>(panel, (nc + SWEEP_COLS - 1)/SWEEP_COLS, J0, cs, nc, out);
+  return 1;
+}
+
 // ---- pose-like blocks: cov[i] = Sigma(s_i .. s_i + d, s_i .. s_i + d), s_i = 6 * solver position of the i-th variable
 __global__ void cov_pose_gather_kernel(const double* __restrict__ tiles, int TPC, const int* __restrict__ spos, int n, int d,
                                        double* __restrict__ out) {

@@ -225,6 +225,15 @@ int dynoba_marginal_keep_points(dynoba_handle h, int32_t n_keep, const int32_t* 
  * DYNOBA_ERR_INDETERMINATE where H is not positive definite (GTSAM throws IndeterminantLinearSystemException), also for
  * a requested landmark no factor touches; single GPU (world > 1: DYNOBA_ERR_UNSUPPORTED). */
 int dynoba_marginal_covariance(dynoba_handle h, int kind, int64_t n, const int32_t* idx, double* cov);
+/* gtsam::Marginals(graph, values, Marginals::CHOLESKY).jointMarginalCovariance(keys) in the caller's order: the n
+ * variables (kind[i], idx[i]) of any kinds, cov = the D x D block of H^-1 over them, D = the sum of their tangent
+ * dimensions (the conventions of dynoba_marginal_covariance), blocks in caller order, row-major, exactly symmetric.
+ * Off-diagonal blocks between any two variables, however far apart in time.  The factor of the reduced system is kept
+ * with the selected inverse's state (a later dynoba_marginal_covariance reuses it) and dropped when the values change;
+ * the LM state is untouched.  DYNOBA_ERR_BAD_ARG (before any device work) for n <= 0, a bad kind, an index out of range, a
+ * variable listed twice or a null array; DYNOBA_ERR_INDETERMINATE where H, or a requested landmark group's own block, is
+ * not positive definite, and for a requested landmark no factor touches; world > 1: DYNOBA_ERR_UNSUPPORTED. */
+int dynoba_joint_marginal_covariance(dynoba_handle h, int32_t n, const int32_t* kind, const int32_t* idx, double* cov);
 /* Optional elimination-order hint for pose-like variables (e.g. the frame id encoded in the key):
  * variables are ordered by (rank, index).  Without it the given order is used. */
 int dynoba_set_pose_order(dynoba_handle h, int64_t n, const int32_t* rank);
