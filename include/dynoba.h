@@ -467,6 +467,48 @@ int dynoba_pnp_ransac_batch(int device, int32_t n_problems, const int32_t* offse
                             const double* points_world, const double* keypoints, const dynoba_pnp_ransac_params* prm,
                             double* pose_out, uint8_t* inlier_out, int32_t* n_inliers, int32_t* status, int32_t* iterations,
                             int32_t* skipped, int32_t* best_hypothesis, int32_t* hyp_counts);
+/* (4) dynoba_object_srif_batch replaces the per-object filter step of ObjectMotionSolverFilter::solveImpl
+ * (src/frontend/vision/MotionSolver.cc:1734-2063) after its PnP: HybridObjectMotionSRIF's predict and robust (IRLS) update
+ * (:1445-1687) for every object of a frame, one CTA per object, one launch per call.  The mathematics is stated in
+ * dynosam_b200/csrc/srif.cuh.  All pointers are HOST memory; the caller keeps the filter state between calls.
+ * Object o owns the correspondences [offsets[o], offsets[o+1]): its PnP inliers in inlier order, each with
+ *   stereo[i][6]        (uL, uR, v) at k-1, then at k;  stereo_valid[i][2]: 1 where that measurement exists;
+ *   points_cam[i][6]    the back-projected camera-frame point at k-1, then at k;
+ *   m_L[i][3], has_point[i]  the tracklet's object-frame point, in / out (initialised here when has_point is 0).
+ * Per object: mode (DYNOBA_SRIF_NEW: not in the filter map; _RESET: resampled and in the map; _CONTINUE), pnp_status
+ * (DYNOBA_TRACK_*: the motion counts as solved only when VALID), pose_prev / pose_cur[12] (X_k-1, X_k), calib6[6]
+ * (fx, fy, skew, u0, v0, baseline: the fake stereo calibration) and state_in / state_out[DYNOBA_SRIF_STATE]
+ * (R row-major [36] | d [6] | H_lin, L_e, prev_H, X_K [12 each]).  NEW and RESET start the filter on the key frame
+ * L_e = (I, X_k-1 * mean of the inliers' points at k-1) and update at k-1 before the update at k.
+ * Outputs per object: status (DYNOBA_SRIF_OK; _TOO_FEW: NEW with fewer than min_new_inliers inliers, no filter is made;
+ * _NO_INLIERS: NEW or RESET with no inlier, where the reference divides by zero -- a deliberate divergence; both leave
+ * state_out = state_in and m_L / has_point untouched), solved (OK and pnp_status VALID), motion_out[36] (the frame-to-frame
+ * motion, the key-framed motion H_W_e_k, the object pose H_W_e_k L_e), cov_out[36] ((R^T R)^-1), errors[2] (the last
+ * update's error and reweighted_error), before_reset[12] (H_lin before a RESET, else the identity) and counts[3] (points
+ * initialised in this call, inliers that already had one, measurements the Huber weight scaled down in the last IRLS
+ * iteration).  R is returned with a non-negative diagonal.  Refused with DYNOBA_ERR_BAD_ARG before any device work: NULL
+ * arrays, bad counts, non-monotone offsets, an unknown mode, a has_point or stereo_valid other than 0 / 1, non-finite poses /
+ * calibration / state / points / valid measurements / parameters, fx, fy or baseline <= 0, P0, Q or R_noise not symmetric
+ * positive definite, huber_k <= 0, irls_iterations < 1, min_new_inliers < 0.  n_objects = 0 is a no-op.  The call shares
+ * the batch entry points' per-device stream and workspace. */
+enum { DYNOBA_SRIF_NEW = 0, DYNOBA_SRIF_RESET = 1, DYNOBA_SRIF_CONTINUE = 2 };
+enum { DYNOBA_SRIF_OK = 0, DYNOBA_SRIF_TOO_FEW = 1, DYNOBA_SRIF_NO_INLIERS = 2 };
+#define DYNOBA_SRIF_STATE 90
+typedef struct {
+  double P0[36];                /* initial covariance, row-major (0.3 I) */
+  double Q[36];                 /* process noise (0.2 I) */
+  double R_noise[9];            /* stereo measurement covariance (I) */
+  double huber_k;               /* 0.1 */
+  int32_t irls_iterations;      /* 2 */
+  int32_t min_new_inliers;      /* 4: a NEW object needs this many inliers */
+} dynoba_object_srif_params;
+void dynoba_object_srif_default_params(dynoba_object_srif_params* p);
+int dynoba_object_srif_batch(int device, int32_t n_objects, const int32_t* offsets, const int32_t* mode,
+                             const int32_t* pnp_status, const double* pose_prev, const double* pose_cur, const double* calib6,
+                             const dynoba_object_srif_params* prm, const double* state_in, double* state_out,
+                             const double* stereo, const uint8_t* stereo_valid, const double* points_cam, double* m_L,
+                             uint8_t* has_point, int32_t* status, uint8_t* solved, double* motion_out, double* cov_out,
+                             double* errors, double* before_reset, int32_t* counts);
 
 /* Combined IMU preintegration of many frame intervals in one launch: gtsam::PreintegratedCombinedMeasurements (GTSAM 4.2.0,
  * ManifoldPreintegration, no Coriolis) integrateMeasurement once per sample, as ImuFrontend::preintegrateImuMeasurements
