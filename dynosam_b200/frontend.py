@@ -19,7 +19,7 @@ EXPORTS = ["dynofront_create", "dynofront_destroy", "dynofront_last_error", "dyn
            "dynofront_homography_last_trace", "dynofront_homography_record_counts", "dynofront_klt_track_points",
            "dynofront_klt_dynamic_default_params", "dynofront_track_dynamic_klt", "dynofront_fundamental_default_params",
            "dynofront_find_fundamental_batch", "dynofront_fundamental_last_trace", "dynofront_fundamental_record", "dynofront_set_right",
-           "dynofront_stereo_match"]
+           "dynofront_stereo_match", "dynofront_object_boundary"]
 
 
 class TrackParamsC(C.Structure):
@@ -189,6 +189,7 @@ def load():
         L.dynofront_pin_host.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         L.dynofront_unpin_host.argtypes = [C.c_void_p, C.c_void_p]
         L.dynofront_get_motion_mask.argtypes = [C.c_void_p, C.c_void_p]
+        L.dynofront_object_boundary.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_int32)] + [C.c_void_p]*4 + [C.POINTER(C.c_float)]
         L.dynofront_anms_range_tree.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p]*4 + [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)]
         L.dynofront_sample_dynamic.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(TrackParamsC), C.POINTER(C.c_int64),
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32] + [C.c_void_p]*5 + [C.POINTER(C.c_int32), C.POINTER(C.c_float)]
@@ -325,6 +326,20 @@ class FeatureTrackerGPU:
         out = np.zeros((self.H, self.W), np.int32)
         self._ck(self.lib.dynofront_get_motion_mask(self.h, _p(out)))
         return out
+
+    def object_boundary(self, thickness=-1, want_mask=False, capacity=255):
+        """FeatureTracker::objectDetection with a provided mask (dynofront_object_boundary): computeObjectMaskBoundaryMask on the
+        current motion mask as uploaded.  thickness < 0: the reference's scaled value for the frame size.  The boundary mask becomes
+        the current frame's (as if uploaded through next_frame).  Returns (objects [n] ascending, bb [n][4], inner_bb [n][4], and
+        with want_mask the boundary mask u8[H][W], else None); capacity limits the rows returned."""
+        cap = int(capacity)
+        objs = np.zeros(max(cap, 1), np.int32); bb = np.zeros((max(cap, 1), 4), np.int32); ib = np.zeros((max(cap, 1), 4), np.int32)
+        mask = np.zeros((self.H, self.W), np.uint8) if want_mask else None
+        n = C.c_int32(); ms = C.c_float()
+        self._ck(self.lib.dynofront_object_boundary(self.h, int(thickness), cap, C.byref(n), _p(objs), _p(bb), _p(ib), _p(mask), C.byref(ms)))
+        self.last_ms = ms.value; self.last_n_objects = n.value
+        s = min(n.value, cap)
+        return objs[:s], bb[:s], ib[:s], mask
 
     def track_dynamic(self, prev_pred_kp, prev_label, prev_age, prev_tracklet, prm: TrackParams, next_tracklet_id: int, want_masks=True):
         kp = np.ascontiguousarray(prev_pred_kp, dtype=np.float64).reshape(-1, 2); n = kp.shape[0]

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/dynofront.h"
+#include "boundary.cuh"
 
 #define FCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { h->err = std::string(#call) + ": " + cudaGetErrorString(e_); return -3; } } while (0)
 
@@ -92,6 +93,9 @@ struct dynofront_ctx {
   // bb[4][64], K, cand, off, corners, selected), tracked sort keys, eigen image, GFTT corners, output features
   DevBuf<unsigned char> tk_rows, tk_cnt; DevBuf<int> tk_int, tk_corners; DevBuf<unsigned long long> tk_keys; DevBuf<float> tk_eig;
   DevBuf<double> tk_kp; DevBuf<int32_t> tk_age, tk_lab, tk_src; DevBuf<long long> tk_tid;
+  // object boundary mask (dynofront_object_boundary): T, the boundary mask until it replaces det, the extent tables and their
+  // pinned host copy; mask_propagated: dynofront_propagate_mask has modified the resident current motion mask since its upload
+  DevBuf<uint8_t> bd_T, bd_mask; DevBuf<int> bd_tab; int* bd_host = nullptr; bool mask_propagated = false, bd_smem_set = false;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
 };
 // grows each (buffer, element count) pair in turn; 0, or -3 with the error at the first allocation that fails
@@ -2313,6 +2317,149 @@ __global__ void __launch_bounds__(1024) tk_construct_kernel(const unsigned long 
   if (threadIdx.x == 0) cnt->features = ntr + base;
 }
 
+// ---------------------------------------------------------------------------------------------------- object boundary mask
+// vision_tools::computeObjectMaskBoundaryMask on the resident current motion mask, in the restatement of boundary.cuh.  Both
+// kernels work on 64 x 32 pixel tiles with 256 threads; the per-label extents are folded per thread (runs of one label down
+// its column), then per CTA in shared memory, then once per (CTA, label) into the global tables with atomicMax, which makes
+// them independent of the order.  Global table: [0, 1024) the extents of M == j, [1024, 2048) those of erode(T) == j, [2048]
+// the flag of a label outside [0, 255].
+#define BD_TW 64
+#define BD_TH 32
+#define BD_THREADS 256
+#define BD_RS (BD_THREADS/BD_TW)          // row step between the pixels of one thread
+#define BD_PP (BD_TH/BD_RS)               // pixels per thread
+#define BD_TAB (8*(BOUNDARY_MAX_LABEL + 1) + 1)
+#define BD_CHUNKS ((BD_TW + 2*BOUNDARY_MAX_THICKNESS + 31)/32)   // 32-column chunks of the widest tile row
+#define BD_LEVELS 8                       // sparse-table levels of the widest run, 2*BOUNDARY_MAX_THICKNESS + 1 pixels
+struct BdRows {                           // one element: radius, top level, row half widths per |dy|, and the |dy| range [lo, hi] whose
+  int r, top, hw[BOUNDARY_MAX_THICKNESS + 1], lo[BD_LEVELS], hi[BD_LEVELS];     // runs take each level (hw falls with |dy|)
+};
+struct BdElem { BdRows in, out; };        // E_10 (erosion) and E_t (dilation)
+__device__ __forceinline__ void bd_run_add(int (*s)[4], int lab, int W, int H, int x, int y0, int y1) {
+  atomicMax(&s[lab][0], W - x); atomicMax(&s[lab][1], H - y0); atomicMax(&s[lab][2], x + 1); atomicMax(&s[lab][3], y1 + 1);
+}
+__device__ __forceinline__ void bd_flush(int (*s)[4], int* g) {
+  __syncthreads();
+  for (int l = threadIdx.x; l <= BOUNDARY_MAX_LABEL; l += BD_THREADS)
+    if (s[l][2]) for (int f = 0; f < 4; f++) atomicMax(&g[4*l + f], s[l][f]);
+}
+// T (the 1x11 column max), the label check and the extents of M == j
+__global__ void __launch_bounds__(BD_THREADS) bd_scan_kernel(const int32_t* __restrict__ M, int W, int H, uint8_t* __restrict__ T, int* tab) {
+  __shared__ int s[BOUNDARY_MAX_LABEL + 1][4];
+  for (int i = threadIdx.x; i < 4*(BOUNDARY_MAX_LABEL + 1); i += BD_THREADS) (&s[0][0])[i] = 0;
+  __syncthreads();
+  const int x = blockIdx.x*BD_TW + threadIdx.x % BD_TW, y0 = blockIdx.y*BD_TH + (threadIdx.x/BD_TW)*BD_PP;
+  bool bad = false;
+  if (x < W) {
+    int run = 0, ry0 = 0, ry1 = 0;
+    for (int y = y0; y < min(y0 + BD_PP, H); y++) {
+      T[(size_t)y*W + x] = (uint8_t)boundary_column_max(M, W, H, x, y);
+      const int32_t v = M[(size_t)y*W + x];
+      bad |= !boundary_label_ok(v);
+      const int lab = boundary_label_ok(v) ? v : 0;
+      if (lab == run) { ry1 = y; continue; }
+      if (run) bd_run_add(s, run, W, H, x, ry0, ry1);
+      run = lab; ry0 = ry1 = y;
+    }
+    if (run) bd_run_add(s, run, W, H, x, ry0, ry1);
+  }
+  if (bad) tab[BD_TAB - 1] = 1;
+  bd_flush(s, tab);
+}
+// One morphology pass over the tile: the max (dilation) or min (erosion) of T over the element of radius r, into acc.  The tile
+// and a halo of r are loaded with a border value that never wins; then, level by level, a sparse table of row maxima / minima is
+// built in place (level k holds the op over 2^k pixels starting at each column) and every element row whose run 2w+1 takes
+// level k is answered with two overlapping windows: O(r) per pixel rather than O(r^2).
+template <bool MAX>
+__device__ void bd_pass(uint8_t* buf, const uint8_t* __restrict__ T, int W, int H, int X0, int Y0, const BdRows& E, int tx, int ty0, int* acc) {
+  const int r = E.r, BW = BD_TW + 2*r, BH = BD_TH + 2*r;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int row = warp; row < BH; row += BD_THREADS/32) {     // one warp per row, all of its loads in flight at once
+    const int gy = Y0 - r + row;
+    const bool in_y = gy >= 0 && gy < H;
+    uint8_t* rp = buf + row*BW;
+    int v[BD_CHUNKS];
+#pragma unroll
+    for (int c = 0; c < BD_CHUNKS; c++) {
+      const int bx = 32*c + lane, gx = X0 - r + bx;
+      v[c] = (in_y && bx < BW && gx >= 0 && gx < W) ? T[(size_t)gy*W + gx] : (MAX ? 0 : 255);
+    }
+#pragma unroll
+    for (int c = 0; c < BD_CHUNKS; c++) if (32*c + lane < BW) rp[32*c + lane] = (uint8_t)v[c];
+  }
+  __syncthreads();
+  for (int k = 0; k <= E.top; k++) {
+    if (k > 0) {                          // one warp per row: the whole row of level k - 1 is read before level k is written
+      const int half = 1 << (k - 1), last = BW - (1 << k);
+      for (int row = warp; row < BH; row += BD_THREADS/32) {
+        uint8_t* rp = buf + row*BW;
+        int v[BD_CHUNKS];
+#pragma unroll
+        for (int c = 0; c < BD_CHUNKS; c++) {
+          const int x = 32*c + lane;
+          v[c] = x <= last ? (MAX ? max(rp[x], rp[x + half]) : min(rp[x], rp[x + half])) : 0;
+        }
+        __syncwarp();
+#pragma unroll
+        for (int c = 0; c < BD_CHUNKS; c++) if (32*c + lane <= last) rp[32*c + lane] = (uint8_t)v[c];
+        __syncwarp();
+      }
+      __syncthreads();
+    }
+    for (int a = E.lo[k]; a <= E.hi[k]; a++) {
+      const int o1 = -E.hw[a], o2 = E.hw[a] - (1 << k) + 1;
+      for (int dy = -a; dy <= a; dy += (a ? 2*a : 1)) {
+        const uint8_t* rp = buf + (ty0 + r + dy)*BW + tx + r;
+#pragma unroll
+        for (int j = 0; j < BD_PP; j++) {
+          const int v1 = rp[j*BD_RS*BW + o1], v2 = rp[j*BD_RS*BW + o2];
+          acc[j] = MAX ? max(acc[j], max(v1, v2)) : min(acc[j], min(v1, v2));
+        }
+      }
+    }
+    __syncthreads();
+  }
+}
+// the boundary mask and the extents of erode(T) == j
+__global__ void __launch_bounds__(BD_THREADS) bd_morph_kernel(const uint8_t* __restrict__ T, int W, int H, const __grid_constant__ BdElem E,
+                                                              uint8_t* __restrict__ out, int* tab) {
+  extern __shared__ uint8_t bd_buf[];
+  __shared__ int s[BOUNDARY_MAX_LABEL + 1][4];
+  for (int i = threadIdx.x; i < 4*(BOUNDARY_MAX_LABEL + 1); i += BD_THREADS) (&s[0][0])[i] = 0;
+  const int X0 = blockIdx.x*BD_TW, Y0 = blockIdx.y*BD_TH, tx = threadIdx.x % BD_TW, ty0 = threadIdx.x/BD_TW;
+  int ero[BD_PP], dil[BD_PP];
+#pragma unroll
+  for (int j = 0; j < BD_PP; j++) { ero[j] = 255; dil[j] = 0; }
+  bd_pass<false>(bd_buf, T, W, H, X0, Y0, E.in, tx, ty0, ero);
+  bd_pass<true>(bd_buf, T, W, H, X0, Y0, E.out, tx, ty0, dil);
+  const int x = X0 + tx;
+  int run = 0, ry0 = 0, ry1 = 0;
+#pragma unroll
+  for (int j = 0; j < BD_PP; j++) {
+    const int y = Y0 + ty0 + j*BD_RS;
+    if (x >= W || y >= H) continue;
+    const size_t p = (size_t)y*W + x;
+    out[p] = boundary_value(T[p], dil[j], ero[j]);
+    const int lab = ero[j];
+    if (lab == run) { ry1 = y; continue; }
+    if (run) bd_run_add(s, run, W, H, x, ry0, ry1);
+    run = lab; ry0 = ry1 = y;
+  }
+  if (run) bd_run_add(s, run, W, H, x, ry0, ry1);
+  bd_flush(s, tab + 4*(BOUNDARY_MAX_LABEL + 1));
+}
+static BdRows bd_rows(int r) {
+  BdRows e; e.r = r; e.top = boundary_level(r);
+  for (int k = 0; k < BD_LEVELS; k++) { e.lo[k] = r + 1; e.hi[k] = -1; }
+  for (int a = 0; a <= r; a++) {
+    e.hw[a] = boundary_ellipse_hw(r, a);
+    const int k = boundary_level(e.hw[a]);
+    e.lo[k] = std::min(e.lo[k], a); e.hi[k] = std::max(e.hi[k], a);
+  }
+  return e;
+}
+static size_t bd_smem(int t) { const int R = std::max(t, BOUNDARY_INNER); return (size_t)(BD_TW + 2*R)*(BD_TH + 2*R); }
+
 // ---------------------------------------------------------------------------------------------------- host API
 extern "C" {
 
@@ -2340,6 +2487,7 @@ int dynofront_destroy(dynofront_handle h) {
   cudaSetDevice(h->dev);
   if (h->e0) cudaEventDestroy(h->e0); if (h->e1) cudaEventDestroy(h->e1);
   if (h->s) cudaStreamDestroy(h->s);
+  if (h->bd_host) cudaFreeHost(h->bd_host);
   delete h; return 0;                                           // (the buffers free their device memory)
 }
 int dynofront_set_frame(dynofront_handle h, const float* flow, const int32_t* motion_mask, const uint8_t* detection_mask) {
@@ -2351,6 +2499,7 @@ int dynofront_set_frame(dynofront_handle h, const float* flow, const int32_t* mo
   else h->has_det = false;
   h->det_work_valid = false;
   h->has_depth = false; h->has_right = false; h->has_frame = h->has_frame || motion_mask;
+  if (motion_mask) h->mask_propagated = false;
   FCK(cudaStreamSynchronize(h->s));
   return 0;
 }
@@ -2367,7 +2516,7 @@ int dynofront_next_frame(dynofront_handle h, const uint8_t* gray, const float* f
   FCK(cudaMemcpyAsync(h->mask, motion_mask, npx*sizeof(int32_t), cudaMemcpyHostToDevice, h->s));
   if (detection_mask) { FCK(cudaMemcpyAsync(h->det, detection_mask, npx, cudaMemcpyHostToDevice, h->s)); h->has_det = true; } else h->has_det = false;
   h->det_work_valid = false;
-  h->has_depth = false; h->has_frame = true;
+  h->has_depth = false; h->has_frame = true; h->mask_propagated = false;
   h->have_prev = h->have_cur; h->have_cur = true;
   if (!h->lw.empty()) { std::swap(h->pyr[0], h->pyr[1]); std::swap(h->der, h->der2); }
   h->have_pyr = h->have_pyr_cur; h->have_pyr_cur = true;
@@ -2717,6 +2866,7 @@ int dynofront_propagate_mask(dynofront_handle h, int32_t n, const double* kp, co
     pm_warp_kernel<<<(unsigned)((npx + 255)/256), 256, 0, h->s>>>(npx, h->W, h->H, pmask, pflow, l, *prm, h->pflag, cmask);
   }
   if (!resident) FCK(cudaMemcpyAsync(current_mask, h->cmask, npx*4, cudaMemcpyDeviceToHost, h->s));
+  else h->mask_propagated = true;
   FCK(cudaStreamSynchronize(h->s));
   FCK(cudaGetLastError());
   return 0;
@@ -2725,6 +2875,50 @@ int dynofront_get_motion_mask(dynofront_handle h, int32_t* out) {
   if (!h || !out) return -1;
   cudaSetDevice(h->dev);
   FCK(cudaMemcpyAsync(out, h->mask, (size_t)h->W*h->H*4, cudaMemcpyDeviceToHost, h->s)); FCK(cudaStreamSynchronize(h->s));
+  return 0;
+}
+int dynofront_object_boundary(dynofront_handle h, int32_t thickness, int32_t capacity, int32_t* n_objects, int32_t* objects, int32_t* bb,
+                              int32_t* inner_bb, uint8_t* boundary_out, float* ms_device) {
+  if (!h) return -1;
+  if (!n_objects || capacity < 0 || (capacity > 0 && (!objects || !bb || !inner_bb))) {
+    h->err = "object_boundary: n_objects is required, and objects / bb / inner_bb when capacity > 0"; return -1;
+  }
+  if (!h->has_frame) { h->err = "object_boundary: no motion mask on the device (dynofront_set_frame / dynofront_next_frame)"; return -1; }
+  if (h->mask_propagated) {
+    h->err = "object_boundary: dynofront_propagate_mask has modified this frame's motion mask; the boundary mask is computed before it";
+    return -1;
+  }
+  const int W = h->W, H = h->H, t = thickness < 0 ? boundary_thickness(W, H) : thickness;
+  if (t > BOUNDARY_MAX_THICKNESS) {
+    h->err = "object_boundary: thickness " + std::to_string(t) + " exceeds " + std::to_string(BOUNDARY_MAX_THICKNESS); return -1;
+  }
+  cudaSetDevice(h->dev);
+  const size_t npx = (size_t)W*H;
+  if (grow(h, h->bd_T, npx, h->bd_mask, npx, h->bd_tab, BD_TAB)) return -3;
+  if (!h->bd_host) FCK(cudaMallocHost((void**)&h->bd_host, BD_TAB*sizeof(int)));
+  if (!h->bd_smem_set) {                // the largest tile (thickness BOUNDARY_MAX_THICKNESS) needs more than the default 48 KB
+    FCK(cudaFuncSetAttribute(bd_morph_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bd_smem(BOUNDARY_MAX_THICKNESS)));
+    h->bd_smem_set = true;
+  }
+  const BdElem E{bd_rows(BOUNDARY_INNER), bd_rows(t)};
+  const dim3 grid((unsigned)((W + BD_TW - 1)/BD_TW), (unsigned)((H + BD_TH - 1)/BD_TH));
+  cudaEventRecord(h->e0, h->s);
+  FCK(cudaMemsetAsync(h->bd_tab, 0, BD_TAB*sizeof(int), h->s));
+  bd_scan_kernel<<<grid, BD_THREADS, 0, h->s>>>(h->mask, W, H, h->bd_T, h->bd_tab);
+  bd_morph_kernel<<<grid, BD_THREADS, bd_smem(t), h->s>>>(h->bd_T, W, H, E, h->bd_mask, h->bd_tab);
+  cudaEventRecord(h->e1, h->s);
+  FCK(cudaMemcpyAsync(h->bd_host, h->bd_tab, BD_TAB*sizeof(int), cudaMemcpyDeviceToHost, h->s));
+  FCK(cudaStreamSynchronize(h->s));
+  FCK(cudaGetLastError());
+  if (h->bd_host[BD_TAB - 1]) {
+    h->err = "object_boundary: a motion-mask label is outside [0, 255] (the reference CHECKs labels > 255 and draws a negative one as 0)";
+    return -1;
+  }
+  *n_objects = boundary_finish(h->bd_host, h->bd_host + 4*(BOUNDARY_MAX_LABEL + 1), W, H, capacity, objects, bb, inner_bb);
+  std::swap(h->det, h->bd_mask);       // the boundary mask becomes the current frame's, as an upload through next_frame would
+  h->has_det = true; h->det_work_valid = false;
+  if (ms_device) cudaEventElapsedTime(ms_device, h->e0, h->e1);
+  if (boundary_out) { FCK(cudaMemcpyAsync(boundary_out, h->det, npx, cudaMemcpyDeviceToHost, h->s)); FCK(cudaStreamSynchronize(h->s)); }
   return 0;
 }
 int dynofront_pin_host(dynofront_handle h, void* ptr, size_t bytes) {

@@ -20,6 +20,8 @@
  *   dynofront_back_project      RGBDInstanceFrontendModule::fillOutputPacketWithTracks, per feature  RGBDInstanceFrontendModule.cc:391-486
  *   dynofront_dense_cloud       Frame::projectToDenseCloud          Frame.cc:172-238
  *   dynofront_track_dynamic_klt FeatureTracker::trackDynamicKLT + requiresSampling: LK, checks, circles, GFTT + ANMS per object  FeatureTracker.cc:500-862,1018-1149
+ *   dynofront_object_boundary   FeatureTracker::objectDetection with a provided mask: vision_tools::computeObjectMaskBoundaryMask
+ *                               (FeatureTracker.cc:1151-1210, VisionTools.cc:286-449)
  *   dynofront_klt_track         cv::calcOpticalFlowPyrLK as called by KltFeatureTracker::trackPoints
  *                               (StaticFeatureTracker.cc:420-625) and FeatureTracker::trackDynamicKLT (FeatureTracker.cc:500-862)
  * Images are row-major, tightly packed: flow float32[H][W][2] (CV_32FC2), masks int32[H][W] (CV_32S, ObjectId),
@@ -59,6 +61,26 @@ int dynofront_next_frame(dynofront_handle h, const uint8_t* gray, const float* f
 int dynofront_pin_host(dynofront_handle h, void* ptr, size_t bytes);     /* cudaHostRegister / Unregister of a caller buffer */
 int dynofront_unpin_host(dynofront_handle h, void* ptr);
 int dynofront_get_motion_mask(dynofront_handle h, int32_t* out);          /* the current frame's motion mask as it is on the device */
+
+/* FeatureTracker::objectDetection with prefer_provided_object_detection (FeatureTracker.cc:1151-1210): vision_tools::
+ * computeObjectMaskBoundaryMask (VisionTools.cc:286-449) on the current motion mask as set_frame / next_frame uploaded it (the
+ * reference runs it before propogateMask), in one call; nothing returns to the host between the stages.
+ *   thickness: the outer border in pixels; < 0 takes objectDetection's scaled value std::round(W*H / (640*480) * 640/480 * 7.51)
+ *     for the handle's size.  The inner border is 10 pixels (VisionTools.cc:412);
+ *   objects (the labels > 0 present, ascending), bb [][4] (x, y, w, h: ObjectBoundaryMaskResult::object_bounding_boxes) and
+ *     inner_bb [][4] (inner_boarder_object_bounding_boxes, (0, 0, 0, 0) for an object the inner erosion removes):
+ *     *n_objects = how many objects there are, the first min(n_objects, capacity) rows are written;
+ *   boundary_out (u8[H][W], may be NULL): the boundary mask, 0 in the band around each object and 255 elsewhere.  It also becomes
+ *     the current frame's boundary mask on the device, exactly as if it had been uploaded through next_frame: the detection mask of
+ *     dynofront_track_dynamic / dynofront_track_dynamic_klt (detection_mask_impl), dynofront_detect_static, dynofront_dense_cloud
+ *     and the sampling calls.  objects / inner_bb go to dynofront_track_dynamic_klt as they are.
+ * Divergence: the reference visits labels in unordered_set order, so where the 1x11 dilations of two objects overlap its
+ * drawContours leaves either label; here objects are drawn in ascending label order and the larger label wins.
+ * Refused with -1, the resident boundary mask left as it was: no motion mask uploaded, dynofront_propagate_mask already run on
+ * this frame's resident mask (an upload clears that), a label < 0 or > 255 (the reference CHECKs > 255 and would draw a negative
+ * one as 0), a thickness above 127 (the scaled value reaches 120 at 2560 x 1440). */
+int dynofront_object_boundary(dynofront_handle h, int32_t thickness, int32_t capacity, int32_t* n_objects, int32_t* objects, int32_t* bb,
+                              int32_t* inner_bb, uint8_t* boundary_out, float* ms_device);
 
 /* trackDynamic: n previous dynamic features (predicted key-point at this frame, object label, age, tracklet id),
  * iterated in array order.  Outputs are per input feature (rows of rejected features are zero); new tracklet ids
