@@ -34,6 +34,7 @@ EXPORTS = [
     "dynoba_pnp_ransac_default_params", "dynoba_pnp_ransac_batch",
     "dynoba_imu_default_params", "dynoba_imu_preintegrate_batch",
     "dynoba_object_srif_default_params", "dynoba_object_srif_batch",
+    "dynoba_triangulate_batch",
 ]
 PREINT_OK, PREINT_NOT_PD = 0, 1                               # DYNOBA_PREINT_*
 LM_TRACE_COLS = ("iterations", "inner", "lambda", "oldLin", "lin", "err", "nerr", "solved", "success", "stop")
@@ -41,6 +42,7 @@ TRACK_VALID, TRACK_FEW_MATCHES, TRACK_INVALID = 0, 2, 3      # DYNOBA_TRACK_* (d
 SRIF_NEW, SRIF_RESET, SRIF_CONTINUE = 0, 1, 2                # DYNOBA_SRIF_* modes
 SRIF_OK, SRIF_TOO_FEW, SRIF_NO_INLIERS = 0, 1, 2             # DYNOBA_SRIF_* statuses
 SRIF_STATE = 90                                              # DYNOBA_SRIF_STATE: R [36] | d [6] | H_lin, L_e, prev_H, X_K [12]
+TRI_OK, TRI_DEGENERATE, TRI_BEHIND_CAMERA, TRI_OUTLIER = 0, 1, 2, 3  # DYNOBA_TRI_* statuses
 
 
 class LmParams(C.Structure):
@@ -162,6 +164,7 @@ def load():
         L.dynoba_object_srif_default_params.argtypes = [C.POINTER(SrifParams)]
         L.dynoba_object_srif_batch.argtypes = [C.c_int, C.c_int32, c_ip, c_ip, c_ip, c_dp, c_dp, c_dp, C.POINTER(SrifParams), c_dp, c_dp,
                                                c_dp, c_u8p, c_dp, c_dp, c_u8p, c_ip, c_u8p, c_dp, c_dp, c_dp, c_dp, c_ip]
+        L.dynoba_triangulate_batch.argtypes = [C.c_int, C.c_int32, c_ip, c_dp, c_dp, c_dp, C.c_double, C.c_double, c_dp, c_ip, c_dp, c_dp]
         L.dynoba_imu_default_params.argtypes = [C.POINTER(ImuParams)]
         L.dynoba_imu_preintegrate_batch.argtypes = [C.c_int, C.POINTER(ImuParams), C.c_int32, c_ip, c_dp, c_dp, c_dp, c_dp, c_dp,
                                                     c_dp, c_ip]
@@ -768,3 +771,35 @@ def imu_preintegrate_batch(params, stamps, acc_gyr, bias_hat=None, device: int =
     if rc != 0:
         raise DynobaError(rc, L.dynoba_status_string(rc).decode())
     return dict(record=rec, cov=cov, sqrt_info=R, status=status)
+
+
+def triangulate_arrays(problems):
+    """the flat arrays of dynoba_triangulate_batch for a list of problems: dicts with poses [m, 12] (camera poses in the
+    world, R row-major | t), kp [m, 2] (pixels) and calib [5] (fx fy s u0 v0) -- inputs, then zeroed outputs"""
+    n = len(problems)
+    cnt = [np.asarray(q["kp"]).reshape(-1, 2).shape[0] for q in problems]
+    off = np.zeros(n + 1, dtype=np.int32); off[1:] = np.cumsum(cnt)
+    a = dict(off=off, poses=_cat(problems, "poses", 12) if n else np.zeros((0, 12)), kp=_cat(problems, "kp", 2) if n else np.zeros((0, 2)),
+             calib=_cat(problems, "calib", 5) if n else np.zeros((0, 5)))
+    a.update(point=np.zeros((n, 3)), status=np.zeros(n, dtype=np.int32), reproj=np.zeros(n), sv=np.zeros((n, 4)))
+    return a
+
+
+def triangulate_call(fn, a, rank_tol, reproj_threshold, *lead):
+    """fn(*lead, n_problems, <the arrays of dynoba_triangulate_batch>) -> status"""
+    return fn(*lead, len(a["off"]) - 1, _ip(a["off"]), _dp(a["poses"]), _dp(a["kp"]), _dp(a["calib"]), C.c_double(rank_tol),
+              C.c_double(reproj_threshold), _dp(a["point"]), _ip(a["status"]), _dp(a["reproj"]), _dp(a["sv"]))
+
+
+def triangulate_batch(problems, device: int = 0, rank_tol: float = 1.0, reproj_threshold: float = 3.0):
+    """gtsam::triangulateSafe (default TriangulationParameters) and the stereo formulation's reprojection test for every
+    problem in ONE launch (dynoba_triangulate_batch; the reference triangulates one landmark at a time in
+    StaticFormulationUpdater::StereoProjection::addLandmark).  problems: dicts with poses [m, 12], kp [m, 2], calib [5]; a
+    stereo frame is two cameras, the right one at X * (I, (baseline, 0, 0)).  Returns dict(status [n] (TRI_*), point [n, 3],
+    reproj [n] (norm of the stacked reprojection errors), sv [n, 4] (A's singular values, descending))."""
+    L = load()
+    a = triangulate_arrays(problems)
+    rc = triangulate_call(L.dynoba_triangulate_batch, a, rank_tol, reproj_threshold, device)
+    if rc != 0:
+        raise DynobaError(rc, L.dynoba_status_string(rc).decode())
+    return dict(status=a["status"], point=a["point"], reproj=a["reproj"], sv=a["sv"])

@@ -47,6 +47,10 @@ class GraphBuilder:
         L.dynoba_builder_set_imu.argtypes = [C.c_void_p, C.c_int32, c_dp, c_dp]
         L.dynoba_builder_nav_counts.argtypes = [C.c_void_p, c_i64p, c_i64p]
         L.dynoba_builder_get_nav_variables.argtypes = [C.c_void_p, c_dp, c_dp, c_ip, c_ip, c_u64p, c_u64p]
+        L.dynoba_builder_set_static_stereo.argtypes = [C.c_void_p, c_dp, C.c_double, C.c_int]
+        L.dynoba_builder_add_static_stereo.argtypes = [C.c_void_p, C.c_int32, C.c_int64, c_i64p, c_dp]
+        L.dynoba_builder_static_stereo_stats.argtypes = [C.c_void_p, c_i64p, c_i64p, c_i64p]
+        self.calib = None
         prm = BuilderParams(); L.dynoba_builder_default_params(C.byref(prm))
         for k, v in params.items():
             if k in ("odometry_sigma", "smoothing_sigma"):
@@ -97,6 +101,24 @@ class GraphBuilder:
         z = np.ascontiguousarray(record, np.float64).reshape(70); R = np.ascontiguousarray(sqrt_info, np.float64).reshape(225)
         self._ck(self.lib.dynoba_builder_set_imu(self.h, int(frame), _dp(z), _dp(R)))
 
+    def set_static_stereo(self, calib6, sigma_px, device=-1):
+        """static landmarks by stereo projection (STEREO_PROJECTION): calib6 = fx fy s u0 v0 baseline, sigma_px the pixel sigma
+        of the GenericStereoFactors, device the GPU that triangulates at finalize (< 0: the host build)"""
+        K = np.ascontiguousarray(calib6, np.float64).reshape(6)
+        self._ck(self.lib.dynoba_builder_set_static_stereo(self.h, _dp(K), float(sigma_px), int(device)))
+        self.calib = K.copy()
+
+    def add_static_stereo(self, frame, tracklet, stereo):
+        """stereo measurements [n, 3] = (uL, uR, v) of the static tracklets seen at `frame` (uR NaN: no right key-point)"""
+        t = np.ascontiguousarray(tracklet, np.int64); z = np.ascontiguousarray(stereo, np.float64).reshape(-1, 3)
+        self._ck(self.lib.dynoba_builder_add_static_stereo(self.h, int(frame), t.size, t.ctypes.data_as(c_i64p), _dp(z)))
+
+    def static_stereo_stats(self):
+        """dict(added, failed {status: attempts}, never_added) of the stereo landmarks (dynoba_builder_static_stereo_stats)"""
+        added = C.c_int64(); never = C.c_int64(); failed = (C.c_int64*4)()
+        self._ck(self.lib.dynoba_builder_static_stereo_stats(self.h, C.byref(added), failed, C.byref(never)))
+        return dict(added=added.value, failed=list(failed), never_added=never.value)
+
     def problem(self) -> Problem:
         """the emitted SoA problem as a Problem container"""
         L = self.lib
@@ -123,7 +145,8 @@ class GraphBuilder:
         self._ck(L.dynoba_builder_get_nav_variables(self.h, _dp(vel), _dp(bias), vo.ctypes.data_as(c_ip), bo.ctypes.data_as(c_ip),
                                                     self.nav_keys[0].ctypes.data_as(c_u64p), self.nav_keys[1].ctypes.data_as(c_u64p)))
         nav = dict(vel=vel, bias=bias, vel_order=vo, bias_order=bo) if nv.value else {}
-        return Problem(pose, point, aux_pose=aux, blocks=blocks, pose_order=order, pose_keys=pk, point_keys=qk, **nav)
+        extra = dict(calib=self.calib) if self.calib is not None else {}
+        return Problem(pose, point, aux_pose=aux, blocks=blocks, pose_order=order, pose_keys=pk, point_keys=qk, **nav, **extra)
 
     def emit(self, solver):
         """hand the arrays to a dynosam_b200.binding.Solver handle (no Problem container in between)"""

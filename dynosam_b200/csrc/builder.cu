@@ -42,6 +42,7 @@
 #include "../../include/dynoba.h"
 #include "se3.cuh"
 #include "preint.cuh"
+#include "triangulate.cuh"
 
 using namespace dynoba;
 
@@ -69,6 +70,10 @@ struct dynoba_builder {
   std::vector<Obs> stat, dyn;
   std::map<std::pair<int32_t, int32_t>, Pose> motion_init, keyframe_pose;    // (object, frame)
   std::map<int32_t, ImuMeas> imu;                                // frame -> preintegrated measurement from the previous frame
+  // STEREO_PROJECTION static landmarks (dynoba_builder_set_static_stereo): (frame, tracklet, uL uR v) per observation
+  bool stereo = false; double calib6[6] = {}; double sigma_px = 0; int stereo_device = -1;
+  std::vector<Obs> stereo_obs;
+  int64_t st_added = 0, st_failed[4] = {}, st_never = 0;
   // products
   std::vector<double> pose, point, aux; std::vector<int32_t> order; std::vector<uint64_t> pose_keys, point_keys;
   std::vector<double> vel, bias; std::vector<int32_t> nav_order; std::vector<uint64_t> vel_keys, bias_keys;
@@ -105,6 +110,7 @@ int dynoba_builder_add_frame(dynoba_builder_handle b, int32_t frame, const doubl
 }
 int dynoba_builder_add_static(dynoba_builder_handle b, int32_t frame, int64_t n, const int64_t* tracklet, const double* z) {
   BARG(b && n >= 0 && (n == 0 || (tracklet && z)), "bad static observations");
+  BARG(!b->stereo, "static landmarks use the stereo formulation: add them with dynoba_builder_add_static_stereo");
   for (int64_t i = 0; i < n; i++) b->stat.push_back(Obs{ frame, tracklet[i], 0, { z[3*i], z[3*i + 1], z[3*i + 2] } });
   b->finalized = false; return DYNOBA_OK;
 }
@@ -129,6 +135,112 @@ int dynoba_builder_set_imu(dynoba_builder_handle b, int32_t frame, const double*
   ImuMeas& m = b->imu[frame];
   std::copy(record, record + 70, m.z); std::copy(sqrt_info, sqrt_info + 225, m.R);
   b->finalized = false; return DYNOBA_OK;
+}
+
+int dynoba_builder_set_static_stereo(dynoba_builder_handle b, const double* calib6, double sigma_px, int device) {
+  BARG(b && calib6, "null");
+  BARG(b->stat.empty(), "point-to-point static observations were added already");
+  for (int i = 0; i < 6; i++) BARG(std::isfinite(calib6[i]), "calibration not finite");
+  BARG(calib6[0] > 0.0 && calib6[1] > 0.0 && calib6[5] > 0.0, "fx, fy and the baseline must be positive");
+  BARG(std::isfinite(sigma_px) && sigma_px > 0.0, "sigma_px must be positive and finite");
+  b->stereo = true; std::copy(calib6, calib6 + 6, b->calib6); b->sigma_px = sigma_px; b->stereo_device = device;
+  b->finalized = false; return DYNOBA_OK;
+}
+int dynoba_builder_add_static_stereo(dynoba_builder_handle b, int32_t frame, int64_t n, const int64_t* tracklet, const double* stereo) {
+  BARG(b && n >= 0 && (n == 0 || (tracklet && stereo)), "bad static stereo observations");
+  BARG(b->stereo, "select the stereo formulation first (dynoba_builder_set_static_stereo)");
+  for (int64_t i = 0; i < n; i++)
+    BARG(std::isfinite(stereo[3*i]) && std::isfinite(stereo[3*i + 2]) && (std::isfinite(stereo[3*i + 1]) || std::isnan(stereo[3*i + 1])),
+         "a stereo measurement needs finite uL and v, and a finite or NaN uR");
+  for (int64_t i = 0; i < n; i++) b->stereo_obs.push_back(Obs{ frame, tracklet[i], 0, { stereo[3*i], stereo[3*i + 1], stereo[3*i + 2] } });
+  b->finalized = false; return DYNOBA_OK;
+}
+int dynoba_builder_static_stereo_stats(dynoba_builder_handle b, int64_t* added, int64_t* failed, int64_t* never_added) {
+  BARG(b, "null builder"); int rc = dynoba_builder_finalize(b); if (rc) return rc;
+  if (added) *added = b->st_added;
+  if (failed) std::copy(b->st_failed, b->st_failed + 4, failed);
+  if (never_added) *never_added = b->st_never;
+  return DYNOBA_OK;
+}
+
+// STEREO_PROJECTION static landmarks (Formulation-impl.hpp:258-411): attempts in rounds by observation index, one batched
+// triangulation per round (dynoba_triangulate_batch on stereo_device, or the host build of triangulate.cuh), then the
+// landmarks, their initial values and the STEREO3 block
+static int stereo_landmarks(dynoba_builder* b, const std::map<int32_t, int32_t>& cam_index) {
+  b->st_added = b->st_never = 0; std::fill(b->st_failed, b->st_failed + 4, 0);
+  auto by_frame = [](const Obs& a, const Obs& c) { return a.frame < c.frame; };
+  std::stable_sort(b->stereo_obs.begin(), b->stereo_obs.end(), by_frame);
+  std::map<int64_t, size_t> slot; std::vector<int64_t> tid; std::vector<std::vector<size_t>> tracks;   // first-appearance order
+  size_t longest = 0;
+  for (size_t i = 0; i < b->stereo_obs.size(); i++) {
+    const Obs& o = b->stereo_obs[i];
+    BARG(cam_index.count(o.frame), "static observation in an unknown frame");
+    auto it = slot.find(o.tracklet);
+    if (it == slot.end()) { it = slot.emplace(o.tracklet, tracks.size()).first; tid.push_back(o.tracklet); tracks.emplace_back(); }
+    auto& t = tracks[it->second];
+    BARG(t.empty() || b->stereo_obs[t.back()].frame < o.frame, "a static tracklet is observed twice in one frame");
+    t.push_back(i); longest = std::max(longest, t.size());
+  }
+  const double* K = b->calib6; const double base = K[5];
+  auto disparity_ok = [](const Obs& o) { return o.z[0] - o.z[1] > 0.5; };      // false for a NaN uR
+  std::vector<int> added_at(tracks.size(), -1); std::vector<double> point(3*tracks.size());
+  std::vector<int32_t> off, st; std::vector<double> poses, kp, cal, pt; std::vector<size_t> which;
+  for (size_t r = 0; r < longest; r++) {
+    off.assign(1, 0); poses.clear(); kp.clear(); cal.clear(); which.clear();
+    for (size_t ti = 0; ti < tracks.size(); ti++) {
+      if (added_at[ti] >= 0 || tracks[ti].size() <= r) continue;
+      for (size_t j = 0; j <= r; j++) {
+        const Obs& o = b->stereo_obs[tracks[ti][j]];
+        const Pose& X = b->frames.at(o.frame).first;                  // hasInitialSensorPose: the add_frame pose
+        double p[12]; pose_to(X, p);
+        poses.insert(poses.end(), p, p + 12); kp.push_back(o.z[0]); kp.push_back(o.z[2]);
+        if (!std::isnan(o.z[1])) {                                     // right camera X * (I, (b, 0, 0))
+          for (int k = 0; k < 3; k++) p[9 + k] = X.t[k] + base*X.R[3*k];
+          poses.insert(poses.end(), p, p + 12); kp.push_back(o.z[1]); kp.push_back(o.z[2]);
+        }
+      }
+      off.push_back((int32_t)(poses.size()/12)); cal.insert(cal.end(), K, K + 5); which.push_back(ti);
+    }
+    if (which.empty()) continue;
+    const int32_t np = (int32_t)which.size();
+    st.assign(np, 0); pt.assign(3*(size_t)np, 0.0);
+    if (b->stereo_device >= 0) {
+      const int rc = dynoba_triangulate_batch(b->stereo_device, np, off.data(), poses.data(), kp.data(), cal.data(), 1.0, 3.0,
+                                              pt.data(), st.data(), nullptr, nullptr);
+      if (rc) { b->err = "dynoba_triangulate_batch failed"; return rc; }
+    } else {
+      std::vector<double> A;
+      for (int32_t p = 0; p < np; p++) {
+        const int m = off[p + 1] - off[p]; A.resize(8*(size_t)m);
+        TriHostLanes lanes; TriOut o;
+        tri_solve(m, poses.data() + 12*(size_t)off[p], kp.data() + 2*(size_t)off[p], K, 1.0, 3.0, A.data(), lanes, o);
+        st[p] = o.status; for (int k = 0; k < 3; k++) pt[3*(size_t)p + k] = o.point[k];
+      }
+    }
+    for (int32_t p = 0; p < np; p++) {
+      const size_t ti = which[p];
+      if (st[p] != DYNOBA_TRI_OK) { b->st_failed[st[p]]++; continue; }
+      int good = 0;
+      for (size_t j = 0; j <= r; j++) good += disparity_ok(b->stereo_obs[tracks[ti][j]]);
+      if (good < 2) { b->st_failed[DYNOBA_TRI_OK]++; continue; }
+      added_at[ti] = (int)r; for (int k = 0; k < 3; k++) point[3*ti + k] = pt[3*(size_t)p + k];
+    }
+  }
+  Block blk; blk.type = DYNOBA_STEREO3; blk.sigma.assign(3, b->sigma_px); blk.sigma_dim = 3; blk.k = b->prm.huber_k;
+  for (size_t ti = 0; ti < tracks.size(); ti++) {
+    if (added_at[ti] < 0) { b->st_never++; continue; }
+    b->st_added++;
+    const int32_t pi = (int32_t)(b->point.size()/3);
+    b->point.insert(b->point.end(), &point[3*ti], &point[3*ti] + 3); b->point_keys.push_back(sym('l', (uint64_t)tid[ti]));
+    for (size_t j = 0; j < tracks[ti].size(); j++) {
+      const Obs& o = b->stereo_obs[tracks[ti][j]];
+      // at the attempt that added it: the observations with disparity > 0.5; afterwards every one with a right key-point
+      if ((int)j <= added_at[ti] ? !disparity_ok(o) : std::isnan(o.z[1])) continue;
+      blk.idx.push_back(cam_index.at(o.frame)); blk.idx.push_back(pi); blk.meas.insert(blk.meas.end(), o.z, o.z + 3);
+    }
+  }
+  if (blk.n()) b->blocks.push_back(std::move(blk));
+  return DYNOBA_OK;
 }
 
 int dynoba_builder_finalize(dynoba_builder_handle b) {
@@ -190,7 +302,8 @@ int dynoba_builder_finalize(dynoba_builder_handle b) {
     for (auto& o : b->dyn) if (count[{o.object, o.tracklet}] >= min_dyn && seen[{o.object, o.tracklet}]++ >= start_d) dyn.push_back(o);
   }
   // ---- static landmarks: tracklets in order of first appearance (frame-major, insertion order inside a frame)
-  {
+  if (b->stereo) { int rc = stereo_landmarks(b, cam_index); if (rc) return rc; }
+  else {
     std::map<int64_t, std::vector<size_t>> tracks; std::vector<int64_t> first_seen;
     for (size_t i = 0; i < stat.size(); i++) { BARG(cam(stat[i].frame) >= 0, "static observation in an unknown frame");
       auto& t = tracks[stat[i].tracklet]; if (t.empty()) first_seen.push_back(stat[i].tracklet); t.push_back(i); }
@@ -404,6 +517,7 @@ int dynoba_builder_emit(dynoba_builder_handle b, dynoba_handle h) {
   if ((rc = dynoba_set_variables(h, DYNOBA_POSE6, (int64_t)b->pose.size()/12, b->pose_keys.data(), b->pose.data()))) return rc;
   if ((rc = dynoba_set_variables(h, DYNOBA_POINT3, (int64_t)b->point.size()/3, b->point_keys.data(), b->point.data()))) return rc;
   if (!b->aux.empty() && (rc = dynoba_set_aux_poses(h, (int64_t)b->aux.size()/12, b->aux.data()))) return rc;
+  if (b->stereo && (rc = dynoba_set_calibration(h, b->calib6))) return rc;
   const int64_t nn = (int64_t)b->nav_order.size();
   if (nn) {
     if ((rc = dynoba_set_variables(h, DYNOBA_VEL3, nn, b->vel_keys.data(), b->vel.data()))) return rc;

@@ -377,6 +377,28 @@ int dynoba_builder_emit(dynoba_builder_handle b, dynoba_handle h);
  * builder emits what it always did.  dynoba_builder_emit also sets the velocities / biases (keys Symbol('V', frame),
  * Symbol('b', frame)) and their order hints (the frame id). */
 int dynoba_builder_set_imu(dynoba_builder_handle b, int32_t frame, const double* record, const double* sqrt_info);
+/* Static landmarks by stereo projection (the reference's --static_formulation_type=2, STEREO_PROJECTION;
+ * Formulation-impl.hpp:258-411).  set_static_stereo selects it: calib6 = fx fy s u0 v0 baseline (Cal3_S2Stereo), sigma_px
+ * the pixel sigma of every GenericStereoFactor (Diagonal (sigma_px x3), Huber huber_k as the other static factors), device
+ * the GPU that runs the triangulations at finalize (dynoba_triangulate_batch), or < 0 for the host build of the same
+ * statement.  It is refused after dynoba_builder_add_static, and add_static after it.  add_static_stereo adds stereo[n][3] =
+ * (uL, uR, v) of the static tracklets seen at `frame`; uR may be NaN (no right key-point), uL and v must be finite.
+ * At finalize every tracklet is attempted at each of its observations, in frame order, until it is added: the attempt at
+ * its j-th observation triangulates (triangulateSafe, rank_tol 1.0, then the 3 px test; triangulate.cuh) over the left
+ * camera X_i and, where uR is not NaN, the right camera X_i * (I, (baseline, 0, 0)) of its observations 0..j, X_i the
+ * add_frame pose.  A valid point with at least two of those observations with uL - uR > 0.5 adds the landmark with the
+ * triangulated initial value, one STEREO3 factor for each of them and one for each later observation with a right
+ * key-point.  Attempts run in rounds by observation index, one batch per round over the tracklets still pending.
+ * min_static_obs and backtrack do not apply.  Deliberate divergence: the reference CHECK-fails on a measurement without a
+ * right key-point; here it adds only its left camera to an attempt, and no factor.  dynoba_builder_emit also calls
+ * dynoba_set_calibration(calib6).  Refused (DYNOBA_ERR_BAD_ARG): non-finite calib6, fx, fy or baseline <= 0, sigma_px <= 0
+ * or not finite; a tracklet observed twice in one frame or in a frame that was not added (at finalize). */
+int dynoba_builder_set_static_stereo(dynoba_builder_handle b, const double* calib6, double sigma_px, int device);
+int dynoba_builder_add_static_stereo(dynoba_builder_handle b, int32_t frame, int64_t n, const int64_t* tracklet, const double* stereo);
+/* After finalize: *added landmarks; failed[4] attempts that did not add the landmark, by status: failed[DYNOBA_TRI_OK] a
+ * valid point with fewer than two factors, failed[DYNOBA_TRI_DEGENERATE / _BEHIND_CAMERA / _OUTLIER] the others (the ones
+ * for which the reference marks the landmark lmk->inlier = false); *never_added tracklets that no attempt added. */
+int dynoba_builder_static_stereo_stats(dynoba_builder_handle b, int64_t* added, int64_t* failed, int64_t* never_added);
 int dynoba_builder_nav_counts(dynoba_builder_handle b, int64_t* n_vel, int64_t* n_bias);
 int dynoba_builder_get_nav_variables(dynoba_builder_handle b, double* vel, double* bias, int32_t* vel_order, int32_t* bias_order,
                                      uint64_t* vel_keys, uint64_t* bias_keys);
@@ -538,6 +560,24 @@ void dynoba_imu_default_params(dynoba_imu_params* p);
 int dynoba_imu_preintegrate_batch(int device, const dynoba_imu_params* params, int32_t n_intervals, const int32_t* offsets,
                                   const double* stamps, const double* acc_gyr, const double* bias_hat, double* record,
                                   double* cov, double* sqrt_info, int32_t* status);
+
+/* Batched triangulation: gtsam::triangulateSafe with default TriangulationParameters (DLT by SVD, rank test, cheirality)
+ * and the reference's reprojection test, for many landmarks in one launch, one warp per problem.  The mathematics is stated
+ * in dynosam_b200/csrc/triangulate.cuh.  All pointers are HOST memory.  Problem p owns the cameras [offsets[p],
+ * offsets[p+1]) (offsets[0] = 0): poses[c][12] (the camera's pose in the world, R row-major | t) and kp[c][2] (its
+ * measurement in pixels); calib5[p][5] = fx fy s u0 v0 (Cal3_S2).  A stereo frame contributes two cameras.
+ * Outputs per problem: status (DYNOBA_TRI_*: fewer than two cameras, rank < 3 (singular values > rank_tol) or a point at
+ * infinity DEGENERATE; a depth <= 0 in any camera BEHIND_CAMERA; |stacked reprojection errors| > reproj_threshold OUTLIER),
+ * point_out[3] (v[0:3] / v[3]; NaN with fewer than two cameras), reproj_norm (NaN unless OK or OUTLIER) and sv_out[4] (A's
+ * singular values, descending; NaN with fewer than two cameras).  Any output pointer but status may be NULL.  The result
+ * of a problem does not depend on the other problems of the call.  Refused with DYNOBA_ERR_BAD_ARG before any device work:
+ * n_problems < 0 or >= 2^24, NULL arrays, offsets[0] != 0 or decreasing, more than 2^27 cameras, non-finite poses,
+ * key-points or calibration, fx or fy <= 0, rank_tol < 0 or not finite, reproj_threshold NaN or < 0 (+inf turns the test
+ * off).  n_problems = 0 is a no-op.  The call shares the batch entry points' per-device stream and workspace. */
+enum { DYNOBA_TRI_OK = 0, DYNOBA_TRI_DEGENERATE = 1, DYNOBA_TRI_BEHIND_CAMERA = 2, DYNOBA_TRI_OUTLIER = 3 };
+int dynoba_triangulate_batch(int device, int32_t n_problems, const int32_t* offsets, const double* poses, const double* kp,
+                             const double* calib5, double rank_tol, double reproj_threshold, double* point_out,
+                             int32_t* status, double* reproj_norm, double* sv_out);
 
 #ifdef __cplusplus
 }
